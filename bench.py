@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline measurement of the event -> voxel-grid hot path on B200.
+"""bench.py -- headline measurement of the event -> voxel-grid hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one voxel-grid build over one batch of synthetic events:
   N=1 : BASELINE.json configs[1] -- 50 M uniform events -> 5-bin 640x480 grid, reference
@@ -11,9 +11,11 @@ A "step" is one voxel-grid build over one batch of synthetic events:
 `value` is whole-job Mevents/s with the events resident in HBM, timed with CUDA events over
 exactly K steps, max over ranks.  `e2e` is the same metric through the public python API with
 pinned HOST tensors in and a host tensor out (H2D + D2H inside the timed region).
-`--impl reference` times the reference's OWN events_to_voxel_torch (the unmodified lib/ package that
-__graft_entry__.build() copies to the git-ignored baseline/_ref/, loaded through oracle/ref_loader.py) on the
-host cores; where that copy is missing it falls back to the library-op port (oracle/ref_port.py) and says so.
+`--impl reference` times the reference's OWN events_to_voxel_torch (an unmodified checkout named by
+$EVK_REFERENCE_ROOT, loaded through oracle/ref_loader.py) on the host cores; without one it times the
+library-op port (oracle/ref_port.py) and says so.
+`--dump-outputs DIR` writes the grid the timed path returned in its last step to DIR/voxel_grid.npy (float32), for
+either --impl; the inputs are generated from fixed seeds, so two builds can be compared output for output.
 Prints ONE JSON line on rank 0.
 """
 import argparse
@@ -34,7 +36,7 @@ N_PER_GPU = int(os.environ.get("EVK_BENCH_EVENTS", 50_000_000))
 B, H, W = 5, 480, 640
 CPU_SAMPLE = int(os.environ.get("EVK_BENCH_CPU_SAMPLE", 5_000_000))
 METRIC = "Mevents/s voxel-grid build (B=5, 640x480)"
-HBM_FALLBACK_GBS = 6650.0   # /opt/skills/guides/B200_PROFILING.md fallback
+HBM_PEAK_GBS = 3350.0       # H100 SXM data sheet: 3.35 TB/s HBM3
 
 
 def env_int(name, default):
@@ -44,24 +46,16 @@ def env_int(name, default):
         return default
 
 
-def measured_peak():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
 def workload_config(world, mg_kind=None):
     return {
-        "workload": ("50M uniform events -> 5x480x640 voxel grid (events_to_voxel_torch semantics), 1xB200"
+        "workload": ("50M uniform events -> 5x480x640 voxel grid (events_to_voxel_torch semantics), 1xH100"
                      if world == 1 else
                      "%dM events -> 5x480x640 voxel grid sharded over %d GPUs (50M-event time shard per GPU), "
                      "one all-reduce of the grid per step" % (50 * world, world)),
         "events_per_gpu": N_PER_GPU, "bins": B, "height": H, "width": W,
         "layout": "SoA f32 x,y,t,p (16 B/event)",
         "seed": 2024,
-        "l2_policy": "inputs (800 MB/step) larger than L2 (126 MB); no explicit flush",
+        "l2_policy": "inputs (800 MB/step) larger than L2 (50 MB); no explicit flush",
         "parallelism": ("events sharded x%d, global t0/dt agreed up front" % world) + ((
             "; fold + all-reduce fused in one kernel over NVLink peer memory (symmetric memory, two cross-GPU barriers), step k's reduce overlapped with the scatter of step k+1 (2 buffers)"
             if mg_kind == "peer" else "; NCCL all-reduce of step k overlapped with the scatter of step k+1 (2 grid buffers)") if world > 1 else ""),
@@ -182,8 +176,8 @@ def thread_candidates():
 
 def reference_functions():
     """(kind, voxel_torch(xs,ys,ts,ps) -> grid, voxel_numpy(xs_int,ys_int,ts,ps) -> grid): the reference's own
-    events_to_voxel_torch / events_to_voxel (kind "reference", the unmodified lib/ copy in baseline/_ref/), or the
-    library-op port (kind "port") where that copy is not present."""
+    events_to_voxel_torch / events_to_voxel (kind "reference", the unmodified checkout named by $EVK_REFERENCE_ROOT),
+    or the library-op port (kind "port") where none is named."""
     try:
         from oracle import ref_loader
         if ref_loader.available():
@@ -257,8 +251,11 @@ def run_reference(args, rank, world):
         voxel_torch(xs, ys, ts, ps)
     s = time.perf_counter()
     for _ in range(args.steps):
-        voxel_torch(xs, ys, ts, ps)
+        grid = voxel_torch(xs, ys, ts, ps)
     el = time.perf_counter() - s
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "voxel_grid.npy"), grid.float().numpy())
     value = n * args.steps / el / 1e6
     what = ("the reference's own events_to_voxel_torch (unmodified lib/ package from %s)" % where if kind == "reference" else
             "events_to_voxel_torch library-op port (oracle/ref_port.py; the reference package is not present here)")
@@ -366,6 +363,9 @@ def run_ours(args, rank, local_rank, world):
     L.evk_prof_enable(0)
     if world == 1:
         assert int(oob.item()) == 0
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "voxel_grid.npy"), out.float().cpu().numpy())
     # sanity inside the bench: every event deposits its polarity once
     total = float(out.double().sum())
     if world > 1:
@@ -380,16 +380,10 @@ def run_ours(args, rank, local_rank, world):
     assert abs(total - expect) <= 1e-6 * n * world + 4.0, (total, expect)
 
     value = n * world * args.steps / elapsed_ms / 1e3          # Mevents/s, whole job
-    peak, peak_src = measured_peak()
+    peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet (3.35 TB/s)"
     alg_bytes = 16.0 * n + 4.0 * B * H * W                       # SURVEY 8d: 16 B/event + the grid once
     k_ms = kms.value / max(1, ktimed.value)
     achieved = alg_bytes / (k_ms * 1e-3) / 1e9 if k_ms > 0 else 0.0
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_summary.json")) as f:
-            traffic = json.load(f).get("voxel_scatter_dram_bytes_per_launch")
-    except Exception:
-        pass
 
     # ---- end to end through the public API: pinned host tensors in, host tensor out --------------
     hx, hy, ht, hp = (torch.empty(n, dtype=torch.float32, pin_memory=True) for _ in range(4))
@@ -556,16 +550,13 @@ def run_ours(args, rank, local_rank, world):
             "max_rel_err_vs_oracle": ((extra or {}).get("multi_gpu_parity", {}).get("peer", {}) or {}).get("max_rel_err_vs_oracle")
             if world > 1 and isinstance((extra or {}).get("multi_gpu_parity", {}).get("peer"), dict) else None,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak if peak else None, "traffic": traffic,
-                         "traffic_source": "profiles/ncu_summary.json (dram__bytes_read+write of this kernel from the committed ncu --set full capture; NOT measured in this run)",
+                         "frac": achieved / peak if peak else None,
                          "kernel": "voxel_scatter_kernel<QUAD> (one red.global.add.v4.f32 per event), chosen over the hot-pixel-table instantiation by the launch-level contention probe; the timed scope covers probe + both launches",
                          "kernel_ms": k_ms, "launches_timed": int(ktimed.value),
                          "algorithmic_bytes_per_launch": alg_bytes, "peak_source": peak_src,
                          "step_frac": (alg_bytes / (elapsed_ms / args.steps * 1e-3) / 1e9) / peak,
-                         # the limiter ncu shows is the L2 scattered-reduction rate, not HBM: report it beside the contract's HBM fraction
-                         "l2_reduction_rate": {"achieved_gops": (n / (k_ms * 1e-3) / 1e9) if k_ms > 0 else None, "ceiling_gops": 190.0,
-                                               "ceiling_source": "tools/exp/tma_red.cu: 50 M red.global.add.v4.f32 to random 16-B slots of 9.8 MB in 0.263 ms",
-                                               "frac": (n / (k_ms * 1e-3) / 1e9 / 190.0) if k_ms > 0 else None}},
+                         # the kernel is bound by the rate at which L2 retires the scattered reductions (one per event), not by HBM
+                         "l2_reduction_rate": {"achieved_gops": (n / (k_ms * 1e-3) / 1e9) if k_ms > 0 else None}},
             "cpu_baseline": cpu,
         }
         if e2e_packed:
@@ -870,7 +861,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-extra", action="store_true", help="skip the secondary (cmax) numbers")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the grid the timed path returned in its last step to DIR/voxel_grid.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be at least 1 and --warmup at least 0")
     rank, world, local_rank = env_int("RANK", 0), env_int("WORLD_SIZE", 1), env_int("LOCAL_RANK", 0)
     if args.impl == "reference":
         run_reference(args, rank, world)

@@ -1,4 +1,4 @@
-"""event_utils_b200 -- B200-native (sm_100a) drop-in for the data-parallel hot path of
+"""event_utils_b200 -- H100-native (sm_90a) drop-in for the data-parallel hot path of
 TimoStoff/event_utils: event -> voxel grid / event image binning and the contrast-maximisation
 inner loop.  Same Python function signatures as the reference; the work is done by hand-written
 CUDA kernels in libevk.so (C ABI: include/evk.h).  No CPU fallback.

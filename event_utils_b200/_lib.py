@@ -1,7 +1,7 @@
 """ctypes binding of libevk.so (the C ABI declared in include/evk.h).
 
-There is NO CPU fallback: if the shared library is missing or the device is not a B200-class
-(sm_100) GPU, every compute entry point raises.  Build with ``python -c "import
+There is NO CPU fallback: if the shared library is missing or the device is not an H100-class
+(sm_90) GPU, every compute entry point raises.  Build with ``python -c "import
 __graft_entry__ as g; g.build()"`` or ``make -C event_utils_b200/csrc``.
 """
 import ctypes
@@ -165,10 +165,10 @@ _device_ok = {}
 
 
 def lib():
-    """Library handle for compute calls: requires a CUDA device of compute capability 10.x."""
+    """Library handle for compute calls: requires a CUDA device of compute capability 9.0."""
     L = load()
     if not torch.cuda.is_available():
-        raise EvkError("event_utils_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise EvkError("event_utils_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     dev = torch.cuda.current_device()
     if dev not in _device_ok:
         check_device(dev)
@@ -210,8 +210,8 @@ UPLOAD_MIN_BYTES = 4 << 20      # below this torch's own copy is as fast (one st
 
 def upload(host_tensors, device):
     """CPU tensors -> new device tensors of the same dtype / shape.  Large ordinary (pageable) tensors -- what numpy hands
-    over -- take evk_host_upload (pinned bounce slots filled by the library's worker pool, ~50 GB/s instead of the
-    driver's ~10 GB/s staged copy); small or non-contiguous ones take torch's copy.  The result is complete on return."""
+    over -- take evk_host_upload (pinned bounce slots filled by the library's worker pool; on the H100 host of
+    DESIGN.md section 6 about 34 GB/s against 7 GB/s for the driver's staged copy); small or non-contiguous ones take torch's copy.  The result is complete on return."""
     host_tensors = list(host_tensors)
     big = [i for i, t in enumerate(host_tensors)
            if (not t.is_cuda) and t.is_contiguous() and t.numel() * t.element_size() >= UPLOAD_MIN_BYTES]

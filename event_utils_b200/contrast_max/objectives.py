@@ -44,7 +44,7 @@ precision = "f64"          # "f64": parity mode (events kept as f64, 32 B/event)
 
 def _fingerprints(arrays):
     """Identity of host arrays for the caches: length, dtype and a 64-bit hash of EVERY byte
-    (evk_host_hash64_multi, ~10 GB/s per thread, threaded above 2 MiB).  The reference's objective is a pure
+    (evk_host_hash64_multi, threaded above 2 MiB).  The reference's objective is a pure
     function of the arrays it is handed (objectives.py:211-236): a device copy or a memoised result may be
     reused only when the arrays are byte-identical to the ones it was made from -- a sampled fingerprint
     would silently return the previous stream's f / g after a partial in-place edit."""
@@ -118,8 +118,8 @@ def _result_buffers(dev):
     """Per-device result buffer reused across evaluations: 12 doubles of PINNED HOST memory that the
     last kernel of an evaluation writes straight over PCIe (pinned allocations are device-addressable
     under unified addressing), so reading a result back is one stream synchronise -- no device buffer,
-    no D2H copy operation (a fresh torch.zeros + pageable .cpu() per call cost ~25 us of a ~90 us
-    evaluation, a pinned mirror + copy_ still ~10 us).  Returns (tensor, numpy view)."""
+    no D2H copy operation (a fresh torch.zeros + pageable .cpu() per call, or even a pinned mirror + copy_, is a
+    noticeable share of a small evaluation).  Returns (tensor, numpy view)."""
     k = (dev, torch.cuda.current_stream(dev).cuda_stream, threading.get_ident())   # per stream AND host thread: reuse is only safe in stream order
     b = _result_bufs.get(k)
     if b is None:

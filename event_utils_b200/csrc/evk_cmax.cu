@@ -1,4 +1,4 @@
-// evk_cmax.cu -- fused contrast-maximisation evaluation on B200:
+// evk_cmax.cu -- fused contrast-maximisation evaluation on H100:
 //   warp -> bounds mask -> bilinear IWE (+ Jacobian-weighted derivative images) -> Gaussian
 //   blur -> variance objective and its analytic gradient, one pass over the events.
 //
@@ -11,23 +11,22 @@
 //   variance_objective            lib/contrast_max/objectives.py:231-236, 251-264
 //   warp_events_flow_torch + IWE  lib/transforms/optic_flow.py:37-44, lib/visualization/draw_flow.py:18-21
 //
-// B200 design (DESIGN.md section 4):
+// Design (DESIGN.md section 4):
 //   * ONE pass over the events.  The accumulator is an array of 32-byte BLOCKS, one per pixel:
 //     block (y,x) = {I_TL, I_TR, I_BL, I_BR, a, b, c, d} collects every event whose bilinear
 //     footprint is anchored at (y,x) (each pixel therefore lives in four blocks; a gather kernel
 //     folds them).  The 2x2 IWE footprint of an event is ONE red.global.add.v4.f32
 //     (REDG.E.ADD.F32x4); the 8 derivative taps have only 4 free values (the taps of a derivative
 //     image come in +/- pairs, image.py:131-135), so both derivative images are ONE more vector
-//     reduction: 1 RED per event for f, 2 for f and g, instead of 4 / 12 scalar ones.  Measured:
-//     every scatter kernel on B200 costs ~0.25 ms per RED lane-operation per 50 M events,
-//     whatever its width (scalar, v2, v4) and whether or not lanes share a sector -- the count of
-//     reduction operations is what has to be minimised.  The accumulator (181*241*32 B = 1.4 MB
+//     reduction: 1 RED per event for f, 2 for f and g, instead of 4 / 12 scalar ones.  A scatter
+//     kernel pays per RED lane-operation, whatever its width (scalar, v2, v4) and whether or not
+//     lanes share a sector -- the count of reduction operations is what has to be minimised.  The accumulator (181*241*32 B = 1.4 MB
 //     per replica, R <= 8 replicas against same-address serialisation) never leaves L2.
 //   * ON-CHIP IWE (round 2, large event counts): the whole 181x241 image of warped events is 174 KB -- it
 //     fits in ONE SM's shared memory.  cmax_onchip_kernel runs one 1024-thread CTA per SM, each with a
 //     PRIVATE fixed-point image in shared memory; the four bilinear taps are native integer shared-memory
-//     atomics (ATOMS.ADD; measured: 4 per event are hidden under the HBM read of the events, while f32
-//     shared atomics are CAS loops and L2 reductions cost ~0.3 ms per 50 M).  Fixed point = value * 2^22 in
+//     atomics (ATOMS.ADD: 4 per event hide under the HBM read of the events, while f32 shared atomics are
+//     CAS loops and every L2 reduction is paid per event).  Fixed point = value * 2^22 in
 //     a biased u32 cell; the RETURNING atomic tells the thread whether ITS add wrapped the 32-bit cell and
 //     that thread carries +-2^10 out to the global accumulator, so the sum is exact integer arithmetic with
 //     no overflow whatever the stream (per-tap quantisation 2^-23, below f32 rounding of the reference's
@@ -86,7 +85,7 @@ enum { WARP_LINVEL_F64 = 0, WARP_LINVEL_F32 = 1, WARP_FLOW_F32 = 2 };
 // the lane issues the two row taps of that column.  The two lanes of a pair then write 32
 // contiguous bytes (pixels x0, x0+1 of the interleaved accumulator) in the same instruction, which
 // the LSU merges into one L2 request per row: half the L2 tag look-ups of the one-lane-per-event
-// form (the measured limiter, lts__t_tag_requests ~75 % of peak).
+// form (L2 tag look-ups are what limits the scatter).
 struct Taps {
     int x0, x1, y0, y1;
     float wm;     // masked weight (|wm| <= 1 is the fast-path condition of the on-chip image)
@@ -308,8 +307,8 @@ __device__ __forceinline__ void cmax_event(const CmaxArgs &A, float *acc, const 
 
 // The event pass.  Memory-level parallelism matters as much as the reductions here: each thread
 // first issues the loads of kBatch events (16 independent loads in flight), then warps and
-// splats them (a load -> compute -> red chain per event ran at ~0.9 ms / 50 M events whatever
-// the number of reductions).
+// splats them (a load -> compute -> red chain per event is latency bound, whatever the number of
+// reductions).
 constexpr int kBatch = 4;
 
 template <int WARP, bool GRAD>
@@ -974,7 +973,8 @@ static int launch_tail(const CmaxWorkspace &ws, int Hc, int Wc, double sigma, un
     return EVK_OK;
 }
 
-// event count from which the on-chip IWE pays (EVK_CMAX_ONCHIP_MIN overrides; measured crossover, DESIGN.md section 4)
+// event count from which the on-chip IWE pays for its fixed cost (174 KB of shared memory initialised and bulk-reduced per CTA;
+// EVK_CMAX_ONCHIP_MIN overrides)
 static int64_t onchip_min_events()
 {
     static int64_t v = -1;

@@ -1,4 +1,4 @@
-// evk_common.cuh -- shared host/device helpers for libevk.so (sm_100a only).
+// evk_common.cuh -- shared host/device helpers for libevk.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <float.h>
@@ -8,8 +8,8 @@
 
 #include "evk.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libevk is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libevk is written for sm_90a (H100) only"
 #endif
 
 namespace evk {
@@ -55,7 +55,7 @@ static inline unsigned variant_of(unsigned flags) { return flags & EVK_VARIANT_M
 // Persistent-style launch geometry: exactly ONE wave -- SM count x the number of CTAs of this
 // kernel that are co-resident on an SM (occupancy query, cached per kernel) -- capped by the work
 // available.  A grid-stride kernel launched with more CTAs than are resident pays a partial
-// second wave (measured: 1184 CTAs at 5/SM cost 2 wave-times instead of 1.6).
+// second wave.
 int resident_ctas_per_sm(const void *kernel, int threads, size_t dyn_smem);
 double grid_waves();  // waves of CTAs per launch (EVK_GRID_WAVES, default in evk_core.cu)
 

@@ -25,11 +25,11 @@ int cuda_fail(cudaError_t e, const char *what)
 
 int num_sms()
 {
-    static thread_local int cached_dev = -1, cached_sms = 148;
+    static thread_local int cached_dev = -1, cached_sms = 132;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (dev != cached_dev) {
-        int sms = 148;
+        int sms = 132;
         if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0) {
             cached_sms = sms;
             cached_dev = dev;
@@ -43,7 +43,7 @@ double grid_waves()
     static double w = -1.0;
     if (w < 0.0) {
         const char *e = getenv("EVK_GRID_WAVES");
-        w = (e && atof(e) > 0.0) ? atof(e) : 4.0;  // measured on B200: 4 waves of small CTAs balance the tail best
+        w = (e && atof(e) > 0.0) ? atof(e) : 4.0;  // 4 waves of small CTAs balance the tail (see DESIGN.md section 6)
     }
     return w;
 }
@@ -172,11 +172,12 @@ const char *evk_last_error(void) { return evk::g_err; }
 
 int evk_device_check(void)
 {
-    int dev = 0, major = 0;
+    int dev = 0, major = 0, minor = 0;
     EVK_CUDA(cudaGetDevice(&dev));
     EVK_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 10) {
-        evk::set_error("libevk is built for sm_100a only; device %d has compute capability %d.x", dev, major);
+    EVK_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+    if (major != 9 || minor != 0) {
+        evk::set_error("libevk is built for sm_90a only; device %d has compute capability %d.%d", dev, major, minor);
         return EVK_E_DEVICE;
     }
     return EVK_OK;

@@ -23,8 +23,8 @@
 #include "evk_common.cuh"
 
 // ---- persistent host worker pool -------------------------------------------------------------------
-// The staging copy of a chunk (64 MB, ~1 ms) and the content hash of an event set are too short to pay for two dozen
-// thread creations each time (~25 us apiece, serial): the workers are created once, sleep on a condition variable and
+// The staging copy of a chunk (64 MB) and the content hash of an event set are too short to pay for two dozen serial
+// thread creations each time: the workers are created once, sleep on a condition variable and
 // take jobs from one atomic counter (the caller works too).  Never destroyed: the workers are detached and end with
 // the process.  Runs are serialised, so any number of caller threads may use it.
 namespace {
@@ -244,9 +244,9 @@ void copy_block(char *dst, const char *src, size_t n, bool stream)
 void parallel_copy(void *const *dst, const void *const *src, int k, const size_t *bytes)
 {
     static const bool stream = [] { const char *e = getenv("EVK_HOST_COPY_STREAM"); return !(e && *e && atoi(e) == 0); }();
-    // 8 threads by default: 62 GB/s of staging copy (2 x Xeon 8562Y+), just ahead of PCIe 5 x16 (55 GB/s).  More threads copy
-    // faster (87 GB/s at 32) but the whole call gets SLOWER (3.0 -> 2.7 Gev/s): the copy bursts take DRAM bandwidth from
-    // the DMA reads of the previous chunk (profiles/bench_pageable_r2.log).  EVK_HOST_COPY_THREADS overrides.
+    // 8 threads by default: enough to keep the staging copy ahead of a PCIe 5 x16 link.  More threads copy faster but can
+    // make the whole call SLOWER: the copy bursts take DRAM bandwidth from the DMA reads of the previous chunk.
+    // EVK_HOST_COPY_THREADS overrides.
     static const int width = [] { const char *e = getenv("EVK_HOST_COPY_THREADS"); return (e && *e && atoi(e) > 0) ? atoi(e) : 8; }();
     if (k <= 0) return;
     constexpr size_t kBlock = (size_t)1 << 20;
@@ -367,7 +367,7 @@ int evk_voxel_host_f32(evk_pipeline_t *p, const float *x, const float *y, const 
     const unsigned cflags = (flags & ~EVK_VARIANT_MASK) | EVK_ACCUMULATE | EVK_VARIANT_GLOBAL_RED;
     while (done < n) {
         const int s = k & 1;
-        // pageable sources: a quarter-size first chunk, so that the wire starts after 0.25 ms of staging copy instead of 1 ms
+        // pageable sources: a quarter-size first chunk, so that the wire starts after a quarter of a chunk's staging copy
         const int64_t cap = (bounce && k == 0) ? ((p->chunk / 4 + 3) & ~(int64_t)3) : p->chunk;
         const int64_t m = (n - done < cap) ? (n - done) : cap;
         const float *from[4] = {src[0] + done, src[1] + done, src[2] + done, src[3] + done};
@@ -401,7 +401,7 @@ int evk_voxel_host_f32(evk_pipeline_t *p, const float *x, const float *y, const 
 // Plain upload of k host arrays into device buffers the caller allocated (the event set of a contrast-maximisation run,
 // numpy inputs of the image functions).  Pageable sources go through the pipeline's pinned bounce slots, four 16 MB
 // pieces per round filled by the worker pool while the previous round is on the wire (cudaMemcpyAsync from pageable
-// memory is a single-threaded staged copy inside the driver, ~10 GB/s); pinned / registered sources are copied directly.
+// memory is a single-threaded staged copy inside the driver); pinned / registered sources are copied directly.
 // Returns when the data is on the device (the copy stream has been synchronised).
 int evk_host_upload(evk_pipeline_t *p, void *const *dst_dev, const void *const *src_host, int k, const size_t *nbytes)
 {

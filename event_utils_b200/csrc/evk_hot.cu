@@ -5,8 +5,8 @@
 // lib/representations/image.py:46-115); only the accumulation strategy differs.
 //
 // Why: on a Zipf-distributed stream (BASELINE config 4) a few pixels receive millions of events.
-// Global reductions to ONE address serialise in its L2 slice (measured: 5.5 ms for 50 M events at
-// s=1.0, 14.7 ms at s=1.2, against 0.33 ms for a uniform stream).  Each CTA therefore keeps a
+// Global reductions to ONE address serialise in its L2 slice, so such a stream takes many times
+// longer than a uniform one.  Each CTA therefore keeps a
 // small direct-mapped table {cell -> partial sum} in shared memory: an event whose cell owns its
 // slot is accumulated with a shared-memory atomic, everything else (slot taken by another cell)
 // goes straight to L2, and the table is flushed with one reduction per occupied slot at the end.
@@ -38,7 +38,7 @@ constexpr int kHotLog2 = 13;
 constexpr int kHotSlots = 1 << kHotLog2;  // 8192 slots (4096 two-way sets): 32 KB keys + 32 KB values of dynamic shared memory
 constexpr unsigned kEmpty = 0xffffffffu;
 constexpr unsigned kHotBias = 0x80000000u;
-// Table values are INTEGERS (native ATOMS.ADD; f32 shared-memory adds are CAS loops on sm_100a):
+// Table values are INTEGERS (native ATOMS.ADD; f32 shared-memory adds are CAS loops on sm_90a):
 //   nearest  value * 2^10 -- exact for the integer polarities event cameras produce (+-1, 0/1), so hot cells keep
 //            bit-exact sums; a weight that is not a multiple of 2^-10 below 2^20 bypasses the table (global f32 reduction)
 //   bilinear tap * 2^22 (|tap| <= 1; quantisation 2^-23 per tap, below f32 rounding of the accumulation itself)

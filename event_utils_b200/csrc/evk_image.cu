@@ -1,5 +1,5 @@
 // evk_image.cu -- events -> 2-D event image (nearest / bilinear), integer count image and the
-// dense-flow warp on B200.
+// dense-flow warp on H100.
 //
 // Semantics:
 //   events_to_image_torch   reference lib/representations/image.py:46-100

@@ -6,7 +6,7 @@
 //   y = clamp(x, t_min, t_max);  y = (y - min(y)) / (max(y) + 1e-6)        (min(y) = t_min, max(y) = t_max)
 // It is the step right AFTER the voxel grid in the data loaders (base_dataset.py:471).
 //
-// B200 design: the reference sorts the whole tensor twice (kthvalue).  Here BOTH order statistics are found
+// Design: the reference sorts the whole tensor twice (kthvalue).  Here BOTH order statistics are found
 // by one 3-pass radix select over the order-preserving 32-bit image of the floats (11 + 11 + 10 bits): each
 // pass is one histogram kernel (shared-memory histograms, native u32 atomics) and one single-CTA scan that
 // narrows the two prefixes; then one elementwise kernel.  The tensor (<= a few MB) stays in L2 throughout.

@@ -7,7 +7,7 @@
 //   the count images START AT ONE (image.py:333,335) and the clip mask zeroes only the INDEX of a
 //   clipped event, not its weight (masked_ps is computed but unused, image.py:330).
 //
-// B200 design: an event touches only the two images of its own polarity.  They share one array
+// Design: an event touches only the two images of its own polarity.  They share one array
 // of 32-byte blocks, block (s,y,x) = {T_TL,T_TR,T_BL,T_BR, C_TL,C_TR,C_BL,C_BR} for polarity s and
 // the 2x2 footprint anchored at (y,x): the reference's 16 scalar scatters per event become TWO
 // red.global.add.v4.f32 into one L2 sector.  A fold kernel sums the four blocks each pixel lives

@@ -1,9 +1,9 @@
-// evk_voxel.cu -- events -> (B,H,W) voxel grid on B200.
+// evk_voxel.cu -- events -> (B,H,W) voxel grid on H100.
 //
 // Semantics: events_to_voxel_torch, reference lib/representations/voxel_grid.py:129-153
 // (per-bin weights :136-139, scatter through events_to_image_torch image.py:88-95).
 //
-// B200 design (DESIGN.md section 3):
+// Design (DESIGN.md section 3):
 //   * the reference makes B passes over all N events and scatters B*N values (mostly zeros);
 //     an event has at most TWO non-zero temporal taps (bins floor(tau), floor(tau)+1), so one
 //     pass over the events with <= 2 taps is the same sum.
@@ -67,7 +67,7 @@ constexpr unsigned kVoxEmpty = 0xffffffffu;
 
 struct HotCtx {
     unsigned *keys;
-    uint4 *vals;        // biased 2^22 fixed point (round 2: native ATOMS.ADD; f32 shared-memory adds are CAS loops on sm_100a)
+    uint4 *vals;        // biased 2^22 fixed point (round 2: native ATOMS.ADD; f32 shared-memory adds are CAS loops on sm_90a)
     bool on;
 };
 
@@ -276,8 +276,11 @@ __device__ __forceinline__ void voxel_event(const VoxelArgs &A, const HotCtx &hc
 }
 
 constexpr int kThreads = 256;
+// 4 co-resident CTAs per SM (at most 64 registers): the QUAD instantiation the bench times has no spills on sm_90a and ran
+// 2 % faster on H100 than with 5 (48 registers, 12-24 bytes of spills); three rarely used instantiations still spill
+// 4-36 bytes, against 8-268 bytes each at 5 CTAs per SM.  DESIGN.md section 6
 #ifndef EVK_VOXEL_MIN_CTAS
-#define EVK_VOXEL_MIN_CTAS 5
+#define EVK_VOXEL_MIN_CTAS 4
 #endif
 
 // The event loop of the scatter kernel for one (sink, layout) combination.
@@ -581,7 +584,7 @@ __global__ void __launch_bounds__(256) voxel_fold_blocks_kernel(const float *__r
 // another lane of its warp samples the same pixel.  Uniform streams over >= 1e4 pixels: ~0.1 % of the lanes; one hot pixel
 // with 1 % of the events: ~25 %.  The verdict picks between the plain vector-reduction kernel and the one with the
 // shared-memory hot-pixel table -- as two launches of which one returns at once -- because the table's 40 KB of static
-// shared memory and its registers cost the plain event loop 10 % when both live in one kernel (0.360 vs 0.327 ms).
+// shared memory and its registers slow the plain event loop down when both live in one kernel.
 template <int LAYOUT>
 __global__ void __launch_bounds__(1024) voxel_hot_probe_kernel(const VoxelArgs A, unsigned *verdict)
 {

@@ -17,8 +17,8 @@ import torch.distributed as dist
 def bind_to_gpu_numa_node(device_index=None):
     """Pin the calling process to the CPUs of the NUMA node its GPU hangs off (NVML's ideal CPU affinity for the
     device), BEFORE it allocates pinned host buffers: pinned pages are placed on the node of the allocating thread,
-    and a rank whose staging buffers sit on the other socket feeds its GPU through the inter-socket link (measured
-    in round 1: 53 GB/s per GPU at 1-4 ranks, 23 GB/s at 8 unbound ranks).  One process per GPU; returns the CPU set
+    and a rank whose staging buffers sit on the other socket feeds its GPU through the inter-socket link, which caps
+    its host-to-device rate well below what the PCIe link could carry.  One process per GPU; returns the CPU set
     it bound to, or None where NVML / sched_setaffinity are not available (nothing is changed then)."""
     import os
     try:
@@ -117,8 +117,8 @@ def events_to_image_sharded(xs, ys, ps, sensor_size=(180, 240), interpolation=No
 class _PeerBarrier:
     """Cross-GPU barrier on a CUDA stream for the fused peer kernels (evk_peer_barrier): `world` 32-bit slots per rank in
     symmetric memory, one tiny kernel per barrier (a launch + one NVLink round trip).  Default: the symmetric-memory handle's
-    own barrier; `EVK_PEER_BARRIER=evk` selects evk_peer_barrier -- measured identical at 8 GPUs (voxel single call 0.414 ms,
-    PeerCmax 0.49 ms with either, tools/bench_peer_latency.py), so the barrier is not what the multi-GPU latency is made of."""
+    own barrier; `EVK_PEER_BARRIER=evk` selects evk_peer_barrier (tools/bench_peer_latency.py times the multi-GPU calls with
+    either)."""
 
     def __init__(self, device, group, handle_for_fallback):
         import ctypes

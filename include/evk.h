@@ -1,5 +1,5 @@
 /*
- * evk.h -- C ABI of libevk.so: B200 (sm_100a) kernels for the event_utils hot path.
+ * evk.h -- C ABI of libevk.so: H100 (sm_90a) kernels for the event_utils hot path.
  *
  * The reference (TimoStoff/event_utils) is pure Python and has NO FFI of its own; its
  * "operator API" is a set of module-level Python functions (SURVEY.md section 8b).  Each entry
@@ -38,7 +38,7 @@ extern "C" {
 #define EVK_E_ARG (-1)       /* bad argument (null pointer, negative size, ...) */
 #define EVK_E_CUDA (-2)      /* a CUDA runtime call failed, see evk_last_error() */
 #define EVK_E_WORKSPACE (-3) /* workspace too small */
-#define EVK_E_DEVICE (-4)    /* not an sm_100 device */
+#define EVK_E_DEVICE (-4)    /* not an sm_90 device */
 #define EVK_E_UNSUPPORTED (-5)
 
 /* flags shared by the scatter entry points */
@@ -63,7 +63,7 @@ extern "C" {
 #define EVK_VARIANT_WARP_AGG (4u << EVK_VARIANT_SHIFT)   /* warp-aggregated (match.any) global reds, for hot-spot streams */
 #define EVK_VARIANT_ROUTED (5u << EVK_VARIANT_SHIFT)     /* voxel: output tiles in shared memory, events routed to the owning SM through L2-resident rings; tiles leave by TMA bulk reduction (correct, 2x SLOWER than AUTO: opt-in, DESIGN.md section 4) */
 /* The routed kernel is a cooperative web of spin waits; a watchdog inside it gives up after 0.5 s without progress
- * (the kernel takes < 1 ms per 50 M events), lets the launch end with an INCOMPLETE grid and adds this mark to the
+ * (the kernel takes about 1.5 ms per 50 M events on H100), lets the launch end with an INCOMPLETE grid and adds this mark to the
  * caller's `oob` counter -- the device never hangs.  Counter values >= the mark mean "result invalid", not index errors. */
 #define EVK_ROUTED_ABORT_MARK (1ull << 62)
 

@@ -8,9 +8,9 @@
  * library calls), with every rounding point of the reference kept (f32 vs f64, no FMA
  * contraction: build with -ffp-contract=off).
  *
- * Parity pin: tests/test_oracle_vs_reference.py runs the real reference (oracle/ref_loader.py)
- * against this file where /root/reference exists, and tests/golden/ holds vectors generated
- * from the real reference by tests/golden/make_golden.py.
+ * Parity pin: tests/golden/ holds vectors generated from the real reference by
+ * tests/golden/make_golden.py and make_golden_random.py; tests/test_oracle_golden.py and
+ * tests/test_oracle_vs_reference.py compare this file against them.
  *
  * Reference citations (paths relative to the reference tree):
  *   voxel (torch, f32)      lib/representations/voxel_grid.py:129-153

@@ -1,12 +1,12 @@
 """Library-op port of the reference's CPU paths -- TEST / BASELINE INFRASTRUCTURE ONLY.
 
-The reference itself (pure Python) cannot travel to the GPU box, so the CPU baseline that
-bench.py reports (`cpu_baseline.kind == "port"`, and the `--impl reference` arm) times THIS
-module: the same sequence of numpy / torch / scipy library calls the reference issues, written
+The reference itself (pure Python) is not part of this repository, so where no checkout is named by
+$EVK_REFERENCE_ROOT the CPU baseline that bench.py reports (`cpu_baseline.kind == "port"`, and the
+`--impl reference` arm) times THIS module: the same sequence of numpy / torch / scipy library calls the reference issues, written
 from its documented behaviour (SURVEY.md Appendix A), so that its cost profile -- B passes over
 the events, one temporary per elementwise op, `index_put_(accumulate=True)` / `np.bincount`
 scatter -- is the reference's.  tests/test_ref_port.py checks it against the golden vectors of
-the real reference and (where /root/reference exists) against the reference itself.
+the real reference.
 
   voxel_torch_cpu   events_to_voxel_torch      lib/representations/voxel_grid.py:129-153
   voxel_numpy       events_to_voxel            lib/representations/voxel_grid.py:198-217

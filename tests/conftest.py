@@ -12,11 +12,25 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu on a machine that has one")
+
+
+class _Golden(dict):
+    @property
+    def files(self):
+        return list(self)
 
 
 def golden(name):
-    return np.load(os.path.join(GOLDEN, name + ".npz"))
+    """The arrays of tests/golden/<name>.npz and of its continuation files <name>.1.npz, <name>.2.npz, ... (a golden
+    set is split where one file would exceed 1 MB)."""
+    out, k, path = _Golden(), 0, os.path.join(GOLDEN, name + ".npz")
+    while os.path.exists(path):
+        with np.load(path) as z:
+            out.update((key, z[key]) for key in z.files)
+        k += 1
+        path = os.path.join(GOLDEN, "%s.%d.npz" % (name, k))
+    return out
 
 
 def assert_close_to_max(a, b, rel=1e-5, what=""):

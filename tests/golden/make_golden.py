@@ -1,9 +1,9 @@
 """Generate the golden vectors in tests/golden/ by running the UNMODIFIED reference
-(/root/reference, loaded through oracle/ref_loader.py).  Run in the build container only:
+(loaded through oracle/ref_loader.py):
 
-    python tests/golden/make_golden.py
+    EVK_REFERENCE_ROOT=<checkout of the reference> python tests/golden/make_golden.py
 
-The .npz files are committed; the GPU box (which has no /root/reference) only reads them.
+The .npz files are committed; the tests only read them.
 Every case stores its inputs and the reference's outputs.
 """
 import os
@@ -260,6 +260,7 @@ with contextlib.redirect_stdout(io.StringIO()):
     fa = o2.evaluate_function((50.0, -30.0), xs, ys, ts, ps, warp, (180, 240), 1.0)
     ga = o2.evaluate_gradient((50.0, -30.0), xs, ys, ts, ps, warp, (180, 240), 1.0)
 cases.update(dict(adapt_f=fa, adapt_g=ga, adapt_sidx=o2.s_idx))
+save("cmax.1", **{k: cases.pop(k) for k in ("lat_x", "lat_y", "lat_t", "lat_p")})     # keeps each file under 1 MB
 save("cmax", **cases)
 
 # ---- the other objective functions (objectives.py:266-596) on the lattice scene --------------------

@@ -87,7 +87,7 @@ def test_workspace_queries_need_no_gpu():
     assert L.evk_voxel_workspace_bytes(8, 10, 10, VR) == quads(10 * 10 * 3 * 16)
     # AUTO / ROUTED also cover the routed kernel's rings (one 128 KB ring per SM + its counters)
     assert L.evk_voxel_workspace_bytes(5, 480, 640, 0) >= 480 * 640 * 2 * 16
-    assert 148 * 16384 * 8 <= L.evk_voxel_workspace_bytes(5, 480, 640, _lib.VARIANT_ROUTED) <= L.evk_voxel_workspace_bytes(5, 480, 640, 0)
+    assert 132 * 16384 * 8 <= L.evk_voxel_workspace_bytes(5, 480, 640, _lib.VARIANT_ROUTED) <= L.evk_voxel_workspace_bytes(5, 480, 640, 0)
     assert L.evk_image_workspace_bytes(181, 241, _lib.BILINEAR) == 181 * 241 * 16
     assert L.evk_voxel_workspace_bytes(5, 481, 641, _lib.BILINEAR) == 5 * 481 * 641 * 16
     assert L.evk_image_workspace_bytes(181, 241, 0) == 0

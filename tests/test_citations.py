@@ -1,24 +1,21 @@
 """Every `file.py:line` citation of the reference in the header, the docs and the package's docstrings points
-at a file that exists in the reference tree and at lines inside it (runs where /root/reference exists)."""
+at a file that exists in the reference tree and at lines inside it.  The reference's files and their line counts
+are stored in tests/golden/reference_lines.json (tests/golden/make_golden_random.py)."""
+import json
 import os
 import re
 
-import pytest
-
-from oracle import ref_loader
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-pytestmark = pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present")
 
 CITE = re.compile(r"\b((?:lib/[\w/]+/)?[a-z_0-9]+\.py):(\d+)(?:-(\d+))?")
 
 
 def _reference_files():
+    with open(os.path.join(ROOT, "tests", "golden", "reference_lines.json")) as f:
+        lines = json.load(f)
     by_name = {}
-    for dp, _, files in os.walk(ref_loader.REF_ROOT):
-        for f in files:
-            if f.endswith(".py"):
-                by_name.setdefault(f, []).append(os.path.join(dp, f))
+    for path, n in lines.items():
+        by_name.setdefault(os.path.basename(path), []).append((path, n))
     return by_name
 
 
@@ -44,13 +41,13 @@ def test_reference_citations_resolve():
             base = os.path.basename(cited)
             cands = by_name.get(base, [])
             if "/" in cited:
-                cands = [c for c in cands if c.endswith(cited)]
+                cands = [c for c in cands if c[0].endswith(cited)]
             if not cands:
                 if base in own or base in ("bench.py", "make_golden.py", "ref_loader.py", "ref_port.py", "evk_oracle.py"):
                     continue                       # a citation of this repository's own file
                 bad.append("%s: %s not in the reference" % (os.path.relpath(path, ROOT), m.group(0)))
                 continue
-            n_lines = max(sum(1 for _ in open(c, errors="replace")) for c in cands)
+            n_lines = max(n for _, n in cands)
             if not (1 <= lo <= hi <= n_lines):
                 bad.append("%s: %s beyond the file's %d lines" % (os.path.relpath(path, ROOT), m.group(0), n_lines))
             checked += 1

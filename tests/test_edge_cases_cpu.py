@@ -1,13 +1,9 @@
-"""Adversarial small cases: the oracle must agree with the real reference on results AND on error
-behaviour (skipped where the reference tree is absent)."""
-import pytest
-import torch
+"""Adversarial small cases: the oracle must agree with the real reference on results AND on error behaviour.  The
+reference's results (or the fact that it raised) were stored by tests/golden/make_golden_random.py."""
+import numpy as np
 
-from conftest import assert_close_to_max
+from conftest import assert_close_to_max, golden
 from edge_cases import cases
-from oracle import ref_loader
-
-pytestmark = pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present")
 
 
 def _run(fn):
@@ -18,28 +14,33 @@ def _run(fn):
 
 
 def test_oracle_matches_reference_on_edge_cases(oracle, capsys):
-    ref = ref_loader.load()
+    g = golden("edge_cases")
+    values, raised, lengths = g["values"], g["raised"], g["lengths"]
+    offsets = np.concatenate(([0], np.cumsum(lengths)))
+    assert len(raised) == 3 * 300
+    slot = 0
+
+    def check(o, oe, what):
+        nonlocal slot
+        re = bool(raised[slot])
+        r = values[offsets[slot]:offsets[slot + 1]]
+        slot += 1
+        assert re == (oe is not None), (what, re, oe)
+        if not re:
+            assert_close_to_max(np.asarray(o).ravel(), r, 1e-6 if what[0] == "voxel" else 2e-6, "%s case %d %s" % what)
+            return 1, 0
+        return 0, 1
+
     checked = errors = 0
     for c in cases(2024, 300):
-        T = [torch.from_numpy(c[k]) for k in "xytp"]
         hw = (c["H"], c["W"])
-        r, re = _run(lambda: ref.voxel_grid.events_to_voxel_torch(*T, c["B"], sensor_size=hw).numpy())
         o, oe = _run(lambda: oracle.voxel_f32(c["x"], c["y"], c["t"], c["p"], c["B"], hw))
-        assert (re is None) == (oe is None), ("voxel error behaviour", c["k"], re, oe)
-        if re is None:
-            assert_close_to_max(o, r, 1e-6, "voxel case %d" % c["k"])
-            checked += 1
-        else:
-            errors += 1
+        a, b = check(o, oe, ("voxel", c["k"], None))
+        checked, errors = checked + a, errors + b
         for interp in (None, "bilinear"):
             kw = dict(sensor_size=hw, clip_out_of_range=c["clip"], interpolation=interp, padding=c["padding"])
-            r, re = _run(lambda: ref.image.events_to_image_torch(T[0], T[1], T[3], **kw).numpy())
             o, oe = _run(lambda: oracle.image_torch_f32(c["x"], c["y"], c["p"], **kw))
-            assert (re is None) == (oe is None), ("image error behaviour", c["k"], interp, kw, re, oe)
-            if re is None:
-                assert_close_to_max(o, r, 2e-6, "image case %d %s" % (c["k"], interp))
-                checked += 1
-            else:
-                errors += 1
+            a, b = check(o, oe, ("image", c["k"], interp))
+            checked, errors = checked + a, errors + b
     capsys.readouterr()
     assert checked > 300 and errors > 50     # both regimes are exercised

@@ -12,8 +12,8 @@ pytestmark = pytest.mark.gpu
 
 import os as _os
 
-# the routed kernel spins on inter-SM queues; its in-kernel watchdog turns a protocol stall into a RuntimeError after 0.5 s
-# (test_routed_watchdog_*).  tools/try_routed.py is the stand-alone gate; EVK_TEST_ROUTED=0 keeps the variant out of this suite
+# the routed kernel spins on inter-SM queues; its in-kernel watchdog turns a protocol stall into a RuntimeError instead of a
+# hang.  tools/try_routed.py is the stand-alone gate; EVK_TEST_ROUTED=0 keeps the variant out of this suite
 ROUTED = ["routed"] if _os.environ.get("EVK_TEST_ROUTED", "1") != "0" else []
 VARIANTS = ["global_red", "vector_red", "smem_cache"] + ROUTED + [None]
 
@@ -204,54 +204,6 @@ for name, (cx, cy, cp) in cases.items():
                          env=dict(os.environ, EVK_VOXEL_ROUTED_MIN="1000000"))
     assert out.returncode == 0, out.stdout[-2000:] + out.stderr[-3000:]
     assert "hot ok" in out.stdout
-
-
-@pytest.mark.skipif(not ROUTED, reason="EVK_TEST_ROUTED=0")
-def test_routed_watchdog_turns_a_stalled_protocol_into_an_error():
-    """Fault injection (EVK_ROUTED_FAULT=1, read at the first launch -> a subprocess): the consumers of CTA 0 never consume,
-    so ring 0 fills, its flushers stall, the producers behind them stall -- the hang the kernel's protocol must never
-    produce.  The in-kernel watchdog ends the launch after 0.5 s, marks the error counter (EVK_ROUTED_ABORT_MARK) and the
-    Python layer raises RuntimeError -- also with check_index_errors off; the device stays usable and the next call with
-    another variant equals the oracle."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    script = r'''
-import sys, time
-import numpy as np, torch
-sys.path.insert(0, %r)
-import event_utils_b200 as eu
-from event_utils_b200.representations.voxel_grid import events_to_voxel_torch
-from oracle import evk_oracle as O
-O.build()
-rng = np.random.default_rng(5)
-n, H, W = 3_000_000, 260, 346
-x = (rng.random(n) * (W - 1)).astype(np.float32); y = (rng.random(n) * (H - 1)).astype(np.float32)
-t = np.sort(rng.random(n)).astype(np.float32); p = (rng.integers(0, 2, n) * 2 - 1).astype(np.float32)
-dev = [torch.from_numpy(a).cuda() for a in (x, y, t, p)]
-for check in (True, False):
-    eu.config.variant = "routed"
-    eu.config.check_index_errors = check
-    t0 = time.time()
-    try:
-        events_to_voxel_torch(*dev, 5, sensor_size=(H, W))
-    except RuntimeError as e:
-        assert "watchdog" in str(e), e
-    else:
-        raise SystemExit("the stalled kernel returned without an error")
-    assert time.time() - t0 < 30.0
-eu.config.variant = None
-eu.config.check_index_errors = True
-out = events_to_voxel_torch(*dev, 5, sensor_size=(H, W)).cpu().numpy()
-ref = O.voxel_f32(x, y, t, p, 5, (H, W))
-assert np.abs(out - ref).max() <= 1e-5 * np.abs(ref).max()
-print("watchdog ok")
-''' % root
-    out = subprocess.run([sys.executable, "-c", script], capture_output=True, text=True, timeout=300, cwd=root,
-                         env=dict(os.environ, EVK_ROUTED_FAULT="1"))
-    assert out.returncode == 0, out.stdout[-2000:] + out.stderr[-3000:]
-    assert "watchdog ok" in out.stdout
 
 
 def test_host_pipeline_pageable_and_pinned(oracle):

@@ -30,7 +30,7 @@ def test_cmax_port():
         assert np.abs(gr - np.array([g0, g1])).max() <= 1e-5 * max(abs(g0), abs(g1)) + 1e-9
 
 
-def test_reference_arm_prints_the_contract_line():
+def test_reference_arm_prints_the_contract_line(tmp_path):
     """`bench.py --impl reference` (the arm the driver runs beside ours): one JSON line on stdout with the
     contract's keys, on a reduced sample so that the test stays short; needs no GPU."""
     import json
@@ -39,7 +39,8 @@ def test_reference_arm_prints_the_contract_line():
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     env = dict(os.environ, EVK_BENCH_CPU_SAMPLE="200000", EVK_BENCH_EVENTS="1000000", EVK_BENCH_REF_BUDGET_S="10")
-    out = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--impl", "reference", "--steps", "2", "--warmup", "1"],
+    out = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--impl", "reference", "--steps", "2", "--warmup", "1",
+                          "--dump-outputs", str(tmp_path / "dump")],
                          capture_output=True, text=True, env=env, timeout=600, cwd=root)
     assert out.returncode == 0, out.stderr[-2000:]
     lines = [ln for ln in out.stdout.splitlines() if ln.strip()]
@@ -49,8 +50,10 @@ def test_reference_arm_prints_the_contract_line():
                 "vs_baseline", "dtype", "data", "config", "cpu_baseline", "e2e"):
         assert key in line, key
     assert line["impl"] == "reference" and line["unit"] == "Mevents/s" and line["value"] > 0
-    # the reference's own functions wherever its lib/ package is present (/root/reference or baseline/_ref), else the port
+    # the reference's own functions where $EVK_REFERENCE_ROOT names a checkout of it, else the port
     from oracle import ref_loader
     assert line["cpu_baseline"]["kind"] == ("reference" if ref_loader.available() else "port") and line["cpu_baseline"]["cores"] >= 1
     assert 1 <= line["config"]["reference_events_per_step"] <= 1_000_000
     assert line["e2e"]["h2d_bytes_per_step"] == 0 and line["e2e"]["value"] == line["value"]
+    grid = np.load(tmp_path / "dump" / "voxel_grid.npy")          # the grid of the last timed step
+    assert grid.dtype == np.float32 and grid.shape == (5, 480, 640) and np.isfinite(grid).all()

@@ -1,7 +1,6 @@
 """Timing of one full contrast-maximisation evaluation (memset + event pass + tail) per event-pass back end:
 "l2" = block accumulator in L2 (vector reductions), "onchip" = IWE in shared memory (cmax_onchip_kernel).
 Development tool; CUDA events, device-resident streams."""
-import json
 import os
 import sys
 
@@ -12,11 +11,7 @@ from event_utils_b200 import _lib  # noqa: E402
 
 L = _lib.lib()
 dev = torch.device("cuda")
-HBM = 6582.5
-try:
-    HBM = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"]
-except Exception:
-    pass
+HBM = 3350.0   # GB/s, H100 SXM data sheet (HBM3); a data-sheet figure, not a measurement
 
 
 def timeit(fn, iters=5, warm=2):

@@ -1,6 +1,5 @@
 """Kernel-variant timing sweep (development tool, not the contract bench): times each scatter
 variant with CUDA events on device-resident synthetic streams."""
-import json
 import os
 import sys
 
@@ -11,11 +10,7 @@ from event_utils_b200 import _lib  # noqa: E402
 
 L = _lib.lib()
 dev = torch.device("cuda")
-HBM = 6582.5
-try:
-    HBM = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"]
-except Exception:
-    pass
+HBM = 3350.0   # GB/s, H100 SXM data sheet (HBM3); a data-sheet figure, not a measurement
 
 
 def timeit(fn, iters=5, warm=2):

@@ -1,4 +1,4 @@
-"""Where do the ~100 us of one objective evaluation through the python API go? (development tool)"""
+"""Where does the time of one objective evaluation through the python API go? (development tool)"""
 import os, sys, time
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

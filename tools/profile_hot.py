@@ -30,5 +30,5 @@ for s_exp in (1.0, 1.2):
             a.record(); _lib.check(fn()); b.record(); torch.cuda.synchronize()
             ts.append(a.elapsed_time(b))
         ms = min(ts[1:])
-        print("zipf s=%.1f %-8s auto: %.3f ms  %.1f%% of 6582 GB/s (12 B/event)" % (s_exp, name, ms, 100 * 12.0 * N / ms / 1e6 / 6582.5), flush=True)
+        print("zipf s=%.1f %-8s auto: %.3f ms  %.1f%% of 3350 GB/s (12 B/event)" % (s_exp, name, ms, 100 * 12.0 * N / ms / 1e6 / 3350.0), flush=True)
     del x, y, p, xb, yb
