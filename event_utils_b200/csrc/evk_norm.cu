@@ -3,7 +3,10 @@
 // Semantics: RobustNorm.__call__ / .percentile, reference lib/data_loaders/data_augmentation.py:82-130
 //   t = kthvalue(x, k), k = 1 + round(.01 q (numel-1))           (exact order statistic, no interpolation)
 //   if t_max == 0 and t_min == 0: return x
-//   y = clamp(x, t_min, t_max);  y = (y - min(y)) / (max(y) + 1e-6)        (min(y) = t_min, max(y) = t_max)
+//   y = clamp(x, t_min, t_max);  y = (y - min(y)) / (max(y) + 1e-6)        (min(y) = min(t_min, t_max), max(y) = t_max)
+// NaN: kthvalue ranks every NaN above +inf whatever its sign bit, and torch.min / torch.max of a tensor holding a NaN
+// are NaN, so any NaN in x makes every output NaN unless the identity short-cut is taken.  ordered_key maps every NaN
+// to the top key and the first histogram pass (which sees every key) counts them.
 // It is the step right AFTER the voxel grid in the data loaders (base_dataset.py:471).
 //
 // Design: the reference sorts the whole tensor twice (kthvalue).  Here BOTH order statistics are found
@@ -18,11 +21,15 @@ struct SelectState {
     unsigned prefix[2];          // key bits decided so far, per target
     unsigned long long rank[2];  // remaining 1-based rank inside the prefix class
     float value[2];              // the selected values (after the last pass)
+    unsigned long long nans;     // NaNs in x (counted by the first pass)
 };
+
+constexpr unsigned kNanKey = 0xffffffffu;   // above +inf (0xff800000); the last bin of every pass
 
 __device__ __forceinline__ unsigned ordered_key(float f)
 {
     const unsigned b = __float_as_uint(f);
+    if ((b & 0x7fffffffu) > 0x7f800000u) return kNanKey;   // NaN of either sign ranks last, as in kthvalue
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 __device__ __forceinline__ float key_to_float(unsigned u)
@@ -70,6 +77,7 @@ __global__ void __launch_bounds__(64) select_scan_kernel(unsigned *hist, int shi
             cum += c;
         }
         if (b == nb) b = nb - 1;
+        if (t == 0 && shift + nbits >= 32) st->nans = hist[nb - 1];   // first pass: every key was counted, kNanKey in the last bin
         st->prefix[t] |= (unsigned)b << shift;
         st->rank[t] = rank - cum;
         if (last) st->value[t] = key_to_float(st->prefix[t]);
@@ -83,14 +91,18 @@ __global__ void __launch_bounds__(256) robust_norm_kernel(const float *__restric
 {
     const float t_min = st->value[0], t_max = st->value[1];
     const bool identity = (t_max == 0.0f && t_min == 0.0f);     // data_augmentation.py:124-125
+    const bool all_nan = !identity && st->nans != 0;           // min(y) / max(y) are NaN (data_augmentation.py:129)
+    // min(clamp(x, t_min, t_max)): t_min, or t_max when t_min > t_max (torch.clamp then yields t_max everywhere)
+    const float lo = fminf(t_min, t_max);
     const float denom = __fadd_rn(t_max, 1e-6f);
     const int64_t stride = (int64_t)gridDim.x * 256;
     for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += stride) {
         const float v = x[i];
         if (identity) { out[i] = v; continue; }
-        // torch.clamp(x, min, max) = min(max(x, t_min), t_max); NaN propagates
-        float c = (v != v) ? v : fminf(fmaxf(v, t_min), t_max);
-        out[i] = __fdiv_rn(__fsub_rn(c, t_min), denom);
+        if (all_nan) { out[i] = __int_as_float(0x7fffffff); continue; }
+        // torch.clamp(x, min, max) = min(max(x, t_min), t_max)
+        float c = fminf(fmaxf(v, t_min), t_max);
+        out[i] = __fdiv_rn(__fsub_rn(c, lo), denom);
     }
 }
 

@@ -348,7 +348,8 @@ int evk_cmax_flow_variance_f32(const float *x, const float *y, const float *t, c
  * RobustNorm.__call__ / .percentile, lib/data_loaders/data_augmentation.py:82-130 (two kthvalue sorts),
  * the step after the voxel grid in the loaders (base_dataset.py:471).
  *   k_low / k_top: 1-based ranks, k = 1 + round(.01 q (n-1)) computed by the caller (:100)
- *   out = x if both statistics are 0, else (clamp(x, t_min, t_max) - t_min) / (t_max + 1e-6)
+ *   out = x if both statistics are 0, else (clamp(x, t_min, t_max) - min(t_min, t_max)) / (t_max + 1e-6);
+ *   NaNs rank above +inf (as in kthvalue), and any NaN in x makes every element of out NaN unless out = x
  *   t_min_max: optional 2 floats on the device receiving the two statistics.
  * --------------------------------------------------------------------------------------------- */
 size_t evk_robust_norm_workspace_bytes(void);

@@ -40,6 +40,34 @@ static inline int64_t trunc_to_long(float v)
     return (int64_t)v;
 }
 
+/* ------------------------------------------------------------------------------------------
+ * Exact mode.  Every scatter function below sends each of its taps through add_tap(); with a
+ * non-NULL `ex` (3 * cells doubles, cells = the size of all its output planes together) the tap
+ * is also accumulated into ex[0*cells + j] (f64 sum of the f32 taps), ex[1*cells + j] (f64 sum
+ * of |tap|) and ex[2*cells + j] (number of non-zero taps).  The f32 outputs are unchanged: tests
+ * bound a kernel's per-cell error by these, independently of the order it adds the taps in.
+ * `j` = plane offset + cell index inside the plane.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+    double *sum, *abs, *cnt;
+} evo_exact;
+
+static inline evo_exact exact_of(double *ex, int64_t cells)
+{
+    evo_exact e = {ex, ex ? ex + cells : NULL, ex ? ex + 2 * cells : NULL};
+    return e;
+}
+
+static inline void add_tap(float *out, const evo_exact *e, int64_t plane, int64_t i, float w)
+{
+    out[i] += w;
+    if (e->sum && w != 0.0f) {
+        e->sum[plane + i] += (double)w;
+        e->abs[plane + i] += fabs((double)w);
+        e->cnt[plane + i] += 1.0;
+    }
+}
+
 /* python / torch advanced-index wrap: [-size,-1] wraps, anything else outside [0,size) is an error */
 static inline int wrap_index(int64_t i, int64_t size, int64_t *out)
 {
@@ -57,9 +85,10 @@ static inline int wrap_index(int64_t i, int64_t size, int64_t *out)
  * in *oob and nothing is written for that event.
  * ------------------------------------------------------------------------------------------ */
 EVO_API int64_t evo_voxel_f32(const float *x, const float *y, const float *t, const float *p,
-                              int64_t n, float t0, float dt, int B, int H, int W, float *out)
+                              int64_t n, float t0, float dt, int B, int H, int W, float *out, double *ex)
 {
     int64_t oob = 0;
+    const evo_exact e = exact_of(ex, (int64_t)B * H * W);
     const float bm1 = (float)(B - 1);
     for (int64_t i = 0; i < n; ++i) {
         int64_t xi, yi;
@@ -76,7 +105,7 @@ EVO_API int64_t evo_voxel_f32(const float *x, const float *y, const float *t, co
             /* torch.max(zeros, w): NaN if w is NaN, else the larger */
             float wb = (w != w) ? w : (w > 0.0f ? w : 0.0f);
             float wt = p[i] * wb;
-            out[((int64_t)b * H + yi) * W + xi] += wt;
+            add_tap(out, &e, 0, ((int64_t)b * H + yi) * W + xi, wt);
         }
     }
     return oob;
@@ -114,9 +143,10 @@ EVO_API int64_t evo_voxel_f64(const int64_t *x, const int64_t *y, const double *
  * ------------------------------------------------------------------------------------------ */
 EVO_API int64_t evo_image_nearest_f32(const float *x, const float *y, const float *p, int64_t n,
                                       int Himg, int Wimg, int clip, float clipx, float clipy,
-                                      float *out)
+                                      float *out, double *ex)
 {
     int64_t oob = 0;
+    const evo_exact e = exact_of(ex, (int64_t)Himg * Wimg);
     for (int64_t i = 0; i < n; ++i) {
         int64_t m = 1;
         if (clip) m = (x[i] >= clipx ? 0 : 1) * (y[i] >= clipy ? 0 : 1);
@@ -126,7 +156,7 @@ EVO_API int64_t evo_image_nearest_f32(const float *x, const float *y, const floa
         yl = (m ? yl : 0);
         int64_t xi, yi;
         if (!wrap_index(xl, Wimg, &xi) || !wrap_index(yl, Himg, &yi)) { ++oob; continue; }
-        out[yi * Wimg + xi] += p[i];
+        add_tap(out, &e, 0, yi * Wimg + xi, p[i]);
     }
     return oob;
 }
@@ -139,9 +169,10 @@ EVO_API int64_t evo_image_nearest_f32(const float *x, const float *y, const floa
  * ------------------------------------------------------------------------------------------ */
 EVO_API int64_t evo_image_bilinear_f32(const float *x, const float *y, const float *p, int64_t n,
                                        int Himg, int Wimg, int clip, float clipx, float clipy,
-                                       float *out)
+                                       float *out, double *ex)
 {
     int64_t oob = 0;
+    const evo_exact e = exact_of(ex, (int64_t)Himg * Wimg);
     for (int64_t i = 0; i < n; ++i) {
         float m = 1.0f;
         if (clip) m = (x[i] >= clipx ? 0.0f : 1.0f) * (y[i] >= clipy ? 0.0f : 1.0f);
@@ -153,10 +184,10 @@ EVO_API int64_t evo_image_bilinear_f32(const float *x, const float *y, const flo
         if (!wrap_index(px, Wimg, &x0) || !wrap_index(px + 1, Wimg, &x1) ||
             !wrap_index(py, Himg, &y0) || !wrap_index(py + 1, Himg, &y1)) { ++oob; continue; }
         float ox = 1.0f - dx, oy = 1.0f - dy;
-        out[y0 * Wimg + x0] += (w * ox) * oy;
-        out[y0 * Wimg + x1] += (w * dx) * oy;
-        out[y1 * Wimg + x0] += (w * ox) * dy;
-        out[y1 * Wimg + x1] += (w * dx) * dy;
+        add_tap(out, &e, 0, y0 * Wimg + x0, (w * ox) * oy);
+        add_tap(out, &e, 0, y0 * Wimg + x1, (w * dx) * oy);
+        add_tap(out, &e, 0, y1 * Wimg + x0, (w * ox) * dy);
+        add_tap(out, &e, 0, y1 * Wimg + x1, (w * dx) * dy);
     }
     return oob;
 }
@@ -212,11 +243,12 @@ EVO_API void evo_warp_flow_f32(const float *x, const float *y, const float *t, i
 EVO_API int64_t evo_iwe_linvel(const double *x, const double *y, const double *t, const double *p,
                                int64_t n, double vx, double vy, double t_ref,
                                int Hm, int Wm, int Hs, int Ws, int use_polarity,
-                               float *iwe, float *diwe)
+                               float *iwe, float *diwe, double *ex)
 {
     const int Hc = Hs + 1, Wc = Ws + 1;
     const float clipx = (float)(Wc - 1), clipy = (float)(Hc - 1);
     const int64_t plane = (int64_t)Hc * Wc;
+    const evo_exact e = exact_of(ex, plane * 3);   /* planes: IWE, dIWE[0], dIWE[1] */
     int64_t oob = 0;
     for (int64_t i = 0; i < n; ++i) {
         double pp = use_polarity ? p[i] : fabs(p[i]);
@@ -236,23 +268,23 @@ EVO_API int64_t evo_iwe_linvel(const double *x, const double *y, const double *t
         if (!wrap_index(px, Wc, &x0) || !wrap_index(px + 1, Wc, &x1) ||
             !wrap_index(py, Hc, &y0) || !wrap_index(py + 1, Hc, &y1)) { ++oob; continue; }
         float ox = 1.0f - dx, oy = 1.0f - dy;
-        iwe[y0 * Wc + x0] += (w * ox) * oy;
-        iwe[y0 * Wc + x1] += (w * dx) * oy;
-        iwe[y1 * Wc + x0] += (w * ox) * dy;
-        iwe[y1 * Wc + x1] += (w * dx) * dy;
+        add_tap(iwe, &e, 0, y0 * Wc + x0, (w * ox) * oy);
+        add_tap(iwe, &e, 0, y0 * Wc + x1, (w * dx) * oy);
+        add_tap(iwe, &e, 0, y1 * Wc + x0, (w * ox) * dy);
+        add_tap(iwe, &e, 0, y1 * Wc + x1, (w * dx) * dy);
         if (diwe) {
             /* image.py:211-213: w1 = jacobian_x * masked_ps, w2 = jacobian_y * masked_ps with
              * jacobian_x = [-d; 0], jacobian_y = [0; -d] (warps.py:57-60). image.py:131-135. */
             float a = jf * w, z = 0.0f * w;
             float *d0 = diwe, *d1 = diwe + plane;
-            d0[y0 * Wc + x0] += a * (-oy) + z * (-ox);
-            d0[y0 * Wc + x1] += a * oy + z * (-dx);
-            d0[y1 * Wc + x0] += a * (-dy) + z * ox;
-            d0[y1 * Wc + x1] += a * dy + z * dx;
-            d1[y0 * Wc + x0] += z * (-oy) + a * (-ox);
-            d1[y0 * Wc + x1] += z * oy + a * (-dx);
-            d1[y1 * Wc + x0] += z * (-dy) + a * ox;
-            d1[y1 * Wc + x1] += z * dy + a * dx;
+            add_tap(d0, &e, plane, y0 * Wc + x0, a * (-oy) + z * (-ox));
+            add_tap(d0, &e, plane, y0 * Wc + x1, a * oy + z * (-dx));
+            add_tap(d0, &e, plane, y1 * Wc + x0, a * (-dy) + z * ox);
+            add_tap(d0, &e, plane, y1 * Wc + x1, a * dy + z * dx);
+            add_tap(d1, &e, 2 * plane, y0 * Wc + x0, z * (-oy) + a * (-ox));
+            add_tap(d1, &e, 2 * plane, y0 * Wc + x1, z * oy + a * (-dx));
+            add_tap(d1, &e, 2 * plane, y1 * Wc + x0, z * (-dy) + a * ox);
+            add_tap(d1, &e, 2 * plane, y1 * Wc + x1, z * dy + a * dx);
         }
     }
     return oob;
@@ -387,14 +419,16 @@ EVO_API void evo_bounds_mask_f64(const double *x, const double *y, int64_t n, do
  *   four bilinear accumulations: tn*[p>0], [p>0], tn*[p<=0], [p<=0]; the two count images
  *   start at ONE (image.py:333,335); the clip mask zeroes the INDEX only, never the weights
  *   (masked_ps is computed but unused, image.py:330); result = sum / count with count==0 -> 1.
- * out: pos then neg, each Himg*Wimg.
+ * out: pos then neg, each Himg*Wimg.  ex (exact mode): the four accumulation images Tpos, Cpos, Tneg,
+ * Cneg, each without the count images' initial one.
  * ------------------------------------------------------------------------------------------ */
 EVO_API int64_t evo_timestamp_image_f32(const float *x, const float *y, const float *t, const float *p, int64_t n,
                                         float t_first, float t_last, int reverse, int Himg, int Wimg, int clip,
-                                        float clipx, float clipy, float *out)
+                                        float clipx, float clipy, float *out, double *ex)
 {
     const int64_t np_ = (int64_t)Himg * Wimg;
     float *acc = (float *)calloc((size_t)np_ * 4, sizeof(float)); /* Tpos, Cpos, Tneg, Cneg */
+    const evo_exact e = exact_of(ex, np_ * 4);
     int64_t oob = 0;
     const float denom = (t_last - t_first) + 1e-6f;
     for (int64_t i = 0; i < np_; ++i) { acc[np_ + i] = 1.0f; acc[3 * np_ + i] = 1.0f; }
@@ -413,10 +447,10 @@ EVO_API int64_t evo_timestamp_image_f32(const float *x, const float *y, const fl
         float ox = 1.0f - dx, oy = 1.0f - dy;
         for (int k = 0; k < 4; ++k) {
             float *im = acc + k * np_;
-            im[y0 * Wimg + x0] += (w[k] * ox) * oy;
-            im[y0 * Wimg + x1] += (w[k] * dx) * oy;
-            im[y1 * Wimg + x0] += (w[k] * ox) * dy;
-            im[y1 * Wimg + x1] += (w[k] * dx) * dy;
+            add_tap(im, &e, k * np_, y0 * Wimg + x0, (w[k] * ox) * oy);
+            add_tap(im, &e, k * np_, y0 * Wimg + x1, (w[k] * dx) * oy);
+            add_tap(im, &e, k * np_, y1 * Wimg + x0, (w[k] * ox) * dy);
+            add_tap(im, &e, k * np_, y1 * Wimg + x1, (w[k] * dx) * dy);
         }
     }
     for (int s = 0; s < 2; ++s)

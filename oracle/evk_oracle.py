@@ -3,7 +3,12 @@
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
 import this module.  The product package (event_utils_b200) never does.
 Each function cites the reference lines it restates; see the C file for the arithmetic.
+
+Exact mode (``exact=True`` on the scatter functions): besides the f32 result, the f64 sum of the f32 taps of
+every output cell, the f64 sum of their absolute values and the number of non-zero taps, from the same tap code
+as the f32 result (evk_oracle.c add_tap).  It returns the out-of-range event count instead of raising.
 """
+import collections
 import ctypes
 import os
 import subprocess
@@ -30,19 +35,19 @@ def lib():
         i64, f32, f64, ci = ctypes.c_int64, ctypes.c_float, ctypes.c_double, ctypes.c_int
         vp = ctypes.c_void_p
         L.evo_voxel_f32.restype = i64
-        L.evo_voxel_f32.argtypes = [vp, vp, vp, vp, i64, f32, f32, ci, ci, ci, vp]
+        L.evo_voxel_f32.argtypes = [vp, vp, vp, vp, i64, f32, f32, ci, ci, ci, vp, vp]
         L.evo_voxel_f64.restype = i64
         L.evo_voxel_f64.argtypes = [vp, vp, vp, vp, i64, f64, f64, ci, ci, ci, vp]
         L.evo_image_nearest_f32.restype = i64
-        L.evo_image_nearest_f32.argtypes = [vp, vp, vp, i64, ci, ci, ci, f32, f32, vp]
+        L.evo_image_nearest_f32.argtypes = [vp, vp, vp, i64, ci, ci, ci, f32, f32, vp, vp]
         L.evo_image_bilinear_f32.restype = i64
-        L.evo_image_bilinear_f32.argtypes = [vp, vp, vp, i64, ci, ci, ci, f32, f32, vp]
+        L.evo_image_bilinear_f32.argtypes = [vp, vp, vp, i64, ci, ci, ci, f32, f32, vp, vp]
         L.evo_timestamp_image_f32.restype = i64
-        L.evo_timestamp_image_f32.argtypes = [vp, vp, vp, vp, i64, f32, f32, ci, ci, ci, ci, f32, f32, vp]
+        L.evo_timestamp_image_f32.argtypes = [vp, vp, vp, vp, i64, f32, f32, ci, ci, ci, ci, f32, f32, vp, vp]
         L.evo_warp_flow_f32.restype = None
         L.evo_warp_flow_f32.argtypes = [vp, vp, vp, i64, vp, ci, ci, f32, vp, vp]
         L.evo_iwe_linvel.restype = i64
-        L.evo_iwe_linvel.argtypes = [vp, vp, vp, vp, i64, f64, f64, f64, ci, ci, ci, ci, ci, vp, vp]
+        L.evo_iwe_linvel.argtypes = [vp, vp, vp, vp, i64, f64, f64, f64, ci, ci, ci, ci, ci, vp, vp, vp]
         L.evo_gaussian_filter_f32.restype = ci
         L.evo_gaussian_filter_f32.argtypes = [vp, vp, ci, f64]
         L.evo_variance_f.restype = f64
@@ -67,8 +72,21 @@ class OracleIndexError(IndexError):
     """The reference would have raised IndexError / ValueError on these inputs."""
 
 
-def voxel_f32(xs, ys, ts, ps, B, sensor_size=(180, 240), t0=None, dt=None):
-    """events_to_voxel_torch, voxel_grid.py:129-153 (f32).  t0/dt default to ts[0], ts[-1]-ts[0]."""
+# per output cell: f64 sum of the f32 taps, f64 sum of |tap|, number of non-zero taps (arrays shaped like the output)
+Exact = collections.namedtuple("Exact", "sum abs cnt")
+
+
+def _exact_buf(shape, want):
+    return np.zeros((3,) + tuple(shape), np.float64) if want else None
+
+
+def _exact(buf):
+    return Exact(buf[0], buf[1], buf[2])
+
+
+def voxel_f32(xs, ys, ts, ps, B, sensor_size=(180, 240), t0=None, dt=None, exact=False):
+    """events_to_voxel_torch, voxel_grid.py:129-153 (f32).  t0/dt default to ts[0], ts[-1]-ts[0].
+    exact=True -> (out, Exact, oob count)."""
     x, y, t, p = (_c(a, np.float32) for a in (xs, ys, ts, ps))
     n = x.shape[0]
     H, W = int(sensor_size[0]), int(sensor_size[1])
@@ -77,7 +95,11 @@ def voxel_f32(xs, ys, ts, ps, B, sensor_size=(180, 240), t0=None, dt=None):
     if dt is None:
         dt = np.float32(t[-1]) - np.float32(t[0])
     out = np.zeros((B, H, W), np.float32)
-    oob = lib().evo_voxel_f32(_p(x), _p(y), _p(t), _p(p), n, float(t0), float(dt), B, H, W, _p(out))
+    ex = _exact_buf(out.shape, exact)
+    oob = lib().evo_voxel_f32(_p(x), _p(y), _p(t), _p(p), n, float(t0), float(dt), B, H, W, _p(out),
+                              _p(ex) if exact else None)
+    if exact:
+        return out, _exact(ex), oob
     if oob:
         raise OracleIndexError("%d events index outside the grid" % oob)
     return out
@@ -100,8 +122,9 @@ def voxel_f64(xs, ys, ts, ps, B, sensor_size=(180, 240), t0=None, dt=None):
 
 
 def image_torch_f32(xs, ys, ps, sensor_size=(180, 240), clip_out_of_range=True,
-                    interpolation=None, padding=True, default=0):
-    """events_to_image_torch, image.py:46-100 (+102-115): returns the un-cropped canvas."""
+                    interpolation=None, padding=True, default=0, exact=False):
+    """events_to_image_torch, image.py:46-100 (+102-115): returns the un-cropped canvas.
+    exact=True -> (canvas, Exact of the taps (the background not included), oob count)."""
     x, y, p = (_c(a, np.float32) for a in (xs, ys, ps))
     bil = interpolation == "bilinear"
     H, W = int(sensor_size[0]), int(sensor_size[1])
@@ -112,18 +135,23 @@ def image_torch_f32(xs, ys, ps, sensor_size=(180, 240), clip_out_of_range=True,
     else:
         clipx, clipy = W - 1, H - 1
     out = np.full((H, W), default, np.float32)
+    ex = _exact_buf(out.shape, exact)
     fn = lib().evo_image_bilinear_f32 if bil else lib().evo_image_nearest_f32
     oob = fn(_p(x), _p(y), _p(p), x.shape[0], H, W, int(bool(clip_out_of_range)),
-             float(clipx), float(clipy), _p(out))
+             float(clipx), float(clipy), _p(out), _p(ex) if exact else None)
+    if exact:
+        return out, _exact(ex), oob
     if oob:
         raise OracleIndexError("%d events index outside the image" % oob)
     return out
 
 
 def timestamp_image_f32(xs, ys, ts, ps, sensor_size=(180, 240), clip_out_of_range=True, interpolation='bilinear',
-                        padding=True, timestamp_reverse=False, normalize_timestamps=True):
+                        padding=True, timestamp_reverse=False, normalize_timestamps=True, exact=False):
     """events_to_timestamp_image_torch, image.py:286-353 -> (img_pos, img_neg).
-    normalize_timestamps=False: the numpy flavour's raw-stamp weights (image.py:261)."""
+    normalize_timestamps=False: the numpy flavour's raw-stamp weights (image.py:261).
+    exact=True -> (img_pos, img_neg, Exact of the four accumulations [Tpos, Cpos, Tneg, Cneg] -- the count images
+    WITHOUT their initial one, oob count)."""
     x, y, t, p = (_c(np.asarray(a).reshape(-1), np.float32) for a in (xs, ys, ts, ps))
     H, W = int(sensor_size[0]), int(sensor_size[1])
     if padding:
@@ -133,10 +161,13 @@ def timestamp_image_f32(xs, ys, ts, ps, sensor_size=(180, 240), clip_out_of_rang
     else:
         clipx, clipy = W - 1, H - 1
     out = np.zeros((2, H, W), np.float32)
+    ex = _exact_buf((4, H, W), exact)
     oob = lib().evo_timestamp_image_f32(_p(x), _p(y), _p(t), _p(p), x.shape[0], float(t[0]), float(t[-1]),
                                         int(bool(timestamp_reverse)) if normalize_timestamps else 2, H, W,
                                         int(bool(clip_out_of_range)),
-                                        float(clipx), float(clipy), _p(out))
+                                        float(clipx), float(clipy), _p(out), _p(ex) if exact else None)
+    if exact:
+        return out[0], out[1], _exact(ex), oob
     if oob:
         raise OracleIndexError("%d events index outside the image" % oob)
     return out[0], out[1]
@@ -157,18 +188,22 @@ def warp_flow_f32(xs, ys, ts, flow, t0=None):
 
 
 def iwe_linvel(params, xs, ys, ts, ps, img_size, compute_gradient=False, use_polarity=True,
-               sensor_size=(180, 240), t_ref=None):
+               sensor_size=(180, 240), t_ref=None, exact=False):
     """get_iwe with linvel_warp, objectives.py:184-192 -> (iwe, d_iwe or None).
     t_ref: reference time of the warp; the reference uses ts[-1] (objectives.py:186), a shard of a
-    longer stream passes the stream's last timestamp."""
+    longer stream passes the stream's last timestamp.
+    exact=True -> (iwe, d_iwe or None, Exact of the planes [IWE, dIWE[0], dIWE[1]], out-of-canvas count)."""
     x, y, t, p = (_c(a, np.float64) for a in (xs, ys, ts, ps))
     Hs, Ws = int(sensor_size[0]), int(sensor_size[1])
     iwe = np.zeros((Hs + 1, Ws + 1), np.float32)
     d = np.zeros((2, Hs + 1, Ws + 1), np.float32) if compute_gradient else None
+    ex = _exact_buf((3, Hs + 1, Ws + 1), exact)
     oob = lib().evo_iwe_linvel(_p(x), _p(y), _p(t), _p(p), x.shape[0], float(params[0]),
                                float(params[1]), float(t[-1] if t_ref is None else t_ref), int(img_size[0]), int(img_size[1]),
                                Hs, Ws, int(bool(use_polarity)), _p(iwe),
-                               _p(d) if d is not None else None)
+                               _p(d) if d is not None else None, _p(ex) if exact else None)
+    if exact:
+        return iwe, d, _exact(ex), oob
     if oob:
         raise OracleIndexError("%d warped events index outside the IWE canvas" % oob)
     return iwe, d

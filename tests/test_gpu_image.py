@@ -125,21 +125,11 @@ def test_hot_spot_bilinear_and_signed(oracle):
     x = x + rng.random(n).astype(np.float32) * np.float32(0.999)
     y = y + rng.random(n).astype(np.float32) * np.float32(0.999)
     p = (rng.integers(0, 2, n) * 2 - 1).astype(np.float32)
-    # f32 tap weights exactly as image.py:79-86,111-114 computes them, accumulated in f64
-    px, py = np.floor(x), np.floor(y)
-    dx, dy = x - px, y - py
-    keep = ((x < W) & (y < H)).astype(np.float32)
-    ix, iy = (px * keep).astype(np.int64), (py * keep).astype(np.int64)
-    w = p * keep
-    one = np.float32(1.0)
-    exact = np.zeros((H + 1, W + 1), np.float64)
-    cnt = np.zeros((H + 1, W + 1), np.int64)
-    for oy_, ox_, tap in ((0, 0, w * (one - dx) * (one - dy)), (0, 1, w * dx * (one - dy)),
-                          (1, 0, w * (one - dx) * dy), (1, 1, w * dx * dy)):
-        np.add.at(exact, (iy + oy_, ix + ox_), tap.astype(np.float64))
-        np.add.at(cnt, (iy + oy_, ix + ox_), 1)
+    # the oracle's f32 taps (image.py:79-86,111-114) accumulated in f64, and the number of taps per cell
+    ref, ex, oob = oracle.image_torch_f32(x, y, p, sensor_size=(H, W), interpolation='bilinear', exact=True)
+    assert oob == 0
+    exact, cnt = ex.sum, ex.cnt
     bound = 2.0 * np.sqrt(cnt.max()) * np.finfo(np.float32).eps * np.abs(exact).max()
-    ref = oracle.image_torch_f32(x, y, p, sensor_size=(H, W), interpolation='bilinear')
     assert np.abs(ref - exact).max() <= bound
     for variant in ("smem_cache", "vector_red", "global_red", None):
         eu.config.variant = variant
