@@ -76,6 +76,20 @@ def _declare(L):
     L.evk_timestamp_image_workspace_bytes.argtypes = [ci, ci]
     L.evk_timestamp_image_f32.restype = ci
     L.evk_timestamp_image_f32.argtypes = [vp, vp, vp, vp, i64, f32, f32, ci, ci, f32, f32, cu, vp, vp, vp, sz, vp, vp]
+    L.evk_timestamp_image_counts_f32.restype = ci
+    L.evk_timestamp_image_counts_f32.argtypes = [vp, vp, vp, vp, i64, f32, f32, ci, ci, f32, f32, cu, vp, vp, vp, vp, vp, sz,
+                                                 vp, vp]
+    L.evk_image_grad_f32.restype = ci
+    L.evk_image_grad_f32.argtypes = [vp, vp, vp, i64, ci, ci, f32, f32, cu, vp, vp, vp, vp, vp]
+    L.evk_timestamp_image_grad_workspace_bytes.restype = sz
+    L.evk_timestamp_image_grad_workspace_bytes.argtypes = [ci, ci]
+    L.evk_timestamp_image_grad_f32.restype = ci
+    L.evk_timestamp_image_grad_f32.argtypes = [vp, vp, vp, vp, i64, f32, f32, ci, ci, f32, f32, cu, vp, vp, vp, vp, vp, vp,
+                                               vp, vp, vp, vp, vp, sz, vp]
+    L.evk_warp_flow_grad_workspace_bytes.restype = sz
+    L.evk_warp_flow_grad_workspace_bytes.argtypes = [ci, ci]
+    L.evk_warp_flow_grad_f32.restype = ci
+    L.evk_warp_flow_grad_f32.argtypes = [vp, vp, vp, i64, vp, ci, ci, f32, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
     L.evk_count_u32.restype = ci
     L.evk_count_u32.argtypes = [vp, vp, i64, ci, ci, f32, f32, cu, vp, vp, vp]
     L.evk_splat_idx_f32.restype = ci

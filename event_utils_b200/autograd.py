@@ -1,0 +1,168 @@
+"""Autograd for the torch functions whose reference versions are plain, differentiable torch ops.
+
+The reference builds its event images, timestamp images and flow warp from `index_put_(accumulate=True)`,
+`grid_sample` and weights made of `xs - floor(xs)` (image.py:46-100, image.py:286-353, optic_flow.py:5-46), so
+autograd runs through them: flow -> warp -> event image -> loss -> backward() into the flow.  Our forwards are
+CUDA kernels, so each function gets a torch.autograd.Function here whose forward is the existing kernel path
+(bit-identical outputs) and whose backward is one pass of a kernel of csrc/evk_grad.cu.
+
+Which inputs get a gradient (as in the reference; the others get None):
+    events_to_image_torch            bilinear: xs, ys, ps;  nearest (or integer coordinates): ps
+    events_to_timestamp_image_torch  xs, ys, ts
+    warp_events_flow_torch           xt, yt, tt, flow_field, t0 (when it is a tensor; t0=None means tt[-1])
+
+The public functions take this path only when grad mode is on and one of those inputs requires grad; every
+other call runs the plain forward.  Gradients come back in each input's shape, dtype and device.  The
+backwards are not themselves differentiable (no double backward).
+"""
+import numpy as np
+import torch
+from torch.autograd.function import once_differentiable
+
+from . import _lib
+
+
+def _meta(t):
+    return (t.shape, t.dtype, t.device) if isinstance(t, torch.Tensor) else None
+
+
+def _as_input(g, meta):
+    """A per-event gradient (flat f32 on the compute device) in the shape, dtype and device of its input."""
+    if g is None or meta is None:
+        return None
+    shape, dtype, device = meta
+    return g.reshape(shape).to(device=device, dtype=dtype)
+
+
+def _grad_in(g, dev):
+    """The incoming gradient as contiguous f32 on the compute device (autograd hands zeros for an unused output, and
+    an expanded gradient such as the one of img.sum() has stride 0)."""
+    return g.to(device=dev, dtype=torch.float32).contiguous()
+
+
+class EventImage(torch.autograd.Function):
+    """events_to_image_torch (image.py:46-100)."""
+
+    @staticmethod
+    def forward(ctx, xs, ys, ps, opts):
+        from .representations.image import _image_device, _image_inputs
+        device, sensor_size, clip, interpolation, padding, default = opts
+        dev, (H, W), clipx, clipy, flags, x, y, p = _image_inputs(xs, ys, ps, sensor_size, clip, interpolation, padding)
+        img = _image_device(x, y, p, H, W, clipx, clipy, flags, default)
+        ctx.save_for_backward(x, y, p)
+        ctx.geom = (dev, H, W, clipx, clipy, flags)
+        ctx.metas = tuple(_meta(t) for t in (xs, ys, ps))
+        return img if img.device == device else img.to(device)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, y, p = ctx.saved_tensors
+        dev, H, W, clipx, clipy, flags = ctx.geom
+        bil = bool(flags & _lib.BILINEAR)
+        need = ctx.needs_input_grad
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g = _grad_in(g, dev)
+            gx = torch.empty_like(x) if bil and need[0] else None
+            gy = torch.empty_like(y) if bil and need[1] else None
+            gp = torch.empty_like(p) if need[2] else None
+            _lib.check(L.evk_image_grad_f32(_lib.ptr(x), _lib.ptr(y), _lib.ptr(p), x.shape[0], H, W, clipx, clipy, flags,
+                                            _lib.ptr(g), _lib.ptr(gx), _lib.ptr(gy), _lib.ptr(gp), _lib.stream()))
+        return _as_input(gx, ctx.metas[0]), _as_input(gy, ctx.metas[1]), _as_input(gp, ctx.metas[2]), None
+
+
+class TimestampImages(torch.autograd.Function):
+    """events_to_timestamp_image_torch (image.py:286-353).  The forward also keeps the two count images."""
+
+    @staticmethod
+    def forward(ctx, xs, ys, ts, ps, opts):
+        from .representations.image import _timestamp_images, _timestamp_inputs, _ts_canvas_and_clip, _ts_flags
+        device, sensor_size, clip, interpolation, padding, reverse = opts
+        dev, x, y, t, p, fl = _timestamp_inputs(xs, ys, ts, ps)
+        pos, neg, cpos, cneg = _timestamp_images(x, y, t, p, fl[0], fl[1], sensor_size, clip, interpolation, padding,
+                                                 reverse, counts=True)
+        ctx.save_for_backward(x, y, t, p, pos, neg, cpos, cneg)
+        _, clipx, clipy = _ts_canvas_and_clip(sensor_size, interpolation, padding)
+        ctx.geom = (dev, fl[0], fl[1], clipx, clipy, _ts_flags(clip, reverse), reverse)
+        ctx.metas = tuple(_meta(a) for a in (xs, ys, ts))
+        if pos.device != device:
+            pos, neg = pos.to(device), neg.to(device)
+        return pos, neg
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_pos, g_neg):
+        x, y, t, p, pos, neg, cpos, cneg = ctx.saved_tensors
+        dev, t_first, t_last, clipx, clipy, flags, reverse = ctx.geom
+        need = ctx.needs_input_grad
+        H, W = pos.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g_pos, g_neg = _grad_in(g_pos, dev), _grad_in(g_neg, dev)
+            gx = torch.empty_like(x) if need[0] else None
+            gy = torch.empty_like(y) if need[1] else None
+            gt = torch.empty_like(t) if need[2] else None
+            sums = torch.empty(2, dtype=torch.float64, device=dev)
+            ws = torch.empty(L.evk_timestamp_image_grad_workspace_bytes(H, W), dtype=torch.uint8, device=dev)
+            _lib.check(L.evk_timestamp_image_grad_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), x.shape[0], t_first, t_last, H, W, clipx, clipy, flags,
+                _lib.ptr(g_pos), _lib.ptr(g_neg), _lib.ptr(pos), _lib.ptr(neg), _lib.ptr(cpos), _lib.ptr(cneg),
+                _lib.ptr(gx), _lib.ptr(gy), _lib.ptr(gt), _lib.ptr(sums), _lib.ptr(ws), ws.numel(), _lib.stream()))
+            if gt is not None and gt.numel():
+                # tn's denominator D = ts[-1] - ts[0] + 1e-6 (f32, as the kernels form it) also depends on ts[0], ts[-1]
+                D = float(np.float32(np.float32(t_last) - np.float32(t_first)) + np.float32(1e-6))
+                s0, s1 = sums[0], sums[1]
+                if reverse:
+                    d_first, d_last = s1 / D, (s0 - s1) / D
+                else:
+                    d_first, d_last = (s1 - s0) / D, -s1 / D
+                gt[0] += d_first.to(torch.float32)
+                gt[-1] += d_last.to(torch.float32)
+        return _as_input(gx, ctx.metas[0]), _as_input(gy, ctx.metas[1]), _as_input(gt, ctx.metas[2]), None, None
+
+
+class WarpFlow(torch.autograd.Function):
+    """warp_events_flow_torch (optic_flow.py:5-46), with t0 a tensor (tt[-1] when the caller gave none, so that its
+    gradient reaches the last event)."""
+
+    @staticmethod
+    def forward(ctx, xt, yt, tt, t0, flow_field, out_device):
+        from .transforms.optic_flow import _flow_inputs, _warp_device
+        dev, x, y, t, f = _flow_inputs(xt, yt, tt, flow_field)
+        with torch.cuda.device(dev):
+            # dt = tt - t0 in the dtype the plain path forms it in (the kernel's f32 subtraction for f32 stamps, the
+            # input dtype's otherwise), then the kernel runs with t0 = 0: the same warped coordinates, bit for bit
+            rt = torch.result_type(t, 1.0)
+            t_rel = (t.to(rt) - t0.detach().to(device=dev, dtype=rt)).to(torch.float32).contiguous()
+            xw, yw = _warp_device(x, y, t_rel, f, 0.0)
+        ctx.save_for_backward(x, y, t_rel, f)
+        ctx.dev = dev
+        ctx.metas = tuple(_meta(a) for a in (xt, yt, tt, t0, flow_field))
+        if xw.device != out_device:
+            xw, yw = xw.to(out_device), yw.to(out_device)
+        return xw, yw
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_xw, g_yw):
+        x, y, t, f = ctx.saved_tensors
+        dev = ctx.dev
+        need = ctx.needs_input_grad
+        H, W = f.shape[1], f.shape[2]
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g_xw, g_yw = _grad_in(g_xw, dev), _grad_in(g_yw, dev)
+            gx = torch.empty_like(x) if need[0] else None
+            gy = torch.empty_like(y) if need[1] else None
+            gt = torch.empty_like(t) if need[2] or need[3] else None
+            gf = torch.empty_like(f)
+            s = torch.empty(1, dtype=torch.float64, device=dev)
+            ws = torch.empty(L.evk_warp_flow_grad_workspace_bytes(H, W), dtype=torch.uint8, device=dev)
+            _lib.check(L.evk_warp_flow_grad_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t), x.shape[0], _lib.ptr(f), H, W, 0.0, _lib.ptr(g_xw), _lib.ptr(g_yw),
+                _lib.ptr(gx), _lib.ptr(gy), _lib.ptr(gt), _lib.ptr(gf), _lib.ptr(s), _lib.ptr(ws), ws.numel(), _lib.stream()))
+        m = ctx.metas
+        g_t0 = _as_input(-s, m[3]) if need[3] else None
+        return (_as_input(gx, m[0]), _as_input(gy, m[1]), _as_input(gt, m[2]) if need[2] else None, g_t0,
+                _as_input(gf, m[4]) if need[4] else None, None)

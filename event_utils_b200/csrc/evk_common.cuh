@@ -49,6 +49,8 @@ int launch_image_hot(const float *x, const float *y, const float *p, int64_t n, 
 
 // evk_image.cu: dense flow [2][H][W] -> interleaved [H][W] {u, v} pairs (see flow_row below)
 void launch_flow_interleave(const float *flow, int64_t npix, float2 *uv, cudaStream_t st);
+// evk_image.cu: 2x2-block workspace [H][W][4] {TL,TR,BL,BR} -> out[H][W] (overwritten)
+void launch_image_fold(const float *ws, float *out, int H, int W, cudaStream_t st);
 
 static inline unsigned variant_of(unsigned flags) { return flags & EVK_VARIANT_MASK; }
 

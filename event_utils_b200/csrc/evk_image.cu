@@ -291,6 +291,12 @@ void launch_flow_interleave(const float *flow, int64_t npix, float2 *uv, cudaStr
     flow_interleave_kernel<<<grid_simple(npix, 256), 256, 0, st>>>(flow, npix, uv);
 }
 
+void launch_image_fold(const float *ws, float *out, int H, int W, cudaStream_t st)
+{
+    prof_count(1);
+    image_fold_kernel<false><<<grid_simple((int64_t)H * W, 256), 256, 0, st>>>(ws, out, H, W, 0.0f);
+}
+
 }  // namespace evk
 
 extern "C" {

@@ -69,8 +69,11 @@ __global__ void __launch_bounds__(256) tsimg_scatter_kernel(const TsArgs A)
     flush_oob(A.oob, oob);
 }
 
+// CNT: also store the count images C (after the zero guard), which the backward needs (evk_grad.cu)
+template <bool CNT>
 __global__ void __launch_bounds__(256) tsimg_fold_kernel(const float *__restrict__ ws, float *__restrict__ out_pos,
-                                                         float *__restrict__ out_neg, int H, int W)
+                                                         float *__restrict__ out_neg, float *__restrict__ cnt_pos,
+                                                         float *__restrict__ cnt_neg, int H, int W)
 {
     const int64_t npix = (int64_t)H * W;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -86,6 +89,7 @@ __global__ void __launch_bounds__(256) tsimg_fold_kernel(const float *__restrict
         float c = __fadd_rn(1.0f, csum);  // count images are initialised to ones (image.py:333,335)
         if (c == 0.0f) c = 1.0f;
         (s ? out_neg : out_pos)[i] = __fdiv_rn(tsum, c);
+        if (CNT) (s ? cnt_neg : cnt_pos)[i] = c;
     }
 }
 
@@ -99,18 +103,19 @@ size_t evk_timestamp_image_workspace_bytes(int Himg, int Wimg)
     return (size_t)2 * Himg * Wimg * 8 * sizeof(float);
 }
 
-int evk_timestamp_image_f32(const float *x, const float *y, const float *t, const float *p, int64_t n, float t_first,
-                            float t_last, int Himg, int Wimg, float clipx, float clipy, unsigned flags, float *out_pos,
-                            float *out_neg, void *workspace, size_t workspace_bytes, unsigned long long *oob, void *stream)
+static int timestamp_image(const float *x, const float *y, const float *t, const float *p, int64_t n, float t_first,
+                           float t_last, int Himg, int Wimg, float clipx, float clipy, unsigned flags, float *out_pos,
+                           float *out_neg, float *cnt_pos, float *cnt_neg, void *workspace, size_t workspace_bytes,
+                           unsigned long long *oob, void *stream, const char *name)
 {
     using namespace evk;
     if (n < 0 || Himg < 2 || Wimg < 2 || !out_pos || !out_neg || (n > 0 && (!x || !y || !t || !p))) {
-        set_error("evk_timestamp_image_f32: bad arguments");
+        set_error("%s: bad arguments", name);
         return EVK_E_ARG;
     }
     const size_t need = evk_timestamp_image_workspace_bytes(Himg, Wimg);
     if (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 15)) {
-        set_error("evk_timestamp_image_f32: 16-byte aligned workspace of %zu bytes required", need);
+        set_error("%s: 16-byte aligned workspace of %zu bytes required", name, need);
         return EVK_E_WORKSPACE;
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -129,9 +134,32 @@ int evk_timestamp_image_f32(const float *x, const float *y, const float *t, cons
         tsimg_scatter_kernel<<<grid_for(tsimg_scatter_kernel, 256, n, 256 * 8), 256, 0, st>>>(A);
     }
     prof_count(1);
-    tsimg_fold_kernel<<<grid_simple((int64_t)2 * Himg * Wimg, 256), 256, 0, st>>>(A.ws, out_pos, out_neg, Himg, Wimg);
+    const int g2 = grid_simple((int64_t)2 * Himg * Wimg, 256);
+    if (cnt_pos) tsimg_fold_kernel<true><<<g2, 256, 0, st>>>(A.ws, out_pos, out_neg, cnt_pos, cnt_neg, Himg, Wimg);
+    else tsimg_fold_kernel<false><<<g2, 256, 0, st>>>(A.ws, out_pos, out_neg, nullptr, nullptr, Himg, Wimg);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
+}
+
+int evk_timestamp_image_f32(const float *x, const float *y, const float *t, const float *p, int64_t n, float t_first,
+                            float t_last, int Himg, int Wimg, float clipx, float clipy, unsigned flags, float *out_pos,
+                            float *out_neg, void *workspace, size_t workspace_bytes, unsigned long long *oob, void *stream)
+{
+    return timestamp_image(x, y, t, p, n, t_first, t_last, Himg, Wimg, clipx, clipy, flags, out_pos, out_neg, nullptr,
+                           nullptr, workspace, workspace_bytes, oob, stream, "evk_timestamp_image_f32");
+}
+
+int evk_timestamp_image_counts_f32(const float *x, const float *y, const float *t, const float *p, int64_t n,
+                                   float t_first, float t_last, int Himg, int Wimg, float clipx, float clipy,
+                                   unsigned flags, float *out_pos, float *out_neg, float *cnt_pos, float *cnt_neg,
+                                   void *workspace, size_t workspace_bytes, unsigned long long *oob, void *stream)
+{
+    if (!cnt_pos || !cnt_neg) {
+        evk::set_error("evk_timestamp_image_counts_f32: bad arguments");
+        return EVK_E_ARG;
+    }
+    return timestamp_image(x, y, t, p, n, t_first, t_last, Himg, Wimg, clipx, clipy, flags, out_pos, out_neg, cnt_pos,
+                           cnt_neg, workspace, workspace_bytes, oob, stream, "evk_timestamp_image_counts_f32");
 }
 
 }  // extern "C"

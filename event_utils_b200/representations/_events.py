@@ -19,6 +19,11 @@ def as_tensor(a):
     return torch.from_numpy(np.ascontiguousarray(a))
 
 
+def needs_grad(*inputs):
+    """True when autograd has to record the call: grad mode is on and one of the differentiable inputs requires grad."""
+    return torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in inputs)
+
+
 def compute_device(*tensors):
     """CUDA device the kernels run on: the inputs' device, or the default one for host inputs."""
     for t in tensors:

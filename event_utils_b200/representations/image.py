@@ -51,11 +51,25 @@ def events_to_image_torch(xs, ys, ps,
     with clip_out_of_range the INDEX of a clipped event is zeroed but its weight is not in
     nearest mode (image.py:94-95), negative indices wrap, the default padding=True makes the
     last row/column count as out of range.
+    Differentiable like the reference: bilinear w.r.t. xs, ys and ps, nearest w.r.t. ps
+    (event_utils_b200.autograd).
     """
     xs_t = E.as_tensor(xs)
     if device is None:
         device = xs_t.device
     device = torch.device(device)
+    if E.needs_grad(*((xs, ys, ps) if interpolation == 'bilinear' else (ps,))):
+        from ..autograd import EventImage
+        return EventImage.apply(xs, ys, ps, (device, sensor_size, clip_out_of_range, interpolation, padding, default))
+    dev, (Himg, Wimg), clipx, clipy, flags, x, y, p = _image_inputs(xs, ys, ps, sensor_size, clip_out_of_range,
+                                                                    interpolation, padding)
+    img = _image_device(x, y, p, Himg, Wimg, clipx, clipy, flags, default)
+    return img if img.device == device else img.to(device)
+
+
+def _image_inputs(xs, ys, ps, sensor_size, clip_out_of_range, interpolation, padding):
+    """events_to_image_torch's kernel inputs: compute device, canvas, clip thresholds, flags and f32 x, y, p."""
+    xs_t = E.as_tensor(xs)
     dev = E.compute_device(xs, ys, ps)
     (Himg, Wimg), clipx, clipy = _canvas_and_clip(sensor_size, interpolation, padding)
     # image.py:78: integer coordinates fall back to the nearest branch (on the padded canvas)
@@ -71,8 +85,7 @@ def events_to_image_torch(xs, ys, ps,
     else:
         x, y = E.coords_f32(xs, dev), E.coords_f32(ys, dev)
     p = E.weights_f32(ps_t.squeeze() if bilinear else ps_t, dev)
-    img = _image_device(x, y, p, Himg, Wimg, clipx, clipy, flags, default)
-    return img if img.device == device else img.to(device)
+    return dev, (Himg, Wimg), clipx, clipy, flags, x, y, p
 
 
 def events_to_image(xs, ys, ps, sensor_size=(180, 240), interpolation=None, padding=False, meanval=False, default=0):
@@ -182,27 +195,55 @@ def image_to_event_weights(xs, ys, img):
         return out.cpu().numpy()
 
 
-def _timestamp_images(x, y, t, p, t_first, t_last, sensor_size, clip_out_of_range, interpolation, padding, reverse,
-                      raw=False):
-    L = _lib.lib()
-    dev = x.device
+def _ts_canvas_and_clip(sensor_size, interpolation, padding):
+    """image.py:305-312: the canvas of the timestamp images and the clip thresholds."""
     if padding:
         img_size = (int(sensor_size[0]) + 1, int(sensor_size[1]) + 1)
     else:
         img_size = (int(sensor_size[0]), int(sensor_size[1]))
     clipx = img_size[1] if interpolation is None and padding == False else img_size[1] - 1  # noqa: E712
     clipy = img_size[0] if interpolation is None and padding == False else img_size[0] - 1  # noqa: E712
+    return img_size, float(clipx), float(clipy)
+
+
+def _ts_flags(clip_out_of_range, reverse, raw=False):
+    return (_lib.CLIP if clip_out_of_range else 0) | (_lib.TS_REVERSE if reverse else 0) | (_lib.TS_RAW if raw else 0)
+
+
+def _timestamp_images(x, y, t, p, t_first, t_last, sensor_size, clip_out_of_range, interpolation, padding, reverse,
+                      raw=False, counts=False):
+    """The two timestamp images; with `counts` also the two count images they were divided by (for the backward)."""
+    L = _lib.lib()
+    dev = x.device
+    img_size, clipx, clipy = _ts_canvas_and_clip(sensor_size, interpolation, padding)
     with torch.cuda.device(dev):
         pos = torch.empty(img_size, dtype=torch.float32, device=dev)
         neg = torch.empty(img_size, dtype=torch.float32, device=dev)
         ws = _lib.scratch("tsimg_ws", L.evk_timestamp_image_workspace_bytes(*img_size), dev)
         oob = _lib.oob_counter(dev)
-        flags = (_lib.CLIP if clip_out_of_range else 0) | (_lib.TS_REVERSE if reverse else 0) | (_lib.TS_RAW if raw else 0)
-        _lib.check(L.evk_timestamp_image_f32(_lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), x.shape[0], t_first, t_last,
-                                             img_size[0], img_size[1], float(clipx), float(clipy), flags, _lib.ptr(pos),
-                                             _lib.ptr(neg), _lib.ptr(ws), ws.numel(), _lib.ptr(oob), _lib.stream()))
+        flags = _ts_flags(clip_out_of_range, reverse, raw)
+        if counts:
+            cpos, cneg = torch.empty_like(pos), torch.empty_like(neg)
+            _lib.check(L.evk_timestamp_image_counts_f32(_lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), x.shape[0],
+                                                        t_first, t_last, img_size[0], img_size[1], clipx, clipy, flags,
+                                                        _lib.ptr(pos), _lib.ptr(neg), _lib.ptr(cpos), _lib.ptr(cneg),
+                                                        _lib.ptr(ws), ws.numel(), _lib.ptr(oob), _lib.stream()))
+        else:
+            _lib.check(L.evk_timestamp_image_f32(_lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), x.shape[0], t_first, t_last,
+                                                 img_size[0], img_size[1], clipx, clipy, flags, _lib.ptr(pos),
+                                                 _lib.ptr(neg), _lib.ptr(ws), ws.numel(), _lib.ptr(oob), _lib.stream()))
         E.raise_if_oob(oob, "timestamp image", img_size)
+    if counts:
+        return pos, neg, cpos, cneg
     return pos, neg
+
+
+def _timestamp_inputs(xs, ys, ts, ps):
+    """events_to_timestamp_image_torch's kernel inputs: compute device, f32 x, y, t, p and (ts[0], ts[-1])."""
+    dev = E.compute_device(xs, ys, ts, ps)
+    x, y, t, p = (E.to_device(E.as_tensor(a).squeeze().reshape(-1), dev).to(torch.float32).contiguous() for a in (xs, ys, ts, ps))
+    fl = torch.stack((t[0], t[-1])).tolist()
+    return dev, x, y, t, p, fl
 
 
 def events_to_timestamp_image_torch(xs, ys, ts, ps,
@@ -211,16 +252,19 @@ def events_to_timestamp_image_torch(xs, ys, ts, ps,
     """
     Average-timestamp images (Zhu et al. 2019) of the positive and negative events; drop-in for
     image.py:286-353.  Quirks kept: the count images start at one, and a clipped event keeps its
-    weight (only its index is zeroed).
+    weight (only its index is zeroed).  Differentiable like the reference w.r.t. xs, ys and ts
+    (event_utils_b200.autograd).
     @returns img_pos, img_neg (canvas (H+1,W+1) with padding)
     """
     xs_t = E.as_tensor(xs)
     if device is None:
         device = xs_t.device
     device = torch.device(device)
-    dev = E.compute_device(xs, ys, ts, ps)
-    x, y, t, p = (E.to_device(E.as_tensor(a).squeeze().reshape(-1), dev).to(torch.float32).contiguous() for a in (xs, ys, ts, ps))
-    fl = torch.stack((t[0], t[-1])).tolist()
+    if E.needs_grad(xs, ys, ts):
+        from ..autograd import TimestampImages
+        return TimestampImages.apply(xs, ys, ts, ps, (device, sensor_size, clip_out_of_range, interpolation, padding,
+                                                      timestamp_reverse))
+    dev, x, y, t, p, fl = _timestamp_inputs(xs, ys, ts, ps)
     pos, neg = _timestamp_images(x, y, t, p, fl[0], fl[1], sensor_size, clip_out_of_range, interpolation, padding,
                                  timestamp_reverse)
     if pos.device != device:

@@ -184,6 +184,13 @@ int evk_timestamp_image_f32(const float *x, const float *y, const float *t, cons
                             float t_first, float t_last, int Himg, int Wimg, float clipx, float clipy,
                             unsigned flags, float *out_pos, float *out_neg, void *workspace,
                             size_t workspace_bytes, unsigned long long *oob, void *stream);
+/* Same, and also writes the count images the division uses (image.py:333-351: one plus the bilinear
+ * count, a zero replaced by one) into cnt_pos / cnt_neg (Himg*Wimg floats each), which the backward
+ * evk_timestamp_image_grad_f32 needs.  out_pos / out_neg are bit-identical to evk_timestamp_image_f32's. */
+int evk_timestamp_image_counts_f32(const float *x, const float *y, const float *t, const float *p, int64_t n,
+                                   float t_first, float t_last, int Himg, int Wimg, float clipx, float clipy,
+                                   unsigned flags, float *out_pos, float *out_neg, float *cnt_pos, float *cnt_neg,
+                                   void *workspace, size_t workspace_bytes, unsigned long long *oob, void *stream);
 
 /* Integer-exact event-count image (nearest, weight +1 per event): out is u32 [Himg][Wimg].
  * The bit-exact form of events_to_image(_torch) for ps == 1 (image.py:37-38, :95). */
@@ -225,6 +232,53 @@ size_t evk_warp_flow_workspace_bytes(int H, int W);
 int evk_warp_flow_f32(const float *x, const float *y, const float *t, int64_t n, const float *flow,
                       int H, int W, float t0, float *xw, float *yw, void *workspace,
                       size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Backward passes.  The reference's torch functions are plain torch ops that autograd runs through
+ * (events_to_image_torch image.py:46-100 with interpolate_to_image :102-115, events_to_timestamp_image_torch
+ * image.py:286-353, warp_events_flow_torch optic_flow.py:5-46); these entry points give the same gradients
+ * for the forward entry points above, one pass over the events each.  Arguments that name the forward's
+ * inputs take the values the forward was called with.  Per-event gradient outputs are n floats and may be
+ * NULL (not written).  floor() has zero derivative, so gradients are one-sided at integer coordinates.
+ *
+ *   evk_image_grad_f32   gradient of evk_image_f32 (flags: EVK_BILINEAR, EVK_CLIP) given grad_img
+ *                        [Himg][Wimg].  Bilinear: grad_x, grad_y through the fractions x - floor(x),
+ *                        y - floor(y) (unmasked, as in the forward), grad_p = mask * the gathered taps.
+ *                        Nearest: grad_p = grad_img[trunc(y)*m][trunc(x)*m] (clipped events read [0][0],
+ *                        negative indices wrap); grad_x / grad_y are not written (the reference's .long()
+ *                        cuts them off).  Events outside the canvas get 0.
+ *   evk_timestamp_image_grad_f32
+ *                        gradient of evk_timestamp_image_counts_f32 (flags EVK_CLIP, EVK_TS_REVERSE; not
+ *                        EVK_TS_RAW) given grad_pos / grad_neg, the outputs and the count images.  Writes
+ *                        grad_x, grad_y (through the sum and the count image) and grad_t = g_tn * dtn/dt
+ *                        (+-1/D, D = t_last - t_first + 1e-6); sums (2 doubles on the device, may be NULL)
+ *                        receives sum(g_tn) and sum(g_tn * tn), from which the caller adds the t_first /
+ *                        t_last terms: forward (S1 - S0)/D to t_first and -S1/D to t_last; reverse S1/D to
+ *                        t_first and (S0 - S1)/D to t_last.  Polarity gets no gradient.
+ *                        workspace: evk_timestamp_image_grad_workspace_bytes() bytes, 16-byte aligned.
+ *   evk_warp_flow_grad_f32
+ *                        gradient of evk_warp_flow_f32 given grad_xw / grad_yw: grad_x, grad_y (1 + dt * the
+ *                        flow's derivative at the sample), grad_t = g_x u + g_y v, *sum_grad_t (one double on
+ *                        the device, may be NULL) = sum of grad_t (t0's gradient is its negative) and
+ *                        grad_flow [2][H][W] (overwritten; taps outside the field get nothing, as zero
+ *                        padding implies).  workspace: evk_warp_flow_grad_workspace_bytes() bytes,
+ *                        16-byte aligned (2x2-block accumulators for the flow gradient).
+ * --------------------------------------------------------------------------------------------- */
+int evk_image_grad_f32(const float *x, const float *y, const float *p, int64_t n, int Himg, int Wimg,
+                       float clipx, float clipy, unsigned flags, const float *grad_img, float *grad_x,
+                       float *grad_y, float *grad_p, void *stream);
+size_t evk_timestamp_image_grad_workspace_bytes(int Himg, int Wimg);
+int evk_timestamp_image_grad_f32(const float *x, const float *y, const float *t, const float *p, int64_t n,
+                                 float t_first, float t_last, int Himg, int Wimg, float clipx, float clipy,
+                                 unsigned flags, const float *grad_pos, const float *grad_neg,
+                                 const float *out_pos, const float *out_neg, const float *cnt_pos,
+                                 const float *cnt_neg, float *grad_x, float *grad_y, float *grad_t,
+                                 double *sums, void *workspace, size_t workspace_bytes, void *stream);
+size_t evk_warp_flow_grad_workspace_bytes(int H, int W);
+int evk_warp_flow_grad_f32(const float *x, const float *y, const float *t, int64_t n, const float *flow,
+                           int H, int W, float t0, const float *grad_xw, const float *grad_yw, float *grad_x,
+                           float *grad_y, float *grad_t, float *grad_flow, double *sum_grad_t,
+                           void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Contrast maximisation, fused: linvel warp -> bounds mask -> bilinear IWE (+ derivative
