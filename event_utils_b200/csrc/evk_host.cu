@@ -363,8 +363,13 @@ int evk_voxel_host_f32(evk_pipeline_t *p, const float *x, const float *y, const 
     // a few host threads fill while the previous chunk is on the wire
     const bool bounce = n > 0 && (is_pageable(x) || is_pageable(y) || is_pageable(t) || is_pageable(pol));
     if (bounce) { int rc = ensure_bounce(p); if (rc) return rc; }
+    // EVK_AUTO_SPAN: the span of the WHOLE stream, read here from the host arrays; a chunk's kernel would take its own
+    if ((flags & EVK_AUTO_SPAN) && n > 0) {
+        t0 = t[0];
+        dt = t[n - 1] - t[0];
+    }
     // every chunk accumulates into the same grid; chunk 0 has already been zeroed above
-    const unsigned cflags = (flags & ~EVK_VARIANT_MASK) | EVK_ACCUMULATE | EVK_VARIANT_GLOBAL_RED;
+    const unsigned cflags = (flags & ~(EVK_VARIANT_MASK | EVK_AUTO_SPAN)) | EVK_ACCUMULATE | EVK_VARIANT_GLOBAL_RED;
     while (done < n) {
         const int s = k & 1;
         // pageable sources: a quarter-size first chunk, so that the wire starts after a quarter of a chunk's staging copy
@@ -464,6 +469,11 @@ int evk_voxel_host_packed_f32(evk_pipeline_t *p, const int16_t *x, const int16_t
     }
     EVK_CUDA(cudaMemsetAsync(p->oob_dev, 0, sizeof(unsigned long long), p->compute));
     EVK_CUDA(cudaMemsetAsync(p->grid, 0, grid_bytes, p->compute));
+    // EVK_AUTO_SPAN: first and last stamp of the whole stream, as evk_voxel_packed_f32 takes them on the device
+    if ((flags & EVK_AUTO_SPAN) && n > 0) {
+        t_first = t[0];
+        t_last = t[n - 1];
+    }
     const unsigned cflags = (flags & ~(EVK_VARIANT_MASK | EVK_AUTO_SPAN)) | EVK_ACCUMULATE | EVK_VARIANT_GLOBAL_RED;
     int64_t done = 0;
     int k = 0;

@@ -416,6 +416,10 @@ int evk_robust_norm_f32(const float *x, int64_t n, int64_t k_low, int64_t k_top,
  * staging area so the H2D copy of chunk k+1 overlaps the scatter of chunk k; the finished grid
  * is copied back to `out_host`.  Synchronous (returns when out_host is complete).
  * *oob_host receives the out-of-range event count.
+ * With EVK_AUTO_SPAN the span is that of the whole stream, read from the host arrays before the first
+ * chunk: t0 = t[0], dt = t[n-1] - t[0] in float32 (evk_voxel_host_f32), t_first = t[0], t_last = t[n-1]
+ * in float64 (evk_voxel_host_packed_f32); the t0 / dt / t_first / t_last arguments are then ignored.
+ * Every chunk is scattered with that one span.
  * --------------------------------------------------------------------------------------------- */
 typedef struct evk_pipeline evk_pipeline_t;
 int evk_pipeline_create(evk_pipeline_t **pipe, int64_t chunk_events);

@@ -91,3 +91,131 @@ def replicate(case, n):
         c[key] = np.resize(case[key], n).astype(_F32)
     c["k"] = "%s*%d" % (case["k"], n)
     return c
+
+
+# ---- exactly summable streams ----------------------------------------------------------------------------------------
+# Every tap of these streams is a multiple of 2^-g and every partial sum a kernel can form stays below 2^(24-g): any
+# summation order, fixed-point quantisation, flush and carry is then exact, and a kernel's output must equal the f64
+# sum of the taps BIT FOR BIT (tests/exact_bounds.py assert_exactly_summable / assert_exact).
+#   hot cells   a few pixels with most of the events, signs in one run of + then one run of - by event index, so that
+#               the fixed-point table slot of every CTA that holds a hot cell wraps upward and back downward at the
+#               launch geometry of the exact-sum tests (exact_bounds.table_wraps checks it; values below)
+#   fine cells  everything else: taps on a 2^-12 grid, a |tap| sum per cell below the wrap threshold of any table,
+#               quarter-pixel coordinates on and beyond the borders, polarities with |p| > 1 that bypass the tables
+# No output cell receives taps of both classes.
+EXACT_FINE_P = np.array([1.0, -1.0, -1.25, 3.0, 0.5, -0.75, 2.5, 0.25], np.float32)
+EXACT_KINDS = ("voxel", "nearest", "bilinear", "cmax")
+
+
+def _fine_coords(rng, n, size):
+    """Quarter-pixel coordinates over [-1, size], with the border values size-1, size-1/4, -1/4 (trunc 0, floor -1),
+    -1 (wraps) and, for ~1 % of the events, whole pixels out of range (size, -size-1)."""
+    v = rng.integers(-4, 4 * size + 1, n) / 4.0
+    special = np.array([size - 1, size - 0.25, -0.25, -1.0, 0.0, size - 0.5])
+    pick = rng.random(n) < 0.1
+    v[pick] = rng.choice(special, int(pick.sum()))
+    out = rng.random(n) < 0.01
+    v[out] = rng.choice(np.array([float(size), -size - 1.0]), int(out.sum()))
+    return v
+
+
+# events per stream of the exact-sum tests: the voxel table launches with 1024 events per CTA reach their one-wave cap
+# (4 waves of at most 5 CTAs per SM) only from about 3.4 M events, and need ~1300 same-slot events per CTA to wrap both ways
+EXACT_SIZES = dict(voxel=(4 << 20) + 4099, nearest=(1 << 20) + 5, bilinear=(1 << 20) + 5, cmax=(4 << 20) + 3)
+
+
+def exact_streams(seed, kind, n, fine=20000, pos_frac=None):
+    """One exactly summable stream of `n` events for the scatter path `kind`:
+      voxel     B = 5, t0 = 0.5, dt = 2: tau = (t - t0) / dt * 4 is a multiple of 2^-6 in [-1, 5].  Hot pixel A (96 %
+                of the hot events): p = +-1 at tau = 0, one integer tap in bin 0 (g = 0), so that one table slot takes
+                all of it; hot pixel B (4 %): tau = 7/2, taps of 1/2 in bins 3 and 4 (g = 1), so that the routed tile
+                carries from both of an event's bins.  + run 60 %, - run 40 %: every CTA of the table launches wraps
+                up and back down (mostly with a zero net carry, so a carry of one direction that is lost or
+                mis-signed shows)
+      nearest   hot p = +-2^19: in the 2^10 image table q = 2^29, so a slot wraps every four same-sign adds
+      bilinear  one hot point at (i + 1/2, j), p = +-1: taps of 1/2 into the top-left and top-right cells, g = 1 (an
+                image CTA takes four 2048-event rounds: 1/2-unit taps are what wraps its slot both ways)
+      cmax      f64 events, velocity (32, -16), t_ref = 0, stamps on a 2^-6 grid in [-1, 0]: the warped coordinates are
+                quarter pixels; each hot event warps onto one of two half-pixel points (taps 1/4), |d| <= 2^-5 so that
+                the dIWE taps stay small
+    `fine` events (at most) are fine, the rest hot; the first `pos_frac` of the hot events are +, the rest - (default
+    0.6 for voxel, 0.7 for the others: their cells also end with net carries, since up and down wraps that cancel
+    would hide a carry sent to the wrong cell).  Returns a dict: x, y, t, p (float32; float64 for cmax), `hot` (the
+    class of each event), `group` (0 fine, 1 hot point A, 2 hot point B), `pos_frac` and the parameters of the call
+    (B, H, W, t0, dt; cmax: vx, vy, t_ref, Hs, Ws)."""
+    assert kind in EXACT_KINDS
+    rng = np.random.default_rng(seed)
+    H, W = (40, 56) if kind == "cmax" else (32, 48)
+    hot = np.zeros(n, bool)
+    hot[rng.permutation(n)[:max(n - fine, n // 2)]] = True
+    nh, nf = int(hot.sum()), int(n - hot.sum())
+    # the hot points: interior pixels, (hx, hy) and (hx2, hy2), each with half of the hot events (alternating by index)
+    hx, hy, hx2, hy2 = W // 3, H // 3, 2 * W // 3, 2 * H // 3
+    if pos_frac is None:
+        pos_frac = 0.6 if kind == "voxel" else 0.7
+    which = {"voxel": (np.arange(nh) % 25 == 0).astype(int), "bilinear": np.zeros(nh, int)}.get(kind, np.arange(nh) % 2)
+    sign = np.where(np.arange(nh) < int(pos_frac * nh), 1.0, -1.0)
+    # fine events stay out of a 7x7 moat around each hot point (no tap of one class lands in a cell of the other)
+    fx, fy = _fine_coords(rng, 2 * nf + 64, W), _fine_coords(rng, 2 * nf + 64, H)
+    keep = ~(((np.abs(fx - hx) < 4) & (np.abs(fy - hy) < 4)) | ((np.abs(fx - hx2) < 4) & (np.abs(fy - hy2) < 4)))
+    fx, fy = fx[keep][:nf], fy[keep][:nf]
+    assert fx.shape[0] == nf
+    fp = rng.choice(EXACT_FINE_P, nf)
+    x, y, p, t = np.empty(n), np.empty(n), np.empty(n), np.empty(n)
+    x[~hot], y[~hot], p[~hot] = fx, fy, fp
+    group = np.zeros(n, int)
+    group[hot] = 1 + which
+    c = dict(kind=kind, H=H, W=W, hot=hot, group=group, pos_frac=pos_frac)
+    if kind == "cmax":
+        vx, vy = 32.0, -16.0
+        ft = -rng.integers(0, 65, nf) / 64.0                         # d = t - t_ref in [-1, 0], 2^-6 grid
+        t[~hot] = ft
+        x[~hot] += ft * vx                                            # warped x - d vx: the fine grid above
+        y[~hot] += ft * vy
+        ht = -rng.integers(0, 3, nh) / 64.0
+        t[hot] = ht
+        x[hot] = np.where(which, hx2, hx) + 0.5 + ht * vx
+        y[hot] = np.where(which, hy2, hy) + 0.5 + ht * vy
+        p[hot] = sign
+        c.update(vx=vx, vy=vy, t_ref=0.0, Hs=H, Ws=W)
+        c.update(x=x, y=y, t=t, p=p)
+        return c
+    B, t0, dt = 5, 0.5, 2.0
+    t[~hot] = t0 + dt * rng.integers(-64, 321, nf) / 256.0           # tau in [-1, 5] on a 2^-6 grid
+    if kind == "voxel":
+        x[hot] = np.where(which, hx2 + 0.75, hx + 0.25)
+        y[hot] = np.where(which, hy2 + 0.5, hy)
+        t[hot] = t0 + dt * np.where(which, 3.5, 0.0) / 4.0
+        p[hot] = sign
+    elif kind == "nearest":
+        x[hot] = np.where(which, hx2 + 0.75, hx)
+        y[hot] = np.where(which, hy2 + 0.25, hy + 0.5)
+        t[hot] = t0 + dt * rng.integers(0, 257, nh) / 256.0
+        p[hot] = sign * 2.0 ** 19
+    else:
+        x[hot] = np.where(which, hx2, hx) + 0.5
+        y[hot] = np.where(which, hy2, hy)
+        t[hot] = t0 + dt * rng.integers(0, 257, nh) / 256.0
+        p[hot] = sign
+    t[0], t[-1] = t0, t0 + dt                                        # EVK_AUTO_SPAN finds the same span
+    c.update(B=B, t0=_F32(t0), dt=_F32(dt))
+    c.update({k: v.astype(_F32) for k, v in dict(x=x, y=y, t=t, p=p).items()})
+    return c
+
+
+def packed_of(c, T0=1.7e9):
+    """The storage-layout (int16 x / y, float64 absolute stamps, uint8 polarity) form of a float32 stream, as the
+    HDF5 / memmap loaders hand it over, plus the float32 events the kernel turns it into:
+      x, y  floor to int16 (a coordinate at -ulp becomes -1 and wraps)
+      t     T0 + t in float64; t_first = T0 + t0, t_last = t_first + dt
+      p     uint8 [p > 0], which the kernel maps to +-1 (finite polarities only: uint8 holds no NaN)
+    Returns (x16, y16, T, p8, t_first, t_last, f32) with f32 = dict(x, y, t, p, t0, dt) for the oracle."""
+    x16 = np.floor(c["x"].astype(np.float64)).astype(np.int16)
+    y16 = np.floor(c["y"].astype(np.float64)).astype(np.int16)
+    T = T0 + c["t"].astype(np.float64)
+    t_first = T0 + float(c["t0"])
+    t_last = t_first + float(c["dt"])
+    p8 = (c["p"] > 0).astype(np.uint8)
+    f32 = dict(x=x16.astype(_F32), y=y16.astype(_F32), t=(T - t_first).astype(_F32),
+               p=np.where(p8 != 0, 1.0, -1.0).astype(_F32), t0=_F32(0.0), dt=_F32(t_last - t_first))
+    return x16, y16, T, p8, t_first, t_last, f32

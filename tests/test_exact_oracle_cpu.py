@@ -157,3 +157,46 @@ def test_kthvalue_ranks_every_nan_last():
     x = torch.from_numpy(np.concatenate([np.float32([1, 2, -1]), neg_nan]))
     assert x.kthvalue(1).values.item() == -1.0
     assert np.isnan(x.kthvalue(4).values.item())
+
+
+# ---- exactly summable streams: the oracle's own f32 sums must equal the exact sums bit for bit ---------------------------
+@pytest.mark.parametrize("kind", ["voxel", "trilinear", "nearest", "bilinear", "cmax"])
+def test_exact_streams_are_exactly_summable(oracle, kind):
+    """exact_streams(): the oracle's sequential f32 sums equal the f64 sums bit for bit, for the stream as generated,
+    reversed and shuffled -- the streams are exactly summable in practice, not only by the argument of
+    exact_bounds.assert_exactly_summable (which is checked as well)."""
+    from edge_cases import exact_streams
+    from exact_bounds import assert_exact, check_exactly_summable, exact_outputs, select_events
+    for seed in (1, 2, 3):
+        c = exact_streams(seed, "voxel" if kind == "trilinear" else kind, 200003)
+        kws = [dict(bilinear=True, clip=False), dict(bilinear=True, clip=True)] if kind == "trilinear" else \
+            [dict(clip=False, padding=False), dict(clip=True, padding=True)] if kind in ("nearest", "bilinear") else \
+            [dict(), dict(abs_polarity=True)] if kind == "cmax" else [dict()]
+        for kw in kws:
+            outs = check_exactly_summable(oracle, c, **kw)
+            n = c["hot"].shape[0]
+            for order in (np.arange(n), np.arange(n)[::-1], np.random.default_rng(seed).permutation(n)):
+                for pl in exact_outputs(oracle, select_events(c, order), **kw):
+                    assert_exact(pl.out, pl.ex, what="%s %s seed %d" % (pl.name, kw, seed))
+            if kind != "cmax" and not kw.get("clip"):
+                assert all(pl.oob > 0 for pl in outs), "the stream has out-of-range events"
+            assert max((pl.ex.abs > 2 ** 14).sum() for pl in outs) > 0, "no hot cell"
+
+
+@pytest.mark.parametrize("kind", ["voxel", "nearest", "bilinear", "cmax"])
+def test_exact_streams_wrap_every_table_slot(kind):
+    """At the sizes of tests/test_gpu_exact_sums.py and the launch geometry of an H100 SXM (132 SMs), every CTA's hot
+    table slot wraps upward and back downward (exact_bounds.assert_tables_wrap), so the carries of both signs run."""
+    from edge_cases import EXACT_SIZES, exact_streams
+    from exact_bounds import assert_tables_wrap
+    assert_tables_wrap(exact_streams(7, kind, EXACT_SIZES[kind]), 132, what=kind)
+
+
+def test_table_wraps_model():
+    """The slot model of table_wraps on hand-counted runs (F = 22: the slot holds +-512, a wrap carries 1024)."""
+    from exact_bounds import table_wraps
+    for P, M, up, down in ((800, 200, 1, 0), (511, 1000, 0, 0), (512, 0, 1, 0), (600, 900, 1, 1), (1600, 400, 2, 1),
+                           (0, 513, 0, 1)):
+        v = np.concatenate([np.ones(P), -np.ones(M)])
+        u, d, net = table_wraps(v, 22, 1, 1)
+        assert (u[0], d[0], net[0]) == (up, down, up - down), (P, M)

@@ -3,14 +3,15 @@ past the size at which AUTO switches to the contended-stream kernels -- each out
 oracle's exact per-cell sums (exact_bounds.assert_within_exact: |gpu - exact| <= gamma(k+4) S + k q), and the
 out-of-range counts exactly.  A tap that is lost, doubled or sent to the wrong cell shows up in the cell it belongs to,
 however hot the rest of the image is."""
+import ctypes
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from exact_bounds import Q22, assert_within_exact
-from edge_cases import hard_cases, replicate
+from exact_bounds import Q22, Exact_of as _sel, assert_within_exact
+from edge_cases import hard_cases, packed_of, replicate
 
 pytestmark = pytest.mark.gpu
 
@@ -43,8 +44,6 @@ def _lib():
     return _lib, _lib.lib()
 
 
-def _sel(ex, k):
-    return type(ex)(*(a[k] for a in ex))
 
 
 def _voxel_variants():
@@ -57,9 +56,22 @@ def _voxel_variants():
 
 
 # ---- voxel grids -----------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("big", [False, True])
-def test_voxel(oracle, big):
+@pytest.fixture
+def host_pipeline():
+    """A host pipeline with 4096-event chunks (a big case makes ~256 of them), destroyed after the test."""
     _l, L = _lib()
+    h = ctypes.c_void_p()
+    _l.check(L.evk_pipeline_create(ctypes.byref(h), 4096))
+    yield h
+    torch.cuda.synchronize()
+    L.evk_pipeline_destroy(h)
+
+
+@pytest.mark.parametrize("big", [False, True])
+def test_voxel(oracle, big, host_pipeline):
+    """SoA (aligned and not), AoS, the packed storage layout and the two host pipelines."""
+    _l, L = _lib()
+    pipe = host_pipeline
     for c in _cases(big, VOXEL_BIG):
         B, H, W, n = c["B"], c["H"], c["W"], c["x"].shape[0]
         t0, dt = float(c["t0"]), float(c["dt"])
@@ -89,6 +101,28 @@ def test_voxel(oracle, big):
             torch.cuda.synchronize()
             assert int(oob.item()) == o_oob
             assert_within_exact(out.cpu().numpy(), ex, Q22, what="voxel aos case %s %s" % (c["k"], name))
+        # the storage layout (int16 x / y, f64 absolute stamps, uint8 polarity: finite polarities only) against the
+        # oracle of the float32 events the kernel makes of it
+        x16, y16, TT, p8, t_first, t_last, f = packed_of(c)
+        _, pex, p_oob = oracle.voxel_f32(f["x"], f["y"], f["t"], f["p"], B, (H, W), t0=f["t0"], dt=f["dt"], exact=True)
+        PX, PY, PT, PP = dev(x16), dev(y16), dev(TT), dev(p8)
+        for name, var in _voxel_variants():
+            oob.zero_()
+            _l.check(L.evk_voxel_packed_f32(_p(PX), _p(PY), _p(PT), _p(PP), n, t_first, t_last, B, H, W, var, _p(out),
+                                            _p(ws), ws.numel(), _p(oob), None))
+            torch.cuda.synchronize()
+            assert int(oob.item()) == p_oob
+            assert_within_exact(out.cpu().numpy(), pex, Q22, what="voxel packed case %s %s" % (c["k"], name))
+        # the host pipelines, in chunks of 4096 events
+        for packed, arrays, span, ref, r_oob in ((False, [c[k] for k in "xytp"], (t0, dt), ex, o_oob),
+                                                 (True, [x16, y16, TT, p8], (t_first, t_last), pex, p_oob)):
+            grid = np.full((B, H, W), np.nan, np.float32)
+            h_oob = ctypes.c_ulonglong(0)
+            fn = L.evk_voxel_host_packed_f32 if packed else L.evk_voxel_host_f32
+            _l.check(fn(pipe, *(a.ctypes.data for a in arrays), n, span[0], span[1], B, H, W, 0, grid.ctypes.data,
+                        ctypes.byref(h_oob)))
+            assert h_oob.value == r_oob
+            assert_within_exact(grid, ref, what="voxel host packed=%d case %s" % (packed, c["k"]))
 
 
 @pytest.mark.parametrize("big", [False, True])
