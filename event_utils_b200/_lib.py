@@ -22,6 +22,8 @@ WINDOW_PAIRS = 0x100000
 WINDOW_NEGPOS = 0x400000
 NO_FOLD = 0x800000
 PEER_MULTICAST = 0x1000000
+WINDOW_OVERLAP = 0x2000000
+EVENTS_AOS = 0x4000000
 AUTO_SPAN = 0x200000
 VARIANT_AUTO = 0 << 8
 VARIANT_GLOBAL_RED = 1 << 8
@@ -90,6 +92,10 @@ def _declare(L):
     L.evk_warp_flow_grad_workspace_bytes.argtypes = [ci, ci]
     L.evk_warp_flow_grad_f32.restype = ci
     L.evk_warp_flow_grad_f32.argtypes = [vp, vp, vp, i64, vp, ci, ci, f32, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    L.evk_voxel_grad_workspace_bytes.restype = sz
+    L.evk_voxel_grad_workspace_bytes.argtypes = [ci, ci, ci, ci, cu]
+    L.evk_voxel_grad_f32.restype = ci
+    L.evk_voxel_grad_f32.argtypes = [vp, vp, vp, vp, i64, vp, ci, ci, ci, ci, cu, vp, vp, vp, vp, sz, vp]
     L.evk_count_u32.restype = ci
     L.evk_count_u32.argtypes = [vp, vp, i64, ci, ci, f32, f32, cu, vp, vp, vp]
     L.evk_splat_idx_f32.restype = ci

@@ -10,6 +10,9 @@ Which inputs get a gradient (as in the reference; the others get None):
     events_to_image_torch            bilinear: xs, ys, ps;  nearest (or integer coordinates): ps
     events_to_timestamp_image_torch  xs, ys, ts
     warp_events_flow_torch           xt, yt, tt, flow_field, t0 (when it is a tensor; t0=None means tt[-1])
+    events_to_voxel_torch            ps, ts (voxel_grid.py:114-153); also through voxel_grids_fixed_n/_t_torch and
+                                     events_to_voxel_timesync_torch
+    events_to_neg_pos_voxel_torch    ts (voxel_grid.py:155-182)
 
 The public functions take this path only when grad mode is on and one of those inputs requires grad; every
 other call runs the plain forward.  Gradients come back in each input's shape, dtype and device.  The
@@ -166,3 +169,58 @@ class WarpFlow(torch.autograd.Function):
         g_t0 = _as_input(-s, m[3]) if need[3] else None
         return (_as_input(gx, m[0]), _as_input(gy, m[1]), _as_input(gt, m[2]) if need[2] else None, g_t0,
                 _as_input(gf, m[4]) if need[4] else None, None)
+
+
+class VoxelGrid(torch.autograd.Function):
+    """events_to_voxel_torch (voxel_grid.py:114-153), both grids of events_to_neg_pos_voxel_torch (:155-182, one
+    (2,B,H,W) output) and the stacked (nw,B,H,W) windows of voxel_grids_fixed_n/_t_torch (:37-80).  opts = (device,
+    B, H, W, negpos, windows) with windows None or (starts, ends).  Each grid or window is normalised by its own first
+    and last stamp, so those two stamps get extra gradient terms (evk.h, evk_voxel_grad_f32)."""
+
+    @staticmethod
+    def forward(ctx, xs, ys, ts, ps, opts):
+        from .representations import _events as E
+        from .representations.voxel_grid import _device_events, _negpos_device, _voxel_device, _windows_device
+        device, B, H, W, negpos, windows = opts
+        dev = E.compute_device(xs, ys, ts, ps)
+        aos = pairs = None
+        overlap = False
+        if windows is not None:
+            starts, ends = windows
+            x, y, t, p = xs, ys, ts, ps
+            out, pairs = _windows_device(xs, ys, ts, ps, starts, ends, B, H, W)
+            s, e = np.asarray(starts), np.asarray(ends)
+            order = np.argsort(s, kind="stable")
+            s, e = s[order], e[order]
+            # searchsorted ends of voxel_grids_fixed_t_torch can reach past the next window's start through rounding
+            overlap = bool(len(s) > 1 and (np.maximum.accumulate(e)[:-1] > s[1:]).any())
+        else:
+            # host inputs are uploaded: the backward runs on the device
+            aos, x, y, t, p, t0, dt, flags = _device_events(xs, ys, ts, ps, dev, aos_ok=not negpos)
+            out = _negpos_device(x, y, t, p, t0, dt, B, H, W, flags) if negpos else \
+                _voxel_device(x, y, t, p, t0, dt, B, H, W, flags=flags, aos=aos)
+        ctx.save_for_backward(aos, x, y, t, p, pairs)
+        ctx.geom = (dev, B, H, W, negpos, overlap)
+        ctx.metas = (_meta(ts), _meta(ps))
+        return out if out.device == device else out.to(device)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        aos, x, y, t, p, pairs = ctx.saved_tensors
+        dev, B, H, W, negpos, overlap = ctx.geom
+        need = ctx.needs_input_grad
+        n = (aos if aos is not None else x).shape[0]
+        nw = 1 if pairs is None else pairs.shape[0] // 2
+        flags = ((_lib.WINDOW_NEGPOS if negpos else 0) | (_lib.WINDOW_OVERLAP if overlap else 0) |
+                 (_lib.EVENTS_AOS if aos is not None else 0))
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g = _grad_in(g, dev)
+            gt = torch.empty(n, dtype=torch.float32, device=dev) if need[2] else None
+            gp = torch.empty(n, dtype=torch.float32, device=dev) if need[3] and not negpos else None
+            ws = torch.empty(L.evk_voxel_grad_workspace_bytes(nw, B, H, W, flags), dtype=torch.uint8, device=dev)
+            _lib.check(L.evk_voxel_grad_f32(
+                _lib.ptr(aos if aos is not None else x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), n, _lib.ptr(pairs), nw,
+                B, H, W, flags, _lib.ptr(g), _lib.ptr(gp), _lib.ptr(gt), _lib.ptr(ws), ws.numel(), _lib.stream()))
+        return None, None, _as_input(gt, ctx.metas[0]), _as_input(gp, ctx.metas[1]), None

@@ -4,6 +4,7 @@
 //   events_to_image_torch            image.py:46-100 (interpolate_to_image :102-115, index_put_ :95)
 //   events_to_timestamp_image_torch  image.py:286-353
 //   warp_events_flow_torch           optic_flow.py:5-46 (grid_sample bilinear, zeros, align_corners=True)
+//   events_to_voxel_torch            voxel_grid.py:114-153, and its neg/pos and windowed callers :37-112, :155-182
 // Each kernel here takes one pass over the events and recomputes the forward's per-event quantities (index,
 // clip, wrap, fractions, weights) with the same arithmetic as the forward kernel, so that the taps it reads
 // are the taps the forward wrote.  floor() has zero derivative: the gradient is one-sided at integer
@@ -286,6 +287,205 @@ __global__ void __launch_bounds__(kGradThreads) warp_flow_grad_kernel(const Flow
     block_red_add_f64(s, A.sum_gt);
 }
 
+// ---- voxel grid (evk_voxel_f32 / _aos_f32 / _negpos_f32 / _windows_f32) -------------------------
+// The reference's bin weight is ps * max(0, 1 - |tn - b|) with tn = ((t - t0) / dt) * (B-1) per window
+// (voxel_grid.py:133-139); autograd reaches ps and, through tn, ts.  The incoming gradient is re-laid out once per
+// call as pixel-major rows of S = roundup(B, 4) floats ([w][grid][H*W][S]), so that an event's bins floor(tn)-1 ..
+// floor(tn)+2 are one or two 16-byte loads from one 32-byte sector (B <= 8) instead of up to four sectors.
+struct VoxGradArgs {
+    const float *x, *y, *t, *p;  // SoA; AoS: x is the [n][4] record array and y / t / p point into it
+    int64_t n;
+    int ev_stride;               // floats between consecutive events: 1 (SoA) or 4 (AoS)
+    const int64_t *pairs;        // [nw][2] (start, end), or null: one window [0, n)
+    int nw, slices;              // CTA (w, s) takes slice s of window w
+    int B, H, W, S;
+    float bm1;
+    int negpos, atomic_out;      // atomic_out: windows may overlap, per-event outputs are added (zeroed first)
+    const float *gi;             // [nw][grids][H*W][S]
+    float *gp, *gt;              // per event, each may be null
+    double *sums;                // [nw][2]: sum G, sum G * tn
+};
+
+// One bin of the reference's autograd through w = p * max(0, v), v = 1 - |d|, d = tn - b, with torch's subgradients:
+// maximum() gives half the gradient to each side on a tie (v == 0) and all of it to a NaN; abs'(d) = sign(d), and
+// sign(0) = sign(NaN) = 0.  Same f32 operations as the forward (voxel_event / add_all_bins_slow).
+__device__ __forceinline__ void voxel_bin_grad(float tn, int b, float p, float g, float &gp, float &gtn)
+{
+    const float d = __fsub_rn(tn, (float)b);
+    const float v = __fsub_rn(1.0f, fabsf(d));
+    const float bw = (v != v) ? v : (v > 0.0f ? v : 0.0f);
+    gp = __fadd_rn(gp, __fmul_rn(g, bw));
+    float gv = __fmul_rn(g, p);
+    if (v == 0.0f) gv = __fmul_rn(gv, 0.5f);
+    if (v < 0.0f) gv = 0.0f;
+    const float sg = d > 0.0f ? 1.0f : (d < 0.0f ? -1.0f : 0.0f);
+    gtn = __fadd_rn(gtn, __fmul_rn(-gv, sg));
+}
+
+// finite tn and p: every bin outside floor(tn)-1 .. floor(tn)+2 has v < 0 and adds 0.  Bin floor(tn)+2 has weight 0 but
+// a tie when tn lies within half an ulp of 1 below an integer: d = frac - 2 rounds to -1 (tn = 1 - 2^-24, or tn = -2^-149)
+__device__ __forceinline__ void voxel_bins_near(const float *row, int B, float tn, float p, float &gp, float &gtn)
+{
+    const int f = (int)floorf(tn);
+    const int lo = f - 1 < 0 ? 0 : f - 1, hi = f + 2 > B - 1 ? B - 1 : f + 2;
+    if (lo > hi) return;
+    const float4 *r4 = reinterpret_cast<const float4 *>(row);
+    const float4 q0 = __ldg(r4 + (lo >> 2));
+    const float4 q1 = (hi >> 2) != (lo >> 2) ? __ldg(r4 + (hi >> 2)) : q0;
+#pragma unroll
+    for (int k = -1; k <= 2; ++k) {
+        const int b = f + k;
+        if (b < lo || b > hi) continue;
+        const float4 q = (b >> 2) == (lo >> 2) ? q0 : q1;
+        const int j = b & 3;
+        voxel_bin_grad(tn, b, p, j == 0 ? q.x : j == 1 ? q.y : j == 2 ? q.z : q.w, gp, gtn);
+    }
+}
+
+// rare path (non-finite tn or p): every bin, so that NaN reaches the gradients exactly where autograd puts it
+__device__ __noinline__ float2 voxel_bins_all(const float *row, int B, float tn, float p)
+{
+    float gp = 0.0f, gtn = 0.0f;
+    for (int b = 0; b < B; ++b) voxel_bin_grad(tn, b, p, row[b], gp, gtn);
+    return make_float2(gp, gtn);
+}
+
+// grad_p and G = dL/dtn of one event; the pixel and tn exactly as voxel_event forms them
+__device__ __forceinline__ void voxel_grad_event(const VoxGradArgs &A, const float *gw, float t0, float dt, float x, float y,
+                                                 float t, float p, float &gp, float &gtn, float &tn)
+{
+    gp = 0.0f; gtn = 0.0f;
+    tn = __fmul_rn(__fdiv_rn(__fsub_rn(t, t0), dt), A.bm1);
+    int xi, yi;
+    if (!wrap_trunc_index(x, A.W, xi) || !wrap_trunc_index(y, A.H, yi)) return;  // outside the grid: no taps
+    const int64_t grid = (int64_t)A.H * A.W * A.S;
+    const float *row = gw + ((int64_t)yi * A.W + xi) * A.S;
+    const bool tfin = fabsf(tn) < 1.0e9f;
+    if (A.negpos) {
+        // weights [p>0] into grid 0 and [p<=0] into grid 1 (voxel_grid.py:172-175); ps gets no gradient
+        const float wpos = p > 0.0f ? 1.0f : 0.0f, wneg = p <= 0.0f ? 1.0f : 0.0f;
+        float unused = 0.0f;
+        if (tfin) {
+            if (wpos != 0.0f || wneg != 0.0f) voxel_bins_near(row + (wneg != 0.0f ? grid : 0), A.B, tn, 1.0f, unused, gtn);
+        } else {
+            const float2 a = voxel_bins_all(row, A.B, tn, wpos), b = voxel_bins_all(row + grid, A.B, tn, wneg);
+            gtn = __fadd_rn(a.y, b.y);
+        }
+    } else if (tfin && fabsf(p) <= FLT_MAX) {
+        voxel_bins_near(row, A.B, tn, p, gp, gtn);
+    } else {
+        const float2 a = voxel_bins_all(row, A.B, tn, p);
+        gp = a.x; gtn = a.y;
+    }
+}
+
+__device__ __forceinline__ void store_grad(float *dst, int atomic_out, float v)
+{
+    if (atomic_out) red_add(dst, v); else __stcs(dst, v);
+}
+
+template <bool VEC4>
+__global__ void __launch_bounds__(kGradThreads) voxel_grad_kernel(const VoxGradArgs A)
+{
+    const int w = blockIdx.x / A.slices, s = blockIdx.x - w * A.slices;
+    const int64_t first = A.pairs ? A.pairs[2 * w] : 0, last = A.pairs ? A.pairs[2 * w + 1] : A.n;
+    double s_g = 0.0, s_gt = 0.0;
+    if (last > first) {
+        // t0 / dt of the window as voxel_windows_kernel and EVK_AUTO_SPAN take them
+        const float t0 = A.t[first * A.ev_stride], dt = __fsub_rn(A.t[(last - 1) * A.ev_stride], t0);
+        const float *gw = A.gi + (int64_t)w * (A.negpos ? 2 : 1) * A.H * A.W * A.S;
+        const int64_t tid = (int64_t)s * kGradThreads + threadIdx.x, stride = (int64_t)A.slices * kGradThreads;
+        // 16-byte body [a, b) four events at a time; the scalar head [first, a) and tail [b, last)
+        int64_t a = first, b = first;
+        if (VEC4) {
+            a = (first + 3) & ~(int64_t)3;
+            if (a > last) a = last;
+            b = a + ((last - a) & ~(int64_t)3);
+        }
+        for (int64_t q = (a >> 2) + tid; q < (b >> 2); q += stride) {
+            float4 X, Y, T, P;
+            if (A.ev_stride == 4) {
+                const float4 e0 = ld_stream4(A.x + 16 * q), e1 = ld_stream4(A.x + 16 * q + 4);
+                const float4 e2 = ld_stream4(A.x + 16 * q + 8), e3 = ld_stream4(A.x + 16 * q + 12);
+                X = make_float4(e0.x, e1.x, e2.x, e3.x); Y = make_float4(e0.y, e1.y, e2.y, e3.y);
+                T = make_float4(e0.z, e1.z, e2.z, e3.z); P = make_float4(e0.w, e1.w, e2.w, e3.w);
+            } else {
+                X = ld_stream4(A.x + 4 * q); Y = ld_stream4(A.y + 4 * q); T = ld_stream4(A.t + 4 * q); P = ld_stream4(A.p + 4 * q);
+            }
+            float4 gp, G, tn;
+            voxel_grad_event(A, gw, t0, dt, X.x, Y.x, T.x, P.x, gp.x, G.x, tn.x);
+            voxel_grad_event(A, gw, t0, dt, X.y, Y.y, T.y, P.y, gp.y, G.y, tn.y);
+            voxel_grad_event(A, gw, t0, dt, X.z, Y.z, T.z, P.z, gp.z, G.z, tn.z);
+            voxel_grad_event(A, gw, t0, dt, X.w, Y.w, T.w, P.w, gp.w, G.w, tn.w);
+            s_g += ((double)G.x + (double)G.y) + ((double)G.z + (double)G.w);
+            s_gt += ((double)G.x * (double)tn.x + (double)G.y * (double)tn.y) + ((double)G.z * (double)tn.z + (double)G.w * (double)tn.w);
+            if (A.gp) {
+                if (A.atomic_out) red_add4(A.gp + 4 * q, gp); else __stcs(reinterpret_cast<float4 *>(A.gp + 4 * q), gp);
+            }
+            if (A.gt) {
+                // dL/dt = G * (B-1) / dt, the reference's two f32 steps
+                const float4 g4 = make_float4(__fdiv_rn(__fmul_rn(G.x, A.bm1), dt), __fdiv_rn(__fmul_rn(G.y, A.bm1), dt),
+                                              __fdiv_rn(__fmul_rn(G.z, A.bm1), dt), __fdiv_rn(__fmul_rn(G.w, A.bm1), dt));
+                if (A.atomic_out) red_add4(A.gt + 4 * q, g4); else __stcs(reinterpret_cast<float4 *>(A.gt + 4 * q), g4);
+            }
+        }
+        const int64_t nhead = a - first, nrest = nhead + (last - b);
+        for (int64_t j = tid; j < nrest; j += stride) {
+            const int64_t i = j < nhead ? first + j : b + (j - nhead);
+            float ex, ey, et, ep;
+            if (A.ev_stride == 4) {
+                const float4 e = ld_stream4(A.x + 4 * i);
+                ex = e.x; ey = e.y; et = e.z; ep = e.w;
+            } else {
+                ex = ld_stream(A.x + i); ey = ld_stream(A.y + i); et = ld_stream(A.t + i); ep = ld_stream(A.p + i);
+            }
+            float gp, G, tn;
+            voxel_grad_event(A, gw, t0, dt, ex, ey, et, ep, gp, G, tn);
+            s_g += (double)G;
+            s_gt += (double)G * (double)tn;
+            if (A.gp) store_grad(A.gp + i, A.atomic_out, gp);
+            if (A.gt) store_grad(A.gt + i, A.atomic_out, __fdiv_rn(__fmul_rn(G, A.bm1), dt));
+        }
+    }
+    block_red_add_f64(s_g, A.sums + 2 * w);
+    block_red_add_f64(s_gt, A.sums + 2 * w + 1);
+}
+
+// t0 = t[first] and dt = t[last-1] - t[first] depend on the window's end stamps:
+//   t[first] += ((sum G * tn) - (B-1) * sum G) / dt,   t[last-1] += -(sum G * tn) / dt
+// (atomic: with overlapping windows an end stamp may belong to two windows)
+__global__ void __launch_bounds__(128) voxel_grad_ends_kernel(const VoxGradArgs A)
+{
+    const int w = blockIdx.x * 128 + threadIdx.x;
+    if (w >= A.nw) return;
+    const int64_t first = A.pairs ? A.pairs[2 * w] : 0, last = A.pairs ? A.pairs[2 * w + 1] : A.n;
+    if (last <= first) return;
+    const float t0 = A.t[first * A.ev_stride], dt = __fsub_rn(A.t[(last - 1) * A.ev_stride], t0);
+    const double s0 = A.sums[2 * w], s1 = A.sums[2 * w + 1];
+    atomicAdd(A.gt + first, (float)((s1 - (double)A.bm1 * s0) / (double)dt));
+    atomicAdd(A.gt + last - 1, (float)(-s1 / (double)dt));
+}
+
+// planar [k][B][npix] -> pixel-major rows [k][npix][S], zero-padded past B
+__global__ void __launch_bounds__(256) voxel_grad_interleave_kernel(const float *__restrict__ g, int64_t rows, int64_t npix, int B,
+                                                                   int S, float *__restrict__ out)
+{
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += stride) {
+        const int64_t k = r / npix, pix = r - k * npix;
+        const float *src = g + k * B * npix + pix;
+        float4 *dst = reinterpret_cast<float4 *>(out + r * S);
+        for (int c = 0; c < S; c += 4) {
+            float v[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) v[j] = c + j < B ? src[(int64_t)(c + j) * npix] : 0.0f;
+            dst[c >> 2] = make_float4(v[0], v[1], v[2], v[3]);
+        }
+    }
+}
+
+static inline int voxel_grad_row(int B) { return (B + 3) & ~3; }
+
 static inline bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 
 }  // namespace evk
@@ -403,6 +603,80 @@ int evk_warp_flow_grad_f32(const float *x, const float *y, const float *t, int64
     const float *ws = static_cast<const float *>(workspace);
     launch_image_fold(ws, grad_flow, H, W, st);
     launch_image_fold(ws + npix * 4, grad_flow + npix, H, W, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_voxel_grad_workspace_bytes(int n_windows, int B, int H, int W, unsigned flags)
+{
+    if (n_windows < 1 || B < 1 || H < 1 || W < 1) return 0;
+    const size_t sums = ((size_t)n_windows * 2 * sizeof(double) + 255) & ~(size_t)255;
+    const size_t grids = (flags & EVK_WINDOW_NEGPOS) ? 2 : 1;
+    return sums + (size_t)n_windows * grids * H * W * evk::voxel_grad_row(B) * sizeof(float);
+}
+
+int evk_voxel_grad_f32(const float *x, const float *y, const float *t, const float *p, int64_t n, const int64_t *pairs,
+                       int n_windows, int B, int H, int W, unsigned flags, const float *grad_out, float *grad_p,
+                       float *grad_t, void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const bool aos = (flags & EVK_EVENTS_AOS) != 0, negpos = (flags & EVK_WINDOW_NEGPOS) != 0;
+    if (n < 0 || n_windows < 1 || B < 1 || H < 1 || W < 1 || !grad_out || (!pairs && n_windows != 1) ||
+        (n > 0 && (!x || (!aos && (!y || !t || !p)))) || (aos && ((uintptr_t)x & 15)) || (flags & EVK_NEGPOS_TRUTHY) ||
+        (flags & EVK_BILINEAR) || (int64_t)B * H * W >= ((int64_t)1 << 40)) {
+        set_error("evk_voxel_grad_f32: bad arguments");
+        return EVK_E_ARG;
+    }
+    const size_t need = evk_voxel_grad_workspace_bytes(n_windows, B, H, W, flags);
+    if (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 255)) {
+        set_error("evk_voxel_grad_f32: 256-byte aligned workspace of %zu bytes required", need);
+        return EVK_E_WORKSPACE;
+    }
+    if (negpos) grad_p = nullptr;
+    if (n == 0 || (!grad_p && !grad_t)) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    VoxGradArgs A{};
+    A.x = x; A.n = n;
+    if (aos) { A.y = x + 1; A.t = x + 2; A.p = x + 3; A.ev_stride = 4; }
+    else { A.y = y; A.t = t; A.p = p; A.ev_stride = 1; }
+    A.pairs = pairs; A.nw = n_windows;
+    A.B = B; A.H = H; A.W = W; A.S = voxel_grad_row(B); A.bm1 = (float)(B - 1);
+    A.negpos = negpos ? 1 : 0;
+    A.atomic_out = (flags & EVK_WINDOW_OVERLAP) ? 1 : 0;
+    A.gp = grad_p; A.gt = grad_t;
+    A.sums = static_cast<double *>(workspace);
+    const size_t sums_bytes = ((size_t)n_windows * 2 * sizeof(double) + 255) & ~(size_t)255;
+    float *gi = reinterpret_cast<float *>(static_cast<char *>(workspace) + sums_bytes);
+    A.gi = gi;
+    EVK_CUDA(cudaMemsetAsync(A.sums, 0, (size_t)n_windows * 2 * sizeof(double), st));
+    if (pairs) {
+        // events outside every window get 0; overlapping windows add into the zeroed outputs
+        if (A.gp) EVK_CUDA(cudaMemsetAsync(A.gp, 0, (size_t)n * sizeof(float), st));
+        if (A.gt) EVK_CUDA(cudaMemsetAsync(A.gt, 0, (size_t)n * sizeof(float), st));
+    } else {
+        A.atomic_out = 0;
+    }
+    const int64_t npix = (int64_t)H * W, rows = (int64_t)n_windows * (negpos ? 2 : 1) * npix;
+    prof_count(1);
+    voxel_grad_interleave_kernel<<<grid_simple(rows, 256), 256, 0, st>>>(grad_out, rows, npix, B, A.S, gi);
+    const bool vec = (aos || (aligned16(x) && aligned16(y) && aligned16(t) && aligned16(p))) && aligned16(A.gp) &&
+                     aligned16(A.gt);
+    // slices per window: a full wave for one window; for many, enough CTAs to fill the machine, at most one per 2K events
+    const int cap = grid_for(voxel_grad_kernel<true>, kGradThreads, (int64_t)1 << 40, 1);
+    const int64_t per = n / n_windows;
+    int64_t slices = (per + kGradThreads * 8 - 1) / (kGradThreads * 8);
+    const int64_t fill = (cap + n_windows - 1) / n_windows;
+    if (slices > fill) slices = fill;
+    if (slices < 1) slices = 1;
+    if ((int64_t)n_windows * slices > 0x7fffffffLL) { set_error("evk_voxel_grad_f32: too many windows"); return EVK_E_ARG; }
+    A.slices = (int)slices;
+    prof_count(1);
+    if (vec) voxel_grad_kernel<true><<<(unsigned)(n_windows * slices), kGradThreads, 0, st>>>(A);
+    else voxel_grad_kernel<false><<<(unsigned)(n_windows * slices), kGradThreads, 0, st>>>(A);
+    if (A.gt) {
+        prof_count(1);
+        voxel_grad_ends_kernel<<<(n_windows + 127) / 128, 128, 0, st>>>(A);
+    }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }

@@ -71,6 +71,23 @@ def _times_f32(ts, dev):
     return t, float(t[0].item()), float((t[-1] - t[0]).item())
 
 
+def _device_events(xs, ys, ts, ps, dev, aos_ok=True):
+    """The events as the voxel kernels take them on `dev`: (aos, x, y, t, p, t0, dt, flags).  aos is the (N,4) view when
+    the four arrays are the columns of one CUDA tensor (x, y, t, p are then None).  t0 / dt are read on the device
+    (EVK_AUTO_SPAN in flags) when the stamps are f32 on the device already."""
+    aos = E.aos_base(xs, ys, ts, ps) if aos_ok and isinstance(xs, torch.Tensor) and xs.is_cuda else None
+    if aos is not None:
+        # t0 / dt are read on the device (EVK_AUTO_SPAN): no host round trip before the launch
+        return aos, None, None, None, None, 0.0, 1.0, _lib.AUTO_SPAN
+    ts_t = E.as_tensor(ts)
+    if ts_t.is_cuda and ts_t.dtype == torch.float32 and ts_t.dim() == 1:
+        t, t0, dt, flags = ts_t.contiguous(), 0.0, 1.0, _lib.AUTO_SPAN
+    else:
+        t, t0, dt = _times_f32(ts, dev)
+        flags = 0
+    return None, E.coords_f32(xs, dev), E.coords_f32(ys, dev), t, E.weights_f32(ps, dev), t0, dt, flags
+
+
 def events_to_voxel_torch(xs, ys, ts, ps, B, device=None, sensor_size=(180, 240), temporal_bilinear=True):
     """
     Turn a set of events into a (B,H,W) float32 voxel grid with temporal bilinear interpolation.
@@ -81,6 +98,7 @@ def events_to_voxel_torch(xs, ys, ts, ps, B, device=None, sensor_size=(180, 240)
     @param sensor_size (H, W)
     @param temporal_bilinear only True is defined (the reference's False branch raises NameError)
     @returns voxel grid tensor
+    Differentiable like the reference w.r.t. ps and ts (event_utils_b200.autograd).
     """
     assert(len(xs) == len(ys) and len(ys) == len(ts) and len(ts) == len(ps))
     if not temporal_bilinear:
@@ -99,6 +117,9 @@ def events_to_voxel_torch(xs, ys, ts, ps, B, device=None, sensor_size=(180, 240)
         raise RuntimeError("Index put requires the source and destination dtypes match, "
                            "got Float for the destination and Double for the source.")
     dev = E.compute_device(xs, ys, ts, ps)
+    if E.needs_grad(ps, ts):
+        from ..autograd import VoxelGrid
+        return VoxelGrid.apply(xs, ys, ts, ps, (device, B, H, W, False, None))
 
     host_f32 = all(isinstance(a, torch.Tensor) and not a.is_cuda and a.dtype == torch.float32
                    and a.dim() == 1 and a.is_contiguous() for a in (xs, ys, ts, ps))
@@ -117,18 +138,8 @@ def events_to_voxel_torch(xs, ys, ts, ps, B, device=None, sensor_size=(180, 240)
             raise IndexError("%d events index outside the voxel grid of shape %s" % (bad.value, (B, H, W)))
         return out if device.type == "cpu" else out.to(device)
 
-    aos = E.aos_base(xs, ys, ts, ps) if isinstance(xs, torch.Tensor) and xs.is_cuda else None
-    ts_t = E.as_tensor(ts)
-    if aos is not None:
-        # t0 / dt are read on the device (EVK_AUTO_SPAN): no host round trip before the launch
-        grid = _voxel_device(None, None, None, None, 0.0, 1.0, B, H, W, flags=_lib.AUTO_SPAN, aos=aos)
-    elif ts_t.is_cuda and ts_t.dtype == torch.float32 and ts_t.dim() == 1:
-        grid = _voxel_device(E.coords_f32(xs, dev), E.coords_f32(ys, dev), ts_t.contiguous(), E.weights_f32(ps_t, dev),
-                             0.0, 1.0, B, H, W, flags=_lib.AUTO_SPAN)
-    else:
-        t, t0, dt = _times_f32(ts, dev)
-        grid = _voxel_device(E.coords_f32(xs, dev), E.coords_f32(ys, dev), t, E.weights_f32(ps_t, dev),
-                             t0, dt, B, H, W)
+    aos, x, y, t, p, t0, dt, flags = _device_events(xs, ys, ts, ps, dev)
+    grid = _voxel_device(x, y, t, p, t0, dt, B, H, W, flags=flags, aos=aos)
     return grid if grid.device == device else grid.to(device)
 
 
@@ -182,7 +193,8 @@ def events_to_neg_pos_voxel_torch(xs, ys, ts, ps, B, device=None, sensor_size=(1
     """
     Positive and negative events in separate voxel grids; drop-in for voxel_grid.py:155-182
     (weights [p>0] and [p<=0]).  The reference runs the whole voxel build twice; here both grids
-    come out of ONE pass over the events (evk_voxel_negpos_f32).
+    come out of ONE pass over the events (evk_voxel_negpos_f32).  Differentiable like the reference
+    w.r.t. ts (event_utils_b200.autograd).
     @returns (voxel_pos, voxel_neg)
     """
     assert(len(xs) == len(ys) and len(ys) == len(ts) and len(ts) == len(ps))
@@ -191,30 +203,37 @@ def events_to_neg_pos_voxel_torch(xs, ys, ts, ps, B, device=None, sensor_size=(1
                                   "(voxel_grid.py:144-147 raises NameError)")
     if len(xs) == 0:
         raise IndexError("index -1 is out of bounds for dimension 0 with size 0")
-    L = _lib.lib()
+    _lib.lib()
     if device is None:
         device = E.as_tensor(xs).device
     device = torch.device(device)
     dev = E.compute_device(xs, ys, ts, ps)
     H, W, B = int(sensor_size[0]), int(sensor_size[1]), int(B)
+    if E.needs_grad(ts):
+        from ..autograd import VoxelGrid
+        out = VoxelGrid.apply(xs, ys, ts, ps, (device, B, H, W, True, None))
+        return out[0], out[1]
     with torch.cuda.device(dev):
-        ts_t = E.as_tensor(ts)
-        flags = E.variant_flag()
-        if ts_t.is_cuda and ts_t.dtype == torch.float32 and ts_t.dim() == 1:
-            t, t0, dt = ts_t.contiguous(), 0.0, 1.0
-            flags |= _lib.AUTO_SPAN       # first / last timestamp read on the device
-        else:
-            t, t0, dt = _times_f32(ts, dev)
-        x, y, p = E.coords_f32(xs, dev), E.coords_f32(ys, dev), E.weights_f32(ps, dev)
+        _, x, y, t, p, t0, dt, flags = _device_events(xs, ys, ts, ps, dev, aos_ok=False)
+        out = _negpos_device(x, y, t, p, t0, dt, B, H, W, flags)
+    if out.device != device:
+        out = out.to(device)
+    return out[0], out[1]
+
+
+def _negpos_device(x, y, t, p, t0, dt, B, H, W, flags):
+    """Both grids of events_to_neg_pos_voxel_torch from device-resident f32 arrays: (2,B,H,W) f32."""
+    L = _lib.lib()
+    dev = x.device
+    with torch.cuda.device(dev):
+        flags |= E.variant_flag()
         out = torch.empty((2, B, H, W), dtype=torch.float32, device=dev)
         ws = _lib.scratch("voxel_ws", 2 * L.evk_voxel_workspace_bytes(B, H, W, flags), dev)
         oob = _lib.oob_counter(dev)
         _lib.check(L.evk_voxel_negpos_f32(_lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), x.shape[0], t0, dt, B, H, W,
                                           flags, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.ptr(oob), _lib.stream()))
         E.raise_if_oob(oob, "voxel grid", (B, H, W))
-    if out.device != device:
-        out = out.to(device)
-    return out[0], out[1]
+    return out
 
 
 def events_to_voxel(xs, ys, ts, ps, B, sensor_size=(180, 240), temporal_bilinear=True):
@@ -265,7 +284,7 @@ def events_to_voxel_timesync_torch(xs, ys, ts, ps, B, t0, t1, device=None, np_ts
     """Voxel grid of the events between t0 and t1; drop-in for voxel_grid.py:82-112."""
     assert(t1 > t0)
     if np_ts is None:
-        np_ts = ts.cpu().numpy()
+        np_ts = ts.detach().cpu().numpy()   # the window bounds only: ts may require grad
     if device is None:
         device = xs.device
     start_idx = np.searchsorted(np_ts, t0)
@@ -282,10 +301,19 @@ def _batched_windows(xs, ys, ts, ps, starts, ends, B, sensor_size):
     if not all(isinstance(a, torch.Tensor) and a.is_cuda and a.dtype == torch.float32 and a.dim() == 1
                and a.is_contiguous() for a in (xs, ys, ts, ps)):
         return None
-    nw = len(starts)
     H, W, B = int(sensor_size[0]), int(sensor_size[1]), int(B)
-    if nw == 0:
+    if len(starts) == 0:
         return []
+    if E.needs_grad(ps, ts):
+        from ..autograd import VoxelGrid
+        return list(VoxelGrid.apply(xs, ys, ts, ps, (xs.device, B, H, W, False, (starts, ends))).unbind(0))
+    return list(_windows_device(xs, ys, ts, ps, starts, ends, B, H, W)[0].unbind(0))
+
+
+def _windows_device(xs, ys, ts, ps, starts, ends, B, H, W):
+    """The (nw,B,H,W) grids of the windows [starts[w], ends[w]) of contiguous f32 CUDA arrays, and the device
+    (start, end) pairs."""
+    nw = len(starts)
     L = _lib.lib()
     dev = xs.device
     with torch.cuda.device(dev):
@@ -297,7 +325,7 @@ def _batched_windows(xs, ys, ts, ps, starts, ends, B, sensor_size):
         _lib.check(L.evk_voxel_windows_f32(_lib.ptr(xs), _lib.ptr(ys), _lib.ptr(ts), _lib.ptr(ps), _lib.ptr(pairs), nw, total,
                                            B, H, W, _lib.WINDOW_PAIRS, _lib.ptr(out), _lib.ptr(oob), _lib.stream()))
         E.raise_if_oob(oob, "voxel grid", (B, H, W))
-    return list(out.unbind(0))
+    return out, pairs
 
 
 def voxel_grids_fixed_n_torch(xs, ys, ts, ps, B, n, sensor_size=(180, 240), temporal_bilinear=True):
@@ -316,7 +344,7 @@ def voxel_grids_fixed_n_torch(xs, ys, ts, ps, B, n, sensor_size=(180, 240), temp
 def voxel_grids_fixed_t_torch(xs, ys, ts, ps, B, t, sensor_size=(180, 240), temporal_bilinear=True):
     """List of voxel grids of temporal width t; drop-in for voxel_grid.py:59-80.  CUDA float32
     inputs: every window in one kernel launch."""
-    np_ts = ts.cpu().numpy()
+    np_ts = ts.detach().cpu().numpy()
     t_starts = np.arange(ts[0].item(), ts[-1].item() - t, t)
     if temporal_bilinear:
         starts = [int(np.searchsorted(np_ts, t0)) for t0 in t_starts]

@@ -51,6 +51,8 @@ extern "C" {
 #define EVK_PEER_MULTICAST 0x1000000u /* evk_voxel_fold_allreduce_f32: entry 0 of both pointer arrays is an NVLS multicast address */
 #define EVK_WINDOW_NEGPOS 0x400000u /* evk_voxel_windows_f32: out is [n_windows][2][B][H][W], the [p>0] / [p<=0] split per window */
 #define EVK_NEGPOS_TRUTHY 0x8u /* neg/pos split on numpy truthiness (p != 0) instead of p > 0 */
+#define EVK_WINDOW_OVERLAP 0x2000000u /* evk_voxel_grad_f32: windows may share events; their per-event gradients are added */
+#define EVK_EVENTS_AOS 0x4000000u /* evk_voxel_grad_f32: x is one 16-byte aligned (N,4) [x,y,t,p] array; y, t, p are ignored */
 /* kernel variant selection, bits 8..11 (0 = pick automatically) */
 #define EVK_VARIANT_SHIFT 8
 #define EVK_VARIANT_MASK (0xFu << EVK_VARIANT_SHIFT)
@@ -263,6 +265,28 @@ int evk_warp_flow_f32(const float *x, const float *y, const float *t, int64_t n,
  *                        grad_flow [2][H][W] (overwritten; taps outside the field get nothing, as zero
  *                        padding implies).  workspace: evk_warp_flow_grad_workspace_bytes() bytes,
  *                        16-byte aligned (2x2-block accumulators for the flow gradient).
+ *   evk_voxel_grad_f32   gradient of evk_voxel_f32 / _aos_f32 (nearest, EVK_AUTO_SPAN), evk_voxel_negpos_f32 and
+ *                        evk_voxel_windows_f32 (EVK_WINDOW_PAIRS), i.e. of events_to_voxel_torch voxel_grid.py:114-153,
+ *                        events_to_neg_pos_voxel_torch :155-182 and the windows of voxel_grids_fixed_n/_t_torch
+ *                        :37-80 and events_to_voxel_timesync_torch :82-112.  pairs: n_windows (start, end) int64
+ *                        pairs on the device, or NULL for the one window [0, n).  Each window has its own
+ *                        t0 = t[start], dt = t[end-1] - t0 and tn = ((t - t0) / dt) * (B-1) in f32, as the forward.
+ *                        grad_out: [n_windows][B][H][W], or [n_windows][2][B][H][W] with EVK_WINDOW_NEGPOS (the
+ *                        [p>0] / [p<=0] split; not EVK_NEGPOS_TRUTHY).  With g = grad_out at the event's pixel
+ *                        (truncated, negative indices wrap), v_b = 1 - |tn - b| and torch's subgradients
+ *                        (sign(0) = 0, a tie of max(0, v) splits the gradient in half):
+ *                          grad_p = sum_b g[b] max(0, v_b)               (not written with EVK_WINDOW_NEGPOS)
+ *                          G      = p sum_b g[b] s_b,  s_b = -sign(tn-b) (v_b > 0), -sign(tn-b)/2 (v_b == 0), 0 (v_b < 0)
+ *                          grad_t = G (B-1) / dt, plus ((sum G tn) - (B-1) sum G) / dt at t[start] and
+ *                                   -(sum G tn) / dt at t[end-1] of each window (sums in f64, on the device)
+ *                        Finite events visit bins floor(tn)-1 .. floor(tn)+2 (the last only ties, when tn - b rounds
+ *                        to -1 just below an integer); non-finite tn or p visit every bin, so NaN lands where
+ *                        autograd puts it.
+ *                        Events outside the grid, and with pairs those outside every window, get 0.  Windows that
+ *                        share events need EVK_WINDOW_OVERLAP (the gradients are then added atomically).  With
+ *                        EVK_EVENTS_AOS, x is the (N,4) record array of evk_voxel_aos_f32.
+ *                        workspace: evk_voxel_grad_workspace_bytes() bytes, 256-byte aligned (the per-window sums
+ *                        and grad_out re-laid out pixel-major).  Nothing is read back to the host.
  * --------------------------------------------------------------------------------------------- */
 int evk_image_grad_f32(const float *x, const float *y, const float *p, int64_t n, int Himg, int Wimg,
                        float clipx, float clipy, unsigned flags, const float *grad_img, float *grad_x,
@@ -279,6 +303,11 @@ int evk_warp_flow_grad_f32(const float *x, const float *y, const float *t, int64
                            int H, int W, float t0, const float *grad_xw, const float *grad_yw, float *grad_x,
                            float *grad_y, float *grad_t, float *grad_flow, double *sum_grad_t,
                            void *workspace, size_t workspace_bytes, void *stream);
+size_t evk_voxel_grad_workspace_bytes(int n_windows, int B, int H, int W, unsigned flags);
+int evk_voxel_grad_f32(const float *x, const float *y, const float *t, const float *p, int64_t n,
+                       const int64_t *pairs, int n_windows, int B, int H, int W, unsigned flags,
+                       const float *grad_out, float *grad_p, float *grad_t, void *workspace,
+                       size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Contrast maximisation, fused: linvel warp -> bounds mask -> bilinear IWE (+ derivative
