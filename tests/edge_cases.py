@@ -219,3 +219,58 @@ def packed_of(c, T0=1.7e9):
     f32 = dict(x=x16.astype(_F32), y=y16.astype(_F32), t=(T - t_first).astype(_F32),
                p=np.where(p8 != 0, 1.0, -1.0).astype(_F32), t0=_F32(0.0), dt=_F32(t_last - t_first))
     return x16, y16, T, p8, t_first, t_last, f32
+
+
+# ---- exactly computable gradient streams -------------------------------------------------------------------------------
+# Every per-event gradient of these streams is exact in f32: quarter-pixel coordinates, integer or dyadic polarities and
+# incoming gradients, tn on quarter bins with dt and B-1 powers of two; for the warp W-1 and H-1 powers of two (the
+# normalise round trip is exact), a dyadic flow and dt.  The window sums sum G and sum G tn of the voxel backward and
+# sum grad_t of the warp need MORE than 24 significant bits: the incoming gradient rises with the bin (voxel) and the
+# flow and gradients are biased positive (warp), so the sums grow with n on a fine dyadic grid.  Only f64 accumulation
+# then gives the value the tests expect, rounded once to f32.
+EXACT_GRAD_P = np.array([1.0, 2.0, 3.0, -1.0, 0.5, 3 * 2.0 ** -12, 5 * 2.0 ** -12, -7 * 2.0 ** -12], np.float32)
+
+
+def exact_grad_streams(seed, kind, n, windows=None):
+    """One exactly computable gradient stream of n events for kind "voxel", "image" or "warp".
+      voxel  B = 5, 12x16 sensor (coordinates also beyond it, wrapping or dropped); per window [s, e) the stamps are
+             w + q/16 (q = 0..16, the first 0 and the last 16): t0 = w, dt = 1, tn = q/4.  `windows`: [nw][2] pairs
+             (default one window [0, n)).  g: the incoming gradient [nw][1][B][H][W], 4b + an integer in [-2, 2]
+      image  canvas 13x17, quarter-pixel coordinates over [-1, size], integer polarities, integer g [H][W]
+      warp   33x33 field (W-1 = H-1 = 32), quarter-pixel coordinates over [-2, 34], stamps k/8 in [0, 2] with t0 = 0,
+             flow in quarters biased positive, incoming gradients integers biased positive
+    Returns a dict of f32 arrays and the parameters."""
+    rng = np.random.default_rng(seed)
+    if kind == "voxel":
+        B, H, W = 5, 12, 16
+        if windows is None:
+            windows = np.array([[0, n]], np.int64)
+        windows = np.asarray(windows, np.int64).reshape(-1, 2)
+        t = np.zeros(n, np.float32)
+        for w, (s, e) in enumerate(windows):
+            if e > s:
+                q = rng.integers(0, 17, e - s)
+                q[0], q[-1] = 0, 16
+                t[s:e] = w + q / 16.0
+        x = (rng.integers(-4 * W, 8 * W, n) / 4.0).astype(np.float32)
+        y = (rng.integers(-4 * H, 8 * H, n) / 4.0).astype(np.float32)
+        p = rng.choice(EXACT_GRAD_P, n)
+        g = (4 * np.arange(B)[None, None, :, None, None]
+             + rng.integers(-2, 3, (len(windows), 1, B, H, W))).astype(np.float32)
+        return dict(kind=kind, x=x, y=y, t=t, p=p, B=B, H=H, W=W, g=g, pairs=windows)
+    if kind == "image":
+        H, W = 13, 17
+        x = (rng.integers(-4, 4 * W + 1, n) / 4.0).astype(np.float32)
+        y = (rng.integers(-4, 4 * H + 1, n) / 4.0).astype(np.float32)
+        p = rng.integers(-3, 4, n).astype(np.float32)
+        g = rng.integers(-8, 9, (H, W)).astype(np.float32)
+        return dict(kind=kind, x=x, y=y, p=p, H=H, W=W, g=g)
+    assert kind == "warp"
+    H = W = 33
+    x = (rng.integers(-8, 4 * (W + 1) + 1, n) / 4.0).astype(np.float32)
+    y = (rng.integers(-8, 4 * (H + 1) + 1, n) / 4.0).astype(np.float32)
+    t = (rng.integers(0, 17, n) / 8.0).astype(np.float32)
+    flow = (rng.integers(-4, 13, (2, H, W)) / 4.0).astype(np.float32)
+    gx = rng.integers(-2, 7, n).astype(np.float32)
+    gy = rng.integers(-2, 7, n).astype(np.float32)
+    return dict(kind=kind, x=x, y=y, t=t, flow=flow, gxw=gx, gyw=gy, H=H, W=W, t0=np.float32(0.0))

@@ -68,6 +68,40 @@ def assert_ratio_within_exact(out, num, den, q=0.0, den_offset=1.0, what=""):
         what, int(bad.sum()), np.argwhere(bad)[:3].tolist(), out[bad][:3].tolist(), ref[bad][:3].tolist(), bound[bad][:3].tolist())
 
 
+def assert_within_grad_bound(out, g, what=""):
+    """A backward kernel's per-event output against its f64 reference g (tests/grad_reference.py Grad): every event
+    within (gamma(m) + gamma64(m)) M + extra of the reference value, m being the roundings on the longest path of the
+    kernel's expression.  Where the reference value is not finite the output must match it exactly (NaN where NaN, the
+    same infinity)."""
+    from grad_reference import bound_of
+    out = np.asarray(out, np.float64).reshape(-1)
+    ref = np.asarray(g.v, np.float64).reshape(-1)
+    assert out.shape == ref.shape, (what, out.shape, ref.shape)
+    nr, no = np.isnan(ref), np.isnan(out)
+    assert (nr == no).all(), "%s: NaN pattern differs at %s" % (what, np.flatnonzero(nr != no)[:5].tolist())
+    fin = np.isfinite(ref)
+    inf = ~fin & ~nr
+    assert (out[inf] == ref[inf]).all(), "%s: infinities differ at %s" % (what, np.flatnonzero(inf & (out != ref))[:5].tolist())
+    bound = np.broadcast_to(bound_of(g), ref.shape)
+    assert np.isfinite(bound[fin]).all(), what + ": bound not finite where the reference is"
+    with np.errstate(invalid="ignore"):
+        err = np.abs(out - ref)
+    bad = fin & ~(err <= bound)
+    if bad.any():
+        i = np.flatnonzero(bad)[:5]
+        raise AssertionError("%s: %d events outside the bound, e.g. %s: out %r ref %r bound %r" % (
+            what, int(bad.sum()), i.tolist(), out[i].tolist(), ref[i].tolist(), bound[i].tolist()))
+
+
+def assert_scalar_within(out, ref, bound, what=""):
+    """One f64 sum (value, bound) of a kernel against its reference; a non-finite reference must match exactly."""
+    out, ref = float(out), float(ref)
+    if not np.isfinite(ref):
+        assert (np.isnan(ref) and np.isnan(out)) or out == ref, (what, out, ref)
+        return
+    assert abs(out - ref) <= bound, "%s: %r vs %r (bound %r)" % (what, out, ref, bound)
+
+
 # ---- exactly summable streams (tests/edge_cases.py exact_streams) ----------------------------------------------------
 EXACT_C = 2048            # CTAs that may share a cell in the image and cmax table paths (at most one wave: 4 per SM)
 # The voxel hot-table kernel holds 40 KB of static shared memory, so at most 5 of its CTAs fit on an SM; its launches

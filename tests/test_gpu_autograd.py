@@ -2,8 +2,6 @@
 against autograd on the torch-op ports of the reference (tests/autograd_ports.py, pinned to the reference by
 tests/test_autograd_port.py), on the same device.  Per-event gradients: max error <= 1e-5 of the largest one; the flow
 gradient, a scatter, also cell by cell against exact f64 sums of its f32 taps (tests/exact_bounds.py)."""
-from collections import namedtuple
-
 import numpy as np
 import pytest
 import torch
@@ -14,6 +12,7 @@ from autograd_cases import CASES, forward, run, scene
 from conftest import assert_close_to_max
 from edge_cases import hard_cases
 from exact_bounds import assert_within_exact
+from grad_reference import flow_grad_exact
 
 pytestmark = pytest.mark.gpu
 
@@ -68,33 +67,6 @@ def compare(case, inputs, what, outputs=True):
 @pytest.mark.parametrize("case", CASES, ids=[c["name"] for c in CASES])
 def test_against_port(case, device):
     compare(case, to(scene(case), device), case["name"])
-
-
-Exact = namedtuple("Exact", "sum abs cnt")
-
-
-def flow_grad_exact(x, y, t_rel, gxw, gyw, H, W):
-    """Per cell of the flow gradient: the f64 sum, |sum| and count of the f32 taps g*dt*w the kernel adds
-    (the sample position and weights as flow_one forms them, in f32)."""
-    f32 = np.float32
-    x, y, t_rel, gxw, gyw = (np.asarray(a, np.float32) for a in (x, y, t_rel, gxw, gyw))
-    wm1, hm1 = f32(W - 1), f32(H - 1)
-    ix = (((x / wm1) * f32(2) - f32(1)) + f32(1)) / f32(2) * wm1
-    iy = (((y / hm1) * f32(2) - f32(1)) + f32(1)) / f32(2) * hm1
-    ok = (np.abs(ix) < 1e9) & (np.abs(iy) < 1e9)
-    fx, fy = np.floor(np.where(ok, ix, 0)), np.floor(np.where(ok, iy, 0))
-    wx1, wx0, wy1, wy0 = (fx + f32(1)) - ix, ix - fx, (fy + f32(1)) - iy, iy - fy
-    taps = [(0, 0, wx1 * wy1), (0, 1, wx0 * wy1), (1, 0, wx1 * wy0), (1, 1, wx0 * wy0)]
-    S, A, K = (np.zeros((2, H, W)) for _ in range(3))
-    for c, g in enumerate((gxw * t_rel, gyw * t_rel)):
-        for oy, ox, w in taps:
-            v = (g * w).astype(np.float32)
-            xx, yy = fx.astype(np.int64) + ox, fy.astype(np.int64) + oy
-            m = ok & (xx >= 0) & (xx < W) & (yy >= 0) & (yy < H) & (v != 0)
-            np.add.at(S[c], (yy[m], xx[m]), v[m].astype(np.float64))
-            np.add.at(A[c], (yy[m], xx[m]), np.abs(v[m]).astype(np.float64))
-            np.add.at(K[c], (yy[m], xx[m]), 1.0)
-    return Exact(S, A, K)
 
 
 def check_flow_exact(inputs, grad_flow, weights, t0):
