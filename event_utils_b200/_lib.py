@@ -39,6 +39,7 @@ CMAX_WANT_GRAD = 0x10
 CMAX_ABS_POLARITY = 0x20
 CMAX_NO_CHANNEL_MIX = 0x40
 OBJ_VARIANCE, OBJ_SOS, OBJ_SOE, OBJ_MOA, OBJ_ISOA, OBJ_SOSA = range(6)
+WARP_ROTATION, WARP_XYZTHETA = 1, 2
 
 _lib = None
 _lock = threading.Lock()
@@ -129,6 +130,15 @@ def _declare(L):
     L.evk_cmax_linvel_objective_batch_f64.restype = ci
     L.evk_cmax_linvel_objective_batch_f64.argtypes = [vp, vp, vp, vp, i64, f64, vp, ci, f64, ci, ci, ci, ci, f64, cu, ci, f64,
                                                       vp, vp, sz, vp]
+    L.evk_cmax_warp_objective_f64.restype = ci
+    L.evk_cmax_warp_objective_f64.argtypes = [vp, vp, vp, vp, i64, f64, ci, vp, f64, ci, ci, ci, ci, f64, cu, ci, f64,
+                                              vp, vp, vp, sz, vp]
+    L.evk_cmax_warp_objective_f32.restype = ci
+    L.evk_cmax_warp_objective_f32.argtypes = [vp, vp, vp, vp, i64, f32, ci, vp, ci, ci, ci, ci, f64, cu, ci, f64,
+                                              vp, vp, vp, sz, vp]
+    L.evk_cmax_warp_objective_batch_f64.restype = ci
+    L.evk_cmax_warp_objective_batch_f64.argtypes = [vp, vp, vp, vp, i64, f64, ci, vp, ci, f64, ci, ci, ci, ci, f64, cu, ci,
+                                                    f64, vp, vp, sz, vp]
     L.evk_iwe_objective_f32.restype = ci
     L.evk_iwe_objective_f32.argtypes = [vp, vp, ci, ci, f64, cu, ci, f64, vp, vp, sz, vp]
     L.evk_gaussian_blur_f32.restype = ci

@@ -12,7 +12,7 @@ import numpy as np
 import scipy.optimize as opt
 
 from ..util.event_util import infer_resolution
-from .objectives import evaluate_candidates, get_iwe, pinned_events, soe_objective, variance_objective
+from .objectives import _fused_kind, evaluate_candidates, get_iwe, pinned_events, soe_objective, variance_objective
 from .warps import linvel_warp
 
 
@@ -63,15 +63,17 @@ def optimize_contrast(xs, ys, ts, ps, warp_function, objective, optimizer=opt.fm
     """
     # nothing between here and the return modifies the event arrays (scipy hands the same `args` objects to
     # every f / f' call), so the event set is uploaded and hashed ONCE for the whole optimisation
-    fused = getattr(warp_function, "fused_kind", None) == "linvel"
+    fused = _fused_kind(warp_function) is not None
+    # the start point of the search: linvel keeps the reference's [0, 0]; other models start from zeros(dims)
+    zero = np.array([0, 0]) if getattr(warp_function, "fused_kind", None) == "linvel" else np.zeros(warp_function.dims)
     with (pinned_events(xs, ys, ts, ps) if fused else contextlib.nullcontext()):
         if grid_search_init and x0 is None:
             init_obj = copy.deepcopy(objective)
             init_obj.adaptive_lifespan = False
             x0 = grid_search_initial(xs, ys, ts, ps, warp_function, init_obj, img_size, log_scale=False)["min_params"]
-            x0 = np.array([0, 0]) if x0 is None else np.array(x0)
+            x0 = zero if x0 is None else np.array(x0)
         elif x0 is None:
-            x0 = np.array([0, 0])
+            x0 = zero
         objective.iter_update(x0)
         args = (xs, ys, ts, ps, warp_function, img_size, blur_sigma)
         if numeric_grads:

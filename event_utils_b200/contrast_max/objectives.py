@@ -114,16 +114,17 @@ def clear_cache():
 _result_bufs = {}
 
 
-def _result_buffers(dev):
-    """Per-device result buffer reused across evaluations: 12 doubles of PINNED HOST memory that the
+def _result_buffers(dev, n=12):
+    """Per-device result buffer reused across evaluations: n doubles (12, or 16 for the rotation / 4-DoF
+    models) of PINNED HOST memory that the
     last kernel of an evaluation writes straight over PCIe (pinned allocations are device-addressable
     under unified addressing), so reading a result back is one stream synchronise -- no device buffer,
     no D2H copy operation (a fresh torch.zeros + pageable .cpu() per call, or even a pinned mirror + copy_, is a
     noticeable share of a small evaluation).  Returns (tensor, numpy view)."""
-    k = (dev, torch.cuda.current_stream(dev).cuda_stream, threading.get_ident())   # per stream AND host thread: reuse is only safe in stream order
+    k = (dev, torch.cuda.current_stream(dev).cuda_stream, threading.get_ident(), n)   # per stream AND host thread: reuse is only safe in stream order
     b = _result_bufs.get(k)
     if b is None:
-        host = torch.zeros(12, dtype=torch.float64).pin_memory()
+        host = torch.zeros(n, dtype=torch.float64).pin_memory()
         b = (host, host.numpy())
         _result_bufs[k] = b
     return b
@@ -198,7 +199,94 @@ def _fused_linvel(params, xs, ys, ts, ps, img_size, blur_sigma, want_grad, use_p
         return res, (iwe.cpu().numpy() if iwe is not None else None), (d_iwe.cpu().numpy() if d_iwe is not None else None)
 
 
-def _objective_of_images(iwe, d_iwe, blur_sigma, want_grad, objective=_lib.OBJ_VARIANCE, obj_param=0.0):
+# fused_kind of a warp object -> the EVK_WARP_* code of evk_cmax_warp_objective_* (linvel has entries of its own)
+_MODEL_WARPS = {"rotation": _lib.WARP_ROTATION, "xyztheta": _lib.WARP_XYZTHETA}
+_FUSED_KINDS = ("linvel",) + tuple(_MODEL_WARPS)
+
+
+def _fused_kind(warpfunc):
+    """'linvel', 'rotation', 'xyztheta' for the models the GPU evaluates natively, else None"""
+    kind = getattr(warpfunc, "fused_kind", None)
+    return kind if kind in _FUSED_KINDS else None
+
+
+def _event_range(n_all, first, last):
+    last = n_all if last is None else (last if last >= 0 else n_all + last)
+    first = first if first >= 0 else n_all + first
+    first, last = max(0, min(first, n_all)), max(0, min(last, n_all))
+    return first, last, max(0, last - first)
+
+
+def _fused_model(warpfunc, params, xs, ys, ts, ps, img_size, blur_sigma, want_grad, use_polarity,
+                 first=0, last=None, p_scale=1.0, want_image=False, objective=_lib.OBJ_VARIANCE, obj_param=0.0, ev=None):
+    """One evaluation of a rotation / 4-DoF model (evk_cmax_warp_objective_*) on events [first:last) of the
+    cached device copy: the image pass, the image-space tail and, with want_grad, the gradient pass.
+    Returns (result[16] as numpy f64, iwe or None); the gradient is result[1:1 + dims]."""
+    L = _lib.lib()
+    ev = _device_events(xs, ys, ts, ps) if ev is None else ev
+    n_all = ev.n
+    first, last, n = _event_range(n_all, first, last)
+    if n == 0:
+        raise IndexError("index -1 is out of bounds for axis 0 with size 0")
+    Hs, Ws = SENSOR_SIZE
+    dev = ev.x.device
+    model = np.ascontiguousarray(warpfunc.model(params), dtype=np.float64)
+    warp = _MODEL_WARPS[warpfunc.fused_kind]
+    with _on_device(dev):
+        ws = _lib.scratch("cmax_ws", L.evk_cmax_workspace_bytes(Hs, Ws), dev)
+        result, result_view = _result_buffers(dev, 16)
+        iwe = torch.empty((Hs + 1, Ws + 1), dtype=torch.float32, device=dev) if want_image else None
+        flags = (_lib.CMAX_WANT_GRAD if want_grad else 0) | (0 if use_polarity else _lib.CMAX_ABS_POLARITY) \
+            | {None: 0, "onchip": _lib.VARIANT_SMEM_TILE, "l2": _lib.VARIANT_VECTOR_RED}[event_pass]
+        sigma = float(blur_sigma) if blur_sigma is not None else 0.0
+        if ev.mode == "f64":
+            t_ref = float(ev.t[last - 1].item()) if last != n_all else ev.t_last
+            off = first * 8
+            _lib.check(L.evk_cmax_warp_objective_f64(
+                ev.x.data_ptr() + off, ev.y.data_ptr() + off, ev.t.data_ptr() + off, ev.p.data_ptr() + off, n,
+                float(p_scale), warp, model.ctypes.data, t_ref, int(img_size[0]), int(img_size[1]), Hs, Ws, sigma, flags,
+                int(objective), float(obj_param), _lib.ptr(result), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(), _lib.stream()))
+        else:
+            if last != n_all:
+                raise NotImplementedError("f32 fast mode stores t relative to the last event; "
+                                          "slicing the tail (adaptive_lifespan) needs precision='f64'")
+            off = first * 4
+            _lib.check(L.evk_cmax_warp_objective_f32(
+                ev.x.data_ptr() + off, ev.y.data_ptr() + off, ev.t.data_ptr() + off, ev.p.data_ptr() + off, n,
+                float(p_scale), warp, model.ctypes.data, int(img_size[0]), int(img_size[1]), Hs, Ws, sigma, flags,
+                int(objective), float(obj_param), _lib.ptr(result), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(), _lib.stream()))
+        torch.cuda.current_stream().synchronize()
+        res = result_view.copy()
+        if res[6] != 0:
+            raise IndexError("%d warped events index outside the IWE canvas %s" % (int(res[6]), (Hs + 1, Ws + 1)))
+        return res, (iwe.cpu().numpy() if iwe is not None else None)
+
+
+def _images_objective(iwe, d_iwe, blur_sigma, want_grad, objective=_lib.OBJ_VARIANCE, obj_param=0.0):
+    """(result, gradient or None) of precomputed images.  A (2,H,W) derivative stack is one
+    evk_iwe_objective_f32 call with scipy's mixing of the two channels (objectives.py:253) reproduced.
+    Any other number K of channels -- the stack of a 3- or 4-parameter model -- is taken two channels
+    at a time with EVK_CMAX_NO_CHANNEL_MIX: the exact gradient, channel by channel (the reference can
+    only form two channels, image.py:210, so there is no mixing to reproduce; mixing components of
+    different units would also stop the vector from being a descent direction).  result is the
+    12-double layout of evk_iwe_objective_f32."""
+    if not want_grad or d_iwe is None:
+        return _objective_of_images(iwe, None, blur_sigma, False, objective, obj_param), None
+    d = np.asarray(d_iwe)
+    if d.shape[0] == 2:
+        res = _objective_of_images(iwe, d, blur_sigma, True, objective, obj_param)
+        return res, np.array([res[1], res[2]])
+    K = d.shape[0]
+    g, res = np.zeros(K), None
+    for k in range(0, K, 2):
+        pair = d[k:k + 2] if k + 2 <= K else np.concatenate((d[k:k + 1], np.zeros_like(d[:1])))
+        r = _objective_of_images(iwe, pair, blur_sigma, True, objective, obj_param, channel_mix=False)
+        res = r if res is None else res
+        g[k:k + 2] = r[6:8][:min(2, K - k)]
+    return res, g
+
+
+def _objective_of_images(iwe, d_iwe, blur_sigma, want_grad, objective=_lib.OBJ_VARIANCE, obj_param=0.0, channel_mix=True):
     """objective (+ gradient) of precomputed images, on the GPU (evk_iwe_objective_f32)."""
     L = _lib.lib()
     dev = E.compute_device()
@@ -208,7 +296,7 @@ def _objective_of_images(iwe, d_iwe, blur_sigma, want_grad, objective=_lib.OBJ_V
         d = torch.from_numpy(np.ascontiguousarray(d_iwe, dtype=np.float32)).to(dev) if d_iwe is not None else None
         ws = _lib.scratch("cmax_ws", L.evk_cmax_workspace_bytes(iwe.shape[0] - 1, iwe.shape[1] - 1), dev)
         result = torch.zeros(12, dtype=torch.float64, device=dev)
-        flags = _lib.CMAX_WANT_GRAD if (want_grad and d is not None) else 0
+        flags = (_lib.CMAX_WANT_GRAD if (want_grad and d is not None) else 0) | (0 if channel_mix else _lib.CMAX_NO_CHANNEL_MIX)
         _lib.check(L.evk_iwe_objective_f32(_lib.ptr(a), _lib.ptr(d), iwe.shape[0], iwe.shape[1], float(blur_sigma), flags,
                                            int(objective), float(obj_param), _lib.ptr(result), _lib.ptr(ws), ws.numel(),
                                            _lib.stream()))
@@ -285,13 +373,19 @@ def get_iwe(params, xs, ys, ts, ps, warpfunc, img_size, compute_gradient=False,
     """
     Image of warped events (and dIWE/dparams) for a parameter vector; drop-in for
     objectives.py:165-199.  numpy in, numpy float32 (181,241) / (dims,181,241) out.
+    The rotation / 4-DoF models form the IWE alone in their image pass; with compute_gradient their
+    (dims,181,241) derivative stack comes from the generic path (host warp() + events_to_image_drv).
     @returns tuple: iwe, d_iwe (or None) [, (xs_warped, ys_warped)] [, per-event contrast]
     """
-    fused = getattr(warpfunc, "fused_kind", None) == "linvel"
+    kind = _fused_kind(warpfunc)
+    fused = kind == "linvel"
     if fused and not return_events and not return_per_event_contrast:
         _, iwe, d_iwe = _fused_linvel(params, xs, ys, ts, ps, img_size, 0.0, compute_gradient, use_polarity,
                                       want_images=True)
         return (iwe, d_iwe)
+    if kind in _MODEL_WARPS and not compute_gradient and not return_events and not return_per_event_contrast:
+        _, iwe = _fused_model(warpfunc, params, xs, ys, ts, ps, img_size, 0.0, False, use_polarity, want_image=True)
+        return (iwe, None)
     # generic warp objects (and the two debugging outputs): host warp + mask as in the
     # reference, image formation on the GPU
     xs, ys, ts, ps = (np.asarray(a) for a in (xs, ys, ts, ps))
@@ -333,22 +427,30 @@ class variance_objective(objective_function):
                 self.recompute_lifespan = False
             first, last, scale = int(self.s_idx), -1, 100.0   # xs[s_idx:-1], ps*100 (objectives.py:224-225)
         blur_sigma = self.default_blur if blur_sigma is None else blur_sigma
-        fused = getattr(warpfunc, "fused_kind", None) == "linvel"
+        kind = _fused_kind(warpfunc)
+        fused = kind is not None
         ev = _device_events(xs, ys, ts, ps) if fused else None
-        # memo only for the fused warp: a generic warp object's result depends on that object's identity and state
+        # memo only for the fused warps: a generic warp object's result depends on that object's identity and state
         key = (tuple(float(v) for v in params), ev.key, tuple(img_size), float(blur_sigma), first, last, scale,
                self.use_polarity, precision) if fused else None
+        if kind in _MODEL_WARPS:
+            key += (kind, tuple(warpfunc.model(params)))    # the model block carries xyztheta's centre
         if fused and self._memo is not None and self._memo[0] == key:
             return self._memo[1], self._memo[2]
-        if fused:
+        if kind == "linvel":
             res, _, _ = _fused_linvel(params, xs, ys, ts, ps, img_size, blur_sigma, True, self.use_polarity,
                                       first=first, last=last, p_scale=scale, ev=ev)
+            f, g = float(res[0]), np.array([res[1], res[2]])
+        elif fused:
+            res, _ = _fused_model(warpfunc, params, xs, ys, ts, ps, img_size, blur_sigma, True, self.use_polarity,
+                                  first=first, last=last, p_scale=scale, ev=ev)
+            f, g = float(res[0]), res[1:1 + warpfunc.dims].copy()
         else:
             sl = slice(first, last)
             iwe, d_iwe = get_iwe(params, xs[sl], ys[sl], ts[sl], ps[sl] * scale, warpfunc, img_size,
                                  use_polarity=self.use_polarity, compute_gradient=True)
-            res = _objective_of_images(iwe, d_iwe, blur_sigma, True)
-        f, g = float(res[0]), np.array([res[1], res[2]])
+            res, g = _images_objective(iwe, d_iwe, blur_sigma, True)
+            f = float(res[0])
         self._memo = (key, f, g) if fused else None
         return f, g
 
@@ -366,8 +468,7 @@ class variance_objective(objective_function):
         """Analytic gradient of the objective wrt the warp parameters (np.ndarray[dims])."""
         if iwe is not None and d_iwe is not None:
             blur_sigma = self.default_blur if blur_sigma is None else blur_sigma
-            res = _objective_of_images(iwe, d_iwe, blur_sigma, True)
-            return np.array([res[1], res[2]])
+            return _images_objective(iwe, d_iwe, blur_sigma, True)[1]
         _, g = self._evaluate(params, xs, ys, ts, ps, warpfunc, img_size, blur_sigma)
         return g.copy()
 
@@ -385,25 +486,38 @@ class _fused_objective(objective_function):
         return 0.0
 
     def _result(self, params, xs, ys, ts, ps, warpfunc, img_size, blur_sigma, iwe=None, d_iwe=None, want_grad=True):
+        """the result array of one evaluation: [0] f; [8] mean(G^2) and [9] sum(exp(-p G)) in every layout"""
+        return self._evaluate_point(params, xs, ys, ts, ps, warpfunc, img_size, blur_sigma, iwe, d_iwe, want_grad)[0]
+
+    def _evaluate_point(self, params, xs, ys, ts, ps, warpfunc, img_size, blur_sigma, iwe=None, d_iwe=None, want_grad=True):
+        """(result array, gradient[dims] or None)"""
         blur_sigma = self.default_blur if blur_sigma is None else blur_sigma
         if iwe is not None:
-            return _objective_of_images(iwe, d_iwe, blur_sigma, want_grad and d_iwe is not None, self._kind, self._param())
-        fused = getattr(warpfunc, "fused_kind", None) == "linvel"
+            return _images_objective(iwe, d_iwe, blur_sigma, want_grad and d_iwe is not None, self._kind, self._param())
+        kind = _fused_kind(warpfunc)
+        fused = kind is not None
         ev = _device_events(xs, ys, ts, ps) if fused else None
         key = (tuple(float(v) for v in params), ev.key, tuple(img_size), float(blur_sigma), self.use_polarity,
                precision, self._kind, self._param()) if fused else None
+        if kind in _MODEL_WARPS:
+            key += (kind, tuple(warpfunc.model(params)))
         memo = getattr(self, "_memo", None)
         if fused and memo is not None and memo[0] == key:
             return memo[1]
-        if fused:
+        if kind == "linvel":
             res, _, _ = _fused_linvel(params, xs, ys, ts, ps, img_size, blur_sigma, self.has_derivative, self.use_polarity,
                                       objective=self._kind, obj_param=self._param(), ev=ev)
+            out = (res, np.array([res[1], res[2]]))
+        elif fused:
+            res, _ = _fused_model(warpfunc, params, xs, ys, ts, ps, img_size, blur_sigma, self.has_derivative,
+                                  self.use_polarity, objective=self._kind, obj_param=self._param(), ev=ev)
+            out = (res, res[1:1 + warpfunc.dims].copy())
         else:
             img, dimg = get_iwe(params, xs, ys, ts, ps, warpfunc, img_size, use_polarity=self.use_polarity,
                                 compute_gradient=self.has_derivative)
-            res = _objective_of_images(img, dimg, blur_sigma, self.has_derivative, self._kind, self._param())
-        self._memo = (key, res) if fused else None
-        return res
+            out = _images_objective(img, dimg, blur_sigma, self.has_derivative, self._kind, self._param())
+        self._memo = (key, out) if fused else None
+        return out
 
     def evaluate_function(self, params=None, xs=None, ys=None, ts=None, ps=None,
             warpfunc=None, img_size=None, blur_sigma=None, showimg=False, iwe=None):
@@ -415,8 +529,8 @@ class _fused_objective(objective_function):
             return None
         if iwe is not None and d_iwe is None:
             iwe = None
-        res = self._result(params, xs, ys, ts, ps, warpfunc, img_size, blur_sigma, iwe=iwe, d_iwe=d_iwe)
-        return np.array([res[1], res[2]])
+        g = self._evaluate_point(params, xs, ys, ts, ps, warpfunc, img_size, blur_sigma, iwe=iwe, d_iwe=d_iwe)[1]
+        return g.copy()
 
 
 class rms_objective(_fused_objective):
@@ -576,17 +690,21 @@ class zhu_timestamp_objective(objective_function):
 
 def evaluate_candidates(objective, params_list, xs, ys, ts, ps, warpfunc, img_size, blur_sigma=None, want_grad=False):
     """Objective (and gradient) at MANY parameter points with one pass over the events per 32
-    candidates (evk_cmax_linvel_objective_batch_f64): what grid_search_initial needs
-    (events_cmax.py:300-302 evaluates 25 points per level, one full evaluation each).
-    @returns (f[K], g[K,2] or None)"""
+    candidates (evk_cmax_linvel_objective_batch_f64; evk_cmax_warp_objective_batch_f64 for the rotation /
+    4-DoF models, f only): what grid_search_initial needs (events_cmax.py:300-302 evaluates
+    num_samples^dims points per level, one full evaluation each).
+    @returns (f[K], g[K,dims] or None)"""
     params_list = [tuple(float(v) for v in prm) for prm in params_list]
-    kind = getattr(objective, "_kind", _lib.OBJ_VARIANCE)
+    kind_obj = getattr(objective, "_kind", _lib.OBJ_VARIANCE)
     prm_fn = getattr(objective, "_param", None)
     obj_param = float(prm_fn()) if prm_fn is not None else 0.0
     sigma = objective.default_blur if blur_sigma is None else blur_sigma
-    fused = getattr(warpfunc, "fused_kind", None) == "linvel" and precision == "f64" \
+    kind = _fused_kind(warpfunc)
+    fused = kind is not None and precision == "f64" \
         and not getattr(objective, "adaptive_lifespan", False) and type(objective).evaluate_function in (
             _fused_objective.evaluate_function, variance_objective.evaluate_function)
+    if kind in _MODEL_WARPS and want_grad:
+        fused = False          # the batch entry of these models returns f only
     if not fused:
         f = np.array([objective.evaluate_function(prm, xs, ys, ts, ps, warpfunc, img_size, blur_sigma) for prm in params_list])
         g = np.array([objective.evaluate_gradient(prm, xs, ys, ts, ps, warpfunc, img_size, blur_sigma)
@@ -597,6 +715,23 @@ def evaluate_candidates(objective, params_list, xs, ys, ts, ps, warpfunc, img_si
     Hs, Ws = SENSOR_SIZE
     dev = ev.x.device
     K = len(params_list)
+    if kind in _MODEL_WARPS:
+        models = np.array([warpfunc.model(prm) for prm in params_list], dtype=np.float64)
+        out = np.zeros((K, 16))
+        with torch.cuda.device(dev):
+            ws = _lib.scratch("cmax_ws", L.evk_cmax_workspace_bytes(Hs, Ws), dev)
+            flags = 0 if objective.use_polarity else _lib.CMAX_ABS_POLARITY
+            for lo in range(0, K, 32):
+                chunk = np.ascontiguousarray(models[lo:lo + 32])
+                res = torch.zeros((chunk.shape[0], 16), dtype=torch.float64, device=dev)
+                _lib.check(L.evk_cmax_warp_objective_batch_f64(
+                    ev.x.data_ptr(), ev.y.data_ptr(), ev.t.data_ptr(), ev.p.data_ptr(), ev.n, 1.0, _MODEL_WARPS[kind],
+                    chunk.ctypes.data, chunk.shape[0], ev.t_last, int(img_size[0]), int(img_size[1]), Hs, Ws, float(sigma),
+                    flags, int(kind_obj), obj_param, _lib.ptr(res), _lib.ptr(ws), ws.numel(), _lib.stream()))
+                out[lo:lo + chunk.shape[0]] = res.cpu().numpy()
+        if out[:, 6].any():
+            raise IndexError("warped events index outside the IWE canvas")
+        return out[:, 0].copy(), None
     out = np.zeros((K, 12))
     with torch.cuda.device(dev):
         ws = _lib.scratch("cmax_ws", L.evk_cmax_workspace_bytes(Hs, Ws), dev)
@@ -607,7 +742,7 @@ def evaluate_candidates(objective, params_list, xs, ys, ts, ps, warpfunc, img_si
             _lib.check(L.evk_cmax_linvel_objective_batch_f64(
                 ev.x.data_ptr(), ev.y.data_ptr(), ev.t.data_ptr(), ev.p.data_ptr(), ev.n, 1.0,
                 chunk.ctypes.data, chunk.shape[0], ev.t_last, int(img_size[0]), int(img_size[1]), Hs, Ws, float(sigma), flags,
-                int(kind), obj_param, _lib.ptr(res), _lib.ptr(ws), ws.numel(), _lib.stream()))
+                int(kind_obj), obj_param, _lib.ptr(res), _lib.ptr(ws), ws.numel(), _lib.stream()))
             out[lo:lo + chunk.shape[0]] = res.cpu().numpy()
     if out[:, 4].any():
         raise IndexError("warped events index outside the IWE canvas")

@@ -59,6 +59,12 @@ struct BlurTaps {
     double w[kMaxRadius + 1];  // w[k] = weight at distance k (symmetric)
 };
 
+// Parameters of the rotation / 4-DoF motion models (host order of evk_cmax_warp_objective_*):
+//   rotation  {cx, cy, omega}                  xyztheta  {hx, hy, hz, theta, cx, cy}
+struct WarpModel {
+    double m[6];
+};
+
 struct CmaxArgs {
     const void *x, *y, *t, *p;
     int64_t n;
@@ -75,9 +81,15 @@ struct CmaxArgs {
     int vec16;      // on-chip path: all four event arrays are 16-byte aligned
     float *planar;  // on-chip path: planar f32 image [npix padded to 4] the CTAs' shared-memory images are reduced into
     unsigned long long *oob;
+    WarpModel model;  // rotation / xyztheta
 };
 
-enum { WARP_LINVEL_F64 = 0, WARP_LINVEL_F32 = 1, WARP_FLOW_F32 = 2 };
+enum { WARP_LINVEL_F64 = 0, WARP_LINVEL_F32 = 1, WARP_FLOW_F32 = 2,
+       WARP_ROTATION_F64 = 3, WARP_ROTATION_F32 = 4, WARP_XYZTHETA_F64 = 5, WARP_XYZTHETA_F32 = 6 };
+
+__host__ __device__ constexpr bool is_model_warp(int w) { return w >= WARP_ROTATION_F64; }
+__host__ __device__ constexpr bool is_rotation(int w) { return w == WARP_ROTATION_F64 || w == WARP_ROTATION_F32; }
+__host__ __device__ constexpr int model_dims(int w) { return is_rotation(w) ? 3 : 4; }
 
 // bilinear splat of weight w (and derivative weight a) at (xf, yf) on the canvas:
 // image.py:199-207 (IWE) and :131-135 (derivative images) with w1 = [a;0], w2 = [0;a].
@@ -89,6 +101,7 @@ enum { WARP_LINVEL_F64 = 0, WARP_LINVEL_F32 = 1, WARP_FLOW_F32 = 2 };
 struct Taps {
     int x0, x1, y0, y1;
     float wm;     // masked weight (|wm| <= 1 is the fast-path condition of the on-chip image)
+    float dx, dy; // bilinear fractions (the gradient pass of the motion models gathers with them)
     float4 ti;    // IWE taps TL, TR, BL, BR
     float4 td;    // free values of the derivative taps: a = am*oy, b = am*dy, c = am*ox, d = am*dx
 };
@@ -113,6 +126,7 @@ __device__ __forceinline__ bool splat_taps(const CmaxArgs &A, float xf, float yf
     const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
     const float wl = __fmul_rn(wm, ox), wr = __fmul_rn(wm, dx);
     T.wm = wm;
+    T.dx = dx; T.dy = dy;
     // tap order inside a block: TL (y0,x0), TR (y0,x1), BL (y1,x0), BR (y1,x1)
     T.ti = make_float4(__fmul_rn(wl, oy), __fmul_rn(wr, oy), __fmul_rn(wl, dy), __fmul_rn(wr, dy));
     // image.py:131-135 with w1 = [am;0], w2 = [0;am]:
@@ -215,6 +229,8 @@ __device__ __forceinline__ void splat_onchip(const CmaxArgs &A, float *acc, unsi
 // One event's four components as loaded (f64 in parity mode, f32 otherwise).
 template <int WARP> struct EvT { using type = float; };
 template <> struct EvT<WARP_LINVEL_F64> { using type = double; };
+template <> struct EvT<WARP_ROTATION_F64> { using type = double; };
+template <> struct EvT<WARP_XYZTHETA_F64> { using type = double; };
 
 template <int WARP>
 struct Event {
@@ -244,10 +260,86 @@ __device__ __forceinline__ void ld_vec16(const double *p, double (&v)[2])
     v[0] = q.x; v[1] = q.y;
 }
 
+// ---- rotation and 4-DoF motion models (contrast_max/warps.py defines them; the reference leaves them empty,
+// lib/contrast_max/warps.py:63-83).  dt = t - t0 and the warp undoes the motion during dt:
+//   rotation (cx, cy, omega):  a = omega dt, u = x - cx, v = y - cy
+//     x' = cx + (cos(a) u + sin(a) v)          y' = cy + (cos(a) v - sin(a) u)
+//     dx'/d(cx, cy, omega) = (1 - cos a, -sin a,  dt (cos(a) v - sin(a) u))
+//     dy'/d(cx, cy, omega) = (sin a, 1 - cos a, -dt (cos(a) u + sin(a) v))
+//   xyztheta (hx, hy, hz, theta) about the fixed centre (cx, cy):
+//     x' = x - dt ((hx + hz u) - theta v)      y' = y - dt ((hy + hz v) + theta u)
+//     dx'/d(hx, hy, hz, theta) = (-dt, 0, -dt u,  dt v)
+//     dy'/d(hx, hy, hz, theta) = (0, -dt, -dt v, -dt u)
+// in the order written (no FMA: the library builds with -fmad=false), f64 in parity mode, f32 in fast mode.
+// THE one place that turns an event into its bilinear footprint for these models: warp, bounds mask
+// (event_util.py:26-27), f64 -> f32 cast (image.py:180-183) and splat_taps -- the IWE pass and the gradient
+// pass call it alike, so they see identical taps.  JAC: also the f32 Jacobian rows jx[k] = dx'/dp_k, jy[k].
+__device__ __forceinline__ void sin_cos(double a, double *s, double *c) { sincos(a, s, c); }
+__device__ __forceinline__ void sin_cos(float a, float *s, float *c) { sincosf(a, s, c); }
+
+template <int WARP, bool JAC>
+__device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> &e, const WarpModel &M, unsigned &oob, Taps &T,
+                                           float (&jx)[4], float (&jy)[4])
+{
+    using R = typename EvT<WARP>::type;
+    R p = e.p;
+    if (A.p_scale != 1.0) p = p * (R)A.p_scale;
+    if (A.abs_polarity) p = fabs(p);
+    const R d = (sizeof(R) == 8) ? e.t - (R)A.t_ref : e.t;   // fast mode stores t - t_ref already
+    R xw, yw;
+    if (is_rotation(WARP)) {
+        const R cx = (R)M.m[0], cy = (R)M.m[1], om = (R)M.m[2];
+        R s, c;
+        sin_cos(om * d, &s, &c);
+        const R u = e.x - cx, v = e.y - cy;
+        const R rx = c * u + s * v, ry = c * v - s * u;
+        xw = cx + rx;
+        yw = cy + ry;
+        if (JAC) {
+            jx[0] = (float)((R)1 - c); jx[1] = (float)(-s); jx[2] = (float)(d * ry);
+            jy[0] = (float)s; jy[1] = (float)((R)1 - c); jy[2] = (float)(-(d * rx));
+            jx[3] = jy[3] = 0.0f;
+        }
+    } else {
+        const R hx = (R)M.m[0], hy = (R)M.m[1], hz = (R)M.m[2], th = (R)M.m[3], cx = (R)M.m[4], cy = (R)M.m[5];
+        const R u = e.x - cx, v = e.y - cy;
+        xw = e.x - d * ((hx + hz * u) - th * v);
+        yw = e.y - d * ((hy + hz * v) + th * u);
+        if (JAC) {
+            jx[0] = (float)(-d); jx[1] = 0.0f; jx[2] = (float)(-(d * u)); jx[3] = (float)(d * v);
+            jy[0] = 0.0f; jy[1] = (float)(-d); jy[2] = (float)(-(d * v)); jy[3] = (float)(-(d * u));
+        }
+    }
+    // event_util.py:26-27: keep iff 0 < x' <= Wm and 0 < y' <= Hm (NaN compares false -> kept)
+    const bool keep = !(xw <= (R)0 || xw > (R)A.Wm) && !(yw <= (R)0 || yw > (R)A.Hm);
+    if (!keep) return false;
+    return splat_taps<false>(A, (float)xw, (float)yw, (float)p, 0.0f, true, oob, T);
+}
+
+// pass 1 of the motion models: the IWE only, through the same two accumulator back ends as linvel
+template <int WARP, bool ONCHIP>
+__device__ __forceinline__ void model_splat(const CmaxArgs &A, float *acc, const Event<WARP> &e, unsigned &oob, const WarpModel &M,
+                                            unsigned *simg)
+{
+    Taps T;
+    float jx[4], jy[4];
+    if (!model_taps<WARP, false>(A, e, M, oob, T, jx, jy)) return;
+    if (ONCHIP && fabsf(T.wm) <= 1.0f) {
+        const int r0 = T.y0 * A.Wc, r1 = T.y1 * A.Wc;
+        onchip_taps(simg, acc, r0 + T.x0, r0 + T.x1, r1 + T.x0, r1 + T.x1, T.ti);
+    } else {
+        emit_global<true, false>(A, acc, T);
+    }
+}
+
 template <int WARP, bool GRAD, bool ONCHIP = false>
 __device__ __forceinline__ void cmax_event(const CmaxArgs &A, float *acc, const Event<WARP> &e, unsigned &oob, double cvx,
                                            double cvy, unsigned *simg = nullptr)
 {
+    if constexpr (is_model_warp(WARP)) {
+        model_splat<WARP, ONCHIP>(A, acc, e, oob, A.model, simg);   // IWE pass only: the gradient is cmax_grad_pass_kernel
+        return;
+    }
     if (WARP == WARP_LINVEL_F64) {
         const double x = e.x, y = e.y, t = e.t;
         double p = e.p;
@@ -370,7 +462,7 @@ __global__ void __launch_bounds__(kOnchipThreads, 1) cmax_onchip_kernel(const Cm
         }
         for (int64_t j = nv * EPV + i; j < A.n; j += stride) cmax_event<WARP, GRAD, true>(A, acc, load_event<WARP>(A, j), oob, A.vx, A.vy, simg);
     } else {
-        constexpr int kB = (WARP == WARP_LINVEL_F64) ? 2 : 4;   // loads in flight per thread (64-register budget at 1024 threads)
+        constexpr int kB = (sizeof(typename EvT<WARP>::type) == 8) ? 2 : 4;   // loads in flight per thread (64-register budget at 1024 threads)
         for (; i + (kB - 1) * stride < A.n; i += kB * stride) {
             Event<WARP> ev[kB];
 #pragma unroll
@@ -426,6 +518,93 @@ __global__ void __launch_bounds__(256) cmax_scatter_batch_kernel(const CmaxArgs 
         }
     }
     flush_oob(A.oob, oob);
+}
+
+// The same for the rotation / 4-DoF models: K parameter points per pass over the events, f only
+struct ModelCandidates {
+    int n;
+    WarpModel m[kMaxCandidates];
+};
+
+template <int WARP>
+__global__ void __launch_bounds__(256) cmax_model_batch_kernel(const CmaxArgs A, const ModelCandidates C)
+{
+    unsigned oob = 0;
+    const int64_t acc_stride = (int64_t)A.Hc * A.Wc * kBlockFloats;
+    const int64_t stride = (int64_t)gridDim.x * 256;
+    for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < A.n; i += 2 * stride) {
+        const Event<WARP> e0 = load_event<WARP>(A, i);
+        const bool has1 = i + stride < A.n;
+        const Event<WARP> e1 = has1 ? load_event<WARP>(A, i + stride) : e0;
+        for (int k = 0; k < C.n; ++k) {
+            float *acc = A.acc + k * acc_stride;
+            model_splat<WARP, false>(A, acc, e0, oob, C.m[k], nullptr);
+            if (has1) model_splat<WARP, false>(A, acc, e1, oob, C.m[k], nullptr);
+        }
+    }
+    flush_oob(A.oob, oob);
+}
+
+// ---- pass 2 of the motion models: the gradient, GATHERED from one image instead of scattered into K --------
+// Every objective's gradient is g_k = s * sum_pix C * G(D_k) with a per-pixel coefficient image C (2(I - mu) for the
+// variance, 2I for sos, exp(G) for soe, ...) and D_k the derivative splat of image.py:131-135 with w1 = jx_k wm,
+// w2 = jy_k wm.  G is self-adjoint, so g_k = s * sum_pix W D_k with W = G(C), and per event the four taps of D_k
+// against W are
+//   Sx = oy (W01 - W00) + dy (W11 - W10)      Sy = ox (W10 - W00) + dx (W11 - W01)      U_k += wm (jx_k Sx + jy_k Sy)
+// One persistent CTA per SM holds W (f32, the 174 KB of a 181x241 canvas) in shared memory, recomputes each event's
+// warp and footprint (model_taps, as pass 1), gathers four shared-memory values and sums K products per thread in
+// f64; no reduction per event whatever K is.
+constexpr int kGradThreads = 512;
+
+template <int WARP>
+__global__ void __launch_bounds__(kGradThreads, 1) cmax_grad_pass_kernel(const CmaxArgs A, const float *__restrict__ W, double *U)
+{
+    constexpr int K = model_dims(WARP);
+    extern __shared__ __align__(16) float sW[];
+    __shared__ double part[kGradThreads / 32][K];
+    const int npix = A.Hc * A.Wc;
+    for (int j = threadIdx.x; j < npix; j += kGradThreads) sW[j] = W[j];
+    __syncthreads();
+    double u[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) u[k] = 0.0;
+    unsigned oob = 0;   // counted by pass 1
+    auto one = [&](const Event<WARP> &e) {
+        Taps T;
+        float jx[4], jy[4];
+        if (!model_taps<WARP, true>(A, e, A.model, oob, T, jx, jy)) return;
+        const int r0 = T.y0 * A.Wc, r1 = T.y1 * A.Wc;
+        const double w00 = sW[r0 + T.x0], w01 = sW[r0 + T.x1], w10 = sW[r1 + T.x0], w11 = sW[r1 + T.x1];
+        const double dx = T.dx, dy = T.dy, ox = 1.0 - dx, oy = 1.0 - dy, wm = T.wm;
+        const double sx = oy * (w01 - w00) + dy * (w11 - w10);
+        const double sy = ox * (w10 - w00) + dx * (w11 - w01);
+#pragma unroll
+        for (int k = 0; k < K; ++k) u[k] += wm * ((double)jx[k] * sx + (double)jy[k] * sy);
+    };
+    const int64_t stride = (int64_t)gridDim.x * kGradThreads;
+    int64_t i = (int64_t)blockIdx.x * kGradThreads + threadIdx.x;
+    for (; i + 3 * stride < A.n; i += 4 * stride) {
+        Event<WARP> ev[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) ev[k] = load_event<WARP>(A, i + k * stride);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) one(ev[k]);
+    }
+    for (; i < A.n; i += stride) one(load_event<WARP>(A, i));
+    // CTA reduction, one f64 atomic per component and CTA
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        double v = u[k];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) part[wid][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        double s = 0.0;
+        for (int w = 0; w < kGradThreads / 32; ++w) s += part[w][threadIdx.x];
+        atomicAdd(U + threadIdx.x, s);
+    }
 }
 
 // ---- image-space tail (43.6 K pixels; negligible next to the event pass) ------------------
@@ -707,6 +886,95 @@ __global__ void cmax_obj_final_kernel(int kind, const double *gsums, const unsig
     result[11] = gsums[3];
 }
 
+// ---- image-space tail of the motion models: f, the side values and the gradient pass's W = G(C) -----------
+// gsums: 0 sum(G^2) (f32 products)  1 sum(exp(G))  2 sum(exp(-p G))  3 #(G > thresh)  4 sum(G)  5 sum(G^2) (f64 products)
+// The variance's C = 2(I - mu) blurs to 2(G - mu); the mean drops out of the gradient (the four derivative taps of an
+// event sum to zero), so W = 2G, written here.  The other objectives leave C in w (f64) for one more blur.
+__global__ void __launch_bounds__(256) cmax_model_stats_kernel(const float *__restrict__ G, const float *__restrict__ I, int npix,
+                                                               int kind, double param, double *gsums, unsigned *gmax,
+                                                               double *__restrict__ w, float *__restrict__ Wvar)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    double g2 = 0.0, ge = 0.0, ga = 0.0, gc = 0.0, g1 = 0.0, gd2 = 0.0;
+    float mx = -FLT_MAX;
+    if (i < npix) {
+        const float g = G[i];
+        const double gd = (double)g;
+        g1 = gd;
+        gd2 = gd * gd;
+        g2 = (double)(g * g);
+        if (kind == OBJ_SOE) ge = exp(gd);
+        if (kind == OBJ_SOSA) ga = exp(-param * gd);
+        if (kind == OBJ_ISOA) gc = (g > (float)param) ? 1.0 : 0.0;
+        mx = g;
+        if (kind == OBJ_VARIANCE) {
+            if (Wvar) Wvar[i] = 2.0f * g;
+        } else if (w) {
+            double wi = 0.0;
+            if (kind == OBJ_SOS) wi = (double)(I[i] * 2.0f);
+            else if (kind == OBJ_SOE) wi = ge;
+            else if (kind == OBJ_ISOA) wi = gc;
+            else if (kind == OBJ_SOSA) wi = -param * exp((double)(float)(-param * gd));
+            w[i] = wi;
+        }
+    }
+    block_add(g2, gsums + 0);
+    if (kind == OBJ_SOE) block_add(ge, gsums + 1);
+    if (kind == OBJ_SOSA) block_add(ga, gsums + 2);
+    if (kind == OBJ_ISOA) block_add(gc, gsums + 3);
+    block_add(g1, gsums + 4);
+    block_add(gd2, gsums + 5);
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(gmax, encode_ordered(mx));
+}
+
+// W = G(w) along axis 1 (after cmax_blur_d_axis0_kernel), stored as f32 for the gradient pass
+__global__ void __launch_bounds__(256) cmax_blur_d_axis1_store_kernel(const double *__restrict__ wt, const double *__restrict__ w,
+                                                                      int Hc, int Wc, const BlurTaps taps, int do_blur,
+                                                                      float *__restrict__ Wout)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= Hc * Wc) return;
+    double gw;
+    if (do_blur) {
+        const int y = i / Wc, x = i - y * Wc;
+        const double *row = wt + y * Wc;
+        gw = row[x] * taps.w[0];
+        for (int k = 1; k <= taps.r; ++k) gw += (row[reflect_idx(x - k, Wc)] + row[reflect_idx(x + k, Wc)]) * taps.w[k];
+    } else {
+        gw = w[i];
+    }
+    Wout[i] = (float)gw;
+}
+
+// result (16 doubles): [0] f  [1..4] g (zero past dims)  [5] sum(IWE)  [6] events outside the canvas
+//                      [7] mean(G)  [8] mean(G^2)  [9] sum(exp(-p G))  [10] max(G)  [11] #(G > thresh)  [12..15] 0
+__global__ void cmax_model_final_kernel(int kind, const double *gsums, const unsigned *gmax, const double *sums,
+                                        const unsigned long long *oob, int npix, const double *U, int dims, int want_grad,
+                                        double *result)
+{
+    const double P = (double)npix;
+    const double mx = (double)decode_ordered(*gmax);
+    double f = 0.0, c = 0.0;
+    if (kind == OBJ_VARIANCE) { const double m = gsums[4] / P; f = -(gsums[5] / P - m * m); c = 1.0 / P; }
+    else if (kind == OBJ_SOS) { f = -gsums[0] / P; c = 1.0 / P; }
+    else if (kind == OBJ_SOE) { f = -gsums[1] / P; c = 1.0 / P; }
+    else if (kind == OBJ_MOA) { f = -mx; c = 0.0; }
+    else if (kind == OBJ_ISOA) { f = gsums[3]; c = 1.0; }
+    else if (kind == OBJ_SOSA) { f = -gsums[2]; c = 1.0; }
+    const bool grad = want_grad && kind != OBJ_MOA;
+    result[0] = f;
+    for (int k = 0; k < 4; ++k) result[1 + k] = (grad && k < dims) ? -c * U[k] : 0.0;
+    result[5] = sums[0];
+    result[6] = (double)(*oob);
+    result[7] = gsums[4] / P;
+    result[8] = gsums[0] / P;
+    result[9] = gsums[2];
+    result[10] = mx;
+    result[11] = gsums[3];
+    for (int k = 12; k < 16; ++k) result[k] = 0.0;
+}
+
 // ---- fused variance tail: gather + both blur axes + all sums + the final scalars in ONE launch ---
 // One CTA = an 8x32 tile of pixels.  It gathers the tile plus a halo of `r` pixels (reflected at the image
 // border, like scipy's mode='reflect') straight from the block accumulator into shared memory, blurs
@@ -985,23 +1253,14 @@ static int64_t onchip_min_events()
     return v;
 }
 
-// partial_images != nullptr: stop after the event pass and leave this rank's planar I, D0, D1 ([3][Hc*Wc]) and its
-// out-of-canvas count there (the sharded evaluation's first half; evk_cmax_peer_tail_f32 is the second)
+// The event pass (pass 1): the on-chip fixed-point IWE from onchip_min_events() events up, the L2 block accumulator below
+// that (EVK_VARIANT_SMEM_TILE / EVK_VARIANT_VECTOR_RED force one or the other).  Zeroes the counters, the planar image and
+// the accumulator replicas it uses; leaves the replica count in A.replicas and the planar image (or null) in A.planar.
 template <int WARP>
-static int run_cmax(CmaxArgs A, double sigma, unsigned flags, int objective, double obj_param, double *result,
-                    float *iwe_out, float *diwe_out, void *workspace, size_t workspace_bytes, cudaStream_t st,
-                    float *partial_images = nullptr, unsigned long long *partial_oob = nullptr)
+static int launch_event_pass(CmaxArgs &A, unsigned flags, bool grad, const CmaxWorkspace &ws, cudaStream_t st)
 {
     const int Hs = A.Hc - 1, Ws = A.Wc - 1;
-    if (A.n < 0 || Hs < 1 || Ws < 1 || (!result && !partial_images) || !workspace) { set_error("evk_cmax: bad arguments"); return EVK_E_ARG; }
-    if (((uintptr_t)workspace & 255) != 0) { set_error("evk_cmax: workspace must be 256-byte aligned"); return EVK_E_ARG; }
-    CmaxWorkspace ws;
-    const size_t need = carve(workspace, Hs, Ws, &ws);
-    if (workspace_bytes < need) { set_error("evk_cmax: workspace of %zu bytes required, %zu given", need, workspace_bytes); return EVK_E_WORKSPACE; }
     const int npix = A.Hc * A.Wc;
-    const bool grad = (flags & EVK_CMAX_WANT_GRAD) != 0 && WARP != WARP_FLOW_F32;
-    A.abs_polarity = (flags & EVK_CMAX_ABS_POLARITY) ? 1 : 0;
-    // replicas spread same-address serialisation in L2; small problems do not need them
     int R = (int)(A.n / (1 << 20));
     R = R < 1 ? 1 : (R > kMaxReplicas ? kMaxReplicas : R);
     A.replicas = R;
@@ -1016,7 +1275,6 @@ static int run_cmax(CmaxArgs A, double sigma, unsigned flags, int objective, dou
     if (variant == EVK_VARIANT_VECTOR_RED || variant == EVK_VARIANT_GLOBAL_RED) onchip = false;
     A.planar = onchip ? ws.planar : nullptr;
     A.vec16 = ((((uintptr_t)A.x | (uintptr_t)A.y | (uintptr_t)A.t | (uintptr_t)A.p) & 15) == 0) ? 1 : 0;
-    const float *planar = A.planar;
     if (onchip && !grad) { R = 1; A.replicas = 1; }   // the blocks only receive carries and slow-path taps
     // counters (gsums, gmax, sums, oob), the planar image and the R accumulator replicas are contiguous: one memset
     EVK_CUDA(cudaMemsetAsync(ws.gsums, 0, (size_t)((char *)ws.acc - (char *)ws.gsums) + (size_t)R * npix * kBlockFloats * sizeof(float), st));
@@ -1045,6 +1303,30 @@ static int run_cmax(CmaxArgs A, double sigma, unsigned flags, int objective, dou
         if (grad) cmax_scatter_kernel<WARP, true><<<grid_for(cmax_scatter_kernel<WARP, true>, 256, A.n, 256 * 4), 256, 0, st>>>(A);
         else cmax_scatter_kernel<WARP, false><<<grid_for(cmax_scatter_kernel<WARP, false>, 256, A.n, 256 * 4), 256, 0, st>>>(A);
     }
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+// partial_images != nullptr: stop after the event pass and leave this rank's planar I, D0, D1 ([3][Hc*Wc]) and its
+// out-of-canvas count there (the sharded evaluation's first half; evk_cmax_peer_tail_f32 is the second)
+template <int WARP>
+static int run_cmax(CmaxArgs A, double sigma, unsigned flags, int objective, double obj_param, double *result,
+                    float *iwe_out, float *diwe_out, void *workspace, size_t workspace_bytes, cudaStream_t st,
+                    float *partial_images = nullptr, unsigned long long *partial_oob = nullptr)
+{
+    const int Hs = A.Hc - 1, Ws = A.Wc - 1;
+    if (A.n < 0 || Hs < 1 || Ws < 1 || (!result && !partial_images) || !workspace) { set_error("evk_cmax: bad arguments"); return EVK_E_ARG; }
+    if (((uintptr_t)workspace & 255) != 0) { set_error("evk_cmax: workspace must be 256-byte aligned"); return EVK_E_ARG; }
+    CmaxWorkspace ws;
+    const size_t need = carve(workspace, Hs, Ws, &ws);
+    if (workspace_bytes < need) { set_error("evk_cmax: workspace of %zu bytes required, %zu given", need, workspace_bytes); return EVK_E_WORKSPACE; }
+    const int npix = A.Hc * A.Wc;
+    const bool grad = (flags & EVK_CMAX_WANT_GRAD) != 0 && WARP != WARP_FLOW_F32;
+    A.abs_polarity = (flags & EVK_CMAX_ABS_POLARITY) ? 1 : 0;
+    int rc = launch_event_pass<WARP>(A, flags, grad, ws, st);
+    if (rc) return rc;
+    const int R = A.replicas;
+    const float *planar = A.planar;
     if (partial_images) {
         prof_count(1);
         cmax_gather_kernel<<<(npix + 255) / 256, 256, 0, st>>>(ws.acc, planar, R, A.Hc, A.Wc, partial_images, partial_images + npix,
@@ -1072,6 +1354,88 @@ static int run_cmax(CmaxArgs A, double sigma, unsigned flags, int objective, dou
     prof_count(1);
     cmax_gather_kernel<<<(npix + 255) / 256, 256, 0, st>>>(ws.acc, planar, R, A.Hc, A.Wc, ws.I, ws.D0, ws.D1, iwe_out, diwe_out, ws.sums);
     return launch_tail(ws, A.Hc, A.Wc, sigma, flags, objective, obj_param, grad, result, st);
+}
+
+// Image-space tail of the motion models on the gathered IWE ws.I: blur, f and the side values into gsums / gmax, and
+// (W_out != nullptr) the gradient pass's W = G(C) as f32 into W_out.
+static int model_tail(const CmaxWorkspace &ws, int Hc, int Wc, double sigma, int objective, double obj_param, float *W_out,
+                      cudaStream_t st)
+{
+    const int npix = Hc * Wc;
+    BlurTaps taps{};
+    const int do_blur = sigma > 0.0;
+    if (do_blur) {
+        int rc = make_taps(sigma, &taps);
+        if (rc) return rc;
+    }
+    const int g = (npix + 255) / 256;
+    prof_count(do_blur ? 3 : 2);
+    if (do_blur) cmax_blur_axis0_kernel<<<g, 256, 0, st>>>(ws.I, ws.tmp, Hc, Wc, taps);
+    cmax_blur_axis1_store_kernel<<<g, 256, 0, st>>>(ws.tmp, ws.I, Hc, Wc, taps, do_blur, ws.G);
+    cmax_model_stats_kernel<<<g, 256, 0, st>>>(ws.G, ws.I, npix, objective, obj_param, ws.gsums, ws.gmax, W_out ? ws.w : nullptr, W_out);
+    if (W_out && objective != OBJ_VARIANCE) {
+        prof_count(do_blur ? 2 : 1);
+        if (do_blur) cmax_blur_d_axis0_kernel<<<g, 256, 0, st>>>(ws.w, ws.wt, Hc, Wc, taps);
+        cmax_blur_d_axis1_store_kernel<<<g, 256, 0, st>>>(ws.wt, ws.w, Hc, Wc, taps, do_blur, W_out);
+    }
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+// One evaluation of a motion model: pass 1 (IWE), the image-space tail, pass 2 (gradient) when asked for.
+// The derivative planes D0 / D1 of the workspace are not used by this path: D0 holds W, sums[1..4] the gradient sums U.
+template <int WARP>
+static int run_model(CmaxArgs A, double sigma, unsigned flags, int objective, double obj_param, double *result, float *iwe_out,
+                     void *workspace, size_t workspace_bytes, cudaStream_t st)
+{
+    const int Hs = A.Hc - 1, Ws = A.Wc - 1;
+    if (A.n < 0 || Hs < 1 || Ws < 1 || !result || !workspace) { set_error("evk_cmax_warp: bad arguments"); return EVK_E_ARG; }
+    if (((uintptr_t)workspace & 255) != 0) { set_error("evk_cmax_warp: workspace must be 256-byte aligned"); return EVK_E_ARG; }
+    if (objective < OBJ_VARIANCE || objective > OBJ_SOSA) { set_error("evk_cmax_warp: unknown objective %d", objective); return EVK_E_ARG; }
+    CmaxWorkspace ws;
+    const size_t need = carve(workspace, Hs, Ws, &ws);
+    if (workspace_bytes < need) { set_error("evk_cmax_warp: workspace of %zu bytes required, %zu given", need, workspace_bytes); return EVK_E_WORKSPACE; }
+    const int npix = A.Hc * A.Wc;
+    const size_t w_smem = (size_t)npix * sizeof(float);
+    const bool grad = (flags & EVK_CMAX_WANT_GRAD) != 0 && objective != OBJ_MOA;
+    if (grad && w_smem > (size_t)200 * 1024) {
+        set_error("evk_cmax_warp: the gradient pass holds the %dx%d canvas in shared memory (at most 200 KB)", A.Hc, A.Wc);
+        return EVK_E_UNSUPPORTED;
+    }
+    A.abs_polarity = (flags & EVK_CMAX_ABS_POLARITY) ? 1 : 0;
+    int rc = launch_event_pass<WARP>(A, flags, false, ws, st);
+    if (rc) return rc;
+    prof_count(1);
+    cmax_gather_kernel<<<(npix + 255) / 256, 256, 0, st>>>(ws.acc, A.planar, A.replicas, A.Hc, A.Wc, ws.I, ws.D0, ws.D1, iwe_out, nullptr, ws.sums);
+    rc = model_tail(ws, A.Hc, A.Wc, sigma, objective, obj_param, grad ? ws.D0 : nullptr, st);
+    if (rc) return rc;
+    double *U = ws.sums + 1;
+    if (grad && A.n > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        int64_t need_ctas = (A.n + kGradThreads * 8 - 1) / (kGradThreads * 8);
+        const int g = (int)(need_ctas < num_sms() ? need_ctas : num_sms());
+        EVK_CUDA(cudaFuncSetAttribute(cmax_grad_pass_kernel<WARP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)w_smem));
+        cmax_grad_pass_kernel<WARP><<<g, kGradThreads, w_smem, st>>>(A, ws.D0, U);
+        EVK_CUDA(cudaGetLastError());
+    }
+    cmax_model_final_kernel<<<1, 1, 0, st>>>(objective, ws.gsums, ws.gmax, ws.sums, ws.oob, npix, U, model_dims(WARP), grad ? 1 : 0, result);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+// host model array -> WarpModel (rotation: 3 doubles, xyztheta: 6)
+static int read_model(int warp, const double *model, WarpModel *M, int *n_doubles)
+{
+    if (!model) { set_error("evk_cmax_warp: null model"); return EVK_E_ARG; }
+    int nd;
+    if (warp == EVK_WARP_ROTATION) nd = 3;
+    else if (warp == EVK_WARP_XYZTHETA) nd = 6;
+    else { set_error("evk_cmax_warp: unknown warp %d", warp); return EVK_E_ARG; }
+    *M = WarpModel{};
+    for (int k = 0; k < nd; ++k) M->m[k] = model[k];
+    if (n_doubles) *n_doubles = nd;
+    return EVK_OK;
 }
 
 // precomputed planar iwe / diwe -> the planar working images + their sums (the block accumulator is
@@ -1334,6 +1698,100 @@ int evk_cmax_linvel_objective_batch_f64(const double *x, const double *y, const 
                                                                 ws.D1, nullptr, nullptr, ws.sums);
         int rc = launch_tail(ws, A.Hc, A.Wc, sigma, flags, objective, obj_param, grad, results + 12 * k, st);
         if (rc) return rc;
+    }
+    return EVK_OK;
+}
+
+int evk_cmax_warp_objective_f64(const double *x, const double *y, const double *t, const double *p, int64_t n, double p_scale,
+                                int warp, const double *model, double t_ref, int Hm, int Wm, int Hs, int Ws, double sigma,
+                                unsigned flags, int objective, double obj_param, double *result, float *iwe_out,
+                                void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    if (n > 0 && (!x || !y || !t || !p)) { set_error("evk_cmax_warp_objective_f64: null event array"); return EVK_E_ARG; }
+    CmaxArgs A{};
+    int rc = read_model(warp, model, &A.model, nullptr);
+    if (rc) return rc;
+    A.x = x; A.y = y; A.t = t; A.p = p; A.n = n;
+    A.t_ref = t_ref; A.p_scale = p_scale;
+    A.Hm = Hm; A.Wm = Wm; A.Hc = Hs + 1; A.Wc = Ws + 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (warp == EVK_WARP_ROTATION)
+        return run_model<WARP_ROTATION_F64>(A, sigma, flags, objective, obj_param, result, iwe_out, workspace, workspace_bytes, st);
+    return run_model<WARP_XYZTHETA_F64>(A, sigma, flags, objective, obj_param, result, iwe_out, workspace, workspace_bytes, st);
+}
+
+int evk_cmax_warp_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, int64_t n, float p_scale,
+                                int warp, const double *model, int Hm, int Wm, int Hs, int Ws, double sigma, unsigned flags,
+                                int objective, double obj_param, double *result, float *iwe_out, void *workspace,
+                                size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    if (n > 0 && (!x || !y || !t_rel || !p)) { set_error("evk_cmax_warp_objective_f32: null event array"); return EVK_E_ARG; }
+    CmaxArgs A{};
+    int rc = read_model(warp, model, &A.model, nullptr);
+    if (rc) return rc;
+    A.x = x; A.y = y; A.t = t_rel; A.p = p; A.n = n;
+    A.t_ref = 0.0; A.p_scale = p_scale;
+    A.Hm = Hm; A.Wm = Wm; A.Hc = Hs + 1; A.Wc = Ws + 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (warp == EVK_WARP_ROTATION)
+        return run_model<WARP_ROTATION_F32>(A, sigma, flags, objective, obj_param, result, iwe_out, workspace, workspace_bytes, st);
+    return run_model<WARP_XYZTHETA_F32>(A, sigma, flags, objective, obj_param, result, iwe_out, workspace, workspace_bytes, st);
+}
+
+int evk_cmax_warp_objective_batch_f64(const double *x, const double *y, const double *t, const double *p, int64_t n,
+                                      double p_scale, int warp, const double *models_host, int n_models, double t_ref, int Hm,
+                                      int Wm, int Hs, int Ws, double sigma, unsigned flags, int objective, double obj_param,
+                                      double *results, void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    if (n < 0 || (n > 0 && (!x || !y || !t || !p)) || !models_host || n_models < 1 || n_models > kMaxCandidates || !results ||
+        !workspace || Hs < 1 || Ws < 1) {
+        set_error("evk_cmax_warp_objective_batch_f64: bad arguments (1 <= n_models <= %d)", kMaxCandidates);
+        return EVK_E_ARG;
+    }
+    if (objective < OBJ_VARIANCE || objective > OBJ_SOSA) { set_error("evk_cmax_warp: unknown objective %d", objective); return EVK_E_ARG; }
+    if (((uintptr_t)workspace & 255) != 0) { set_error("evk_cmax_warp batch: workspace must be 256-byte aligned"); return EVK_E_ARG; }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CmaxWorkspace ws;
+    const size_t need = carve(workspace, Hs, Ws, &ws);
+    if (workspace_bytes < need) { set_error("evk_cmax_warp batch: workspace of %zu bytes required", need); return EVK_E_WORKSPACE; }
+    ModelCandidates C{};
+    C.n = n_models;
+    int nd = 0;
+    for (int k = 0; k < n_models; ++k) {
+        int rc = read_model(warp, models_host + (size_t)k * (warp == EVK_WARP_ROTATION ? 3 : 6), &C.m[k], &nd);
+        if (rc) return rc;
+    }
+    CmaxArgs A{};
+    A.x = x; A.y = y; A.t = t; A.p = p; A.n = n;
+    A.t_ref = t_ref; A.p_scale = p_scale;
+    A.Hm = Hm; A.Wm = Wm; A.Hc = Hs + 1; A.Wc = Ws + 1;
+    A.abs_polarity = (flags & EVK_CMAX_ABS_POLARITY) ? 1 : 0;
+    A.replicas = 1; A.acc = ws.acc; A.oob = ws.oob;
+    const int npix = A.Hc * A.Wc;
+    // bsums, btickets, gsums, gmax, sums, oob and the accumulators are contiguous: one memset
+    EVK_CUDA(cudaMemsetAsync(ws.bsums, 0, (size_t)((char *)ws.acc - (char *)ws.bsums) + (size_t)n_models * npix * kBlockFloats * sizeof(float), st));
+    if (n > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        if (warp == EVK_WARP_ROTATION)
+            cmax_model_batch_kernel<WARP_ROTATION_F64><<<grid_for(cmax_model_batch_kernel<WARP_ROTATION_F64>, 256, n, 256 * 2), 256, 0, st>>>(A, C);
+        else
+            cmax_model_batch_kernel<WARP_XYZTHETA_F64><<<grid_for(cmax_model_batch_kernel<WARP_XYZTHETA_F64>, 256, n, 256 * 2), 256, 0, st>>>(A, C);
+        EVK_CUDA(cudaGetLastError());
+    }
+    for (int k = 0; k < n_models; ++k) {
+        // per-candidate image-space tail on the shared scratch images (stream-ordered); the oob counter is kept
+        EVK_CUDA(cudaMemsetAsync(ws.gsums, 0, (size_t)((char *)ws.oob - (char *)ws.gsums), st));
+        prof_count(1);
+        cmax_gather_kernel<<<(npix + 255) / 256, 256, 0, st>>>(ws.acc + (size_t)k * npix * kBlockFloats, nullptr, 1, A.Hc, A.Wc, ws.I, ws.D0,
+                                                                ws.D1, nullptr, nullptr, ws.sums);
+        int rc = model_tail(ws, A.Hc, A.Wc, sigma, objective, obj_param, nullptr, st);
+        if (rc) return rc;
+        cmax_model_final_kernel<<<1, 1, 0, st>>>(objective, ws.gsums, ws.gmax, ws.sums, ws.oob, npix, ws.sums + 1, 4, 0, results + 16 * k);
+        EVK_CUDA(cudaGetLastError());
     }
     return EVK_OK;
 }

@@ -381,6 +381,44 @@ int evk_iwe_objective_f32(const float *iwe, const float *diwe, int Hc, int Wc, d
                           unsigned flags, int objective, double obj_param, double *result,
                           void *workspace, size_t workspace_bytes, void *stream);
 
+/* Rotation and 4-DoF motion models: the reference declares xyztheta_warp and pure_rotation_warp
+ * (lib/contrast_max/warps.py:63-83) with empty warp(); contrast_max/warps.py defines them.  Same
+ * event pass as the linvel entries for the IWE (get_iwe objectives.py:184-192, events_bounds_mask
+ * event_util.py:26-27, events_to_image_drv image.py:179-217), then the objective of
+ * objectives.py:202-523 and, with EVK_CMAX_WANT_GRAD, its exact gradient from a SECOND pass over
+ * the events that gathers W = G(C) (C = the objective's coefficient image) at each event's four
+ * taps -- no derivative images are formed (interpolate_to_derivative_img image.py:131-135 is only
+ * contracted with W).  The gradient is not mixed across parameters (scipy's 3-D blur of the stack,
+ * objectives.py:253, has no meaning for a stack of other than 2 channels).
+ *   warp   : EVK_WARP_ROTATION,  model (host) = {cx, cy, omega}                 (dims 3)
+ *            EVK_WARP_XYZTHETA,  model (host) = {hx, hy, hz, theta, cx, cy}     (dims 4)
+ *   other arguments as evk_cmax_linvel_objective_*; the gradient pass needs (Hs+1)(Ws+1) <= 51200.
+ *   result : 16 doubles -- [0] f, [1..4] g (zero past dims), [5] sum(IWE), [6] events outside the
+ *            canvas, [7] mean(G), [8] mean(G^2), [9] sum(exp(-p G)), [10] max(G), [11] #(G > thresh).
+ *   iwe_out: optional (Hs+1)*(Ws+1) floats (the un-blurred IWE). */
+#define EVK_WARP_ROTATION 1
+#define EVK_WARP_XYZTHETA 2
+int evk_cmax_warp_objective_f64(const double *x, const double *y, const double *t, const double *p,
+                                int64_t n, double p_scale, int warp, const double *model,
+                                double t_ref, int Hm, int Wm, int Hs, int Ws, double sigma,
+                                unsigned flags, int objective, double obj_param, double *result,
+                                float *iwe_out, void *workspace, size_t workspace_bytes, void *stream);
+int evk_cmax_warp_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                int64_t n, float p_scale, int warp, const double *model, int Hm,
+                                int Wm, int Hs, int Ws, double sigma, unsigned flags, int objective,
+                                double obj_param, double *result, float *iwe_out, void *workspace,
+                                size_t workspace_bytes, void *stream);
+/* Up to 32 models per pass over the events, f only (grid_search_initial, events_cmax.py:241-311,
+ * samples 5^dims points per level): models_host = n_models consecutive models (3 or 6 doubles
+ * each, HOST memory); results: 16 doubles per model (layout above, g = 0).  result[6] counts the
+ * out-of-canvas events of all models together. */
+int evk_cmax_warp_objective_batch_f64(const double *x, const double *y, const double *t,
+                                      const double *p, int64_t n, double p_scale, int warp,
+                                      const double *models_host, int n_models, double t_ref, int Hm,
+                                      int Wm, int Hs, int Ws, double sigma, unsigned flags,
+                                      int objective, double obj_param, double *results,
+                                      void *workspace, size_t workspace_bytes, void *stream);
+
 /* scipy.ndimage.gaussian_filter(img, sigma) for a 2-D f32 image (truncate=4, mode='reflect', f64 line
  * accumulation, f32 store after each axis) -- the blur every objective applies (objectives.py:233 ...).
  * tmp: H*W floats of scratch; out may not alias img. */
