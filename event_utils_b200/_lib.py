@@ -155,6 +155,13 @@ def _declare(L):
     L.evk_cmax_peer_tail_f32.argtypes = [vp, vp, ci, ci, ci, f64, cu, vp, vp, sz, vp]
     L.evk_cmax_flow_variance_f32.restype = ci
     L.evk_cmax_flow_variance_f32.argtypes = [vp, vp, vp, vp, i64, vp, f32, ci, ci, f64, cu, vp, vp, vp, sz, vp]
+    L.evk_cmax_flow_objective_workspace_bytes.restype = sz
+    L.evk_cmax_flow_objective_workspace_bytes.argtypes = [ci, ci, ci]
+    L.evk_cmax_flow_objective_f32.restype = ci
+    L.evk_cmax_flow_objective_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, vp, ci, ci, f64, ci, f64, vp, vp, vp, sz, vp]
+    L.evk_cmax_flow_objective_grad_f32.restype = ci
+    L.evk_cmax_flow_objective_grad_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, vp, ci, ci, f64, ci, f64, vp, vp, vp, vp, sz,
+                                                   vp]
     L.evk_robust_norm_workspace_bytes.restype = sz
     L.evk_robust_norm_workspace_bytes.argtypes = []
     L.evk_robust_norm_f32.restype = ci

@@ -13,6 +13,7 @@ Which inputs get a gradient (as in the reference; the others get None):
     events_to_voxel_torch            ps, ts (voxel_grid.py:114-153); also through voxel_grids_fixed_n/_t_torch and
                                      events_to_voxel_timesync_torch
     events_to_neg_pos_voxel_torch    ts (voxel_grid.py:155-182)
+    flow_contrast_objective_torch    flow only (contrast_max/flow_objective.py; the events are data)
 
 The public functions take this path only when grad mode is on and one of those inputs requires grad; every
 other call runs the plain forward.  Gradients come back in each input's shape, dtype and device.  The
@@ -169,6 +170,49 @@ class WarpFlow(torch.autograd.Function):
         g_t0 = _as_input(-s, m[3]) if need[3] else None
         return (_as_input(gx, m[0]), _as_input(gy, m[1]), _as_input(gt, m[2]) if need[2] else None, g_t0,
                 _as_input(gf, m[4]) if need[4] else None, None)
+
+
+class FlowObjective(torch.autograd.Function):
+    """The batched dense-flow contrast objective of contrast_max/flow_objective.py (draw_flow.py:15-26 followed by an
+    objective of objectives.py): f (B,) f64 from flow (B,2,H,W) and the prepared device events.  Only the flow gets a
+    gradient: the exact derivative of f, one pass over the events (evk_cmax_flow_objective_grad_f32)."""
+
+    @staticmethod
+    def forward(ctx, flow, x, y, t_rel, p, offsets, opts):
+        objective, sigma, param = opts
+        dev = x.device
+        B, _, H, W = flow.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            f32 = flow.detach().to(device=dev, dtype=torch.float32).contiguous()
+            f = torch.empty(B, dtype=torch.float64, device=dev)
+            iwe = torch.empty((B, H + 1, W + 1), dtype=torch.float32, device=dev)
+            ws = _lib.scratch("flow_objective", L.evk_cmax_flow_objective_workspace_bytes(B, H, W), dev)
+            _lib.check(L.evk_cmax_flow_objective_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0], _lib.ptr(f32),
+                H, W, sigma, objective, param, _lib.ptr(f), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(), _lib.stream()))
+        ctx.save_for_backward(x, y, t_rel, p, offsets, f32, iwe)
+        ctx.opts = opts
+        ctx.meta = _meta(flow)
+        return f
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, y, t_rel, p, offsets, f32, iwe = ctx.saved_tensors
+        objective, sigma, param = ctx.opts
+        dev = x.device
+        B, _, H, W = f32.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g = _grad_in(g, dev)
+            gf = torch.empty_like(f32)
+            ws = _lib.scratch("flow_objective", L.evk_cmax_flow_objective_workspace_bytes(B, H, W), dev)
+            _lib.check(L.evk_cmax_flow_objective_grad_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0], _lib.ptr(f32),
+                H, W, sigma, objective, param, _lib.ptr(iwe), _lib.ptr(g), _lib.ptr(gf), _lib.ptr(ws), ws.numel(),
+                _lib.stream()))
+        return _as_input(gf, ctx.meta), None, None, None, None, None, None
 
 
 class VoxelGrid(torch.autograd.Function):

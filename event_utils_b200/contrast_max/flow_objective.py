@@ -1,0 +1,86 @@
+"""Dense-flow contrast maximisation as a batched, differentiable torch loss.
+
+The loss of self-supervised optical-flow training: warp each sample's events by the flow the network predicts
+(warp_events_flow_torch, lib/transforms/optic_flow.py:37-44), form the bilinear image of warped events as the
+reference's motion_compensate does (lib/visualization/draw_flow.py:15-26) and score its contrast with an objective of
+lib/contrast_max/objectives.py.  One call evaluates a whole batch on the GPU (evk_cmax_flow_objective_f32) and its
+backward gives the exact gradient of the returned f with respect to the flow (evk_cmax_flow_objective_grad_f32).
+"""
+import torch
+
+from .. import _lib
+from ..representations import _events as E
+
+OBJECTIVES = {"variance": _lib.OBJ_VARIANCE, "sos": _lib.OBJ_SOS, "soe": _lib.OBJ_SOE, "sosa": _lib.OBJ_SOSA}
+DEFAULT_PARAM = {"sosa": 3.0}   # sosa_objective(p=3)
+
+
+def flow_contrast_objective_torch(xs, ys, ts, ps, flow, t0=None, objective="variance", blur_sigma=1.0, obj_param=None,
+                                  batch_end_indices=None):
+    """
+    Contrast objective f_b of every sample b of a batch of event windows warped by a dense flow.
+    Sample b holds the events [start_b, end_b) of the concatenated stream, end_b = batch_end_indices[b] and start_b the
+    previous end (0 for the first sample), and is warped by flow[b]: x' = x + u(x,y) (t - t0_b), y' = y + v(x,y) (t - t0_b)
+    (grid_sample bilinear, zero padding, align_corners, optic_flow.py:37-44; t - t0_b is formed in ts' dtype, then f32).
+    The image of warped events is the bilinear events_to_image_torch canvas (H+1, W+1) with padding (draw_flow.py:18-21),
+    to which an event contributes iff 0 <= x' < W and 0 <= y' < H; other events are dropped (no IndexError, no wrap to
+    the opposite border).  An event whose warped position is not finite makes its sample's f NaN.  Then
+    G = gaussian_filter(image, blur_sigma) (0: no blur) and
+        variance  -var(G)        sos  -mean(G^2)        soe  -mean(exp G)        sosa  -sum(exp(-obj_param G))
+    ('moa' and 'isoa' are piecewise constant in the flow and are rejected).
+    @param xs, ys, ts, ps the concatenated events, (N,) tensors or arrays; they are data, not differentiable
+    @param flow (B,2,H,W) or (2,H,W) for one sample; the only differentiable input (expanded views work)
+    @param t0 None (each sample's last timestamp), a number, or B values
+    @param batch_end_indices the cumulative end indices of BaseVoxelDataset.collate_fn
+           (lib/data_loaders/base_dataset.py:513-539), a list or an int64 tensor; None means one sample of all events
+    @returns (B,) tensor of f in flow's dtype, on flow's device.  With every input already on the GPU neither the
+           forward nor the backward synchronises with the host.
+    """
+    if objective not in OBJECTIVES:
+        if objective in ("moa", "isoa"):
+            raise ValueError("objective %r is piecewise constant in the flow and has no gradient; use one of %s"
+                             % (objective, sorted(OBJECTIVES)))
+        raise ValueError("unknown objective %r (one of %s)" % (objective, sorted(OBJECTIVES)))
+    xs, ys, ts, ps = (E.as_tensor(a).reshape(-1) for a in (xs, ys, ts, ps))
+    if any(a.requires_grad for a in (xs, ys, ts, ps)) or (isinstance(t0, torch.Tensor) and t0.requires_grad):
+        raise ValueError("flow_contrast_objective_torch differentiates with respect to the flow only; the events and t0 "
+                         "must not require grad (detach them)")
+    flow = E.as_tensor(flow)
+    if flow.dim() == 3:
+        flow = flow.unsqueeze(0)
+    if flow.dim() != 4 or flow.shape[1] != 2:
+        raise ValueError("flow must have shape (B,2,H,W) or (2,H,W), got %s" % (tuple(flow.shape),))
+    B, H, W = flow.shape[0], flow.shape[2], flow.shape[3]
+    n = xs.shape[0]
+    if not (ys.shape[0] == ts.shape[0] == ps.shape[0] == n):
+        raise ValueError("xs, ys, ts, ps must have the same length")
+    _lib.lib()
+    dev = E.compute_device(flow, xs, ys, ts, ps)
+    with torch.cuda.device(dev):
+        if batch_end_indices is None:
+            ends = torch.full((1,), n, dtype=torch.int64, device=dev)
+        elif isinstance(batch_end_indices, torch.Tensor):
+            ends = batch_end_indices.reshape(-1).to(device=dev, dtype=torch.int64)
+        else:
+            ends = torch.tensor([int(e) for e in batch_end_indices], dtype=torch.int64).to(dev)
+        if ends.shape[0] != B:
+            raise ValueError("%d samples of events for a batch of %d flows" % (ends.shape[0], B))
+        offsets = torch.cat((torch.zeros(1, dtype=torch.int64, device=dev), ends))
+        x, y, p = (E.to_device(a, dev).to(torch.float32).contiguous() for a in (xs, ys, ps))
+        t = E.to_device(ts, dev)
+        rt = torch.result_type(t, 1.0)
+        t = t.to(rt)
+        if n == 0:
+            t_rel = torch.empty(0, dtype=torch.float32, device=dev)
+        else:
+            if t0 is None:
+                t0b = t[(ends - 1).clamp(0, n - 1)]                     # each sample's last event (as warp_events_flow_torch)
+            else:
+                t0b = torch.as_tensor(t0, dtype=rt).to(dev).reshape(-1).expand(B)
+            # the sample of each event: windows are contiguous, [ends[b-1], ends[b])
+            sample = torch.searchsorted(ends, torch.arange(n, device=dev), right=True).clamp_(max=B - 1)
+            t_rel = (t - t0b.to(rt)[sample]).to(torch.float32).contiguous()
+    from ..autograd import FlowObjective
+    param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
+    f = FlowObjective.apply(flow, x, y, t_rel, p, offsets, (OBJECTIVES[objective], float(blur_sigma), param))
+    return f.to(device=flow.device, dtype=flow.dtype)

@@ -332,6 +332,49 @@ __device__ __forceinline__ void model_splat(const CmaxArgs &A, float *acc, const
     }
 }
 
+// The flow at an event (optic_flow.py:37-44: normalise to [-1,1], grid_sample bilinear, zero padding, align_corners):
+// u, v, and the four grid_sample taps (x0, y0) .. (x0+1, y0+1) with their weights nw, ne, sw, se, which the backward
+// of the flow objective spreads its gradient over.  `sampled` is false for coordinates no tap can reach (u = v = 0).
+struct FlowSample {
+    int x0, y0;
+    float nw, ne, sw, se;
+    float u, v;
+    bool sampled;
+};
+
+template <bool INTERLEAVED>
+__device__ __forceinline__ FlowSample flow_sample(const float *flow, const float2 *uv, int H, int W, float xe, float ye)
+{
+    FlowSample s;
+    const float wm1 = (float)(W - 1), hm1 = (float)(H - 1);
+    const float gx = __fsub_rn(__fmul_rn(__fdiv_rn(xe, wm1), 2.0f), 1.0f);
+    const float gy = __fsub_rn(__fmul_rn(__fdiv_rn(ye, hm1), 2.0f), 1.0f);
+    const float ix = __fmul_rn(__fdiv_rn(__fadd_rn(gx, 1.0f), 2.0f), wm1);
+    const float iy = __fmul_rn(__fdiv_rn(__fadd_rn(gy, 1.0f), 2.0f), hm1);
+    float u = 0.0f, v = 0.0f;
+    s.sampled = fabsf(ix) < 1.0e9f && fabsf(iy) < 1.0e9f;
+    s.x0 = s.y0 = 0;
+    s.nw = s.ne = s.sw = s.se = 0.0f;
+    if (s.sampled) {
+        const float fx = floorf(ix), fy = floorf(iy);
+        const int x0 = (int)fx, y0 = (int)fy;
+        const float xs = fx + 1.0f, ys = fy + 1.0f;
+        const float nw = __fmul_rn(__fsub_rn(xs, ix), __fsub_rn(ys, iy));
+        const float ne = __fmul_rn(__fsub_rn(ix, fx), __fsub_rn(ys, iy));
+        const float sw = __fmul_rn(__fsub_rn(xs, ix), __fsub_rn(iy, fy));
+        const float se = __fmul_rn(__fsub_rn(ix, fx), __fsub_rn(iy, fy));
+        const float4 top = flow_row<INTERLEAVED>(flow, uv, H, W, y0, x0), bot = flow_row<INTERLEAVED>(flow, uv, H, W, y0 + 1, x0);
+        u = __fadd_rn(u, __fmul_rn(top.x, nw)); v = __fadd_rn(v, __fmul_rn(top.y, nw));
+        u = __fadd_rn(u, __fmul_rn(top.z, ne)); v = __fadd_rn(v, __fmul_rn(top.w, ne));
+        u = __fadd_rn(u, __fmul_rn(bot.x, sw)); v = __fadd_rn(v, __fmul_rn(bot.y, sw));
+        u = __fadd_rn(u, __fmul_rn(bot.z, se)); v = __fadd_rn(v, __fmul_rn(bot.w, se));
+        s.x0 = x0; s.y0 = y0;
+        s.nw = nw; s.ne = ne; s.sw = sw; s.se = se;
+    }
+    s.u = u; s.v = v;
+    return s;
+}
+
 template <int WARP, bool GRAD, bool ONCHIP = false>
 __device__ __forceinline__ void cmax_event(const CmaxArgs &A, float *acc, const Event<WARP> &e, unsigned &oob, double cvx,
                                            double cvy, unsigned *simg = nullptr)
@@ -370,27 +413,8 @@ __device__ __forceinline__ void cmax_event(const CmaxArgs &A, float *acc, const 
         const float xe = e.x, ye = e.y, te = e.t;
         float p = e.p;
         if (A.abs_polarity) p = fabsf(p);
-        const int H = A.Hc - 1, W = A.Wc - 1;
-        const float wm1 = (float)(W - 1), hm1 = (float)(H - 1);
-        const float gx = __fsub_rn(__fmul_rn(__fdiv_rn(xe, wm1), 2.0f), 1.0f);
-        const float gy = __fsub_rn(__fmul_rn(__fdiv_rn(ye, hm1), 2.0f), 1.0f);
-        const float ix = __fmul_rn(__fdiv_rn(__fadd_rn(gx, 1.0f), 2.0f), wm1);
-        const float iy = __fmul_rn(__fdiv_rn(__fadd_rn(gy, 1.0f), 2.0f), hm1);
-        float u = 0.0f, v = 0.0f;
-        if (fabsf(ix) < 1.0e9f && fabsf(iy) < 1.0e9f) {
-            const float fx = floorf(ix), fy = floorf(iy);
-            const int x0 = (int)fx, y0 = (int)fy;
-            const float xs = fx + 1.0f, ys = fy + 1.0f;
-            const float nw = __fmul_rn(__fsub_rn(xs, ix), __fsub_rn(ys, iy));
-            const float ne = __fmul_rn(__fsub_rn(ix, fx), __fsub_rn(ys, iy));
-            const float sw = __fmul_rn(__fsub_rn(xs, ix), __fsub_rn(iy, fy));
-            const float se = __fmul_rn(__fsub_rn(ix, fx), __fsub_rn(iy, fy));
-            const float4 top = flow_row<true>(A.flow, A.flow_uv, H, W, y0, x0), bot = flow_row<true>(A.flow, A.flow_uv, H, W, y0 + 1, x0);
-            u = __fadd_rn(u, __fmul_rn(top.x, nw)); v = __fadd_rn(v, __fmul_rn(top.y, nw));
-            u = __fadd_rn(u, __fmul_rn(top.z, ne)); v = __fadd_rn(v, __fmul_rn(top.w, ne));
-            u = __fadd_rn(u, __fmul_rn(bot.x, sw)); v = __fadd_rn(v, __fmul_rn(bot.y, sw));
-            u = __fadd_rn(u, __fmul_rn(bot.z, se)); v = __fadd_rn(v, __fmul_rn(bot.w, se));
-        }
+        const FlowSample s = flow_sample<true>(A.flow, A.flow_uv, A.Hc - 1, A.Wc - 1, xe, ye);
+        const float u = s.u, v = s.v;
         const float d = __fsub_rn(te, A.flow_t0);
         if (ONCHIP) splat_onchip<false>(A, acc, simg, __fadd_rn(xe, __fmul_rn(u, d)), __fadd_rn(ye, __fmul_rn(v, d)), p, 0.0f, true, oob);
         else splat<false>(A, acc, __fadd_rn(xe, __fmul_rn(u, d)), __fadd_rn(ye, __fmul_rn(v, d)), p, 0.0f, true, oob);
@@ -687,10 +711,14 @@ __device__ __forceinline__ int reflect_idx(int i, int n)
     return i < n ? i : period - 1 - i;
 }
 
-// scipy applies axis 0 first and rounds the intermediate to f32
+// scipy applies axis 0 first and rounds the intermediate to f32.
+// The image-space kernels below that take blockIdx.z treat it as the image index of a batch of images laid out one
+// after the other (the flow objective's samples); every other launch has gridDim.z = 1.
 __global__ void __launch_bounds__(256) cmax_blur_axis0_kernel(const float *__restrict__ I, float *__restrict__ tmp,
                                                               int Hc, int Wc, const BlurTaps taps)
 {
+    const size_t img = (size_t)blockIdx.z * Hc * Wc;
+    I += img; tmp += img;
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= Hc * Wc) return;
     const int y = i / Wc, x = i - y * Wc;
@@ -778,6 +806,8 @@ __global__ void __launch_bounds__(256) cmax_blur_axis1_store_kernel(const float 
                                                                     int Hc, int Wc, const BlurTaps taps, int do_blur,
                                                                     float *__restrict__ G)
 {
+    const size_t img = (size_t)blockIdx.z * Hc * Wc;
+    tmp += img; I += img; G += img;
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= Hc * Wc) return;
     if (!do_blur) { G[i] = I[i]; return; }
@@ -825,6 +855,8 @@ __global__ void __launch_bounds__(256) cmax_obj_reduce_kernel(const float *__res
 __global__ void __launch_bounds__(256) cmax_blur_d_axis0_kernel(const double *__restrict__ w, double *__restrict__ wt, int Hc,
                                                                 int Wc, const BlurTaps taps)
 {
+    const size_t img = (size_t)blockIdx.z * Hc * Wc;
+    w += img; wt += img;
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= Hc * Wc) return;
     const int y = i / Wc, x = i - y * Wc;
@@ -894,6 +926,10 @@ __global__ void __launch_bounds__(256) cmax_model_stats_kernel(const float *__re
                                                                int kind, double param, double *gsums, unsigned *gmax,
                                                                double *__restrict__ w, float *__restrict__ Wvar)
 {
+    const size_t img = (size_t)blockIdx.z * npix;
+    G += img; I += img; gsums += 8 * blockIdx.z; gmax += blockIdx.z;
+    if (w) w += img;
+    if (Wvar) Wvar += img;
     const int i = blockIdx.x * 256 + threadIdx.x;
     double g2 = 0.0, ge = 0.0, ga = 0.0, gc = 0.0, g1 = 0.0, gd2 = 0.0;
     float mx = -FLT_MAX;
@@ -933,6 +969,8 @@ __global__ void __launch_bounds__(256) cmax_blur_d_axis1_store_kernel(const doub
                                                                       int Hc, int Wc, const BlurTaps taps, int do_blur,
                                                                       float *__restrict__ Wout)
 {
+    const size_t img = (size_t)blockIdx.z * Hc * Wc;
+    wt += img; w += img; Wout += img;
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= Hc * Wc) return;
     double gw;
@@ -1456,6 +1494,263 @@ __global__ void __launch_bounds__(256) cmax_planar_kernel(const float *__restric
     block_add((double)c, sums + 6);
 }
 
+// ---- dense-flow objective over a batch of samples (evk_cmax_flow_objective_f32 / _grad_f32) -------------------------
+// Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by flow[b] (optic_flow.py:37-44), the bilinear
+// IWE of draw_flow.py:18-21 on the (H+1)x(W+1) canvas keeping only events with 0 <= x' < W and 0 <= y' < H, the blur and
+// one of the objectives of objectives.py:231-236, 308-400, 478-523.  The grid of both event passes is (slices, batch):
+// blockIdx.y is the sample, so no event searches for its sample and the launch count does not depend on the batch.
+//   forward:  one v4 reduction per kept event into the sample's 2x2-block image [B][Hc][Wc][4] (16 B per pixel)
+//   backward: W = g_b G(C_b) per sample (C = df/dG), then per event the four taps of W (L2 gathers) give df/dx', df/dy';
+//             times d they are spread over the event's four grid_sample taps: two v4 reductions into the 2x2-block
+//             flow gradient [B][2][H][W][4] of evk_warp_flow_grad_f32.
+struct FlowObjArgs {
+    CmaxArgs C;                  // canvas (Hc, Wc) for splat_taps
+    const float *x, *y, *t, *p;  // t relative to the sample's t0
+    const int64_t *offsets;
+    int64_t n;
+    const float *flow;           // [B][2][H][W]
+    int H, W;
+    float *acc;                  // forward: [B][Hc][Wc][4]; backward: [B][2][H][W][4]
+    unsigned *nonfinite;         // [B] forward: set when an event's warped position is not finite
+    const float *Wimg;           // backward: [B][Hc][Wc]
+};
+
+constexpr int kFlowObjThreads = 256;
+
+// The warp and the keep rule of one event of sample b; false for events that contribute nothing.
+__device__ __forceinline__ bool flow_obj_warp(const FlowObjArgs &A, const float *flow, float xe, float ye, float d, float p,
+                                              FlowSample &s, Taps &T, bool &nonfinite)
+{
+    s = flow_sample<false>(flow, nullptr, A.H, A.W, xe, ye);
+    const float xw = __fadd_rn(xe, __fmul_rn(s.u, d)), yw = __fadd_rn(ye, __fmul_rn(s.v, d));
+    if (!isfinite(xw) || !isfinite(yw)) { nonfinite = true; return false; }
+    if (!(xw >= 0.0f && xw < (float)A.W && yw >= 0.0f && yw < (float)A.H)) return false;
+    unsigned oob = 0;   // a kept event's footprint lies inside the canvas
+    return splat_taps<false>(A.C, xw, yw, p, 0.0f, true, oob, T);
+}
+
+template <bool GRAD>
+__device__ __forceinline__ void flow_obj_event(const FlowObjArgs &A, const float *flow, float *acc, const float *Wb,
+                                               float xe, float ye, float d, float p, bool &nonfinite)
+{
+    FlowSample s;
+    Taps T;
+    if (!flow_obj_warp(A, flow, xe, ye, d, p, s, T, nonfinite)) return;
+    if (!GRAD) {
+        red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
+        return;
+    }
+    // df/dx' and df/dy' through the four bilinear taps of the IWE (the sx / sy of cmax_grad_pass_kernel)
+    const int r0 = T.y0 * A.C.Wc, r1 = T.y1 * A.C.Wc;
+    const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0), w11 = __ldg(Wb + r1 + T.x1);
+    const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
+    const float sx = T.wm * (oy * (w01 - w00) + T.dy * (w11 - w10));
+    const float sy = T.wm * (ox * (w10 - w00) + T.dx * (w11 - w01));
+    const float gu = sx * d, gv = sy * d;
+    if (!s.sampled || (gu == 0.0f && gv == 0.0f)) return;
+    const int64_t plane4 = (int64_t)A.H * A.W * 4;
+    if (s.x0 >= 0 && s.x0 + 1 < A.W && s.y0 >= 0 && s.y0 + 1 < A.H) {
+        float *blk = acc + ((int64_t)s.y0 * A.W + s.x0) * 4;
+        red_add4(blk, make_float4(gu * s.nw, gu * s.ne, gu * s.sw, gu * s.se));
+        red_add4(blk + plane4, make_float4(gv * s.nw, gv * s.ne, gv * s.sw, gv * s.se));
+    } else {
+        // border footprint: every tap inside the field is the TL tap of its own pixel's block
+        const int xs[4] = {s.x0, s.x0 + 1, s.x0, s.x0 + 1}, ys[4] = {s.y0, s.y0, s.y0 + 1, s.y0 + 1};
+        const float w[4] = {s.nw, s.ne, s.sw, s.se};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            if ((unsigned)xs[k] >= (unsigned)A.W || (unsigned)ys[k] >= (unsigned)A.H) continue;
+            float *blk = acc + ((int64_t)ys[k] * A.W + xs[k]) * 4;
+            red_add(blk, gu * w[k]);
+            red_add(blk + plane4, gv * w[k]);
+        }
+    }
+}
+
+template <bool GRAD>
+__global__ void __launch_bounds__(kFlowObjThreads) flow_obj_event_kernel(const FlowObjArgs A)
+{
+    const int b = blockIdx.y;
+    int64_t first = A.offsets[b], last = A.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > A.n) last = A.n;
+    const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
+    const float *flow = A.flow + (int64_t)b * 2 * A.H * A.W;
+    float *acc = A.acc + (GRAD ? (int64_t)b * 2 * A.H * A.W * 4 : (int64_t)b * npix * 4);
+    const float *Wb = GRAD ? A.Wimg + (int64_t)b * npix : nullptr;
+    bool nonfinite = false;
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
+        float ex[kBatch], ey[kBatch], et[kBatch], ep[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            ex[k] = ld_stream(A.x + i + k * stride); ey[k] = ld_stream(A.y + i + k * stride);
+            et[k] = ld_stream(A.t + i + k * stride); ep[k] = ld_stream(A.p + i + k * stride);
+        }
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) flow_obj_event<GRAD>(A, flow, acc, Wb, ex[k], ey[k], et[k], ep[k], nonfinite);
+    }
+    for (; i < last; i += stride)
+        flow_obj_event<GRAD>(A, flow, acc, Wb, ld_stream(A.x + i), ld_stream(A.y + i), ld_stream(A.t + i), ld_stream(A.p + i),
+                             nonfinite);
+    if (!GRAD && nonfinite) A.nonfinite[b] = 1u;
+}
+
+// blocks -> the IWE of every sample (blockIdx.z); a sample with a non-finite warped position gets an all-NaN IWE, so that
+// its f (and its gradient) is NaN
+__global__ void __launch_bounds__(256) flow_obj_fold_kernel(const float *__restrict__ acc, const unsigned *__restrict__ nonfinite,
+                                                            int Hc, int Wc, float *__restrict__ iwe)
+{
+    const int64_t npix = (int64_t)Hc * Wc;
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= npix) return;
+    acc += blockIdx.z * npix * 4;
+    const int y = i / Wc, x = i - y * Wc;
+    float v = acc[(int64_t)i * 4];
+    if (x > 0) v += acc[(int64_t)(i - 1) * 4 + 1];
+    if (y > 0) v += acc[(int64_t)(i - Wc) * 4 + 2];
+    if (x > 0 && y > 0) v += acc[(int64_t)(i - Wc - 1) * 4 + 3];
+    iwe[blockIdx.z * npix + i] = nonfinite[blockIdx.z] ? __int_as_float(0x7fc00000) : v;
+}
+
+// f of every sample from the sums of cmax_model_stats_kernel (gsums[b][8]: 1 sum(exp G), 2 sum(exp(-p G)), 4 sum(G),
+// 5 sum(G^2) with f64 products)
+__global__ void flow_obj_final_kernel(int kind, const double *gsums, int npix, int batch, double *f_out)
+{
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= batch) return;
+    const double *s = gsums + 8 * b;
+    const double P = (double)npix;
+    double f;
+    if (kind == OBJ_VARIANCE) { const double m = s[4] / P; f = -(s[5] / P - m * m); }
+    else if (kind == OBJ_SOS) f = -s[5] / P;
+    else if (kind == OBJ_SOE) f = -s[1] / P;
+    else f = -s[2];
+    f_out[b] = f;
+}
+
+// g_b * df_b/dG per pixel (before the blur that turns it into W):
+//   variance -2 G / P (the -2 mean(G) / P of the exact derivative is constant over the image; the blur keeps it constant
+//   and the tap differences of the event pass cancel it), sos -2 G / P, soe -exp(G) / P, sosa p exp(-p G)
+__global__ void __launch_bounds__(256) flow_obj_coef_kernel(const float *__restrict__ G, int npix, int kind, double param,
+                                                            const float *__restrict__ grad_f, double *__restrict__ w)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= npix) return;
+    const size_t k = (size_t)blockIdx.z * npix + i;
+    const double g = (double)G[k], P = (double)npix;
+    double c;
+    if (kind == OBJ_SOE) c = -exp(g) / P;
+    else if (kind == OBJ_SOSA) c = param * exp(-param * g);
+    else c = -2.0 * g / P;
+    w[k] = (double)grad_f[blockIdx.z] * c;
+}
+
+// [B][2][H][W][4] blocks -> grad_flow [B][2][H][W]
+__global__ void __launch_bounds__(256) flow_obj_grad_fold_kernel(const float *__restrict__ ws, float *__restrict__ out, int64_t planes,
+                                                                 int H, int W)
+{
+    const int64_t total = planes * H * W;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const int x = (int)(i % W), y = (int)((i / W) % H);
+        float v = ws[i * 4];
+        if (x > 0) v += ws[(i - 1) * 4 + 1];
+        if (y > 0) v += ws[(i - W) * 4 + 2];
+        if (x > 0 && y > 0) v += ws[(i - W - 1) * 4 + 3];
+        out[i] = v;
+    }
+}
+
+struct FlowObjWorkspace {
+    unsigned *nonfinite;   // [B]
+    double *gsums;         // [B][8]
+    unsigned *gmax;        // [B]
+    float *acc;            // [B][Hc][Wc][4] (forward) / [B][2][H][W][4] (backward)
+    float *tmp, *G, *Wimg; // [B][Hc][Wc]
+    double *w, *wt;        // [B][Hc][Wc]
+};
+
+static size_t flow_obj_carve(void *base, int batch, int H, int W, FlowObjWorkspace *ws)
+{
+    const size_t npix = (size_t)(H + 1) * (W + 1), B = (size_t)batch;
+    size_t off = 0;
+    char *b = static_cast<char *>(base);
+    auto take = [&](size_t bytes) { char *p = b ? b + off : nullptr; off += align_up(bytes, 256); return p; };
+    // the counters come first and are directly followed by the accumulator: one memset zeroes them all
+    unsigned *nonfinite = (unsigned *)take(B * sizeof(unsigned));
+    double *gsums = (double *)take(B * 8 * sizeof(double));
+    unsigned *gmax = (unsigned *)take(B * sizeof(unsigned));
+    const size_t acc_floats = npix > (size_t)2 * H * W ? npix : (size_t)2 * H * W;   // the IWE blocks / the flow-gradient blocks
+    float *acc = (float *)take(B * acc_floats * 4 * sizeof(float));
+    float *tmp = (float *)take(B * npix * sizeof(float));
+    float *G = (float *)take(B * npix * sizeof(float));
+    float *Wimg = (float *)take(B * npix * sizeof(float));
+    double *w = (double *)take(B * npix * sizeof(double));
+    double *wt = (double *)take(B * npix * sizeof(double));
+    if (ws) { ws->nonfinite = nonfinite; ws->gsums = gsums; ws->gmax = gmax; ws->acc = acc; ws->tmp = tmp; ws->G = G; ws->Wimg = Wimg; ws->w = w; ws->wt = wt; }
+    return off;
+}
+
+// shared argument checks and set-up of the two entry points
+static int flow_obj_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
+                          int batch, int64_t n, const float *flow, int H, int W, double sigma, int objective, void *workspace,
+                          size_t workspace_bytes, FlowObjArgs &A, FlowObjWorkspace &ws, BlurTaps &taps)
+{
+    if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
+        (n > 0 && (!x || !y || !t || !p))) {
+        set_error("%s: bad arguments (0 <= batch <= 65535, H, W >= 2)", who);
+        return EVK_E_ARG;
+    }
+    if (objective == OBJ_MOA || objective == OBJ_ISOA) {
+        set_error("%s: objective %d (moa / isoa) is piecewise constant in the flow and has no gradient", who, objective);
+        return EVK_E_UNSUPPORTED;
+    }
+    if (objective != OBJ_VARIANCE && objective != OBJ_SOS && objective != OBJ_SOE && objective != OBJ_SOSA) {
+        set_error("%s: unknown objective %d", who, objective);
+        return EVK_E_ARG;
+    }
+    if ((size_t)(H + 1) * (W + 1) > (size_t)1 << 30) { set_error("%s: canvas too large", who); return EVK_E_ARG; }
+    const size_t need = flow_obj_carve(nullptr, batch, H, W, nullptr);
+    if (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 255)) {
+        set_error("%s: 256-byte aligned workspace of %zu bytes required", who, need);
+        return EVK_E_WORKSPACE;
+    }
+    flow_obj_carve(workspace, batch, H, W, &ws);
+    taps = BlurTaps{};
+    if (sigma > 0.0) {
+        int rc = make_taps(sigma, &taps);
+        if (rc) return rc;
+    }
+    A = FlowObjArgs{};
+    A.C.Hc = H + 1; A.C.Wc = W + 1;
+    A.x = x; A.y = y; A.t = t; A.p = p; A.offsets = offsets; A.n = n;
+    A.flow = flow; A.H = H; A.W = W;
+    return EVK_OK;
+}
+
+// (slices, batch) grid of an event pass: about 2K events per CTA, at most ~8 CTAs per SM over the whole batch
+static dim3 flow_obj_grid(int64_t n, int batch)
+{
+    const int64_t per = n / batch;
+    int64_t slices = (per + 2047) / 2048;
+    const int64_t fill = ((int64_t)num_sms() * 8 + batch - 1) / batch;
+    if (slices > fill) slices = fill;
+    if (slices < 1) slices = 1;
+    return dim3((unsigned)slices, (unsigned)batch);
+}
+
+// G = blur(I) for every sample (blockIdx.z), both axes
+static void flow_obj_blur(const FlowObjWorkspace &ws, const float *I, int Hc, int Wc, const BlurTaps &taps, int batch, cudaStream_t st)
+{
+    const int do_blur = taps.r > 0 || taps.w[0] != 0.0;
+    const dim3 g((Hc * Wc + 255) / 256, 1, batch);
+    prof_count(do_blur ? 2 : 1);
+    if (do_blur) cmax_blur_axis0_kernel<<<g, 256, 0, st>>>(I, ws.tmp, Hc, Wc, taps);
+    cmax_blur_axis1_store_kernel<<<g, 256, 0, st>>>(ws.tmp, I, Hc, Wc, taps, do_blur, ws.G);
+}
+
 }  // namespace evk
 
 extern "C" {
@@ -1793,6 +2088,86 @@ int evk_cmax_warp_objective_batch_f64(const double *x, const double *y, const do
         cmax_model_final_kernel<<<1, 1, 0, st>>>(objective, ws.gsums, ws.gmax, ws.sums, ws.oob, npix, ws.sums + 1, 4, 0, results + 16 * k);
         EVK_CUDA(cudaGetLastError());
     }
+    return EVK_OK;
+}
+
+size_t evk_cmax_flow_objective_workspace_bytes(int batch, int H, int W)
+{
+    if (batch < 0 || H < 2 || W < 2) return 0;
+    return evk::flow_obj_carve(nullptr, batch, H, W, nullptr);
+}
+
+int evk_cmax_flow_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                int batch, int64_t n_events, const float *flow, int H, int W, double sigma, int objective,
+                                double obj_param, double *f_out, float *iwe_out, void *workspace, size_t workspace_bytes,
+                                void *stream)
+{
+    using namespace evk;
+    FlowObjArgs A;
+    FlowObjWorkspace ws;
+    BlurTaps taps;
+    int rc = flow_obj_setup("evk_cmax_flow_objective_f32", x, y, t_rel, p, offsets, batch, n_events, flow, H, W, sigma, objective,
+                            workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !iwe_out)) { set_error("evk_cmax_flow_objective_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc;
+    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)batch * npix * 4 * sizeof(float), st));
+    A.acc = ws.acc;
+    A.nonfinite = ws.nonfinite;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        flow_obj_event_kernel<false><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+    }
+    const dim3 g((npix + 255) / 256, 1, batch);
+    prof_count(1);
+    flow_obj_fold_kernel<<<g, 256, 0, st>>>(ws.acc, ws.nonfinite, Hc, Wc, iwe_out);
+    flow_obj_blur(ws, iwe_out, Hc, Wc, taps, batch, st);
+    prof_count(2);
+    cmax_model_stats_kernel<<<g, 256, 0, st>>>(ws.G, iwe_out, npix, objective, obj_param, ws.gsums, ws.gmax, nullptr, nullptr);
+    flow_obj_final_kernel<<<(batch + 127) / 128, 128, 0, st>>>(objective, ws.gsums, npix, batch, f_out);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                     int batch, int64_t n_events, const float *flow, int H, int W, double sigma, int objective,
+                                     double obj_param, const float *iwe, const float *grad_f, float *grad_flow, void *workspace,
+                                     size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    FlowObjArgs A;
+    FlowObjWorkspace ws;
+    BlurTaps taps;
+    int rc = flow_obj_setup("evk_cmax_flow_objective_grad_f32", x, y, t_rel, p, offsets, batch, n_events, flow, H, W, sigma,
+                            objective, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!iwe || !grad_f || !grad_flow)) { set_error("evk_cmax_flow_objective_grad_f32: null array"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc;
+    const int64_t planes = (int64_t)batch * 2;
+    EVK_CUDA(cudaMemsetAsync(ws.acc, 0, (size_t)planes * H * W * 4 * sizeof(float), st));
+    // W = G(g_b C_b): recompute G from the saved IWE, the coefficient image, its blur
+    flow_obj_blur(ws, iwe, Hc, Wc, taps, batch, st);
+    const int do_blur = taps.r > 0 || taps.w[0] != 0.0;
+    const dim3 g((npix + 255) / 256, 1, batch);
+    prof_count(do_blur ? 3 : 2);
+    flow_obj_coef_kernel<<<g, 256, 0, st>>>(ws.G, npix, objective, obj_param, grad_f, ws.w);
+    if (do_blur) cmax_blur_d_axis0_kernel<<<g, 256, 0, st>>>(ws.w, ws.wt, Hc, Wc, taps);
+    cmax_blur_d_axis1_store_kernel<<<g, 256, 0, st>>>(ws.wt, ws.w, Hc, Wc, taps, do_blur, ws.Wimg);
+    A.acc = ws.acc;
+    A.Wimg = ws.Wimg;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        flow_obj_event_kernel<true><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+    }
+    prof_count(1);
+    flow_obj_grad_fold_kernel<<<grid_simple(planes * H * W, 256), 256, 0, st>>>(ws.acc, grad_flow, planes, H, W);
+    EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }
 

@@ -464,6 +464,36 @@ int evk_cmax_flow_variance_f32(const float *x, const float *y, const float *t, c
                                unsigned flags, double *result, float *iwe_out, void *workspace,
                                size_t workspace_bytes, void *stream);
 
+/* Dense-flow contrast maximisation over a batch of samples, as a differentiable loss: the reference's
+ * motion_compensate (lib/visualization/draw_flow.py:15-26: warp_events_flow_torch, then the bilinear
+ * events_to_image_torch) followed by an objective of lib/contrast_max/objectives.py.  Sample b is the events
+ * [offsets[b], offsets[b+1]) (clipped to [0, n_events); end < start is empty), warped by flow[b]:
+ *   x' = x + u(x,y) t_rel,  y' = y + v(x,y) t_rel     (optic_flow.py:37-44; t_rel = t - t0[b], given)
+ * The IWE of sample b is the bilinear splat of p on the (H+1)x(W+1) canvas of every event with 0 <= x' < W and
+ * 0 <= y' < H (f32 comparisons); other events contribute nothing.  An event whose x' or y' is not finite makes the
+ * whole IWE of its sample NaN, and so its f.  Then G = gaussian_filter(IWE, sigma) (sigma 0: no blur) and, P = (H+1)(W+1):
+ *   EVK_OBJ_VARIANCE  f = -var(G)          EVK_OBJ_SOS   f = -mean(G^2)
+ *   EVK_OBJ_SOE       f = -mean(exp G)     EVK_OBJ_SOSA  f = -sum(exp(-obj_param G))
+ * (EVK_OBJ_MOA / EVK_OBJ_ISOA are piecewise constant: EVK_E_UNSUPPORTED.)
+ *   x, y, t_rel, p : n_events floats;  offsets: batch+1 int64 on the device;  flow: [batch][2][H][W] f32
+ *   f_out          : batch doubles;  iwe_out: [batch][H+1][W+1] floats, which the backward takes as `iwe`
+ * evk_cmax_flow_objective_grad_f32 writes grad_flow [batch][2][H][W] = sum_b grad_f[b] df_b/dflow[b], the exact
+ * derivative of the f above (grad_f: batch floats on the device): with W_b = G(grad_f[b] df_b/dG), per kept event
+ *   df/dx' = p[(1-dy)(W01-W00) + dy(W11-W10)],  df/dy' = p[(1-dx)(W10-W00) + dx(W11-W01)]
+ * times t_rel, spread over the four grid_sample taps of the event's (x, y); taps outside the field get nothing.
+ * workspace: evk_cmax_flow_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
+ * Neither call synchronises, and both launch the same kernels whatever the batch. */
+size_t evk_cmax_flow_objective_workspace_bytes(int batch, int H, int W);
+int evk_cmax_flow_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                const int64_t *offsets, int batch, int64_t n_events, const float *flow,
+                                int H, int W, double sigma, int objective, double obj_param, double *f_out,
+                                float *iwe_out, void *workspace, size_t workspace_bytes, void *stream);
+int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                     const int64_t *offsets, int batch, int64_t n_events, const float *flow,
+                                     int H, int W, double sigma, int objective, double obj_param,
+                                     const float *iwe, const float *grad_f, float *grad_flow,
+                                     void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * RobustNorm (row f4): clamp a tensor between two of its order statistics and rescale it.  Replaces
  * RobustNorm.__call__ / .percentile, lib/data_loaders/data_augmentation.py:82-130 (two kthvalue sorts),
