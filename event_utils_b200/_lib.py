@@ -39,7 +39,7 @@ CMAX_WANT_GRAD = 0x10
 CMAX_ABS_POLARITY = 0x20
 CMAX_NO_CHANNEL_MIX = 0x40
 OBJ_VARIANCE, OBJ_SOS, OBJ_SOE, OBJ_MOA, OBJ_ISOA, OBJ_SOSA = range(6)
-WARP_ROTATION, WARP_XYZTHETA = 1, 2
+WARP_ROTATION, WARP_XYZTHETA, WARP_LINVEL = 1, 2, 3
 
 _lib = None
 _lock = threading.Lock()
@@ -162,6 +162,14 @@ def _declare(L):
     L.evk_cmax_flow_objective_grad_f32.restype = ci
     L.evk_cmax_flow_objective_grad_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, vp, ci, ci, f64, ci, f64, vp, vp, vp, vp, sz,
                                                    vp]
+    L.evk_cmax_motion_objective_workspace_bytes.restype = sz
+    L.evk_cmax_motion_objective_workspace_bytes.argtypes = [ci, ci, ci]
+    L.evk_cmax_motion_objective_f32.restype = ci
+    L.evk_cmax_motion_objective_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci, f64, ci, f64, vp, vp,
+                                                vp, sz, vp]
+    L.evk_cmax_motion_objective_grad_f32.restype = ci
+    L.evk_cmax_motion_objective_grad_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci, f64, ci, f64, vp,
+                                                     vp, vp, vp, sz, vp]
     L.evk_robust_norm_workspace_bytes.restype = sz
     L.evk_robust_norm_workspace_bytes.argtypes = []
     L.evk_robust_norm_f32.restype = ci

@@ -14,6 +14,7 @@ Which inputs get a gradient (as in the reference; the others get None):
                                      events_to_voxel_timesync_torch
     events_to_neg_pos_voxel_torch    ts (voxel_grid.py:155-182)
     flow_contrast_objective_torch    flow only (contrast_max/flow_objective.py; the events are data)
+    motion_contrast_objective_torch  params only (contrast_max/motion_objective.py; the events are data)
 
 The public functions take this path only when grad mode is on and one of those inputs requires grad; every
 other call runs the plain forward.  Gradients come back in each input's shape, dtype and device.  The
@@ -40,7 +41,8 @@ def _as_input(g, meta):
 
 def _grad_in(g, dev):
     """The incoming gradient as contiguous f32 on the compute device (autograd hands zeros for an unused output, and
-    an expanded gradient such as the one of img.sum() has stride 0)."""
+    an expanded gradient such as the one of img.sum() has stride 0).  The backward kernels work in f32, so an f64
+    incoming gradient (e.g. of the contrast objectives' f64 f) is rounded to f32 here."""
     return g.to(device=dev, dtype=torch.float32).contiguous()
 
 
@@ -213,6 +215,50 @@ class FlowObjective(torch.autograd.Function):
                 H, W, sigma, objective, param, _lib.ptr(iwe), _lib.ptr(g), _lib.ptr(gf), _lib.ptr(ws), ws.numel(),
                 _lib.stream()))
         return _as_input(gf, ctx.meta), None, None, None, None, None, None
+
+
+class MotionObjective(torch.autograd.Function):
+    """The batched parametric contrast objective of contrast_max/motion_objective.py (get_iwe, objectives.py:184-192, with
+    the linvel, rotation or 4-DoF model, then an objective of objectives.py): f (B,) f64 from params (B,K) and the
+    prepared device events.  Only the parameters get a gradient: the exact derivative of f, one pass over the events
+    (evk_cmax_motion_objective_grad_f32).  opts = (warp code, centre, H, W, objective, sigma, obj_param)."""
+
+    @staticmethod
+    def forward(ctx, params, x, y, t_rel, p, offsets, opts):
+        warp, (cx, cy), H, W, objective, sigma, param = opts
+        dev = x.device
+        B, K = params.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            p64 = params.detach().to(device=dev, dtype=torch.float64).contiguous()
+            f = torch.empty(B, dtype=torch.float64, device=dev)
+            iwe = torch.empty((B, H + 1, W + 1), dtype=torch.float32, device=dev)
+            ws = _lib.scratch("motion_objective", L.evk_cmax_motion_objective_workspace_bytes(B, H, W), dev)
+            _lib.check(L.evk_cmax_motion_objective_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0], warp, _lib.ptr(p64), K,
+                cx, cy, H, W, sigma, objective, param, _lib.ptr(f), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(), _lib.stream()))
+        ctx.save_for_backward(x, y, t_rel, p, offsets, p64, iwe)
+        ctx.opts = opts
+        ctx.meta = _meta(params)
+        return f
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, y, t_rel, p, offsets, p64, iwe = ctx.saved_tensors
+        warp, (cx, cy), H, W, objective, sigma, param = ctx.opts
+        dev = x.device
+        B, K = p64.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g = _grad_in(g, dev)
+            gp = torch.empty_like(p64)
+            ws = _lib.scratch("motion_objective", L.evk_cmax_motion_objective_workspace_bytes(B, H, W), dev)
+            _lib.check(L.evk_cmax_motion_objective_grad_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0], warp, _lib.ptr(p64), K,
+                cx, cy, H, W, sigma, objective, param, _lib.ptr(iwe), _lib.ptr(g), _lib.ptr(gp), _lib.ptr(ws), ws.numel(),
+                _lib.stream()))
+        return _as_input(gp, ctx.meta), None, None, None, None, None, None
 
 
 class VoxelGrid(torch.autograd.Function):

@@ -34,28 +34,51 @@ def flow_contrast_objective_torch(xs, ys, ts, ps, flow, t0=None, objective="vari
     @param batch_end_indices the cumulative end indices of BaseVoxelDataset.collate_fn
            (lib/data_loaders/base_dataset.py:513-539), a list or an int64 tensor; None means one sample of all events
     @returns (B,) tensor of f in flow's dtype, on flow's device.  With every input already on the GPU neither the
-           forward nor the backward synchronises with the host.
+           forward nor the backward synchronises with the host.  The backward rounds the incoming gradient g_b to
+           f32, as it stores W_b = G(g_b df_b/dG) in f32: the gradient is accurate to f32 rounding whatever
+           flow's dtype (an f64 flow does not give an f64-accurate gradient).
     """
-    if objective not in OBJECTIVES:
-        if objective in ("moa", "isoa"):
-            raise ValueError("objective %r is piecewise constant in the flow and has no gradient; use one of %s"
-                             % (objective, sorted(OBJECTIVES)))
-        raise ValueError("unknown objective %r (one of %s)" % (objective, sorted(OBJECTIVES)))
-    xs, ys, ts, ps = (E.as_tensor(a).reshape(-1) for a in (xs, ys, ts, ps))
-    if any(a.requires_grad for a in (xs, ys, ts, ps)) or (isinstance(t0, torch.Tensor) and t0.requires_grad):
-        raise ValueError("flow_contrast_objective_torch differentiates with respect to the flow only; the events and t0 "
-                         "must not require grad (detach them)")
+    _check_objective(objective, "flow")
+    xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "flow_contrast_objective_torch", "the flow")
     flow = E.as_tensor(flow)
     if flow.dim() == 3:
         flow = flow.unsqueeze(0)
     if flow.dim() != 4 or flow.shape[1] != 2:
         raise ValueError("flow must have shape (B,2,H,W) or (2,H,W), got %s" % (tuple(flow.shape),))
     B, H, W = flow.shape[0], flow.shape[2], flow.shape[3]
+    _lib.lib()
+    dev = E.compute_device(flow, xs, ys, ts, ps)
+    x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "flows")
+    from ..autograd import FlowObjective
+    param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
+    f = FlowObjective.apply(flow, x, y, t_rel, p, offsets, (OBJECTIVES[objective], float(blur_sigma), param))
+    return f.to(device=flow.device, dtype=flow.dtype)
+
+
+def _check_objective(objective, wrt):
+    if objective not in OBJECTIVES:
+        if objective in ("moa", "isoa"):
+            raise ValueError("objective %r is piecewise constant in the %s and has no gradient; use one of %s"
+                             % (objective, wrt, sorted(OBJECTIVES)))
+        raise ValueError("unknown objective %r (one of %s)" % (objective, sorted(OBJECTIVES)))
+
+
+def _event_tensors(xs, ys, ts, ps, t0, who, wrt):
+    """the events as flat tensors; they and t0 are data and must not require grad"""
+    xs, ys, ts, ps = (E.as_tensor(a).reshape(-1) for a in (xs, ys, ts, ps))
+    if any(a.requires_grad for a in (xs, ys, ts, ps)) or (isinstance(t0, torch.Tensor) and t0.requires_grad):
+        raise ValueError("%s differentiates with respect to %s only; the events and t0 must not require grad (detach them)"
+                         % (who, wrt))
     n = xs.shape[0]
     if not (ys.shape[0] == ts.shape[0] == ps.shape[0] == n):
         raise ValueError("xs, ys, ts, ps must have the same length")
-    _lib.lib()
-    dev = E.compute_device(flow, xs, ys, ts, ps)
+    return xs, ys, ts, ps
+
+
+def _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what):
+    """The events of a batch of B samples on `dev` as the batched kernels take them: x, y, p f32, t_rel = t - t0_b
+    formed in ts' dtype then cast to f32 (t0 None: each sample's last stamp), and the B+1 int64 sample offsets."""
+    n = xs.shape[0]
     with torch.cuda.device(dev):
         if batch_end_indices is None:
             ends = torch.full((1,), n, dtype=torch.int64, device=dev)
@@ -64,7 +87,7 @@ def flow_contrast_objective_torch(xs, ys, ts, ps, flow, t0=None, objective="vari
         else:
             ends = torch.tensor([int(e) for e in batch_end_indices], dtype=torch.int64).to(dev)
         if ends.shape[0] != B:
-            raise ValueError("%d samples of events for a batch of %d flows" % (ends.shape[0], B))
+            raise ValueError("%d samples of events for a batch of %d %s" % (ends.shape[0], B, what))
         offsets = torch.cat((torch.zeros(1, dtype=torch.int64, device=dev), ends))
         x, y, p = (E.to_device(a, dev).to(torch.float32).contiguous() for a in (xs, ys, ps))
         t = E.to_device(ts, dev)
@@ -80,7 +103,4 @@ def flow_contrast_objective_torch(xs, ys, ts, ps, flow, t0=None, objective="vari
             # the sample of each event: windows are contiguous, [ends[b-1], ends[b])
             sample = torch.searchsorted(ends, torch.arange(n, device=dev), right=True).clamp_(max=B - 1)
             t_rel = (t - t0b.to(rt)[sample]).to(torch.float32).contiguous()
-    from ..autograd import FlowObjective
-    param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
-    f = FlowObjective.apply(flow, x, y, t_rel, p, offsets, (OBJECTIVES[objective], float(blur_sigma), param))
-    return f.to(device=flow.device, dtype=flow.dtype)
+    return x, y, t_rel, p, offsets

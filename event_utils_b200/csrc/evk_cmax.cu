@@ -89,7 +89,8 @@ enum { WARP_LINVEL_F64 = 0, WARP_LINVEL_F32 = 1, WARP_FLOW_F32 = 2,
 
 __host__ __device__ constexpr bool is_model_warp(int w) { return w >= WARP_ROTATION_F64; }
 __host__ __device__ constexpr bool is_rotation(int w) { return w == WARP_ROTATION_F64 || w == WARP_ROTATION_F32; }
-__host__ __device__ constexpr int model_dims(int w) { return is_rotation(w) ? 3 : 4; }
+__host__ __device__ constexpr bool is_linvel(int w) { return w == WARP_LINVEL_F64 || w == WARP_LINVEL_F32; }
+__host__ __device__ constexpr int model_dims(int w) { return is_linvel(w) ? 2 : is_rotation(w) ? 3 : 4; }
 
 // bilinear splat of weight w (and derivative weight a) at (xf, yf) on the canvas:
 // image.py:199-207 (IWE) and :131-135 (derivative images) with w1 = [a;0], w2 = [0;a].
@@ -270,6 +271,8 @@ __device__ __forceinline__ void ld_vec16(const double *p, double (&v)[2])
 //     x' = x - dt ((hx + hz u) - theta v)      y' = y - dt ((hy + hz v) + theta u)
 //     dx'/d(hx, hy, hz, theta) = (-dt, 0, -dt u,  dt v)
 //     dy'/d(hx, hy, hz, theta) = (0, -dt, -dt v, -dt u)
+//   linvel (vx, vy), warps.py:51-61 (the batched motion objective; the single-window linvel entries keep their own
+//   fused pass, cmax_event):  x' = x - dt vx,  y' = y - dt vy,  dx'/d(vx, vy) = (-dt, 0),  dy'/d(vx, vy) = (0, -dt)
 // in the order written (no FMA: the library builds with -fmad=false), f64 in parity mode, f32 in fast mode.
 // THE one place that turns an event into its bilinear footprint for these models: warp, bounds mask
 // (event_util.py:26-27), f64 -> f32 cast (image.py:180-183) and splat_taps -- the IWE pass and the gradient
@@ -287,7 +290,16 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
     if (A.abs_polarity) p = fabs(p);
     const R d = (sizeof(R) == 8) ? e.t - (R)A.t_ref : e.t;   // fast mode stores t - t_ref already
     R xw, yw;
-    if (is_rotation(WARP)) {
+    if (is_linvel(WARP)) {
+        const R vx = (R)M.m[0], vy = (R)M.m[1];
+        xw = e.x - d * vx;
+        yw = e.y - d * vy;
+        if (JAC) {
+            jx[0] = (float)(-d); jx[1] = 0.0f;
+            jy[0] = 0.0f; jy[1] = (float)(-d);
+            jx[2] = jx[3] = jy[2] = jy[3] = 0.0f;
+        }
+    } else if (is_rotation(WARP)) {
         const R cx = (R)M.m[0], cy = (R)M.m[1], om = (R)M.m[2];
         R s, c;
         sin_cos(om * d, &s, &c);
@@ -1663,16 +1675,18 @@ __global__ void __launch_bounds__(256) flow_obj_grad_fold_kernel(const float *__
     }
 }
 
-struct FlowObjWorkspace {
+// ---- shared by the batched objectives (dense flow above, parametric motion below): workspace, checks, image tail ----
+struct BatchObjWorkspace {
     unsigned *nonfinite;   // [B]
     double *gsums;         // [B][8]
     unsigned *gmax;        // [B]
-    float *acc;            // [B][Hc][Wc][4] (forward) / [B][2][H][W][4] (backward)
+    float *acc;            // [B][acc_blocks][4]: the 2x2-block IWE (forward); the flow objective's flow-gradient blocks
     float *tmp, *G, *Wimg; // [B][Hc][Wc]
     double *w, *wt;        // [B][Hc][Wc]
 };
 
-static size_t flow_obj_carve(void *base, int batch, int H, int W, FlowObjWorkspace *ws)
+// acc_blocks: 16-byte blocks of the accumulator per sample
+static size_t batch_obj_carve(void *base, int batch, int H, int W, size_t acc_blocks, BatchObjWorkspace *ws)
 {
     const size_t npix = (size_t)(H + 1) * (W + 1), B = (size_t)batch;
     size_t off = 0;
@@ -1682,8 +1696,7 @@ static size_t flow_obj_carve(void *base, int batch, int H, int W, FlowObjWorkspa
     unsigned *nonfinite = (unsigned *)take(B * sizeof(unsigned));
     double *gsums = (double *)take(B * 8 * sizeof(double));
     unsigned *gmax = (unsigned *)take(B * sizeof(unsigned));
-    const size_t acc_floats = npix > (size_t)2 * H * W ? npix : (size_t)2 * H * W;   // the IWE blocks / the flow-gradient blocks
-    float *acc = (float *)take(B * acc_floats * 4 * sizeof(float));
+    float *acc = (float *)take(B * acc_blocks * 4 * sizeof(float));
     float *tmp = (float *)take(B * npix * sizeof(float));
     float *G = (float *)take(B * npix * sizeof(float));
     float *Wimg = (float *)take(B * npix * sizeof(float));
@@ -1693,18 +1706,19 @@ static size_t flow_obj_carve(void *base, int batch, int H, int W, FlowObjWorkspa
     return off;
 }
 
-// shared argument checks and set-up of the two entry points
-static int flow_obj_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
-                          int batch, int64_t n, const float *flow, int H, int W, double sigma, int objective, void *workspace,
-                          size_t workspace_bytes, FlowObjArgs &A, FlowObjWorkspace &ws, BlurTaps &taps)
+// the flow objective's accumulator: the IWE blocks (forward) or the flow-gradient blocks (backward), whichever is larger
+static size_t flow_obj_acc_blocks(int H, int W)
 {
-    if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
-        (n > 0 && (!x || !y || !t || !p))) {
-        set_error("%s: bad arguments (0 <= batch <= 65535, H, W >= 2)", who);
-        return EVK_E_ARG;
-    }
+    const size_t npix = (size_t)(H + 1) * (W + 1), grad = (size_t)2 * H * W;
+    return npix > grad ? npix : grad;
+}
+
+// the checks and set-up every batched objective entry shares: objective, canvas, workspace (carved into ws), blur taps
+static int batch_obj_check(const char *who, const char *wrt, int batch, int H, int W, double sigma, int objective, size_t acc_blocks,
+                           void *workspace, size_t workspace_bytes, BatchObjWorkspace &ws, BlurTaps &taps)
+{
     if (objective == OBJ_MOA || objective == OBJ_ISOA) {
-        set_error("%s: objective %d (moa / isoa) is piecewise constant in the flow and has no gradient", who, objective);
+        set_error("%s: objective %d (moa / isoa) is piecewise constant in the %s and has no gradient", who, objective, wrt);
         return EVK_E_UNSUPPORTED;
     }
     if (objective != OBJ_VARIANCE && objective != OBJ_SOS && objective != OBJ_SOE && objective != OBJ_SOSA) {
@@ -1712,17 +1726,32 @@ static int flow_obj_setup(const char *who, const float *x, const float *y, const
         return EVK_E_ARG;
     }
     if ((size_t)(H + 1) * (W + 1) > (size_t)1 << 30) { set_error("%s: canvas too large", who); return EVK_E_ARG; }
-    const size_t need = flow_obj_carve(nullptr, batch, H, W, nullptr);
+    const size_t need = batch_obj_carve(nullptr, batch, H, W, acc_blocks, nullptr);
     if (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 255)) {
         set_error("%s: 256-byte aligned workspace of %zu bytes required", who, need);
         return EVK_E_WORKSPACE;
     }
-    flow_obj_carve(workspace, batch, H, W, &ws);
+    batch_obj_carve(workspace, batch, H, W, acc_blocks, &ws);
     taps = BlurTaps{};
     if (sigma > 0.0) {
         int rc = make_taps(sigma, &taps);
         if (rc) return rc;
     }
+    return EVK_OK;
+}
+
+// shared argument checks and set-up of the two flow entry points
+static int flow_obj_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
+                          int batch, int64_t n, const float *flow, int H, int W, double sigma, int objective, void *workspace,
+                          size_t workspace_bytes, FlowObjArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
+{
+    if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
+        (n > 0 && (!x || !y || !t || !p))) {
+        set_error("%s: bad arguments (0 <= batch <= 65535, H, W >= 2)", who);
+        return EVK_E_ARG;
+    }
+    int rc = batch_obj_check(who, "flow", batch, H, W, sigma, objective, flow_obj_acc_blocks(H, W), workspace, workspace_bytes, ws, taps);
+    if (rc) return rc;
     A = FlowObjArgs{};
     A.C.Hc = H + 1; A.C.Wc = W + 1;
     A.x = x; A.y = y; A.t = t; A.p = p; A.offsets = offsets; A.n = n;
@@ -1742,13 +1771,171 @@ static dim3 flow_obj_grid(int64_t n, int batch)
 }
 
 // G = blur(I) for every sample (blockIdx.z), both axes
-static void flow_obj_blur(const FlowObjWorkspace &ws, const float *I, int Hc, int Wc, const BlurTaps &taps, int batch, cudaStream_t st)
+static void batch_obj_blur(const BatchObjWorkspace &ws, const float *I, int Hc, int Wc, const BlurTaps &taps, int batch, cudaStream_t st)
 {
     const int do_blur = taps.r > 0 || taps.w[0] != 0.0;
     const dim3 g((Hc * Wc + 255) / 256, 1, batch);
     prof_count(do_blur ? 2 : 1);
     if (do_blur) cmax_blur_axis0_kernel<<<g, 256, 0, st>>>(I, ws.tmp, Hc, Wc, taps);
     cmax_blur_axis1_store_kernel<<<g, 256, 0, st>>>(ws.tmp, I, Hc, Wc, taps, do_blur, ws.G);
+}
+
+// forward tail after the event pass: the 2x2-block images in ws.acc -> iwe_out (NaN for a sample flagged in ws.nonfinite),
+// its blur and f of every sample
+static void batch_obj_forward_tail(const BatchObjWorkspace &ws, int Hc, int Wc, const BlurTaps &taps, int batch, int objective,
+                                   double obj_param, float *iwe_out, double *f_out, cudaStream_t st)
+{
+    const int npix = Hc * Wc;
+    const dim3 g((npix + 255) / 256, 1, batch);
+    prof_count(1);
+    flow_obj_fold_kernel<<<g, 256, 0, st>>>(ws.acc, ws.nonfinite, Hc, Wc, iwe_out);
+    batch_obj_blur(ws, iwe_out, Hc, Wc, taps, batch, st);
+    prof_count(2);
+    cmax_model_stats_kernel<<<g, 256, 0, st>>>(ws.G, iwe_out, npix, objective, obj_param, ws.gsums, ws.gmax, nullptr, nullptr);
+    flow_obj_final_kernel<<<(batch + 127) / 128, 128, 0, st>>>(objective, ws.gsums, npix, batch, f_out);
+}
+
+// first half of a backward: W_b = G(grad_f[b] df_b/dG) into ws.Wimg, with G recomputed from the saved IWE
+static void batch_obj_backward_W(const BatchObjWorkspace &ws, const float *iwe, int Hc, int Wc, const BlurTaps &taps, int batch,
+                                 int objective, double obj_param, const float *grad_f, cudaStream_t st)
+{
+    const int npix = Hc * Wc;
+    batch_obj_blur(ws, iwe, Hc, Wc, taps, batch, st);
+    const int do_blur = taps.r > 0 || taps.w[0] != 0.0;
+    const dim3 g((npix + 255) / 256, 1, batch);
+    prof_count(do_blur ? 3 : 2);
+    flow_obj_coef_kernel<<<g, 256, 0, st>>>(ws.G, npix, objective, obj_param, grad_f, ws.w);
+    if (do_blur) cmax_blur_d_axis0_kernel<<<g, 256, 0, st>>>(ws.w, ws.wt, Hc, Wc, taps);
+    cmax_blur_d_axis1_store_kernel<<<g, 256, 0, st>>>(ws.wt, ws.w, Hc, Wc, taps, do_blur, ws.Wimg);
+}
+
+// ---- parametric motion objective over a batch of samples (evk_cmax_motion_objective_f32 / _grad_f32) ---------------
+// Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by its own model params[b] -- linvel, rotation
+// or xyztheta through model_taps, with the bounds mask of event_util.py:26-27 at img_size = (H, W) and the splat of
+// image.py:179-217 on the (H+1)x(W+1) canvas -- then blurred and scored by the flow objective's image-space tail.  The
+// grid of both event passes is (slices, batch), as for the flow objective:
+//   forward:  one v4 reduction per kept event into the sample's 2x2-block image [B][Hc][Wc][4] (16 B per pixel)
+//   backward: W_b = G(g_b C_b) per sample (batch_obj_backward_W), then per event the four taps of W_b (L2 gathers) against
+//             the event's Jacobian (model_taps<..., true>), summed in f64 per thread as cmax_grad_pass_kernel does; a CTA
+//             reduction and one f64 atomic per component and CTA into grad [B][K] -- no reduction per event, and no
+//             canvas-size limit (W is not held in shared memory).
+struct MotionObjArgs {
+    CmaxArgs C;                  // canvas (Hc, Wc) and bounds mask (Hm, Wm) for model_taps; p_scale 1, t_ref 0
+    const float *x, *y, *t, *p;  // t relative to the sample's t0
+    const int64_t *offsets;
+    int64_t n;
+    const double *params;        // [B][K] on the device
+    double cx, cy;               // the centre of xyztheta
+    float *acc;                  // forward: [B][Hc][Wc][4]
+    const float *Wimg;           // backward: [B][Hc][Wc]
+    double *grad;                // backward: [B][K]
+};
+
+template <int WARP, bool GRAD>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_obj_event_kernel(const MotionObjArgs A)
+{
+    constexpr int K = model_dims(WARP);
+    const int b = blockIdx.y;
+    int64_t first = A.offsets[b], last = A.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > A.n) last = A.n;
+    const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
+    WarpModel M{};
+#pragma unroll
+    for (int k = 0; k < K; ++k) M.m[k] = A.params[(int64_t)b * K + k];
+    if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = A.cx; M.m[5] = A.cy; }
+    float *acc = GRAD ? nullptr : A.acc + b * npix * 4;
+    const float *Wb = GRAD ? A.Wimg + b * npix : nullptr;
+    double u[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) u[k] = 0.0;
+    unsigned oob = 0;   // a kept finite event lies inside the canvas; a non-finite one contributes nothing
+    auto one = [&](float xe, float ye, float te, float pe) {
+        Event<WARP> e;
+        e.x = xe; e.y = ye; e.t = te; e.p = pe;
+        Taps T;
+        float jx[4], jy[4];
+        if (!model_taps<WARP, GRAD>(A.C, e, M, oob, T, jx, jy)) return;
+        if (!GRAD) {
+            red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
+            return;
+        }
+        const int64_t r0 = (int64_t)T.y0 * A.C.Wc, r1 = (int64_t)T.y1 * A.C.Wc;
+        const double w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0), w11 = __ldg(Wb + r1 + T.x1);
+        const double dx = T.dx, dy = T.dy, ox = 1.0 - dx, oy = 1.0 - dy, wm = T.wm;
+        const double sx = oy * (w01 - w00) + dy * (w11 - w10);
+        const double sy = ox * (w10 - w00) + dx * (w11 - w01);
+#pragma unroll
+        for (int k = 0; k < K; ++k) u[k] += wm * ((double)jx[k] * sx + (double)jy[k] * sy);
+    };
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
+        float ex[kBatch], ey[kBatch], et[kBatch], ep[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            ex[k] = ld_stream(A.x + i + k * stride); ey[k] = ld_stream(A.y + i + k * stride);
+            et[k] = ld_stream(A.t + i + k * stride); ep[k] = ld_stream(A.p + i + k * stride);
+        }
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) one(ex[k], ey[k], et[k], ep[k]);
+    }
+    for (; i < last; i += stride) one(ld_stream(A.x + i), ld_stream(A.y + i), ld_stream(A.t + i), ld_stream(A.p + i));
+    if (!GRAD) return;
+    // CTA reduction, one f64 atomic per component and CTA
+    __shared__ double part[kFlowObjThreads / 32][K];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        double v = u[k];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) part[wid][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        double s = 0.0;
+        for (int w = 0; w < kFlowObjThreads / 32; ++w) s += part[w][threadIdx.x];
+        atomicAdd(A.grad + (int64_t)b * K + threadIdx.x, s);
+    }
+}
+
+static int motion_obj_dims(int warp)
+{
+    return warp == EVK_WARP_LINVEL ? 2 : warp == EVK_WARP_ROTATION ? 3 : warp == EVK_WARP_XYZTHETA ? 4 : 0;
+}
+
+// shared argument checks and set-up of the two motion entry points
+static int motion_obj_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
+                            int batch, int64_t n, int warp, const double *params, int K, double cx, double cy, int H, int W,
+                            double sigma, int objective, void *workspace, size_t workspace_bytes, MotionObjArgs &A,
+                            BatchObjWorkspace &ws, BlurTaps &taps)
+{
+    if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
+        (n > 0 && (!x || !y || !t || !p))) {
+        set_error("%s: bad arguments (0 <= batch <= 65535, H, W >= 2)", who);
+        return EVK_E_ARG;
+    }
+    const int dims = motion_obj_dims(warp);
+    if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
+    if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
+    int rc = batch_obj_check(who, "parameters", batch, H, W, sigma, objective, (size_t)(H + 1) * (W + 1), workspace, workspace_bytes,
+                             ws, taps);
+    if (rc) return rc;
+    A = MotionObjArgs{};
+    A.C.Hm = H; A.C.Wm = W; A.C.Hc = H + 1; A.C.Wc = W + 1;
+    A.C.p_scale = 1.0;
+    A.x = x; A.y = y; A.t = t; A.p = p; A.offsets = offsets; A.n = n;
+    A.params = params; A.cx = cx; A.cy = cy;
+    return EVK_OK;
+}
+
+template <bool GRAD>
+static void launch_motion_obj_events(int warp, const MotionObjArgs &A, int batch, cudaStream_t st)
+{
+    const dim3 grid = flow_obj_grid(A.n, batch);
+    if (warp == EVK_WARP_LINVEL) motion_obj_event_kernel<WARP_LINVEL_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else if (warp == EVK_WARP_ROTATION) motion_obj_event_kernel<WARP_ROTATION_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else motion_obj_event_kernel<WARP_XYZTHETA_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
 }
 
 }  // namespace evk
@@ -2094,7 +2281,7 @@ int evk_cmax_warp_objective_batch_f64(const double *x, const double *y, const do
 size_t evk_cmax_flow_objective_workspace_bytes(int batch, int H, int W)
 {
     if (batch < 0 || H < 2 || W < 2) return 0;
-    return evk::flow_obj_carve(nullptr, batch, H, W, nullptr);
+    return evk::batch_obj_carve(nullptr, batch, H, W, evk::flow_obj_acc_blocks(H, W), nullptr);
 }
 
 int evk_cmax_flow_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
@@ -2104,7 +2291,7 @@ int evk_cmax_flow_objective_f32(const float *x, const float *y, const float *t_r
 {
     using namespace evk;
     FlowObjArgs A;
-    FlowObjWorkspace ws;
+    BatchObjWorkspace ws;
     BlurTaps taps;
     int rc = flow_obj_setup("evk_cmax_flow_objective_f32", x, y, t_rel, p, offsets, batch, n_events, flow, H, W, sigma, objective,
                             workspace, workspace_bytes, A, ws, taps);
@@ -2121,13 +2308,7 @@ int evk_cmax_flow_objective_f32(const float *x, const float *y, const float *t_r
         prof_count(1);
         flow_obj_event_kernel<false><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
     }
-    const dim3 g((npix + 255) / 256, 1, batch);
-    prof_count(1);
-    flow_obj_fold_kernel<<<g, 256, 0, st>>>(ws.acc, ws.nonfinite, Hc, Wc, iwe_out);
-    flow_obj_blur(ws, iwe_out, Hc, Wc, taps, batch, st);
-    prof_count(2);
-    cmax_model_stats_kernel<<<g, 256, 0, st>>>(ws.G, iwe_out, npix, objective, obj_param, ws.gsums, ws.gmax, nullptr, nullptr);
-    flow_obj_final_kernel<<<(batch + 127) / 128, 128, 0, st>>>(objective, ws.gsums, npix, batch, f_out);
+    batch_obj_forward_tail(ws, Hc, Wc, taps, batch, objective, obj_param, iwe_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }
@@ -2139,7 +2320,7 @@ int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float
 {
     using namespace evk;
     FlowObjArgs A;
-    FlowObjWorkspace ws;
+    BatchObjWorkspace ws;
     BlurTaps taps;
     int rc = flow_obj_setup("evk_cmax_flow_objective_grad_f32", x, y, t_rel, p, offsets, batch, n_events, flow, H, W, sigma,
                             objective, workspace, workspace_bytes, A, ws, taps);
@@ -2147,17 +2328,11 @@ int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float
     if (batch > 0 && (!iwe || !grad_f || !grad_flow)) { set_error("evk_cmax_flow_objective_grad_f32: null array"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc;
+    const int Hc = H + 1, Wc = W + 1;
     const int64_t planes = (int64_t)batch * 2;
     EVK_CUDA(cudaMemsetAsync(ws.acc, 0, (size_t)planes * H * W * 4 * sizeof(float), st));
     // W = G(g_b C_b): recompute G from the saved IWE, the coefficient image, its blur
-    flow_obj_blur(ws, iwe, Hc, Wc, taps, batch, st);
-    const int do_blur = taps.r > 0 || taps.w[0] != 0.0;
-    const dim3 g((npix + 255) / 256, 1, batch);
-    prof_count(do_blur ? 3 : 2);
-    flow_obj_coef_kernel<<<g, 256, 0, st>>>(ws.G, npix, objective, obj_param, grad_f, ws.w);
-    if (do_blur) cmax_blur_d_axis0_kernel<<<g, 256, 0, st>>>(ws.w, ws.wt, Hc, Wc, taps);
-    cmax_blur_d_axis1_store_kernel<<<g, 256, 0, st>>>(ws.wt, ws.w, Hc, Wc, taps, do_blur, ws.Wimg);
+    batch_obj_backward_W(ws, iwe, Hc, Wc, taps, batch, objective, obj_param, grad_f, st);
     A.acc = ws.acc;
     A.Wimg = ws.Wimg;
     if (n_events > 0) {
@@ -2167,6 +2342,70 @@ int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float
     }
     prof_count(1);
     flow_obj_grad_fold_kernel<<<grid_simple(planes * H * W, 256), 256, 0, st>>>(ws.acc, grad_flow, planes, H, W);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W)
+{
+    if (batch < 0 || H < 2 || W < 2) return 0;
+    return evk::batch_obj_carve(nullptr, batch, H, W, (size_t)(H + 1) * (W + 1), nullptr);
+}
+
+int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                  int batch, int64_t n_events, int warp, const double *params, int K, double cx, double cy,
+                                  int H, int W, double sigma, int objective, double obj_param, double *f_out, float *iwe_out,
+                                  void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    MotionObjArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_obj_setup("evk_cmax_motion_objective_f32", x, y, t_rel, p, offsets, batch, n_events, warp, params, K, cx, cy,
+                              H, W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !iwe_out)) { set_error("evk_cmax_motion_objective_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc;
+    // nonfinite stays zero: a motion sample's non-finite events contribute nothing (model_taps), as in the single window
+    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)batch * npix * 4 * sizeof(float), st));
+    A.acc = ws.acc;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_obj_events<false>(warp, A, batch, st);
+    }
+    batch_obj_forward_tail(ws, Hc, Wc, taps, batch, objective, obj_param, iwe_out, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                       int batch, int64_t n_events, int warp, const double *params, int K, double cx, double cy,
+                                       int H, int W, double sigma, int objective, double obj_param, const float *iwe,
+                                       const float *grad_f, double *grad_params, void *workspace, size_t workspace_bytes,
+                                       void *stream)
+{
+    using namespace evk;
+    MotionObjArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_obj_setup("evk_cmax_motion_objective_grad_f32", x, y, t_rel, p, offsets, batch, n_events, warp, params, K, cx,
+                              cy, H, W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!iwe || !grad_f || !grad_params)) { set_error("evk_cmax_motion_objective_grad_f32: null array"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    EVK_CUDA(cudaMemsetAsync(grad_params, 0, (size_t)batch * K * sizeof(double), st));
+    batch_obj_backward_W(ws, iwe, H + 1, W + 1, taps, batch, objective, obj_param, grad_f, st);
+    A.Wimg = ws.Wimg;
+    A.grad = grad_params;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_obj_events<true>(warp, A, batch, st);
+    }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }

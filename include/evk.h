@@ -494,6 +494,42 @@ int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float
                                      const float *iwe, const float *grad_f, float *grad_flow,
                                      void *workspace, size_t workspace_bytes, void *stream);
 
+/* Parametric contrast maximisation over a batch of samples, as a differentiable loss: per sample the f32
+ * fast-mode evaluation of evk_cmax_warp_objective_f32 / evk_cmax_linvel_objective_f32 with Hm = Hs = H,
+ * Wm = Ws = W, p_scale 1 and no flags (get_iwe, lib/contrast_max/objectives.py:184-192).  Sample b is the
+ * events [offsets[b], offsets[b+1]) (clipped to [0, n_events); end < start is empty), warped by its own
+ * parameters params[b] (K doubles, in DEVICE memory) with the model `warp`:
+ *   EVK_WARP_LINVEL    (vx, vy)                K = 2   x' = x - t_rel vx (lib/contrast_max/warps.py:51-61)
+ *   EVK_WARP_ROTATION  (cx, cy, omega)         K = 3
+ *   EVK_WARP_XYZTHETA  (hx, hy, hz, theta)     K = 4   about the centre (cx, cy) given here (ignored otherwise)
+ * in f32, in the order written.  An event is kept iff 0 < x' <= W and 0 < y' <= H (events_bounds_mask,
+ * lib/util/event_util.py:26-27; NaN compares false and is kept, then contributes nothing) and splatted
+ * bilinearly on the (H+1)x(W+1) canvas (events_to_image_drv, lib/representations/image.py:179-217).  Then
+ * G = gaussian_filter(IWE, sigma) and f is one of the four objectives of evk_cmax_flow_objective_f32
+ * (EVK_OBJ_MOA / EVK_OBJ_ISOA: EVK_E_UNSUPPORTED).
+ *   f_out   : batch doubles;  iwe_out: [batch][H+1][W+1] floats, which the backward takes as `iwe`
+ * evk_cmax_motion_objective_grad_f32 writes grad_params [batch][K] doubles = grad_f[b] df_b/dparams[b], the
+ * exact derivative of the f above with the floor and keep decisions held (grad_f: batch floats on the device):
+ * with W_b = G(grad_f[b] df_b/dG), per kept event
+ *   df/dparams_k += p[(1-dy)(W01-W00) + dy(W11-W10)] dx'/dparams_k + p[(1-dx)(W10-W00) + dx(W11-W01)] dy'/dparams_k
+ * For linvel this is not the reference's evaluate_gradient (objectives.py:251-264), which mixes the two
+ * channels in its 3-D blur and multiplies by the un-blurred IWE.  No limit on the canvas size.
+ * workspace: evk_cmax_motion_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
+ * Neither call synchronises, and both launch the same kernels whatever the batch. */
+#define EVK_WARP_LINVEL 3
+size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W);
+int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                  const int64_t *offsets, int batch, int64_t n_events, int warp,
+                                  const double *params, int K, double cx, double cy, int H, int W,
+                                  double sigma, int objective, double obj_param, double *f_out,
+                                  float *iwe_out, void *workspace, size_t workspace_bytes, void *stream);
+int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                       const int64_t *offsets, int batch, int64_t n_events, int warp,
+                                       const double *params, int K, double cx, double cy, int H, int W,
+                                       double sigma, int objective, double obj_param, const float *iwe,
+                                       const float *grad_f, double *grad_params, void *workspace,
+                                       size_t workspace_bytes, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * RobustNorm (row f4): clamp a tensor between two of its order statistics and rescale it.  Replaces
  * RobustNorm.__call__ / .percentile, lib/data_loaders/data_augmentation.py:82-130 (two kthvalue sorts),
