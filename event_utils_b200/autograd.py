@@ -14,6 +14,7 @@ Which inputs get a gradient (as in the reference; the others get None):
                                      events_to_voxel_timesync_torch
     events_to_neg_pos_voxel_torch    ts (voxel_grid.py:155-182)
     flow_contrast_objective_torch    flow only (contrast_max/flow_objective.py; the events are data)
+    flow_timestamp_objective_torch   flow only (contrast_max/flow_timestamp_objective.py; the events are data)
     motion_contrast_objective_torch  params only (contrast_max/motion_objective.py; the events are data)
 
 The public functions take this path only when grad mode is on and one of those inputs requires grad; every
@@ -215,6 +216,50 @@ class FlowObjective(torch.autograd.Function):
                 H, W, sigma, objective, param, _lib.ptr(iwe), _lib.ptr(g), _lib.ptr(gf), _lib.ptr(ws), ws.numel(),
                 _lib.stream()))
         return _as_input(gf, ctx.meta), None, None, None, None, None, None
+
+
+class FlowTimestampObjective(torch.autograd.Function):
+    """The batched dense-flow average-timestamp loss of contrast_max/flow_timestamp_objective.py (optic_flow.py:5-46,
+    image.py:286-353, then the sum of squares of objectives.py:524-551): f (B,) f64 from flow (B,2,H,W) and the prepared
+    device events with their normalised stamps tau.  Only the flow gets a gradient: the exact derivative of f, one pass
+    over the events (evk_flow_timestamp_objective_grad_f32).  The forward keeps the timestamp and count images."""
+
+    @staticmethod
+    def forward(ctx, flow, x, y, t_rel, tau, p, offsets, sigma):
+        dev = x.device
+        B, _, H, W = flow.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            f32 = flow.detach().to(device=dev, dtype=torch.float32).contiguous()
+            f = torch.empty(B, dtype=torch.float64, device=dev)
+            ts_img = torch.empty((B, 2, H + 1, W + 1), dtype=torch.float32, device=dev)
+            cnt_img = torch.empty_like(ts_img)
+            ws = _lib.scratch("flow_timestamp_objective", L.evk_flow_timestamp_objective_workspace_bytes(B, H, W), dev)
+            _lib.check(L.evk_flow_timestamp_objective_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0],
+                _lib.ptr(f32), H, W, sigma, _lib.ptr(f), _lib.ptr(ts_img), _lib.ptr(cnt_img), _lib.ptr(ws), ws.numel(),
+                _lib.stream()))
+        ctx.save_for_backward(x, y, t_rel, tau, p, offsets, f32, ts_img, cnt_img)
+        ctx.sigma = sigma
+        ctx.meta = _meta(flow)
+        return f
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, y, t_rel, tau, p, offsets, f32, ts_img, cnt_img = ctx.saved_tensors
+        dev = x.device
+        B, _, H, W = f32.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g = _grad_in(g, dev)
+            gf = torch.empty_like(f32)
+            ws = _lib.scratch("flow_timestamp_objective", L.evk_flow_timestamp_objective_workspace_bytes(B, H, W), dev)
+            _lib.check(L.evk_flow_timestamp_objective_grad_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0],
+                _lib.ptr(f32), H, W, ctx.sigma, _lib.ptr(ts_img), _lib.ptr(cnt_img), _lib.ptr(g), _lib.ptr(gf),
+                _lib.ptr(ws), ws.numel(), _lib.stream()))
+        return _as_input(gf, ctx.meta), None, None, None, None, None, None, None
 
 
 class MotionObjective(torch.autograd.Function):

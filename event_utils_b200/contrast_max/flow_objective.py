@@ -40,11 +40,7 @@ def flow_contrast_objective_torch(xs, ys, ts, ps, flow, t0=None, objective="vari
     """
     _check_objective(objective, "flow")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "flow_contrast_objective_torch", "the flow")
-    flow = E.as_tensor(flow)
-    if flow.dim() == 3:
-        flow = flow.unsqueeze(0)
-    if flow.dim() != 4 or flow.shape[1] != 2:
-        raise ValueError("flow must have shape (B,2,H,W) or (2,H,W), got %s" % (tuple(flow.shape),))
+    flow = _flow_batch(flow)
     B, H, W = flow.shape[0], flow.shape[2], flow.shape[3]
     _lib.lib()
     dev = E.compute_device(flow, xs, ys, ts, ps)
@@ -53,6 +49,16 @@ def flow_contrast_objective_torch(xs, ys, ts, ps, flow, t0=None, objective="vari
     param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
     f = FlowObjective.apply(flow, x, y, t_rel, p, offsets, (OBJECTIVES[objective], float(blur_sigma), param))
     return f.to(device=flow.device, dtype=flow.dtype)
+
+
+def _flow_batch(flow):
+    """flow as a (B,2,H,W) tensor ((2,H,W) is one sample)"""
+    flow = E.as_tensor(flow)
+    if flow.dim() == 3:
+        flow = flow.unsqueeze(0)
+    if flow.dim() != 4 or flow.shape[1] != 2:
+        raise ValueError("flow must have shape (B,2,H,W) or (2,H,W), got %s" % (tuple(flow.shape),))
+    return flow
 
 
 def _check_objective(objective, wrt):
@@ -75,9 +81,10 @@ def _event_tensors(xs, ys, ts, ps, t0, who, wrt):
     return xs, ys, ts, ps
 
 
-def _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what):
+def _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what, stamps=False):
     """The events of a batch of B samples on `dev` as the batched kernels take them: x, y, p f32, t_rel = t - t0_b
-    formed in ts' dtype then cast to f32 (t0 None: each sample's last stamp), and the B+1 int64 sample offsets."""
+    formed in ts' dtype then cast to f32 (t0 None: each sample's last stamp), and the B+1 int64 sample offsets.
+    With `stamps`, also the stamps on `dev` in that dtype and the sample index of every event."""
     n = xs.shape[0]
     with torch.cuda.device(dev):
         if batch_end_indices is None:
@@ -95,6 +102,7 @@ def _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what):
         t = t.to(rt)
         if n == 0:
             t_rel = torch.empty(0, dtype=torch.float32, device=dev)
+            sample = torch.empty(0, dtype=torch.int64, device=dev)
         else:
             if t0 is None:
                 t0b = t[(ends - 1).clamp(0, n - 1)]                     # each sample's last event (as warp_events_flow_torch)
@@ -103,4 +111,6 @@ def _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what):
             # the sample of each event: windows are contiguous, [ends[b-1], ends[b])
             sample = torch.searchsorted(ends, torch.arange(n, device=dev), right=True).clamp_(max=B - 1)
             t_rel = (t - t0b.to(rt)[sample]).to(torch.float32).contiguous()
+    if stamps:
+        return x, y, t_rel, p, offsets, t, sample
     return x, y, t_rel, p, offsets

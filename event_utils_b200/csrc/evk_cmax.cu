@@ -1541,24 +1541,10 @@ __device__ __forceinline__ bool flow_obj_warp(const FlowObjArgs &A, const float 
     return splat_taps<false>(A.C, xw, yw, p, 0.0f, true, oob, T);
 }
 
-template <bool GRAD>
-__device__ __forceinline__ void flow_obj_event(const FlowObjArgs &A, const float *flow, float *acc, const float *Wb,
-                                               float xe, float ye, float d, float p, bool &nonfinite)
+// The backward of the flow losses: an event's df/dflow = (gu, gv) times the weights of its four grid_sample taps, added to
+// the 2x2-block flow gradient acc [2][H][W][4] of its sample; taps outside the field get nothing.
+__device__ __forceinline__ void flow_obj_spread(const FlowObjArgs &A, float *acc, const FlowSample &s, float gu, float gv)
 {
-    FlowSample s;
-    Taps T;
-    if (!flow_obj_warp(A, flow, xe, ye, d, p, s, T, nonfinite)) return;
-    if (!GRAD) {
-        red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
-        return;
-    }
-    // df/dx' and df/dy' through the four bilinear taps of the IWE (the sx / sy of cmax_grad_pass_kernel)
-    const int r0 = T.y0 * A.C.Wc, r1 = T.y1 * A.C.Wc;
-    const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0), w11 = __ldg(Wb + r1 + T.x1);
-    const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
-    const float sx = T.wm * (oy * (w01 - w00) + T.dy * (w11 - w10));
-    const float sy = T.wm * (ox * (w10 - w00) + T.dx * (w11 - w01));
-    const float gu = sx * d, gv = sy * d;
     if (!s.sampled || (gu == 0.0f && gv == 0.0f)) return;
     const int64_t plane4 = (int64_t)A.H * A.W * 4;
     if (s.x0 >= 0 && s.x0 + 1 < A.W && s.y0 >= 0 && s.y0 + 1 < A.H) {
@@ -1577,6 +1563,26 @@ __device__ __forceinline__ void flow_obj_event(const FlowObjArgs &A, const float
             red_add(blk + plane4, gv * w[k]);
         }
     }
+}
+
+template <bool GRAD>
+__device__ __forceinline__ void flow_obj_event(const FlowObjArgs &A, const float *flow, float *acc, const float *Wb,
+                                               float xe, float ye, float d, float p, bool &nonfinite)
+{
+    FlowSample s;
+    Taps T;
+    if (!flow_obj_warp(A, flow, xe, ye, d, p, s, T, nonfinite)) return;
+    if (!GRAD) {
+        red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
+        return;
+    }
+    // df/dx' and df/dy' through the four bilinear taps of the IWE (the sx / sy of cmax_grad_pass_kernel)
+    const int r0 = T.y0 * A.C.Wc, r1 = T.y1 * A.C.Wc;
+    const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0), w11 = __ldg(Wb + r1 + T.x1);
+    const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
+    const float sx = T.wm * (oy * (w01 - w00) + T.dy * (w11 - w10));
+    const float sy = T.wm * (ox * (w10 - w00) + T.dx * (w11 - w01));
+    flow_obj_spread(A, acc, s, sx * d, sy * d);
 }
 
 template <bool GRAD>
@@ -1936,6 +1942,157 @@ static void launch_motion_obj_events(int warp, const MotionObjArgs &A, int batch
     if (warp == EVK_WARP_LINVEL) motion_obj_event_kernel<WARP_LINVEL_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
     else if (warp == EVK_WARP_ROTATION) motion_obj_event_kernel<WARP_ROTATION_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
     else motion_obj_event_kernel<WARP_XYZTHETA_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
+}
+
+// ---- dense-flow average-timestamp (Zhu) loss over a batch of samples (evk_flow_timestamp_objective_f32 / _grad_f32) --
+// Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by flow[b] with the flow objective's warp and keep
+// rule (flow_obj_warp), then the average-timestamp images of events_to_timestamp_image_torch (image.py:286-353) on the
+// (H+1)x(W+1) canvas, one per polarity s (p > 0 / p <= 0, a NaN p in neither): S_s = sum tau k, C_s = 1 + sum k over the
+// bilinear taps k, T_s = S_s / C_s, and f_b = sum G(T_+)^2 + sum G(T_-)^2.  The 2B images are numbered z = 2b + s, so the
+// batched blur, the statistics and the adjoint blur of the other batched losses run over them as over 2B samples.
+//   forward:  two v4 reductions per kept event into the 32-byte block {S taps, C taps} of its polarity, [B][2][Hc][Wc][8]
+//             (evk_tsimg.cu's layout and arithmetic); a fold to T and C; the blur; per image an f64 sum of G^2.
+//   backward: U_s = G(2 g_b G_s) (f64 adjoint blur); (A_s, B_s) = (U_s / C_s, -U_s T_s / C_s) as f32 pairs
+//             [B][2][Hc][Wc][2]; per kept event the four pairs of its polarity give dF/dk = tau A + B per tap, then
+//             df/dx', df/dy' through the tap weights as in flow_obj_event, spread by flow_obj_spread.
+struct FlowTsArgs {
+    FlowObjArgs F;     // warp, keep rule and samples; F.acc: forward [B][2][Hc][Wc][8], backward the flow-gradient blocks
+    const float *tau;  // the normalised stamp of every event
+    const float2 *ab;  // backward: (A, B) [B][2][Hc][Wc]
+};
+
+// one 32-byte block per canvas pixel and polarity; the backward's flow-gradient blocks ([2][H][W] per sample) are fewer
+static size_t flow_ts_acc_blocks(int H, int W) { return (size_t)2 * (H + 1) * (W + 1); }
+
+template <bool GRAD>
+__device__ __forceinline__ void flow_ts_event(const FlowTsArgs &A, const float *flow, float *acc, const float2 *ab, float xe,
+                                              float ye, float d, float tau, float p, bool &nonfinite)
+{
+    FlowSample s;
+    Taps T;
+    if (!flow_obj_warp(A.F, flow, xe, ye, d, 1.0f, s, T, nonfinite)) return;
+    const bool pos = p > 0.0f;
+    if (!pos && !(p <= 0.0f)) return;   // NaN polarity: in neither image (evk_tsimg.cu)
+    const int Wc = A.F.C.Wc;
+    const int64_t plane = (int64_t)A.F.C.Hc * Wc;
+    const float dx = T.dx, dy = T.dy;
+    const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+    if (!GRAD) {
+        // tsimg_scatter_kernel's taps: tau (1-dx)(1-dy) .. and (1-dx)(1-dy) ..
+        const float tl = __fmul_rn(tau, ox), tr = __fmul_rn(tau, dx);
+        float *blk = acc + ((pos ? 0 : plane) + (int64_t)T.y0 * Wc + T.x0) * 8;
+        red_add4(blk, make_float4(__fmul_rn(tl, oy), __fmul_rn(tr, oy), __fmul_rn(tl, dy), __fmul_rn(tr, dy)));
+        red_add4(blk + 4, make_float4(__fmul_rn(ox, oy), __fmul_rn(dx, oy), __fmul_rn(ox, dy), __fmul_rn(dx, dy)));
+        return;
+    }
+    if (!pos) ab += plane;
+    const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
+    const float2 a00 = __ldg(ab + r0 + T.x0), a01 = __ldg(ab + r0 + T.x1), a10 = __ldg(ab + r1 + T.x0), a11 = __ldg(ab + r1 + T.x1);
+    const float q00 = tau * a00.x + a00.y, q01 = tau * a01.x + a01.y, q10 = tau * a10.x + a10.y, q11 = tau * a11.x + a11.y;
+    const float sx = oy * (q01 - q00) + dy * (q11 - q10);
+    const float sy = ox * (q10 - q00) + dx * (q11 - q01);
+    flow_obj_spread(A.F, acc, s, sx * d, sy * d);
+}
+
+template <bool GRAD>
+__global__ void __launch_bounds__(kFlowObjThreads) flow_ts_event_kernel(const FlowTsArgs A)
+{
+    const int b = blockIdx.y;
+    int64_t first = A.F.offsets[b], last = A.F.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > A.F.n) last = A.F.n;
+    const int64_t npix = (int64_t)A.F.C.Hc * A.F.C.Wc;
+    const float *flow = A.F.flow + (int64_t)b * 2 * A.F.H * A.F.W;
+    float *acc = A.F.acc + (GRAD ? (int64_t)b * 2 * A.F.H * A.F.W * 4 : (int64_t)b * 2 * npix * 8);
+    const float2 *ab = GRAD ? A.ab + (int64_t)b * 2 * npix : nullptr;
+    bool nonfinite = false;
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
+        float ex[kBatch], ey[kBatch], et[kBatch], eu[kBatch], ep[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            ex[k] = ld_stream(A.F.x + i + k * stride); ey[k] = ld_stream(A.F.y + i + k * stride);
+            et[k] = ld_stream(A.F.t + i + k * stride); eu[k] = ld_stream(A.tau + i + k * stride);
+            ep[k] = ld_stream(A.F.p + i + k * stride);
+        }
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) flow_ts_event<GRAD>(A, flow, acc, ab, ex[k], ey[k], et[k], eu[k], ep[k], nonfinite);
+    }
+    for (; i < last; i += stride)
+        flow_ts_event<GRAD>(A, flow, acc, ab, ld_stream(A.F.x + i), ld_stream(A.F.y + i), ld_stream(A.F.t + i),
+                            ld_stream(A.tau + i), ld_stream(A.F.p + i), nonfinite);
+    if (!GRAD && nonfinite) A.F.nonfinite[b] = 1u;
+}
+
+// blocks -> T and C of every image z = 2b + s (blockIdx.z), tsimg_fold_kernel's arithmetic (the count starts at one, so its
+// zero guard never fires); both all-NaN for a sample flagged in nonfinite, so that its f and its gradient are NaN
+__global__ void __launch_bounds__(256) flow_ts_fold_kernel(const float *__restrict__ acc, const unsigned *__restrict__ nonfinite,
+                                                           int Hc, int Wc, float *__restrict__ ts, float *__restrict__ cnt)
+{
+    const int64_t npix = (int64_t)Hc * Wc;
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= npix) return;
+    const int64_t k = blockIdx.z * npix + i;
+    const float *b = acc + k * 8;
+    const int y = i / Wc, x = i - y * Wc;
+    float tsum = b[0], csum = b[4];
+    if (x > 0) { tsum += b[-8 + 1]; csum += b[-8 + 5]; }
+    if (y > 0) { tsum += b[-8 * (int64_t)Wc + 2]; csum += b[-8 * (int64_t)Wc + 6]; }
+    if (x > 0 && y > 0) { tsum += b[-8 * ((int64_t)Wc + 1) + 3]; csum += b[-8 * ((int64_t)Wc + 1) + 7]; }
+    const float c = __fadd_rn(1.0f, csum);
+    const bool bad = nonfinite[blockIdx.z >> 1] != 0;
+    ts[k] = bad ? __int_as_float(0x7fc00000) : __fdiv_rn(tsum, c);
+    cnt[k] = bad ? __int_as_float(0x7fc00000) : c;
+}
+
+// f_b = sum G_+^2 + sum G_-^2 from the f64 sums of cmax_model_stats_kernel (gsums[z][5])
+__global__ void flow_ts_final_kernel(const double *gsums, int batch, double *f_out)
+{
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < batch) f_out[b] = gsums[8 * (2 * b) + 5] + gsums[8 * (2 * b + 1) + 5];
+}
+
+// the coefficient image 2 g_b G_s of df/dG, before the adjoint blur turns it into U_s
+__global__ void __launch_bounds__(256) flow_ts_coef_kernel(const float *__restrict__ G, int npix, const float *__restrict__ grad_f,
+                                                           double *__restrict__ w)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= npix) return;
+    const size_t k = (size_t)blockIdx.z * npix + i;
+    w[k] = 2.0 * (double)grad_f[blockIdx.z >> 1] * (double)G[k];
+}
+
+// dF/dS = U / C and dF/dC = -U T / C per pixel: the pair (A, B) the event pass gathers
+__global__ void __launch_bounds__(256) flow_ts_ab_kernel(const float *__restrict__ U, const float *__restrict__ ts,
+                                                         const float *__restrict__ cnt, int npix, float2 *__restrict__ ab)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= npix) return;
+    const size_t k = (size_t)blockIdx.z * npix + i;
+    const double u = (double)U[k], c = (double)cnt[k];
+    ab[k] = make_float2((float)(u / c), (float)(-u * (double)ts[k] / c));
+}
+
+// shared argument checks and set-up of the two timestamp entry points (those of flow_obj_setup, for 2B images)
+static int flow_ts_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
+                         const int64_t *offsets, int batch, int64_t n, const float *flow, int H, int W, double sigma,
+                         void *workspace, size_t workspace_bytes, FlowTsArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
+{
+    if (batch < 0 || batch > 32767 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
+        (n > 0 && (!x || !y || !t || !tau || !p))) {
+        set_error("%s: bad arguments (0 <= batch <= 32767, H, W >= 2)", who);
+        return EVK_E_ARG;
+    }
+    int rc = batch_obj_check(who, "flow", 2 * batch, H, W, sigma, OBJ_SOS, flow_ts_acc_blocks(H, W), workspace, workspace_bytes,
+                             ws, taps);
+    if (rc) return rc;
+    A = FlowTsArgs{};
+    A.F.C.Hc = H + 1; A.F.C.Wc = W + 1;
+    A.F.x = x; A.F.y = y; A.F.t = t; A.F.p = p; A.F.offsets = offsets; A.F.n = n;
+    A.F.flow = flow; A.F.H = H; A.F.W = W;
+    A.tau = tau;
+    return EVK_OK;
 }
 
 }  // namespace evk
@@ -2406,6 +2563,91 @@ int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const flo
         prof_count(1);
         launch_motion_obj_events<true>(warp, A, batch, st);
     }
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_flow_timestamp_objective_workspace_bytes(int batch, int H, int W)
+{
+    if (batch < 0 || H < 2 || W < 2) return 0;
+    return evk::batch_obj_carve(nullptr, 2 * batch, H, W, evk::flow_ts_acc_blocks(H, W), nullptr);
+}
+
+int evk_flow_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                     const int64_t *offsets, int batch, int64_t n_events, const float *flow, int H, int W,
+                                     double sigma, double *f_out, float *ts_out, float *cnt_out, void *workspace,
+                                     size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    FlowTsArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = flow_ts_setup("evk_flow_timestamp_objective_f32", x, y, t_rel, tau, p, offsets, batch, n_events, flow, H, W, sigma,
+                           workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !ts_out || !cnt_out)) { set_error("evk_flow_timestamp_objective_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch;
+    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)images * npix * 8 * sizeof(float), st));
+    A.F.acc = ws.acc;
+    A.F.nonfinite = ws.nonfinite;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        flow_ts_event_kernel<false><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+    }
+    const dim3 g((npix + 255) / 256, 1, images);
+    prof_count(1);
+    flow_ts_fold_kernel<<<g, 256, 0, st>>>(ws.acc, ws.nonfinite, Hc, Wc, ts_out, cnt_out);
+    batch_obj_blur(ws, ts_out, Hc, Wc, taps, images, st);
+    prof_count(2);
+    cmax_model_stats_kernel<<<g, 256, 0, st>>>(ws.G, ts_out, npix, OBJ_SOS, 0.0, ws.gsums, ws.gmax, nullptr, nullptr);
+    flow_ts_final_kernel<<<(batch + 127) / 128, 128, 0, st>>>(ws.gsums, batch, f_out);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                          const int64_t *offsets, int batch, int64_t n_events, const float *flow, int H, int W,
+                                          double sigma, const float *ts_img, const float *cnt_img, const float *grad_f,
+                                          float *grad_flow, void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    FlowTsArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = flow_ts_setup("evk_flow_timestamp_objective_grad_f32", x, y, t_rel, tau, p, offsets, batch, n_events, flow, H, W,
+                           sigma, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!ts_img || !cnt_img || !grad_f || !grad_flow)) {
+        set_error("evk_flow_timestamp_objective_grad_f32: null array");
+        return EVK_E_ARG;
+    }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch;
+    EVK_CUDA(cudaMemsetAsync(ws.acc, 0, (size_t)images * H * W * 4 * sizeof(float), st));
+    // U = G(2 g_b G_s): recompute G from the saved T, the coefficient image, its adjoint blur (into ws.Wimg)
+    batch_obj_blur(ws, ts_img, Hc, Wc, taps, images, st);
+    const int do_blur = taps.r > 0 || taps.w[0] != 0.0;
+    const dim3 g((npix + 255) / 256, 1, images);
+    prof_count(do_blur ? 4 : 3);
+    flow_ts_coef_kernel<<<g, 256, 0, st>>>(ws.G, npix, grad_f, ws.w);
+    if (do_blur) cmax_blur_d_axis0_kernel<<<g, 256, 0, st>>>(ws.w, ws.wt, Hc, Wc, taps);
+    cmax_blur_d_axis1_store_kernel<<<g, 256, 0, st>>>(ws.wt, ws.w, Hc, Wc, taps, do_blur, ws.Wimg);
+    // the pairs go to ws.wt (8 bytes per pixel), which the blur above has finished reading
+    float2 *ab = reinterpret_cast<float2 *>(ws.wt);
+    flow_ts_ab_kernel<<<g, 256, 0, st>>>(ws.Wimg, ts_img, cnt_img, npix, ab);
+    A.F.acc = ws.acc;
+    A.ab = ab;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        flow_ts_event_kernel<true><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+    }
+    prof_count(1);
+    flow_obj_grad_fold_kernel<<<grid_simple((int64_t)images * H * W, 256), 256, 0, st>>>(ws.acc, grad_flow, images, H, W);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }

@@ -530,6 +530,40 @@ int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const flo
                                        const float *grad_f, double *grad_params, void *workspace,
                                        size_t workspace_bytes, void *stream);
 
+/* Dense-flow average-timestamp loss (Zhu et al., CVPR'19) over a batch of samples, as a differentiable loss:
+ * warp_events_flow_torch (lib/transforms/optic_flow.py:5-46), then the timestamp images of
+ * events_to_timestamp_image_torch (lib/representations/image.py:286-353) on the canvas of motion_compensate
+ * (lib/visualization/draw_flow.py:15-26), blurred and squared as zhu_timestamp_objective does
+ * (lib/contrast_max/objectives.py:524-551), with the sign of a loss to minimise.  Sample b is the events
+ * [offsets[b], offsets[b+1]) (clipped to [0, n_events); end < start is empty), warped by flow[b] and kept exactly
+ * as in evk_cmax_flow_objective_f32 (0 <= x' < W, 0 <= y' < H; a non-finite x' or y' makes the sample's f NaN).
+ * tau is each event's normalised stamp, prepared by the caller: (t - t_first) / (t_last - t_first + 1e-6) of its
+ * sample, or (-t + t_last) / (...) for the reversed images.  Per polarity s (p > 0 / p <= 0; a NaN p is dropped),
+ * with k the bilinear tap weights of the kept events on the (H+1)x(W+1) canvas:
+ *   T_s = S_s / C_s,  S_s = sum tau k,  C_s = 1 + sum k,   f_b = sum gaussian_filter(T_+, sigma)^2 + sum (...T_-...)^2
+ * (sigma 0: no blur).
+ *   x, y, t_rel, tau, p : n_events floats;  offsets: batch+1 int64 on the device;  flow: [batch][2][H][W] f32
+ *   f_out: batch doubles;  ts_out, cnt_out: [batch][2][H+1][W+1] floats (T and C, polarity 0 positive), which the
+ *   backward takes as ts_img, cnt_img.  0 <= batch <= 32767.
+ * evk_flow_timestamp_objective_grad_f32 writes grad_flow [batch][2][H][W] = grad_f[b] df_b/dflow[b], the exact
+ * derivative of the f above with the floor and keep decisions held (grad_f: batch floats on the device): with
+ * U_s = G(2 grad_f[b] G_s), A_s = U_s / C_s and B_s = -U_s T_s / C_s, per kept event of polarity s and each of its
+ * four taps q = tau A_s + B_s, and
+ *   df/dx' = (1-dy)(q01-q00) + dy(q11-q10),  df/dy' = (1-dx)(q10-q00) + dx(q11-q01)
+ * times t_rel, spread over the four grid_sample taps of the event's (x, y); taps outside the field get nothing.
+ * workspace: evk_flow_timestamp_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
+ * Neither call synchronises, and both launch the same kernels whatever the batch. */
+size_t evk_flow_timestamp_objective_workspace_bytes(int batch, int H, int W);
+int evk_flow_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                     const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                     const float *flow, int H, int W, double sigma, double *f_out, float *ts_out,
+                                     float *cnt_out, void *workspace, size_t workspace_bytes, void *stream);
+int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                          const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                          const float *flow, int H, int W, double sigma, const float *ts_img,
+                                          const float *cnt_img, const float *grad_f, float *grad_flow,
+                                          void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * RobustNorm (row f4): clamp a tensor between two of its order statistics and rescale it.  Replaces
  * RobustNorm.__call__ / .percentile, lib/data_loaders/data_augmentation.py:82-130 (two kthvalue sorts),
