@@ -674,7 +674,7 @@ class zhu_timestamp_objective(objective_function):
             pos, neg = _timestamp_images(x, y, t, p, 0.0, float(np.float32(rel[-1])), SENSOR_SIZE, True, 'bilinear', True, False)
             total = 0.0
             for img in (pos, neg):
-                if blur_sigma > 0:
+                if blur_sigma > 0 or blur_sigma != blur_sigma:      # a NaN sigma reaches the library, which rejects it
                     g, tmp = torch.empty_like(img), torch.empty_like(img)
                     _lib.check(L.evk_gaussian_blur_f32(_lib.ptr(img), img.shape[0], img.shape[1], float(blur_sigma), _lib.ptr(g),
                                                        _lib.ptr(tmp), _lib.stream()))

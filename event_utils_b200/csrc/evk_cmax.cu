@@ -1244,10 +1244,26 @@ static void mix_coeffs(const BlurTaps &t, double *a, double *b)
     *a = sa; *b = sb;
 }
 
+// The blur-sigma rule of every entry point that takes a sigma, applied before any CUDA call: NaN is an argument error,
+// sigma <= 0 means no blur, and a positive sigma needs the truncate-4 radius (int)(4 sigma + 0.5) <= kMaxRadius.  The
+// radius is compared in double, so no sigma (+inf, or one past the int range) can overflow the conversion.
+static int check_sigma(const char *who, double sigma)
+{
+    if (sigma != sigma) { set_error("%s: blur sigma is NaN", who); return EVK_E_ARG; }
+    const double r = 4.0 * sigma + 0.5;
+    if (sigma > 0.0 && r >= (double)(kMaxRadius + 1)) {
+        set_error("%s: blur sigma %.3f needs radius %.0f > %d", who, sigma, floor(r), kMaxRadius);
+        return EVK_E_UNSUPPORTED;
+    }
+    return EVK_OK;
+}
+
+// taps of a blur with sigma > 0 (check_sigma's rule)
 static int make_taps(double sigma, BlurTaps *t)
 {
-    int r = (int)(4.0 * sigma + 0.5);
-    if (r > kMaxRadius) { set_error("evk_cmax: blur sigma %.3f needs radius %d > %d", sigma, r, kMaxRadius); return EVK_E_UNSUPPORTED; }
+    int rc = check_sigma("evk_cmax", sigma);
+    if (rc) return rc;
+    const int r = (int)(4.0 * sigma + 0.5);
     t->r = r;
     double s = 0.0;
     for (int k = -r; k <= r; ++k) s += exp(-0.5 / (sigma * sigma) * (double)k * (double)k);
@@ -1384,16 +1400,16 @@ static int run_cmax(CmaxArgs A, double sigma, unsigned flags, int objective, dou
         EVK_CUDA(cudaGetLastError());
         return EVK_OK;
     }
-    if (objective == OBJ_VARIANCE && (sigma <= 0.0 || (int)(4.0 * sigma + 0.5) <= kFusedMaxR)) {
+    BlurTaps taps{};
+    double mix_a = 1.0, mix_b = 0.0;
+    const int do_blur = sigma > 0.0;
+    if (do_blur) {
+        rc = make_taps(sigma, &taps);
+        if (rc) return rc;
+        if (!(flags & EVK_CMAX_NO_CHANNEL_MIX)) mix_coeffs(taps, &mix_a, &mix_b);
+    }
+    if (objective == OBJ_VARIANCE && taps.r <= kFusedMaxR) {
         // launch-bound regime matters most here: gather + blur + sums + final in one kernel
-        BlurTaps taps{};
-        double mix_a = 1.0, mix_b = 0.0;
-        const int do_blur = sigma > 0.0;
-        if (do_blur) {
-            int rc = make_taps(sigma, &taps);
-            if (rc) return rc;
-            if (!(flags & EVK_CMAX_NO_CHANNEL_MIX)) mix_coeffs(taps, &mix_a, &mix_b);
-        }
         prof_count(1);
         dim3 tgrid((A.Wc + kTileX - 1) / kTileX, (A.Hc + kTileY - 1) / kTileY), tblock(kTileX, kTileY);
         cmax_fused_var_tail_kernel_t<false><<<tgrid, tblock, 0, st>>>(CmaxPeers{}, ws.acc, planar, R, A.Hc, A.Wc, taps, do_blur, grad ? 1 : 0, mix_a, mix_b, iwe_out,
@@ -1751,6 +1767,7 @@ static int flow_obj_setup(const char *who, const float *x, const float *y, const
                           int batch, int64_t n, const float *flow, int H, int W, double sigma, int objective, void *workspace,
                           size_t workspace_bytes, FlowObjArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
 {
+    if (int rc = check_sigma(who, sigma)) return rc;
     if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
         (n > 0 && (!x || !y || !t || !p))) {
         set_error("%s: bad arguments (0 <= batch <= 65535, H, W >= 2)", who);
@@ -1916,6 +1933,7 @@ static int motion_obj_setup(const char *who, const float *x, const float *y, con
                             double sigma, int objective, void *workspace, size_t workspace_bytes, MotionObjArgs &A,
                             BatchObjWorkspace &ws, BlurTaps &taps)
 {
+    if (int rc = check_sigma(who, sigma)) return rc;
     if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
         (n > 0 && (!x || !y || !t || !p))) {
         set_error("%s: bad arguments (0 <= batch <= 65535, H, W >= 2)", who);
@@ -2079,6 +2097,7 @@ static int flow_ts_setup(const char *who, const float *x, const float *y, const 
                          const int64_t *offsets, int batch, int64_t n, const float *flow, int H, int W, double sigma,
                          void *workspace, size_t workspace_bytes, FlowTsArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
 {
+    if (int rc = check_sigma(who, sigma)) return rc;
     if (batch < 0 || batch > 32767 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
         (n > 0 && (!x || !y || !t || !tau || !p))) {
         set_error("%s: bad arguments (0 <= batch <= 32767, H, W >= 2)", who);
@@ -2111,6 +2130,7 @@ int evk_cmax_linvel_objective_f64(const double *x, const double *y, const double
                                   float *iwe_out, float *diwe_out, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_cmax_linvel_objective_f64", sigma)) return rc;
     if (n > 0 && (!x || !y || !t || !p)) { set_error("evk_cmax_linvel_objective_f64: null event array"); return EVK_E_ARG; }
     CmaxArgs A{};
     A.x = x; A.y = y; A.t = t; A.p = p; A.n = n;
@@ -2126,6 +2146,7 @@ int evk_cmax_linvel_objective_f32(const float *x, const float *y, const float *t
                                   float *diwe_out, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_cmax_linvel_objective_f32", sigma)) return rc;
     if (n > 0 && (!x || !y || !t_rel || !p)) { set_error("evk_cmax_linvel_objective_f32: null event array"); return EVK_E_ARG; }
     CmaxArgs A{};
     A.x = x; A.y = y; A.t = t_rel; A.p = p; A.n = n;
@@ -2185,6 +2206,7 @@ int evk_cmax_peer_tail_f32(const float *const *peer_images, const unsigned long 
                            double sigma, unsigned flags, double *result, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_cmax_peer_tail_f32", sigma)) return rc;
     if (!peer_images || !peer_oob || world < 1 || world > kMaxCmaxPeers || Hc < 2 || Wc < 2 || !result || !workspace) {
         set_error("evk_cmax_peer_tail_f32: bad arguments (1 <= world <= %d)", kMaxCmaxPeers);
         return EVK_E_ARG;
@@ -2225,6 +2247,7 @@ int evk_cmax_flow_variance_f32(const float *x, const float *y, const float *t, c
                                double *result, float *iwe_out, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_cmax_flow_variance_f32", sigma)) return rc;
     if (!flow || (n > 0 && (!x || !y || !t || !p))) { set_error("evk_cmax_flow_variance_f32: null array"); return EVK_E_ARG; }
     CmaxArgs A{};
     A.x = x; A.y = y; A.t = t; A.p = p; A.n = n;
@@ -2238,6 +2261,7 @@ int evk_iwe_objective_f32(const float *iwe, const float *diwe, int Hc, int Wc, d
                           double obj_param, double *result, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_iwe_objective_f32", sigma)) return rc;
     if (!iwe || !result || !workspace || Hc < 2 || Wc < 2) { set_error("evk_iwe_objective_f32: bad arguments"); return EVK_E_ARG; }
     if (((uintptr_t)workspace & 255) != 0) { set_error("evk_iwe_objective_f32: workspace must be 256-byte aligned"); return EVK_E_ARG; }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2261,6 +2285,7 @@ int evk_variance_objective_f32(const float *iwe, const float *diwe, int Hc, int 
 int evk_gaussian_blur_f32(const float *img, int H, int W, double sigma, float *out, float *tmp, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_gaussian_blur_f32", sigma)) return rc;
     if (!img || !out || !tmp || H < 1 || W < 1) { set_error("evk_gaussian_blur_f32: bad arguments"); return EVK_E_ARG; }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     BlurTaps taps{};
@@ -2283,6 +2308,7 @@ int evk_cmax_linvel_objective_batch_f64(const double *x, const double *y, const 
                                         double *results, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_cmax_linvel_objective_batch_f64", sigma)) return rc;
     if (n < 0 || (n > 0 && (!x || !y || !t || !p)) || !params_host || n_params < 1 || n_params > kMaxCandidates || !results || !workspace) {
         set_error("evk_cmax_linvel_objective_batch_f64: bad arguments (1 <= n_params <= %d)", kMaxCandidates);
         return EVK_E_ARG;
@@ -2312,16 +2338,16 @@ int evk_cmax_linvel_objective_batch_f64(const double *x, const double *y, const 
         else cmax_scatter_batch_kernel<WARP_LINVEL_F64, false><<<grid_for(cmax_scatter_batch_kernel<WARP_LINVEL_F64, false>, 256, n, 256 * 2), 256, 0, st>>>(A, C);
         EVK_CUDA(cudaGetLastError());
     }
-    if (objective == OBJ_VARIANCE && (sigma <= 0.0 || (int)(4.0 * sigma + 0.5) <= kFusedMaxR)) {
+    BlurTaps taps{};
+    double mix_a = 1.0, mix_b = 0.0;
+    const int do_blur = sigma > 0.0;
+    if (do_blur) {
+        int rc = make_taps(sigma, &taps);
+        if (rc) return rc;
+        if (!(flags & EVK_CMAX_NO_CHANNEL_MIX)) mix_coeffs(taps, &mix_a, &mix_b);
+    }
+    if (objective == OBJ_VARIANCE && taps.r <= kFusedMaxR) {
         // all candidates' tails in ONE launch (blockIdx.z = candidate)
-        BlurTaps taps{};
-        double mix_a = 1.0, mix_b = 0.0;
-        const int do_blur = sigma > 0.0;
-        if (do_blur) {
-            int rc = make_taps(sigma, &taps);
-            if (rc) return rc;
-            if (!(flags & EVK_CMAX_NO_CHANNEL_MIX)) mix_coeffs(taps, &mix_a, &mix_b);
-        }
         prof_count(1);
         dim3 tgrid((A.Wc + kTileX - 1) / kTileX, (A.Hc + kTileY - 1) / kTileY, n_params), tblock(kTileX, kTileY);
         cmax_fused_var_tail_kernel_t<false><<<tgrid, tblock, 0, st>>>(CmaxPeers{}, ws.acc, nullptr, 1, A.Hc, A.Wc, taps, do_blur, grad ? 1 : 0, mix_a, mix_b, nullptr,
@@ -2347,6 +2373,7 @@ int evk_cmax_warp_objective_f64(const double *x, const double *y, const double *
                                 void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_cmax_warp_objective_f64", sigma)) return rc;
     if (n > 0 && (!x || !y || !t || !p)) { set_error("evk_cmax_warp_objective_f64: null event array"); return EVK_E_ARG; }
     CmaxArgs A{};
     int rc = read_model(warp, model, &A.model, nullptr);
@@ -2366,6 +2393,7 @@ int evk_cmax_warp_objective_f32(const float *x, const float *y, const float *t_r
                                 size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_cmax_warp_objective_f32", sigma)) return rc;
     if (n > 0 && (!x || !y || !t_rel || !p)) { set_error("evk_cmax_warp_objective_f32: null event array"); return EVK_E_ARG; }
     CmaxArgs A{};
     int rc = read_model(warp, model, &A.model, nullptr);
@@ -2385,6 +2413,7 @@ int evk_cmax_warp_objective_batch_f64(const double *x, const double *y, const do
                                       double *results, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
+    if (int rc = check_sigma("evk_cmax_warp_objective_batch_f64", sigma)) return rc;
     if (n < 0 || (n > 0 && (!x || !y || !t || !p)) || !models_host || n_models < 1 || n_models > kMaxCandidates || !results ||
         !workspace || Hs < 1 || Ws < 1) {
         set_error("evk_cmax_warp_objective_batch_f64: bad arguments (1 <= n_models <= %d)", kMaxCandidates);

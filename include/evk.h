@@ -326,6 +326,10 @@ int evk_voxel_grad_f32(const float *x, const float *y, const float *t, const flo
  *   iwe_out : optional (Hs+1)*(Ws+1) floats (the un-blurred IWE), diwe_out optional 2x that.
  *   p_scale : polarity multiplier (1, or 100 for the adaptive-lifespan branch objectives.py:225)
  *   workspace: evk_cmax_workspace_bytes(Hs,Ws) bytes of device scratch, 256-byte aligned.
+ *   sigma   : the Gaussian blur of the image, scipy's gaussian_filter (truncate 4, mode 'reflect'), radius
+ *             (int)(4 sigma + 0.5).  sigma <= 0: no blur.  NaN: EVK_E_ARG.  A radius above 64 (sigma >= 16.125,
+ *             +inf included): EVK_E_UNSUPPORTED.  The same rule holds for every entry point below that takes a
+ *             sigma, and each checks it first, before any CUDA call.
  * --------------------------------------------------------------------------------------------- */
 size_t evk_cmax_workspace_bytes(int Hs, int Ws);
 int evk_cmax_linvel_variance_f64(const double *x, const double *y, const double *t, const double *p,
@@ -421,7 +425,8 @@ int evk_cmax_warp_objective_batch_f64(const double *x, const double *y, const do
 
 /* scipy.ndimage.gaussian_filter(img, sigma) for a 2-D f32 image (truncate=4, mode='reflect', f64 line
  * accumulation, f32 store after each axis) -- the blur every objective applies (objectives.py:233 ...).
- * tmp: H*W floats of scratch; out may not alias img. */
+ * tmp: H*W floats of scratch; out may not alias img.  sigma <= 0 copies img; NaN and radii above 64 are rejected
+ * (the sigma rule above). */
 int evk_gaussian_blur_f32(const float *img, int H, int W, double sigma, float *out, float *tmp, void *stream);
 
 /* The objective (and gradient) of a PRECOMPUTED image of warped events, i.e. the iwe= / d_iwe=
