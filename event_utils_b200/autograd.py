@@ -16,6 +16,7 @@ Which inputs get a gradient (as in the reference; the others get None):
     flow_contrast_objective_torch    flow only (contrast_max/flow_objective.py; the events are data)
     flow_timestamp_objective_torch   flow only (contrast_max/flow_timestamp_objective.py; the events are data)
     motion_contrast_objective_torch  params only (contrast_max/motion_objective.py; the events are data)
+    motion_timestamp_objective_torch params only (contrast_max/motion_timestamp_objective.py; the events are data)
 
 The public functions take this path only when grad mode is on and one of those inputs requires grad; every
 other call runs the plain forward.  Gradients come back in each input's shape, dtype and device.  The
@@ -304,6 +305,53 @@ class MotionObjective(torch.autograd.Function):
                 cx, cy, H, W, sigma, objective, param, _lib.ptr(iwe), _lib.ptr(g), _lib.ptr(gp), _lib.ptr(ws), ws.numel(),
                 _lib.stream()))
         return _as_input(gp, ctx.meta), None, None, None, None, None, None
+
+
+class MotionTimestampObjective(torch.autograd.Function):
+    """The batched parametric average-timestamp loss of contrast_max/motion_timestamp_objective.py
+    (zhu_timestamp_objective, objectives.py:524-558, with the linvel, rotation or 4-DoF model): f (B,) f64 from params
+    (B,K) and the prepared device events with their normalised stamps tau.  Only the parameters get a gradient: the exact
+    derivative of f, one pass over the events (evk_motion_timestamp_objective_grad_f32).  The forward keeps the timestamp
+    and count images.  opts = (warp code, centre, H, W, sigma)."""
+
+    @staticmethod
+    def forward(ctx, params, x, y, t_rel, tau, p, offsets, opts):
+        warp, (cx, cy), H, W, sigma = opts
+        dev = x.device
+        B, K = params.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            p64 = params.detach().to(device=dev, dtype=torch.float64).contiguous()
+            f = torch.empty(B, dtype=torch.float64, device=dev)
+            ts_img = torch.empty((B, 2, H + 1, W + 1), dtype=torch.float32, device=dev)
+            cnt_img = torch.empty_like(ts_img)
+            ws = _lib.scratch("motion_timestamp_objective", L.evk_motion_timestamp_objective_workspace_bytes(B, H, W), dev)
+            _lib.check(L.evk_motion_timestamp_objective_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0], warp,
+                _lib.ptr(p64), K, cx, cy, H, W, sigma, _lib.ptr(f), _lib.ptr(ts_img), _lib.ptr(cnt_img), _lib.ptr(ws),
+                ws.numel(), _lib.stream()))
+        ctx.save_for_backward(x, y, t_rel, tau, p, offsets, p64, ts_img, cnt_img)
+        ctx.opts = opts
+        ctx.meta = _meta(params)
+        return f
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, y, t_rel, tau, p, offsets, p64, ts_img, cnt_img = ctx.saved_tensors
+        warp, (cx, cy), H, W, sigma = ctx.opts
+        dev = x.device
+        B, K = p64.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g = _grad_in(g, dev)
+            gp = torch.empty_like(p64)
+            ws = _lib.scratch("motion_timestamp_objective", L.evk_motion_timestamp_objective_workspace_bytes(B, H, W), dev)
+            _lib.check(L.evk_motion_timestamp_objective_grad_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0], warp,
+                _lib.ptr(p64), K, cx, cy, H, W, sigma, _lib.ptr(ts_img), _lib.ptr(cnt_img), _lib.ptr(g), _lib.ptr(gp),
+                _lib.ptr(ws), ws.numel(), _lib.stream()))
+        return _as_input(gp, ctx.meta), None, None, None, None, None, None, None
 
 
 class VoxelGrid(torch.autograd.Function):

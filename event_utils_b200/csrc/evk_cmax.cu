@@ -2092,6 +2092,40 @@ __global__ void __launch_bounds__(256) flow_ts_ab_kernel(const float *__restrict
     ab[k] = make_float2((float)(u / c), (float)(-u * (double)ts[k] / c));
 }
 
+// forward image-space half of the timestamp losses, after their event pass: the 32-byte blocks in ws.acc -> T and C of
+// the 2B images (NaN for a sample flagged in ws.nonfinite), the blur, per image an f64 sum of G^2, and f_b
+static void ts_obj_forward_tail(const BatchObjWorkspace &ws, int Hc, int Wc, const BlurTaps &taps, int batch, float *ts_out,
+                                float *cnt_out, double *f_out, cudaStream_t st)
+{
+    const int npix = Hc * Wc, images = 2 * batch;
+    const dim3 g((npix + 255) / 256, 1, images);
+    prof_count(1);
+    flow_ts_fold_kernel<<<g, 256, 0, st>>>(ws.acc, ws.nonfinite, Hc, Wc, ts_out, cnt_out);
+    batch_obj_blur(ws, ts_out, Hc, Wc, taps, images, st);
+    prof_count(2);
+    cmax_model_stats_kernel<<<g, 256, 0, st>>>(ws.G, ts_out, npix, OBJ_SOS, 0.0, ws.gsums, ws.gmax, nullptr, nullptr);
+    flow_ts_final_kernel<<<(batch + 127) / 128, 128, 0, st>>>(ws.gsums, batch, f_out);
+}
+
+// backward image-space half of the timestamp losses, before their event pass: U = G(2 g_b G_s) from the saved T (G
+// recomputed, the coefficient image, its adjoint blur into ws.Wimg), then the (A, B) pairs, which go to ws.wt (8 bytes per
+// pixel), which the blur has finished reading.  Returns the pairs.
+static const float2 *ts_obj_backward_ab(const BatchObjWorkspace &ws, const float *ts_img, const float *cnt_img, int Hc, int Wc,
+                                        const BlurTaps &taps, int batch, const float *grad_f, cudaStream_t st)
+{
+    const int npix = Hc * Wc, images = 2 * batch;
+    batch_obj_blur(ws, ts_img, Hc, Wc, taps, images, st);
+    const int do_blur = taps.r > 0 || taps.w[0] != 0.0;
+    const dim3 g((npix + 255) / 256, 1, images);
+    prof_count(do_blur ? 4 : 3);
+    flow_ts_coef_kernel<<<g, 256, 0, st>>>(ws.G, npix, grad_f, ws.w);
+    if (do_blur) cmax_blur_d_axis0_kernel<<<g, 256, 0, st>>>(ws.w, ws.wt, Hc, Wc, taps);
+    cmax_blur_d_axis1_store_kernel<<<g, 256, 0, st>>>(ws.wt, ws.w, Hc, Wc, taps, do_blur, ws.Wimg);
+    float2 *ab = reinterpret_cast<float2 *>(ws.wt);
+    flow_ts_ab_kernel<<<g, 256, 0, st>>>(ws.Wimg, ts_img, cnt_img, npix, ab);
+    return ab;
+}
+
 // shared argument checks and set-up of the two timestamp entry points (those of flow_obj_setup, for 2B images)
 static int flow_ts_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
                          const int64_t *offsets, int batch, int64_t n, const float *flow, int H, int W, double sigma,
@@ -2112,6 +2146,141 @@ static int flow_ts_setup(const char *who, const float *x, const float *y, const 
     A.F.flow = flow; A.F.H = H; A.F.W = W;
     A.tau = tau;
     return EVK_OK;
+}
+
+// ---- parametric average-timestamp (Zhu) loss over a batch of samples (evk_motion_timestamp_objective_f32 / _grad_f32) --
+// Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by its own model params[b] through model_taps
+// (linvel, rotation or xyztheta, f32, as the motion contrast loss warps), with weight 1: an event contributes iff its splat
+// there is not zero (finite, 0 < x' < W, 0 < y' < H).  Then the images and f_b of the dense-flow timestamp loss above, on
+// the same 2B images z = 2b + s and through the same image-space halves (ts_obj_forward_tail, ts_obj_backward_ab):
+//   forward:  two v4 reductions per contributing event into the 32-byte block {S taps, C taps} of its polarity (the
+//             arithmetic of flow_ts_event); a non-finite x' or y' contributes nothing, so no sample is ever flagged.
+//   backward: per contributing event the four (A, B) pairs of its polarity (L2 gathers), q = tau A + B per tap,
+//             df/dx', df/dy' through the tap weights, contracted with the Jacobian rows of model_taps<..., true> and summed
+//             in f64 per thread; a CTA reduction and one f64 atomic per component and CTA into grad [B][K], as in
+//             motion_obj_event_kernel.
+struct MotionTsArgs {
+    MotionObjArgs M;   // warp, keep rule, samples and parameters; M.acc: forward [B][2][Hc][Wc][8]; M.grad: backward [B][K]
+    const float *tau;  // the normalised stamp of every event
+    const float2 *ab;  // backward: (A, B) [B][2][Hc][Wc]
+};
+
+template <int WARP, bool GRAD>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_ts_event_kernel(const MotionTsArgs A)
+{
+    constexpr int K = model_dims(WARP);
+    const int b = blockIdx.y;
+    int64_t first = A.M.offsets[b], last = A.M.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > A.M.n) last = A.M.n;
+    const int Wc = A.M.C.Wc;
+    const int64_t npix = (int64_t)A.M.C.Hc * Wc;
+    WarpModel M{};
+#pragma unroll
+    for (int k = 0; k < K; ++k) M.m[k] = A.M.params[(int64_t)b * K + k];
+    if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = A.M.cx; M.m[5] = A.M.cy; }
+    float *acc = GRAD ? nullptr : A.M.acc + b * 2 * npix * 8;
+    const float2 *ab = GRAD ? A.ab + b * 2 * npix : nullptr;
+    double u[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) u[k] = 0.0;
+    unsigned oob = 0;   // a contributing event lies inside the canvas; a non-finite one contributes nothing
+    auto one = [&](float xe, float ye, float te, float ue, float pe) {
+        const bool pos = pe > 0.0f;
+        if (!pos && !(pe <= 0.0f)) return;   // NaN polarity: in neither image (evk_tsimg.cu)
+        Event<WARP> e;
+        e.x = xe; e.y = ye; e.t = te; e.p = 1.0f;
+        Taps T;
+        float jx[4], jy[4];
+        if (!model_taps<WARP, GRAD>(A.M.C, e, M, oob, T, jx, jy)) return;
+        const float dx = T.dx, dy = T.dy;
+        const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+        if (!GRAD) {
+            // tsimg_scatter_kernel's taps: tau (1-dx)(1-dy) .. and (1-dx)(1-dy) ..
+            const float tl = __fmul_rn(ue, ox), tr = __fmul_rn(ue, dx);
+            float *blk = acc + ((pos ? 0 : npix) + (int64_t)T.y0 * Wc + T.x0) * 8;
+            red_add4(blk, make_float4(__fmul_rn(tl, oy), __fmul_rn(tr, oy), __fmul_rn(tl, dy), __fmul_rn(tr, dy)));
+            red_add4(blk + 4, make_float4(__fmul_rn(ox, oy), __fmul_rn(dx, oy), __fmul_rn(ox, dy), __fmul_rn(dx, dy)));
+            return;
+        }
+        const float2 *abs_ = pos ? ab : ab + npix;
+        const int64_t r0 = (int64_t)T.y0 * Wc, r1 = (int64_t)T.y1 * Wc;
+        const float2 a00 = __ldg(abs_ + r0 + T.x0), a01 = __ldg(abs_ + r0 + T.x1), a10 = __ldg(abs_ + r1 + T.x0),
+                     a11 = __ldg(abs_ + r1 + T.x1);
+        const double tau = ue;
+        const double q00 = tau * a00.x + a00.y, q01 = tau * a01.x + a01.y, q10 = tau * a10.x + a10.y, q11 = tau * a11.x + a11.y;
+        const double sx = (double)oy * (q01 - q00) + (double)dy * (q11 - q10);
+        const double sy = (double)ox * (q10 - q00) + (double)dx * (q11 - q01);
+#pragma unroll
+        for (int k = 0; k < K; ++k) u[k] += (double)jx[k] * sx + (double)jy[k] * sy;
+    };
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
+        float ex[kBatch], ey[kBatch], et[kBatch], eu[kBatch], ep[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            ex[k] = ld_stream(A.M.x + i + k * stride); ey[k] = ld_stream(A.M.y + i + k * stride);
+            et[k] = ld_stream(A.M.t + i + k * stride); eu[k] = ld_stream(A.tau + i + k * stride);
+            ep[k] = ld_stream(A.M.p + i + k * stride);
+        }
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) one(ex[k], ey[k], et[k], eu[k], ep[k]);
+    }
+    for (; i < last; i += stride)
+        one(ld_stream(A.M.x + i), ld_stream(A.M.y + i), ld_stream(A.M.t + i), ld_stream(A.tau + i), ld_stream(A.M.p + i));
+    if (!GRAD) return;
+    // CTA reduction, one f64 atomic per component and CTA
+    __shared__ double part[kFlowObjThreads / 32][K];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        double v = u[k];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) part[wid][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        double s = 0.0;
+        for (int w = 0; w < kFlowObjThreads / 32; ++w) s += part[w][threadIdx.x];
+        atomicAdd(A.M.grad + (int64_t)b * K + threadIdx.x, s);
+    }
+}
+
+// shared argument checks and set-up of the two parametric timestamp entry points (those of motion_obj_setup, for 2B images)
+static int motion_ts_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
+                           const int64_t *offsets, int batch, int64_t n, int warp, const double *params, int K, double cx,
+                           double cy, int H, int W, double sigma, void *workspace, size_t workspace_bytes, MotionTsArgs &A,
+                           BatchObjWorkspace &ws, BlurTaps &taps)
+{
+    if (int rc = check_sigma(who, sigma)) return rc;
+    if (batch < 0 || batch > 32767 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
+        (n > 0 && (!x || !y || !t || !tau || !p))) {
+        set_error("%s: bad arguments (0 <= batch <= 32767, H, W >= 2)", who);
+        return EVK_E_ARG;
+    }
+    const int dims = motion_obj_dims(warp);
+    if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
+    if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
+    int rc = batch_obj_check(who, "parameters", 2 * batch, H, W, sigma, OBJ_SOS, flow_ts_acc_blocks(H, W), workspace,
+                             workspace_bytes, ws, taps);
+    if (rc) return rc;
+    A = MotionTsArgs{};
+    A.M.C.Hm = H; A.M.C.Wm = W; A.M.C.Hc = H + 1; A.M.C.Wc = W + 1;
+    A.M.C.p_scale = 1.0;
+    A.M.x = x; A.M.y = y; A.M.t = t; A.M.p = p; A.M.offsets = offsets; A.M.n = n;
+    A.M.params = params; A.M.cx = cx; A.M.cy = cy;
+    A.tau = tau;
+    return EVK_OK;
+}
+
+template <bool GRAD>
+static void launch_motion_ts_events(int warp, const MotionTsArgs &A, int batch, cudaStream_t st)
+{
+    const dim3 grid = flow_obj_grid(A.M.n, batch);
+    if (warp == EVK_WARP_LINVEL) motion_ts_event_kernel<WARP_LINVEL_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else if (warp == EVK_WARP_ROTATION) motion_ts_event_kernel<WARP_ROTATION_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else motion_ts_event_kernel<WARP_XYZTHETA_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
 }
 
 }  // namespace evk
@@ -2626,13 +2795,7 @@ int evk_flow_timestamp_objective_f32(const float *x, const float *y, const float
         prof_count(1);
         flow_ts_event_kernel<false><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
     }
-    const dim3 g((npix + 255) / 256, 1, images);
-    prof_count(1);
-    flow_ts_fold_kernel<<<g, 256, 0, st>>>(ws.acc, ws.nonfinite, Hc, Wc, ts_out, cnt_out);
-    batch_obj_blur(ws, ts_out, Hc, Wc, taps, images, st);
-    prof_count(2);
-    cmax_model_stats_kernel<<<g, 256, 0, st>>>(ws.G, ts_out, npix, OBJ_SOS, 0.0, ws.gsums, ws.gmax, nullptr, nullptr);
-    flow_ts_final_kernel<<<(batch + 127) / 128, 128, 0, st>>>(ws.gsums, batch, f_out);
+    ts_obj_forward_tail(ws, Hc, Wc, taps, batch, ts_out, cnt_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }
@@ -2655,21 +2818,10 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
     }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch;
+    const int images = 2 * batch;
     EVK_CUDA(cudaMemsetAsync(ws.acc, 0, (size_t)images * H * W * 4 * sizeof(float), st));
-    // U = G(2 g_b G_s): recompute G from the saved T, the coefficient image, its adjoint blur (into ws.Wimg)
-    batch_obj_blur(ws, ts_img, Hc, Wc, taps, images, st);
-    const int do_blur = taps.r > 0 || taps.w[0] != 0.0;
-    const dim3 g((npix + 255) / 256, 1, images);
-    prof_count(do_blur ? 4 : 3);
-    flow_ts_coef_kernel<<<g, 256, 0, st>>>(ws.G, npix, grad_f, ws.w);
-    if (do_blur) cmax_blur_d_axis0_kernel<<<g, 256, 0, st>>>(ws.w, ws.wt, Hc, Wc, taps);
-    cmax_blur_d_axis1_store_kernel<<<g, 256, 0, st>>>(ws.wt, ws.w, Hc, Wc, taps, do_blur, ws.Wimg);
-    // the pairs go to ws.wt (8 bytes per pixel), which the blur above has finished reading
-    float2 *ab = reinterpret_cast<float2 *>(ws.wt);
-    flow_ts_ab_kernel<<<g, 256, 0, st>>>(ws.Wimg, ts_img, cnt_img, npix, ab);
     A.F.acc = ws.acc;
-    A.ab = ab;
+    A.ab = ts_obj_backward_ab(ws, ts_img, cnt_img, H + 1, W + 1, taps, batch, grad_f, st);
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
@@ -2677,6 +2829,72 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
     }
     prof_count(1);
     flow_obj_grad_fold_kernel<<<grid_simple((int64_t)images * H * W, 256), 256, 0, st>>>(ws.acc, grad_flow, images, H, W);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_motion_timestamp_objective_workspace_bytes(int batch, int H, int W)
+{
+    if (batch < 0 || H < 2 || W < 2) return 0;
+    return evk::batch_obj_carve(nullptr, 2 * batch, H, W, evk::flow_ts_acc_blocks(H, W), nullptr);
+}
+
+int evk_motion_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                       const int64_t *offsets, int batch, int64_t n_events, int warp, const double *params,
+                                       int K, double cx, double cy, int H, int W, double sigma, double *f_out, float *ts_out,
+                                       float *cnt_out, void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    MotionTsArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_ts_setup("evk_motion_timestamp_objective_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp, params,
+                             K, cx, cy, H, W, sigma, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !ts_out || !cnt_out)) { set_error("evk_motion_timestamp_objective_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch;
+    // nonfinite stays zero: a non-finite event contributes nothing (model_taps), as in the motion contrast loss
+    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)images * npix * 8 * sizeof(float), st));
+    A.M.acc = ws.acc;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_ts_events<false>(warp, A, batch, st);
+    }
+    ts_obj_forward_tail(ws, Hc, Wc, taps, batch, ts_out, cnt_out, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                            const int64_t *offsets, int batch, int64_t n_events, int warp, const double *params,
+                                            int K, double cx, double cy, int H, int W, double sigma, const float *ts_img,
+                                            const float *cnt_img, const float *grad_f, double *grad_params, void *workspace,
+                                            size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    MotionTsArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_ts_setup("evk_motion_timestamp_objective_grad_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp,
+                             params, K, cx, cy, H, W, sigma, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!ts_img || !cnt_img || !grad_f || !grad_params)) {
+        set_error("evk_motion_timestamp_objective_grad_f32: null array");
+        return EVK_E_ARG;
+    }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    EVK_CUDA(cudaMemsetAsync(grad_params, 0, (size_t)batch * K * sizeof(double), st));
+    A.ab = ts_obj_backward_ab(ws, ts_img, cnt_img, H + 1, W + 1, taps, batch, grad_f, st);
+    A.M.grad = grad_params;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_ts_events<true>(warp, A, batch, st);
+    }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }

@@ -569,6 +569,43 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
                                           const float *cnt_img, const float *grad_f, float *grad_flow,
                                           void *workspace, size_t workspace_bytes, void *stream);
 
+/* Parametric average-timestamp loss (Zhu et al., CVPR'19) over a batch of samples, as a differentiable loss: the
+ * reference's zhu_timestamp_objective (lib/contrast_max/objectives.py:524-558), driven by its warp_function, with the
+ * sign of a loss to minimise.  Sample b is the events [offsets[b], offsets[b+1]) (clipped to [0, n_events); end < start
+ * is empty), warped by its own parameters params[b] (K doubles in DEVICE memory) with the model `warp` and its f32
+ * arithmetic exactly as in evk_cmax_motion_objective_f32 (EVK_WARP_LINVEL / _ROTATION / _XYZTHETA; the centre (cx, cy)
+ * of xyztheta).  An event contributes iff its splat in that loss is not zero: x', y' finite, 0 < x' < W and
+ * 0 < y' < H (the bounds mask 0 < x' <= W, then the clip that gives x' = W zero weight).  A non-finite x' or y'
+ * contributes nothing and does not poison the sample.  The reference instead zeroes the masked events and piles them
+ * at (0, 0) as events with p = 0 and t = 0 (objectives.py:543-545).  tau and the images are those of
+ * evk_flow_timestamp_objective_f32: per polarity s (p > 0 / p <= 0; a NaN p is dropped), on the (H+1)x(W+1) canvas,
+ *   T_s = S_s / C_s,  S_s = sum tau k,  C_s = 1 + sum k,   f_b = sum gaussian_filter(T_+, blur_sigma)^2 + sum (...T_-...)^2
+ * the negation of zhu_timestamp_objective.evaluate_function.  blur_sigma follows the blur-sigma rule of the other
+ * entries (0 or less: no blur; NaN: EVK_E_ARG; a radius over 64: EVK_E_UNSUPPORTED), checked before any CUDA call.
+ *   x, y, t_rel, tau, p : n_events floats;  offsets: batch+1 int64 on the device
+ *   f_out: batch doubles;  ts_out, cnt_out: [batch][2][H+1][W+1] floats (T and C, polarity 0 positive), which the
+ *   backward takes as ts_img, cnt_img.  0 <= batch <= 32767.
+ * evk_motion_timestamp_objective_grad_f32 writes grad_params [batch][K] doubles = grad_f[b] df_b/dparams[b], the exact
+ * derivative of the f above with the floor and keep decisions held (grad_f: batch floats on the device): with
+ * U_s = G(2 grad_f[b] G_s), A_s = U_s / C_s and B_s = -U_s T_s / C_s, per contributing event of polarity s and each of
+ * its four taps q = tau A_s + B_s,
+ *   df/dx' = (1-dy)(q01-q00) + dy(q11-q10),  df/dy' = (1-dx)(q10-q00) + dx(q11-q01),
+ *   df/dparams_k += df/dx' dx'/dparams_k + df/dy' dy'/dparams_k.
+ * workspace: evk_motion_timestamp_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
+ * Neither call synchronises, and both launch the same kernels whatever the batch. */
+size_t evk_motion_timestamp_objective_workspace_bytes(int batch, int H, int W);
+int evk_motion_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                       const float *p, const int64_t *offsets, int batch, int64_t n_events, int warp,
+                                       const double *params, int K, double cx, double cy, int H, int W, double blur_sigma,
+                                       double *f_out, float *ts_out, float *cnt_out, void *workspace,
+                                       size_t workspace_bytes, void *stream);
+int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                            const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                            int warp, const double *params, int K, double cx, double cy, int H, int W,
+                                            double blur_sigma, const float *ts_img, const float *cnt_img,
+                                            const float *grad_f, double *grad_params, void *workspace,
+                                            size_t workspace_bytes, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * RobustNorm (row f4): clamp a tensor between two of its order statistics and rescale it.  Replaces
  * RobustNorm.__call__ / .percentile, lib/data_loaders/data_augmentation.py:82-130 (two kthvalue sorts),
