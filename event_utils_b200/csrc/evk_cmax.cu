@@ -1707,8 +1707,9 @@ struct BatchObjWorkspace {
     double *w, *wt;        // [B][Hc][Wc]
 };
 
-// acc_blocks: 16-byte blocks of the accumulator per sample
-static size_t batch_obj_carve(void *base, int batch, int H, int W, size_t acc_blocks, BatchObjWorkspace *ws)
+// acc_blocks: 16-byte blocks of the accumulator per sample.  Without `backward` the two f64 images of the adjoint blur
+// are not carved (a forward-only entry, which may use Wimg for its folded images).
+static size_t batch_obj_carve(void *base, int batch, int H, int W, size_t acc_blocks, BatchObjWorkspace *ws, bool backward = true)
 {
     const size_t npix = (size_t)(H + 1) * (W + 1), B = (size_t)batch;
     size_t off = 0;
@@ -1722,8 +1723,8 @@ static size_t batch_obj_carve(void *base, int batch, int H, int W, size_t acc_bl
     float *tmp = (float *)take(B * npix * sizeof(float));
     float *G = (float *)take(B * npix * sizeof(float));
     float *Wimg = (float *)take(B * npix * sizeof(float));
-    double *w = (double *)take(B * npix * sizeof(double));
-    double *wt = (double *)take(B * npix * sizeof(double));
+    double *w = backward ? (double *)take(B * npix * sizeof(double)) : nullptr;
+    double *wt = backward ? (double *)take(B * npix * sizeof(double)) : nullptr;
     if (ws) { ws->nonfinite = nonfinite; ws->gsums = gsums; ws->gmax = gmax; ws->acc = acc; ws->tmp = tmp; ws->G = G; ws->Wimg = Wimg; ws->w = w; ws->wt = wt; }
     return off;
 }
@@ -1737,7 +1738,7 @@ static size_t flow_obj_acc_blocks(int H, int W)
 
 // the checks and set-up every batched objective entry shares: objective, canvas, workspace (carved into ws), blur taps
 static int batch_obj_check(const char *who, const char *wrt, int batch, int H, int W, double sigma, int objective, size_t acc_blocks,
-                           void *workspace, size_t workspace_bytes, BatchObjWorkspace &ws, BlurTaps &taps)
+                           void *workspace, size_t workspace_bytes, BatchObjWorkspace &ws, BlurTaps &taps, bool backward = true)
 {
     if (objective == OBJ_MOA || objective == OBJ_ISOA) {
         set_error("%s: objective %d (moa / isoa) is piecewise constant in the %s and has no gradient", who, objective, wrt);
@@ -1748,12 +1749,12 @@ static int batch_obj_check(const char *who, const char *wrt, int batch, int H, i
         return EVK_E_ARG;
     }
     if ((size_t)(H + 1) * (W + 1) > (size_t)1 << 30) { set_error("%s: canvas too large", who); return EVK_E_ARG; }
-    const size_t need = batch_obj_carve(nullptr, batch, H, W, acc_blocks, nullptr);
+    const size_t need = batch_obj_carve(nullptr, batch, H, W, acc_blocks, nullptr, backward);
     if (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 255)) {
         set_error("%s: 256-byte aligned workspace of %zu bytes required", who, need);
         return EVK_E_WORKSPACE;
     }
-    batch_obj_carve(workspace, batch, H, W, acc_blocks, &ws);
+    batch_obj_carve(workspace, batch, H, W, acc_blocks, &ws, backward);
     taps = BlurTaps{};
     if (sigma > 0.0) {
         int rc = make_taps(sigma, &taps);
@@ -1931,7 +1932,7 @@ static int motion_obj_dims(int warp)
 static int motion_obj_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
                             int batch, int64_t n, int warp, const double *params, int K, double cx, double cy, int H, int W,
                             double sigma, int objective, void *workspace, size_t workspace_bytes, MotionObjArgs &A,
-                            BatchObjWorkspace &ws, BlurTaps &taps)
+                            BatchObjWorkspace &ws, BlurTaps &taps, bool candidates = false, int n_cand = 1)
 {
     if (int rc = check_sigma(who, sigma)) return rc;
     if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
@@ -1942,8 +1943,15 @@ static int motion_obj_setup(const char *who, const float *x, const float *y, con
     const int dims = motion_obj_dims(warp);
     if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
     if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
-    int rc = batch_obj_check(who, "parameters", batch, H, W, sigma, objective, (size_t)(H + 1) * (W + 1), workspace, workspace_bytes,
-                             ws, taps);
+    // the differentiable entries: one canvas per sample; the candidates entry: one forward-only canvas per sample and
+    // candidate (the tail's grid takes at most 65535 canvases)
+    if (candidates && (n_cand < 1 || n_cand > kMaxCandidates || (int64_t)batch * n_cand > 65535)) {
+        set_error("%s: bad arguments (1 <= n_cand <= %d, batch * n_cand <= 65535)", who, kMaxCandidates);
+        return EVK_E_ARG;
+    }
+    const int canvases = candidates ? batch * n_cand : batch;
+    int rc = batch_obj_check(who, "parameters", canvases, H, W, sigma, objective, (size_t)(H + 1) * (W + 1), workspace,
+                             workspace_bytes, ws, taps, !candidates);
     if (rc) return rc;
     A = MotionObjArgs{};
     A.C.Hm = H; A.C.Wm = W; A.C.Hc = H + 1; A.C.Wc = W + 1;
@@ -1960,6 +1968,75 @@ static void launch_motion_obj_events(int warp, const MotionObjArgs &A, int batch
     if (warp == EVK_WARP_LINVEL) motion_obj_event_kernel<WARP_LINVEL_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
     else if (warp == EVK_WARP_ROTATION) motion_obj_event_kernel<WARP_ROTATION_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
     else motion_obj_event_kernel<WARP_XYZTHETA_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
+}
+
+// ---- many parameter vectors per sample in one event pass (evk_cmax_motion_candidates_f32) -------------------------
+// The grid search of grid_search_initial (events_cmax.py:241-311) and the line search of a batched quasi-Newton fit score
+// n_cand parameter vectors of every sample.  On the (slices, batch) grid of the other motion passes, each CTA takes its
+// sample's n_cand x K candidates into shared memory, reads each event ONCE (16 B) and splats it through model_taps under
+// every candidate: one v4 reduction per kept event and candidate into the candidate's 2x2-block image, canvas
+// z = b n_cand + j of [batch][n_cand][Hc][Wc][4].  batch_obj_forward_tail then scores the batch x n_cand canvases exactly
+// as it scores the samples of evk_cmax_motion_objective_f32.
+struct MotionCandArgs {
+    MotionObjArgs M;   // events, samples and canvas; M.params = the candidates [B][n_cand][K]; M.acc = the canvases' blocks
+    int n_cand;
+};
+
+template <int WARP>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_obj_cand_kernel(const MotionCandArgs A)
+{
+    constexpr int K = model_dims(WARP);
+    __shared__ WarpModel cand[kMaxCandidates];
+    const int b = blockIdx.y, J = A.n_cand;
+    for (int j = threadIdx.x; j < J; j += kFlowObjThreads) {
+        WarpModel M{};
+#pragma unroll
+        for (int k = 0; k < K; ++k) M.m[k] = A.M.params[((int64_t)b * J + j) * K + k];
+        if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = A.M.cx; M.m[5] = A.M.cy; }
+        cand[j] = M;
+    }
+    __syncthreads();
+    int64_t first = A.M.offsets[b], last = A.M.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > A.M.n) last = A.M.n;
+    const int Wc = A.M.C.Wc;
+    const int64_t npix = (int64_t)A.M.C.Hc * Wc;
+    float *acc = A.M.acc + (int64_t)b * J * npix * 4;
+    unsigned oob = 0;   // as in motion_obj_event_kernel: a kept finite event lies inside the canvas
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i < last; i += kBatch * stride) {
+        Event<WARP> e[kBatch];
+        int ne = 0;
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int64_t q = i + k * stride;
+            if (q < last) {
+                e[k].x = ld_stream(A.M.x + q); e[k].y = ld_stream(A.M.y + q);
+                e[k].t = ld_stream(A.M.t + q); e[k].p = ld_stream(A.M.p + q);
+                ne = k + 1;
+            }
+        }
+        for (int j = 0; j < J; ++j) {
+            const WarpModel M = cand[j];
+            float *accj = acc + j * npix * 4;
+#pragma unroll
+            for (int k = 0; k < kBatch; ++k) {
+                Taps T;
+                float jx[4], jy[4];
+                if (k < ne && model_taps<WARP, false>(A.M.C, e[k], M, oob, T, jx, jy))
+                    red_add4(accj + ((int64_t)T.y0 * Wc + T.x0) * 4, T.ti);
+            }
+        }
+    }
+}
+
+static void launch_motion_cand_events(int warp, const MotionCandArgs &A, int batch, cudaStream_t st)
+{
+    const dim3 grid = flow_obj_grid(A.M.n, batch);
+    if (warp == EVK_WARP_LINVEL) motion_obj_cand_kernel<WARP_LINVEL_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else if (warp == EVK_WARP_ROTATION) motion_obj_cand_kernel<WARP_ROTATION_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else motion_obj_cand_kernel<WARP_XYZTHETA_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
 }
 
 // ---- dense-flow average-timestamp (Zhu) loss over a batch of samples (evk_flow_timestamp_objective_f32 / _grad_f32) --
@@ -2761,6 +2838,43 @@ int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const flo
         prof_count(1);
         launch_motion_obj_events<true>(warp, A, batch, st);
     }
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_cmax_motion_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
+{
+    if (batch < 0 || n_cand < 1 || n_cand > evk::kMaxCandidates || H < 2 || W < 2) return 0;
+    return evk::batch_obj_carve(nullptr, batch * n_cand, H, W, (size_t)(H + 1) * (W + 1), nullptr, false);
+}
+
+int evk_cmax_motion_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                   int batch, int64_t n_events, int warp, const double *cand, int n_cand, int K, double cx,
+                                   double cy, int H, int W, double blur_sigma, int objective, double obj_param, double *f_out,
+                                   void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    MotionCandArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_obj_setup("evk_cmax_motion_candidates_f32", x, y, t_rel, p, offsets, batch, n_events, warp, cand, K, cx, cy,
+                              H, W, blur_sigma, objective, workspace, workspace_bytes, A.M, ws, taps, true, n_cand);
+    if (rc) return rc;
+    if (batch > 0 && !f_out) { set_error("evk_cmax_motion_candidates_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_cand;
+    // nonfinite stays zero, as in evk_cmax_motion_objective_f32
+    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)canvases * npix * 4 * sizeof(float), st));
+    A.M.acc = ws.acc;
+    A.n_cand = n_cand;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_cand_events(warp, A, batch, st);
+    }
+    // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
+    batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, ws.Wimg, f_out, st);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }

@@ -535,6 +535,26 @@ int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const flo
                                        const float *grad_f, double *grad_params, void *workspace,
                                        size_t workspace_bytes, void *stream);
 
+/* Many parameter vectors per sample in one pass over the events: the sample points of a grid search per window
+ * (grid_search_initial, lib/contrast_max/events_cmax.py:241-311) or the step lengths of a batched line search.
+ * f_out[b][j] is exactly the f_b of evk_cmax_motion_objective_f32 with params[b] = cand[b][j] (get_iwe,
+ * lib/contrast_max/objectives.py:184-192): the same warp, keep rule, splat, blur and objectives, the same argument
+ * checks (EVK_OBJ_MOA / EVK_OBJ_ISOA: EVK_E_UNSUPPORTED) and the blur-sigma rule for blur_sigma (0 or less: no blur;
+ * NaN: EVK_E_ARG; a radius over 64: EVK_E_UNSUPPORTED), all checked before any CUDA call.  Forward only: no image out,
+ * no gradient.
+ *   cand : [batch][n_cand][K] doubles in DEVICE memory, 1 <= n_cand <= 32, batch * n_cand <= 65535
+ *   f_out: [batch][n_cand] doubles
+ * Every event is read once and splatted under each of its sample's n_cand candidates.
+ * workspace: evk_cmax_motion_candidates_workspace_bytes(batch, n_cand, H, W) bytes (about 28 bytes per canvas pixel
+ * and candidate), 256-byte aligned; the query returns 0 for arguments the entry rejects.
+ * The call does not synchronise and launches the same kernels whatever batch and n_cand. */
+size_t evk_cmax_motion_candidates_workspace_bytes(int batch, int n_cand, int H, int W);
+int evk_cmax_motion_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                   const int64_t *offsets, int batch, int64_t n_events, int warp,
+                                   const double *cand, int n_cand, int K, double cx, double cy, int H, int W,
+                                   double blur_sigma, int objective, double obj_param, double *f_out,
+                                   void *workspace, size_t workspace_bytes, void *stream);
+
 /* Dense-flow average-timestamp loss (Zhu et al., CVPR'19) over a batch of samples, as a differentiable loss:
  * warp_events_flow_torch (lib/transforms/optic_flow.py:5-46), then the timestamp images of
  * events_to_timestamp_image_torch (lib/representations/image.py:286-353) on the canvas of motion_compensate
