@@ -65,40 +65,63 @@ def motion_contrast_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None, 
     warp = _warp_code(warpfunc, "motion_contrast_fit_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_contrast_fit_torch", "nothing")
+    sigmas = _fit_arguments("motion_contrast_fit_torch", blur_sigma, line_search_steps, x0, param_ranges)
+    H, W = int(img_size[0]), int(img_size[1])
+    _lib.lib()
+    dev = E.compute_device(*(a for a in (x0, param_ranges, xs, ys, ts, ps) if isinstance(a, torch.Tensor)))
+    B = _window_count(batch_end_indices)
+    x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows")
+
+    def stage(sigma):
+        opts = _model(warp, warpfunc, objective, sigma, obj_param, H, W)
+        return _objective_and_gradient(x, y, t_rel, p, offsets, opts), lambda c: _candidates(x, y, t_rel, p, offsets, c, opts)
+    with torch.cuda.device(dev):
+        return _fit_stages(stage, sigmas, B, warpfunc.dims, dev, x0, param_ranges, num_samples_per_param, grid_levels,
+                           log_scale, param_scale, max_iter, line_search_steps, ftol, gtol)
+
+
+def _fit_arguments(who, blur_sigma, line_search_steps, x0, param_ranges):
+    """the argument checks the fits share, before any CUDA call; returns the blur sigmas of the stages"""
     sigmas = [float(s) for s in (blur_sigma if isinstance(blur_sigma, (list, tuple)) else [blur_sigma])]
     if not sigmas:
         raise ValueError("blur_sigma must be a number or a non-empty sequence")
     if not 1 <= int(line_search_steps) <= 32:
         raise ValueError("line_search_steps must be in 1..32, got %r" % (line_search_steps,))
-    K = warpfunc.dims
-    H, W = int(img_size[0]), int(img_size[1])
     if x0 is None and param_ranges is None:
-        raise ValueError("motion_contrast_fit_torch needs x0 or param_ranges")
-    _lib.lib()
-    dev = E.compute_device(*(a for a in (x0, param_ranges, xs, ys, ts, ps) if isinstance(a, torch.Tensor)))
-    B = _window_count(batch_end_indices)
-    x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows")
-    with torch.cuda.device(dev):
-        if x0 is None:
-            ranges = _per_window(param_ranges, B, (K, 2), "param_ranges", dev)
-            opts = _model(warp, warpfunc, objective, sigmas[0], obj_param, H, W)
-            start = _grid_search(lambda c: _candidates(x, y, t_rel, p, offsets, c, opts), ranges,
-                                 num_samples_per_param, grid_levels, log_scale)
-            scale = (ranges[..., 1] - ranges[..., 0]) / (num_samples_per_param - 1)
-        else:
-            start = _per_window(x0, B, (K,), "x0", dev)
-            scale = torch.ones((B, K), dtype=torch.float64, device=dev)
-        if param_scale is not None:
-            scale = _per_window(param_scale, B, (K,), "param_scale", dev)
-        xk = start
-        iters = torch.zeros(B, dtype=torch.int32, device=dev)
-        status = f = None
-        for sigma in sigmas:
-            opts = _model(warp, warpfunc, objective, sigma, obj_param, H, W)
-            xk, f, status, it = _batched_bfgs(_objective_and_gradient(x, y, t_rel, p, offsets, opts),
-                                              lambda c: _candidates(x, y, t_rel, p, offsets, c, opts), xk, scale,
-                                              max_iter, line_search_steps, ftol, gtol)
-            iters += it
+        raise ValueError("%s needs x0 or param_ranges" % who)
+    return sigmas
+
+
+def _fit_stages(stage, sigmas, B, K, dev, x0, param_ranges, num_samples_per_param, grid_levels, log_scale, param_scale,
+                max_iter, line_search_steps, ftol, gtol, bounds=None, bound_to_ranges=False, unit_first_step=False):
+    """The start point and the BFGS stages the fits share.  stage(sigma) -> (fg, candidates) of the objective at that
+    blur.  bounds ((K,2) or (B,K,2)) confines the line searches; without it, bound_to_ranges confines a grid-started fit
+    to param_ranges widened by one level-0 grid step on each side, and further to take in the grid's best point (a
+    later grid level may lie beyond the ranges).
+    unit_first_step is _batched_bfgs'."""
+    if bounds is not None:
+        bounds = _per_window(bounds, B, (K, 2), "bounds", dev)
+    if x0 is None:
+        ranges = _per_window(param_ranges, B, (K, 2), "param_ranges", dev)
+        start = _grid_search(stage(sigmas[0])[1], ranges, num_samples_per_param, grid_levels, log_scale)
+        scale = (ranges[..., 1] - ranges[..., 0]) / (num_samples_per_param - 1)
+        if bounds is None and bound_to_ranges:
+            # one grid step beyond the ranges: a start on the ranges' edge must be free to step outwards
+            bounds = torch.stack((torch.minimum(ranges[..., 0] - scale, start), torch.maximum(ranges[..., 1] + scale, start)),
+                                 dim=-1)
+    else:
+        start = _per_window(x0, B, (K,), "x0", dev)
+        scale = torch.ones((B, K), dtype=torch.float64, device=dev)
+    if param_scale is not None:
+        scale = _per_window(param_scale, B, (K,), "param_scale", dev)
+    xk = start
+    iters = torch.zeros(B, dtype=torch.int32, device=dev)
+    status = f = None
+    for sigma in sigmas:
+        fg, candidates = stage(sigma)
+        xk, f, status, it = _batched_bfgs(fg, candidates, xk, scale, max_iter, line_search_steps, ftol, gtol, bounds,
+                                          unit_first_step)
+        iters += it
     return MotionFit(xk, f, status, iters)
 
 
@@ -113,11 +136,16 @@ def _window_count(batch_end_indices):
 def _per_window(v, B, shape, name, dev):
     """v of `shape` or (B,)+shape as a (B,)+shape f64 tensor on dev (a host value is copied without a host wait)"""
     t = v if isinstance(v, torch.Tensor) else torch.from_numpy(np.array(v, dtype=np.float64))
+    _check_per_window(t, B, shape, name)
     if tuple(t.shape) == tuple(shape):
         t = t.unsqueeze(0).expand((B,) + tuple(shape))
-    if tuple(t.shape) != (B,) + tuple(shape):
-        raise ValueError("%s must have shape %s or %s, got %s" % (name, tuple(shape), (B,) + tuple(shape), tuple(t.shape)))
     return _to_device(t.to(torch.float64), dev).contiguous()
+
+
+def _check_per_window(v, B, shape, name):
+    got = tuple(v.shape) if isinstance(v, torch.Tensor) else np.shape(v)
+    if got != tuple(shape) and got != (B,) + tuple(shape):
+        raise ValueError("%s must have shape %s or %s, got %s" % (name, tuple(shape), (B,) + tuple(shape), got))
 
 
 def _to_device(t, dev):
@@ -204,10 +232,15 @@ def _grid_search(evaluate, ranges, num_samples_per_param=5, levels=1, log_scale=
     return best
 
 
-def _batched_bfgs(fg, candidates, x0, scale, max_iter=50, line_search_steps=8, ftol=1e-9, gtol=1e-9):
+def _batched_bfgs(fg, candidates, x0, scale, max_iter=50, line_search_steps=8, ftol=1e-9, gtol=1e-9, bounds=None,
+                  unit_first_step=False):
     """
     The BFGS core of motion_contrast_fit_torch, on any batched objective: fg((B,K) x) -> (f (B,), g (B,K)) and
     candidates((B,J,K) points) -> (B,J) f, all f64.  Runs exactly max_iter iterations over every window, under masks.
+    bounds: None, or (B,K,2) [lo, hi] per window: a line-search point outside its window's box scores +inf, so no step
+    leaves the box.
+    unit_first_step: start from H = D / |g * scale| instead of D = diag(scale^2), so that the first step is one unit of
+    scale long whatever the size of g (scipy's BFGS likewise makes its first step about one unit long).
     @returns (x (B,K), f (B,), status (B,) int8, iterations (B,) int32)
     """
     x = x0.to(torch.float64).clone()
@@ -225,6 +258,10 @@ def _batched_bfgs(fg, candidates, x0, scale, max_iter=50, line_search_steps=8, f
     iters = torch.zeros(B, dtype=torch.int32, device=dev)
     scaled = torch.zeros(B, dtype=torch.bool, device=dev)     # H rescaled after the first accepted step
     gam = torch.ones(B, dtype=torch.float64, device=dev)      # the latest s'y / y'Dy: a reset starts from gam D
+    if unit_first_step:
+        gn = (g * scale).norm(dim=1)
+        gam = torch.where(finite & (gn > 0), 1.0 / torch.where(gn > 0, gn, torch.ones_like(gn)), gam)
+        Hinv = gam.view(-1, 1, 1) * D
     reset = torch.zeros(B, dtype=torch.bool, device=dev)      # H reset since the last accepted step
     alphas = torch.pow(2.0, -torch.arange(line_search_steps, dtype=torch.float64, device=dev))
     for _ in range(max_iter):
@@ -232,6 +269,9 @@ def _batched_bfgs(fg, candidates, x0, scale, max_iter=50, line_search_steps=8, f
         slope = (g * d).sum(1)
         pts = x.unsqueeze(1) + alphas.view(1, -1, 1) * d.unsqueeze(1)
         fc = torch.nan_to_num(candidates(pts), nan=float("inf"))
+        if bounds is not None:
+            inside = ((pts >= bounds[:, None, :, 0]) & (pts <= bounds[:, None, :, 1])).all(2)
+            fc = torch.where(inside, fc, float("inf"))
         armijo = fc <= f.unsqueeze(1) + ARMIJO_C1 * alphas.unsqueeze(0) * slope.unsqueeze(1)
         j_best = fc.argmin(1)
         j = torch.where(armijo.any(1), armijo.to(torch.int8).argmax(1), j_best)

@@ -14,7 +14,7 @@ from .. import _lib
 from ..representations import _events as E
 from .flow_objective import _batch_events, _event_tensors
 from .flow_timestamp_objective import _normalised_stamps
-from .motion_objective import _WARPS
+from .motion_objective import _WARPS, MAX_CANDIDATES, _warp_code
 
 
 def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, blur_sigma=2.0, timestamp_reverse=False,
@@ -84,3 +84,76 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
     centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
     f = MotionTimestampObjective.apply(params, x, y, t_rel, tau, p, offsets, (warp, centre, H, W, float(blur_sigma)))
     return f.to(device=params.device, dtype=params.dtype)
+
+
+# The workspace of one evk_motion_timestamp_candidates_f32 call stays below this many bytes: larger batches of windows
+# run in chunks (96 bytes per canvas pixel and candidate: 16 GiB hold 119 windows x 32 candidates at 180x240, about as
+# many windows per chunk as the contrast loss's candidates pass takes).
+TIMESTAMP_CANDIDATES_WORKSPACE_BYTES = 16 << 30
+
+
+def motion_timestamp_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=None, blur_sigma=2.0, timestamp_reverse=False,
+                                      img_size=(180, 240), batch_end_indices=None):
+    """
+    The average-timestamp loss of every window b under each of its J candidate parameter vectors candidates[b, j]:
+    f[b, j] is the f_b that motion_timestamp_objective_torch returns with params[b] = candidates[b, j] (same windows, t0,
+    stamps, keep rule, blur and canvas).  Each pass over the events scores up to 32 candidates of every window
+    (evk_motion_timestamp_candidates_f32): the grid search and the line search of motion_timestamp_fit_torch.  J is split
+    into passes of at most 32 candidates, and the windows into chunks whose workspace stays under
+    TIMESTAMP_CANDIDATES_WORKSPACE_BYTES; neither split changes a value's arithmetic.
+    @param candidates (B,J,K) parameter vectors, any float dtype, K = warpfunc.dims, any J >= 1
+    @returns (B,J) f64 tensor of values (no autograd graph) on candidates' device
+    """
+    warp = _warp_code(warpfunc, "motion_timestamp_candidates_torch")
+    xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_timestamp_candidates_torch", "nothing")
+    cand = E.as_tensor(candidates)
+    if not cand.is_floating_point():
+        raise ValueError("candidates must be a floating-point tensor, got %s" % cand.dtype)
+    if cand.dim() != 3 or cand.shape[2] != warpfunc.dims or cand.shape[1] < 1:
+        raise ValueError("candidates must have shape (B,J,%d) with J >= 1 for %s, got %s"
+                         % (warpfunc.dims, type(warpfunc).__name__, tuple(cand.shape)))
+    B = cand.shape[0]
+    H, W = int(img_size[0]), int(img_size[1])
+    _lib.lib()
+    dev = E.compute_device(cand, xs, ys, ts, ps)
+    x, y, t_rel, p, offsets, t, sample = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "candidate sets",
+                                                       stamps=True)
+    with torch.cuda.device(dev):
+        tau = _normalised_stamps(t, sample, offsets, timestamp_reverse)
+        c64 = cand.detach().to(device=dev, dtype=torch.float64)
+        f = _ts_candidates(x, y, t_rel, tau, p, offsets, c64, _ts_model(warp, warpfunc, blur_sigma, H, W))
+    return f.to(cand.device)
+
+
+def _ts_model(warp, warpfunc, blur_sigma, H, W):
+    """the scalar arguments the motion timestamp entries share: (warp code, (cx, cy), H, W, sigma)"""
+    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
+    return warp, centre, H, W, float(blur_sigma)
+
+
+def _ts_candidates(x, y, t_rel, tau, p, offsets, c64, opts):
+    """f (B,J) f64 of the prepared device events under the device candidates c64 (B,J,K) f64, in passes of at most
+    MAX_CANDIDATES candidates over chunks of windows whose workspace fits TIMESTAMP_CANDIDATES_WORKSPACE_BYTES"""
+    warp, (cx, cy), H, W, sigma = opts
+    B, J, K = c64.shape
+    L = _lib.lib()
+    dev = x.device
+    f = torch.empty((B, J), dtype=torch.float64, device=dev)
+    if B == 0:
+        return f
+    jc = min(J, MAX_CANDIDATES)
+    per_window = L.evk_motion_timestamp_candidates_workspace_bytes(1, jc, H, W)
+    wb = max(1, min(B, TIMESTAMP_CANDIDATES_WORKSPACE_BYTES // per_window, 32767 // jc))
+    ws = _lib.scratch("motion_timestamp_candidates", L.evk_motion_timestamp_candidates_workspace_bytes(wb, jc, H, W), dev)
+    for b0 in range(0, B, wb):
+        b1 = min(B, b0 + wb)
+        for j0 in range(0, J, MAX_CANDIDATES):
+            j1 = min(J, j0 + MAX_CANDIDATES)
+            c = c64[b0:b1, j0:j1].contiguous()
+            out = torch.empty((b1 - b0, j1 - j0), dtype=torch.float64, device=dev)
+            _lib.check(L.evk_motion_timestamp_candidates_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets[b0:]), b1 - b0,
+                x.shape[0], warp, _lib.ptr(c), j1 - j0, K, cx, cy, H, W, sigma, _lib.ptr(out), _lib.ptr(ws), ws.numel(),
+                _lib.stream()))
+            f[b0:b1, j0:j1] = out
+    return f

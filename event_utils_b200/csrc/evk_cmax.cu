@@ -2324,11 +2324,23 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_ts_event_kernel(const 
     }
 }
 
-// shared argument checks and set-up of the two parametric timestamp entry points (those of motion_obj_setup, for 2B images)
+// the candidates entry's workspace for `images` = 2 batch n_cand images: the forward-only carve (no f64 adjoint images;
+// the T images go to its Wimg), then the C images the fold writes, which nothing reads
+static size_t motion_ts_cand_head(int images, int H, int W)
+{
+    return batch_obj_carve(nullptr, images, H, W, flow_ts_acc_blocks(H, W), nullptr, false);
+}
+static size_t motion_ts_cand_bytes(int images, int H, int W)
+{
+    return motion_ts_cand_head(images, H, W) + align_up((size_t)images * (H + 1) * (W + 1) * sizeof(float), 256);
+}
+
+// shared argument checks and set-up of the parametric timestamp entry points (those of motion_obj_setup, for 2B images;
+// with `candidates`, for 2 B n_cand forward-only images)
 static int motion_ts_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
                            const int64_t *offsets, int batch, int64_t n, int warp, const double *params, int K, double cx,
                            double cy, int H, int W, double sigma, void *workspace, size_t workspace_bytes, MotionTsArgs &A,
-                           BatchObjWorkspace &ws, BlurTaps &taps)
+                           BatchObjWorkspace &ws, BlurTaps &taps, bool candidates = false, int n_cand = 1)
 {
     if (int rc = check_sigma(who, sigma)) return rc;
     if (batch < 0 || batch > 32767 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
@@ -2339,9 +2351,19 @@ static int motion_ts_setup(const char *who, const float *x, const float *y, cons
     const int dims = motion_obj_dims(warp);
     if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
     if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
-    int rc = batch_obj_check(who, "parameters", 2 * batch, H, W, sigma, OBJ_SOS, flow_ts_acc_blocks(H, W), workspace,
-                             workspace_bytes, ws, taps);
+    // the tail's grid takes at most 65535 images, two per sample and candidate
+    if (candidates && (n_cand < 1 || n_cand > kMaxCandidates || (int64_t)batch * n_cand > 32767)) {
+        set_error("%s: bad arguments (1 <= n_cand <= %d, batch * n_cand <= 32767)", who, kMaxCandidates);
+        return EVK_E_ARG;
+    }
+    const int images = 2 * batch * (candidates ? n_cand : 1);
+    int rc = batch_obj_check(who, "parameters", images, H, W, sigma, OBJ_SOS, flow_ts_acc_blocks(H, W), workspace,
+                             workspace_bytes, ws, taps, !candidates);
     if (rc) return rc;
+    if (candidates && workspace_bytes < motion_ts_cand_bytes(images, H, W)) {
+        set_error("%s: 256-byte aligned workspace of %zu bytes required", who, motion_ts_cand_bytes(images, H, W));
+        return EVK_E_WORKSPACE;
+    }
     A = MotionTsArgs{};
     A.M.C.Hm = H; A.M.C.Wm = W; A.M.C.Hc = H + 1; A.M.C.Wc = W + 1;
     A.M.C.p_scale = 1.0;
@@ -2358,6 +2380,86 @@ static void launch_motion_ts_events(int warp, const MotionTsArgs &A, int batch, 
     if (warp == EVK_WARP_LINVEL) motion_ts_event_kernel<WARP_LINVEL_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
     else if (warp == EVK_WARP_ROTATION) motion_ts_event_kernel<WARP_ROTATION_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
     else motion_ts_event_kernel<WARP_XYZTHETA_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
+}
+
+// ---- many parameter vectors per sample in one event pass (evk_motion_timestamp_candidates_f32) --------------------
+// The grid search and the line search of a batched fit of the timestamp loss score n_cand parameter vectors of every
+// sample.  On the (slices, batch) grid, each CTA takes its sample's n_cand x K candidates into shared memory, reads each
+// event ONCE (x, y, t, tau, p: 20 B) and, under every candidate that keeps it, makes the two v4 reductions of
+// motion_ts_event_kernel's forward into the 32-byte {S, C} block of its polarity, image pair z = 2 (b n_cand + j) + s of
+// [batch][n_cand][2][Hc][Wc][8].  ts_obj_forward_tail then treats the batch x n_cand pairs as the samples of
+// evk_motion_timestamp_objective_f32, so f comes out in [batch][n_cand] order.
+struct MotionTsCandArgs {
+    MotionTsArgs T;    // events, stamps, samples and canvas; T.M.params = the candidates [B][n_cand][K]; T.M.acc = the blocks
+    int n_cand;
+};
+
+template <int WARP>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_ts_cand_kernel(const MotionTsCandArgs A)
+{
+    constexpr int K = model_dims(WARP);
+    __shared__ WarpModel cand[kMaxCandidates];
+    const MotionObjArgs &M0 = A.T.M;
+    const int b = blockIdx.y, J = A.n_cand;
+    for (int j = threadIdx.x; j < J; j += kFlowObjThreads) {
+        WarpModel M{};
+#pragma unroll
+        for (int k = 0; k < K; ++k) M.m[k] = M0.params[((int64_t)b * J + j) * K + k];
+        if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = M0.cx; M.m[5] = M0.cy; }
+        cand[j] = M;
+    }
+    __syncthreads();
+    int64_t first = M0.offsets[b], last = M0.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > M0.n) last = M0.n;
+    const int Wc = M0.C.Wc;
+    const int64_t npix = (int64_t)M0.C.Hc * Wc;
+    float *acc = M0.acc + (int64_t)b * J * 2 * npix * 8;
+    unsigned oob = 0;   // as in motion_ts_event_kernel: a contributing event lies inside the canvas
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i < last; i += kBatch * stride) {
+        Event<WARP> e[kBatch];
+        float eu[kBatch];
+        int64_t plane[kBatch];   // 0 for a positive event, npix for a negative one, -1 for none (NaN polarity, past the end)
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int64_t q = i + k * stride;
+            plane[k] = -1;
+            if (q < last) {
+                e[k].x = ld_stream(M0.x + q); e[k].y = ld_stream(M0.y + q); e[k].t = ld_stream(M0.t + q); e[k].p = 1.0f;
+                eu[k] = ld_stream(A.T.tau + q);
+                const float pe = ld_stream(M0.p + q);
+                if (pe > 0.0f) plane[k] = 0;
+                else if (pe <= 0.0f) plane[k] = npix;   // NaN polarity: in neither image (evk_tsimg.cu)
+            }
+        }
+        for (int j = 0; j < J; ++j) {
+            const WarpModel M = cand[j];
+            float *accj = acc + (int64_t)j * 2 * npix * 8;
+#pragma unroll
+            for (int k = 0; k < kBatch; ++k) {
+                Taps T;
+                float jx[4], jy[4];
+                if (plane[k] < 0 || !model_taps<WARP, false>(M0.C, e[k], M, oob, T, jx, jy)) continue;
+                const float dx = T.dx, dy = T.dy;
+                const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+                // tsimg_scatter_kernel's taps, as motion_ts_event_kernel forms them
+                const float tl = __fmul_rn(eu[k], ox), tr = __fmul_rn(eu[k], dx);
+                float *blk = accj + (plane[k] + (int64_t)T.y0 * Wc + T.x0) * 8;
+                red_add4(blk, make_float4(__fmul_rn(tl, oy), __fmul_rn(tr, oy), __fmul_rn(tl, dy), __fmul_rn(tr, dy)));
+                red_add4(blk + 4, make_float4(__fmul_rn(ox, oy), __fmul_rn(dx, oy), __fmul_rn(ox, dy), __fmul_rn(dx, dy)));
+            }
+        }
+    }
+}
+
+static void launch_motion_ts_cand_events(int warp, const MotionTsCandArgs &A, int batch, cudaStream_t st)
+{
+    const dim3 grid = flow_obj_grid(A.T.M.n, batch);
+    if (warp == EVK_WARP_LINVEL) motion_ts_cand_kernel<WARP_LINVEL_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else if (warp == EVK_WARP_ROTATION) motion_ts_cand_kernel<WARP_ROTATION_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else motion_ts_cand_kernel<WARP_XYZTHETA_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
 }
 
 }  // namespace evk
@@ -3009,6 +3111,43 @@ int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, cons
         prof_count(1);
         launch_motion_ts_events<true>(warp, A, batch, st);
     }
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_motion_timestamp_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
+{
+    if (batch < 0 || n_cand < 1 || n_cand > evk::kMaxCandidates || H < 2 || W < 2) return 0;
+    return evk::motion_ts_cand_bytes(2 * batch * n_cand, H, W);
+}
+
+int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                        const int64_t *offsets, int batch, int64_t n_events, int warp, const double *cand,
+                                        int n_cand, int K, double cx, double cy, int H, int W, double blur_sigma, double *f_out,
+                                        void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    MotionTsCandArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_ts_setup("evk_motion_timestamp_candidates_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp, cand,
+                             K, cx, cy, H, W, blur_sigma, workspace, workspace_bytes, A.T, ws, taps, true, n_cand);
+    if (rc) return rc;
+    if (batch > 0 && !f_out) { set_error("evk_motion_timestamp_candidates_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch * n_cand;
+    // nonfinite stays zero, as in evk_motion_timestamp_objective_f32
+    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)images * npix * 8 * sizeof(float), st));
+    A.T.M.acc = ws.acc;
+    A.n_cand = n_cand;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_ts_cand_events(warp, A, batch, st);
+    }
+    float *cnt = reinterpret_cast<float *>(static_cast<char *>(workspace) + motion_ts_cand_head(images, H, W));
+    ts_obj_forward_tail(ws, Hc, Wc, taps, batch * n_cand, ws.Wimg, cnt, f_out, st);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }

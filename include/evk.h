@@ -626,6 +626,24 @@ int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, cons
                                             const float *grad_f, double *grad_params, void *workspace,
                                             size_t workspace_bytes, void *stream);
 
+/* Many parameter vectors per sample in one pass over the events, for the average-timestamp loss: the sample points of a
+ * grid search per window or the step lengths of a batched line search.  f_out[b][j] is exactly the f_b of
+ * evk_motion_timestamp_objective_f32 with params[b] = cand[b][j]: the same warp, keep rule, NaN-polarity rule, stamps
+ * tau and blur, the same argument checks and the blur-sigma rule for blur_sigma (0 or less: no blur; NaN: EVK_E_ARG; a
+ * radius over 64: EVK_E_UNSUPPORTED), all checked before any CUDA call.  Forward only: no image out, no gradient.
+ *   cand : [batch][n_cand][K] doubles in DEVICE memory, 1 <= n_cand <= 32, batch * n_cand <= 32767
+ *   f_out: [batch][n_cand] doubles
+ * Every event is read once and splatted under each of its sample's n_cand candidates.
+ * workspace: evk_motion_timestamp_candidates_workspace_bytes(batch, n_cand, H, W) bytes (about 96 bytes per canvas pixel
+ * and candidate), 256-byte aligned; the query returns 0 for arguments the entry rejects.
+ * The call does not synchronise and launches the same kernels whatever batch and n_cand. */
+size_t evk_motion_timestamp_candidates_workspace_bytes(int batch, int n_cand, int H, int W);
+int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                        const float *p, const int64_t *offsets, int batch, int64_t n_events, int warp,
+                                        const double *cand, int n_cand, int K, double cx, double cy, int H, int W,
+                                        double blur_sigma, double *f_out, void *workspace, size_t workspace_bytes,
+                                        void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * RobustNorm (row f4): clamp a tensor between two of its order statistics and rescale it.  Replaces
  * RobustNorm.__call__ / .percentile, lib/data_loaders/data_augmentation.py:82-130 (two kthvalue sorts),
