@@ -5,7 +5,8 @@ start, then scipy's BFGS (optimize_contrast, events_cmax.py:313-346), with one f
 per f / f' call.  motion_contrast_fit_torch fits B windows at once: every grid level and every line search is ONE
 candidates pass over the events (motion_contrast_candidates_torch), f and its gradient are one call each of the
 batched loss's C entries, and the BFGS state is a set of (B,K) / (B,K,K) tensors updated under per-window masks.  The
-number of iterations is fixed, so with every input on the GPU the fit never synchronises with the host.
+number of iterations is fixed, so with every input on the GPU the fit never synchronises with the host.  Every call of
+an entry takes a chunk of the windows, at most as many as the entry's batch limit and its workspace budget allow.
 """
 import collections
 
@@ -55,8 +56,13 @@ def motion_contrast_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None, 
     values bit for bit while the others iterate.
     blur_sigma may be a sequence: stage i refines at blur_sigma[i] from stage i-1's result, and the grid search runs
     at blur_sigma[0] only (grid_cmax's grid at blur 2, then refinement at 1, events_cmax.py:28-76).
-    Every stage runs exactly max_iter iterations on all windows, so with the events, the window ends and x0 (or
-    param_ranges) on the GPU the fit never synchronises with the host, and its launch sequence does not depend on B.
+    Every stage runs exactly max_iter iterations on all windows (max_iter = 0 returns the start), so with the events,
+    the window ends and x0 (or param_ranges) on the GPU the fit never synchronises with the host.
+    Any number of windows B: each candidates call runs the windows in chunks of
+    max(1, min(B, CANDIDATES_WORKSPACE_BYTES // its workspace per window, 65535 // min(J, 32))) windows (J the candidates
+    of the call: num_samples_per_param^K for a grid level, line_search_steps for a line search), and each forward and
+    gradient call in chunks of max(1, min(B, FIT_WORKSPACE_BYTES // (workspace + image per window), 65535)).  The launch
+    sequence therefore depends on B only through those numbers of chunks.
     @returns MotionFit(params (B,K) f64, f (B,) f64 at params for the last stage's blur, status (B,) int8, iterations
              (B,) int32 summed over the stages) on the events' device.  status: 0 converged, 1 iteration limit,
              2 no descent, 3 non-finite start, f or g at a stage's start (the window keeps that start).  An empty window,
@@ -157,8 +163,21 @@ def _to_device(t, dev):
     return t.to(dev)
 
 
+def fit_window_chunk(B, per_window_bytes, budget, cap):
+    """Windows per call of a fit's forward and gradient entries: at most `cap` (the entries' batch limit) and at most
+    as many as fit `budget` bytes of workspace and images, but at least one"""
+    return max(1, min(B, budget // per_window_bytes, cap))
+
+
+# One forward + gradient call of motion_contrast_fit_torch takes at most this many windows (the entries' batch limit)
+# and at most as many as fit FIT_WORKSPACE_BYTES of workspace and images; larger batches run in chunks of windows.
+FIT_MAX_WINDOWS = 65535
+FIT_WORKSPACE_BYTES = 4 << 30
+
+
 def _objective_and_gradient(x, y, t_rel, p, offsets, opts):
-    """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_cmax_motion_objective_f32 / _grad_f32 (grad_f = 1)"""
+    """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_cmax_motion_objective_f32 / _grad_f32 (grad_f = 1), in
+    chunks of windows (fit_window_chunk); the windows are independent, so a chunk changes no value's arithmetic"""
     warp, (cx, cy), H, W, objective, sigma, param = opts
     L = _lib.lib()
     dev = x.device
@@ -168,14 +187,19 @@ def _objective_and_gradient(x, y, t_rel, p, offsets, opts):
         prm = params.contiguous()
         f = torch.empty(B, dtype=torch.float64, device=dev)
         g = torch.empty((B, K), dtype=torch.float64, device=dev)
-        iwe = torch.empty((B, H + 1, W + 1), dtype=torch.float32, device=dev)
-        ones = torch.ones(B, dtype=torch.float32, device=dev)
-        ws = _lib.scratch("motion_objective", L.evk_cmax_motion_objective_workspace_bytes(B, H, W), dev)
-        ev = (_lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0], warp, _lib.ptr(prm),
-              K, cx, cy, H, W, sigma, objective, param)
-        _lib.check(L.evk_cmax_motion_objective_f32(*ev, _lib.ptr(f), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(), _lib.stream()))
-        _lib.check(L.evk_cmax_motion_objective_grad_f32(*ev, _lib.ptr(iwe), _lib.ptr(ones), _lib.ptr(g), _lib.ptr(ws),
-                                                        ws.numel(), _lib.stream()))
+        per_window = L.evk_cmax_motion_objective_workspace_bytes(1, H, W) + 4 * (H + 1) * (W + 1)
+        wb = fit_window_chunk(B, per_window, FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS)
+        iwe = torch.empty((wb, H + 1, W + 1), dtype=torch.float32, device=dev)
+        ones = torch.ones(wb, dtype=torch.float32, device=dev)
+        ws = _lib.scratch("motion_objective", L.evk_cmax_motion_objective_workspace_bytes(wb, H, W), dev)
+        for b0 in range(0, B, wb):
+            b1 = min(B, b0 + wb)
+            ev = (_lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(offsets[b0:]), b1 - b0, x.shape[0], warp,
+                  _lib.ptr(prm[b0:b1]), K, cx, cy, H, W, sigma, objective, param)
+            _lib.check(L.evk_cmax_motion_objective_f32(*ev, _lib.ptr(f[b0:b1]), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(),
+                                                       _lib.stream()))
+            _lib.check(L.evk_cmax_motion_objective_grad_f32(*ev, _lib.ptr(iwe), _lib.ptr(ones), _lib.ptr(g[b0:b1]),
+                                                            _lib.ptr(ws), ws.numel(), _lib.stream()))
         return f, g
     return fg
 

@@ -12,9 +12,13 @@ from .. import _lib
 from ..representations import _events as E
 from .flow_objective import _batch_events, _event_tensors
 from .flow_timestamp_objective import _normalised_stamps
-from .motion_fit import _check_per_window, _fit_arguments, _fit_stages, _window_count
+from .motion_fit import FIT_WORKSPACE_BYTES, _check_per_window, _fit_arguments, _fit_stages, _window_count, fit_window_chunk
 from .motion_objective import _warp_code
 from .motion_timestamp_objective import _ts_candidates, _ts_model
+
+# One forward + gradient call of motion_timestamp_fit_torch takes at most this many windows (the entries' batch limit:
+# two tail images per window) and at most as many as fit motion_fit.FIT_WORKSPACE_BYTES
+TIMESTAMP_FIT_MAX_WINDOWS = 32767
 
 
 def motion_timestamp_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None, t0=None, blur_sigma=2.0,
@@ -31,6 +35,11 @@ def motion_timestamp_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None,
     Start point, refinement, stages (blur_sigma may be a sequence), tolerances, statuses and the absence of host
     synchronisation are those of motion_contrast_fit_torch, with f and g from evk_motion_timestamp_objective_f32 /
     _grad_f32 and every grid level and line search one evk_motion_timestamp_candidates_f32 pass.
+    Any number of windows B: each candidates call runs the windows in chunks of
+    max(1, min(B, TIMESTAMP_CANDIDATES_WORKSPACE_BYTES // its workspace per window, 32767 // min(J, 32))) windows (J the
+    candidates of the call: num_samples_per_param^K for a grid level, line_search_steps for a line search), and each
+    forward and gradient call in chunks of max(1, min(B, FIT_WORKSPACE_BYTES // (workspace + images per window), 32767)).
+    The launch sequence depends on B only through those numbers of chunks.
     One difference: the inverse Hessian starts as diag(param_scale^2) / |g * param_scale|, so that the first step is one
     unit of param_scale long.  This loss's gradient is large against its scale (f is a sum over the canvas, not a
     mean), and a first step of H g with H = diag(param_scale^2) overshoots by far more than the 2^-(line_search_steps-1)
@@ -68,7 +77,9 @@ def motion_timestamp_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None,
 
 
 def _objective_and_gradient(x, y, t_rel, tau, p, offsets, opts):
-    """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_motion_timestamp_objective_f32 / _grad_f32 (grad_f = 1)"""
+    """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_motion_timestamp_objective_f32 / _grad_f32 (grad_f = 1),
+    in chunks of at most TIMESTAMP_FIT_MAX_WINDOWS windows whose workspace and images fit FIT_WORKSPACE_BYTES; the windows
+    are independent, so a chunk changes no value's arithmetic"""
     warp, (cx, cy), H, W, sigma = opts
     L = _lib.lib()
     dev = x.device
@@ -78,15 +89,19 @@ def _objective_and_gradient(x, y, t_rel, tau, p, offsets, opts):
         prm = params.contiguous()
         f = torch.empty(B, dtype=torch.float64, device=dev)
         g = torch.empty((B, K), dtype=torch.float64, device=dev)
-        T = torch.empty((B, 2, H + 1, W + 1), dtype=torch.float32, device=dev)
+        per_window = L.evk_motion_timestamp_objective_workspace_bytes(1, H, W) + 16 * (H + 1) * (W + 1)
+        wb = fit_window_chunk(B, per_window, FIT_WORKSPACE_BYTES, TIMESTAMP_FIT_MAX_WINDOWS)
+        T = torch.empty((wb, 2, H + 1, W + 1), dtype=torch.float32, device=dev)
         C = torch.empty_like(T)
-        ones = torch.ones(B, dtype=torch.float32, device=dev)
-        ws = _lib.scratch("motion_timestamp_objective", L.evk_motion_timestamp_objective_workspace_bytes(B, H, W), dev)
-        ev = (_lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets), B, x.shape[0], warp,
-              _lib.ptr(prm), K, cx, cy, H, W, sigma)
-        _lib.check(L.evk_motion_timestamp_objective_f32(*ev, _lib.ptr(f), _lib.ptr(T), _lib.ptr(C), _lib.ptr(ws), ws.numel(),
-                                                        _lib.stream()))
-        _lib.check(L.evk_motion_timestamp_objective_grad_f32(*ev, _lib.ptr(T), _lib.ptr(C), _lib.ptr(ones), _lib.ptr(g),
-                                                             _lib.ptr(ws), ws.numel(), _lib.stream()))
+        ones = torch.ones(wb, dtype=torch.float32, device=dev)
+        ws = _lib.scratch("motion_timestamp_objective", L.evk_motion_timestamp_objective_workspace_bytes(wb, H, W), dev)
+        for b0 in range(0, B, wb):
+            b1 = min(B, b0 + wb)
+            ev = (_lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets[b0:]), b1 - b0,
+                  x.shape[0], warp, _lib.ptr(prm[b0:b1]), K, cx, cy, H, W, sigma)
+            _lib.check(L.evk_motion_timestamp_objective_f32(*ev, _lib.ptr(f[b0:b1]), _lib.ptr(T), _lib.ptr(C), _lib.ptr(ws),
+                                                            ws.numel(), _lib.stream()))
+            _lib.check(L.evk_motion_timestamp_objective_grad_f32(*ev, _lib.ptr(T), _lib.ptr(C), _lib.ptr(ones),
+                                                                 _lib.ptr(g[b0:b1]), _lib.ptr(ws), ws.numel(), _lib.stream()))
         return f, g
     return fg
