@@ -175,6 +175,22 @@ def _declare(L):
     L.evk_cmax_motion_candidates_f32.restype = ci
     L.evk_cmax_motion_candidates_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, ci, f64, f64, ci, ci, f64, ci, f64, vp,
                                                  vp, sz, vp]
+    L.evk_cmax_motion_segment_workspace_bytes.restype = sz
+    L.evk_cmax_motion_segment_workspace_bytes.argtypes = [ci, ci, ci, ci]
+    L.evk_cmax_motion_segment_f32.restype = ci
+    L.evk_cmax_motion_segment_f32.argtypes = [vp, vp, vp, vp, vp, ci, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci, f64, ci, f64,
+                                              vp, vp, vp, sz, vp]
+    L.evk_cmax_motion_segment_grad_f32.restype = ci
+    L.evk_cmax_motion_segment_grad_f32.argtypes = [vp, vp, vp, vp, vp, ci, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci, f64, ci,
+                                                   f64, vp, vp, vp, vp, vp, sz, vp]
+    L.evk_cmax_motion_segment_candidates_workspace_bytes.restype = sz
+    L.evk_cmax_motion_segment_candidates_workspace_bytes.argtypes = [ci, ci, ci, ci, ci]
+    L.evk_cmax_motion_segment_candidates_f32.restype = ci
+    L.evk_cmax_motion_segment_candidates_f32.argtypes = [vp, vp, vp, vp, vp, ci, vp, ci, i64, ci, vp, ci, ci, f64, f64, ci, ci,
+                                                         f64, ci, f64, vp, vp, sz, vp]
+    L.evk_cmax_motion_segment_assign_f32.restype = ci
+    L.evk_cmax_motion_segment_assign_f32.argtypes = [vp, vp, vp, ci, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci, vp, f64, f64,
+                                                     vp, vp, sz, vp]
     L.evk_flow_timestamp_objective_workspace_bytes.restype = sz
     L.evk_flow_timestamp_objective_workspace_bytes.argtypes = [ci, ci, ci]
     L.evk_flow_timestamp_objective_f32.restype = ci

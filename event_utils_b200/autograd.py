@@ -16,6 +16,7 @@ Which inputs get a gradient (as in the reference; the others get None):
     flow_contrast_objective_torch    flow only (contrast_max/flow_objective.py; the events are data)
     flow_timestamp_objective_torch   flow only (contrast_max/flow_timestamp_objective.py; the events are data)
     motion_contrast_objective_torch  params only (contrast_max/motion_objective.py; the events are data)
+    motion_segmentation_objective_torch  params and weights (contrast_max/motion_segmentation.py; the events are data)
     motion_timestamp_objective_torch params only (contrast_max/motion_timestamp_objective.py; the events are data)
 
 The public functions take this path only when grad mode is on and one of those inputs requires grad; every
@@ -305,6 +306,53 @@ class MotionObjective(torch.autograd.Function):
                 cx, cy, H, W, sigma, objective, param, _lib.ptr(iwe), _lib.ptr(g), _lib.ptr(gp), _lib.ptr(ws), ws.numel(),
                 _lib.stream()))
         return _as_input(gp, ctx.meta), None, None, None, None, None, None
+
+
+class MotionSegmentationObjective(torch.autograd.Function):
+    """The weighted multi-model contrast of contrast_max/motion_segmentation.py: f (B,M) f64 from params (B,M,K), the
+    memberships weights (N,M) and the prepared device events.  The parameters and the memberships get gradients, one
+    pass over the events for both (evk_cmax_motion_segment_grad_f32); the membership gradient only when weights
+    requires grad.  opts = (warp code, centre, H, W, objective, sigma, obj_param)."""
+
+    @staticmethod
+    def forward(ctx, params, weights, x, y, t_rel, p, offsets, opts):
+        warp, (cx, cy), H, W, objective, sigma, param = opts
+        dev = x.device
+        B, M, K = params.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            p64 = params.detach().to(device=dev, dtype=torch.float64).contiguous()
+            w32 = weights.detach().to(device=dev, dtype=torch.float32).contiguous()
+            f = torch.empty((B, M), dtype=torch.float64, device=dev)
+            iwe = torch.empty((B, M, H + 1, W + 1), dtype=torch.float32, device=dev)
+            ws = _lib.scratch("motion_segment", L.evk_cmax_motion_segment_workspace_bytes(B, M, H, W), dev)
+            _lib.check(L.evk_cmax_motion_segment_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(w32), M, _lib.ptr(offsets), B, x.shape[0], warp,
+                _lib.ptr(p64), K, cx, cy, H, W, sigma, objective, param, _lib.ptr(f), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(),
+                _lib.stream()))
+        ctx.save_for_backward(x, y, t_rel, p, w32, offsets, p64, iwe)
+        ctx.opts = opts
+        ctx.metas = (_meta(params), _meta(weights))
+        return f
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, y, t_rel, p, w32, offsets, p64, iwe = ctx.saved_tensors
+        warp, (cx, cy), H, W, objective, sigma, param = ctx.opts
+        dev = x.device
+        B, M, K = p64.shape
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g = _grad_in(g, dev)
+            gp = torch.empty_like(p64)
+            gw = torch.zeros_like(w32) if ctx.needs_input_grad[1] else None      # rows outside every window: 0
+            ws = _lib.scratch("motion_segment", L.evk_cmax_motion_segment_workspace_bytes(B, M, H, W), dev)
+            _lib.check(L.evk_cmax_motion_segment_grad_f32(
+                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(w32), M, _lib.ptr(offsets), B, x.shape[0], warp,
+                _lib.ptr(p64), K, cx, cy, H, W, sigma, objective, param, _lib.ptr(iwe), _lib.ptr(g), _lib.ptr(gp), _lib.ptr(gw),
+                _lib.ptr(ws), ws.numel(), _lib.stream()))
+        return _as_input(gp, ctx.metas[0]), _as_input(gw, ctx.metas[1]), None, None, None, None, None, None
 
 
 class MotionTimestampObjective(torch.autograd.Function):

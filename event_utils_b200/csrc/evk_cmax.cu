@@ -2039,6 +2039,301 @@ static void launch_motion_cand_events(int warp, const MotionCandArgs &A, int bat
     else motion_obj_cand_kernel<WARP_XYZTHETA_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
 }
 
+// ---- motion segmentation by motion compensation (evk_cmax_motion_segment_*) ----------------------------------------
+// Stoffregen, Gallego, Drummond, Kleeman, Scaramuzza (ICCV 2019): M motion models per sample and a soft membership
+// w[e][m] of every event in every model.  Image (b, m) is the IWE of sample b's events warped by params[b][m], each
+// event splatted with the f32 weight p_e w[e][m] through model_taps -- exactly the taps of the motion objective run on
+// p * w[:, m] -- and canvas z = b M + m (candidates: (b M + m) J + j) goes through the same image tail.
+//   forward / candidates: motion_seg_cand_kernel on the (slices, batch) grid, the sample's M x J models in shared
+//             memory; each event is read once (16 B and its row of M weights) and costs one v4 reduction per kept
+//             event and model / candidate.
+//   backward: motion_seg_grad_kernel on (slices, batch, M): per event the unweighted taps of model m (so that an event
+//             of weight 0 still has its footprint), four gathers of W_bm, the parameter gradient of
+//             motion_obj_event_kernel<.., true> with wm = p w[e][m], and optionally dF/dw[e][m] = p sum_taps k W_bm.
+//   assignment (E-step): motion_seg_assign_kernel, per event and model c = max(0, sum_taps k G_bm) with the
+//             polarity- and weight-free bilinear fractions k, then w'[e][m] = (c_m + eps) / (sum c + M eps).
+constexpr int kMaxSegModels = 8;
+
+struct MotionSegArgs {
+    MotionObjArgs O;         // events, samples, canvas; O.params [B][M][J][K]; O.acc; O.Wimg [B][M]; O.grad [B][M][K]
+    const float *weights;    // [n][M]
+    int M, J;
+    int wvec4;               // the weight rows load as float4s (M a multiple of 4, 16-byte aligned)
+    const float *grad_f;     // backward: [B][M]
+    const double *gsums;     // backward with the variance: the stats of every G_bm (sum(G) in [4])
+    float *grad_w;           // backward: [n][M] or null
+    const float *G;          // assignment: [B][M][Hc][Wc]
+    double eps;              // assignment
+    float *w_out;            // assignment: [n][M]
+};
+
+__device__ __forceinline__ void load_seg_weights(const MotionSegArgs &A, int64_t i, float (&w)[kMaxSegModels])
+{
+    const float *r = A.weights + i * A.M;
+    if (A.wvec4) {
+#pragma unroll
+        for (int q = 0; q < kMaxSegModels; q += 4) {
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (q < A.M) v = ld_stream4(r + q);
+            w[q] = v.x; w[q + 1] = v.y; w[q + 2] = v.z; w[q + 3] = v.w;
+        }
+    } else {
+#pragma unroll
+        for (int m = 0; m < kMaxSegModels; ++m) w[m] = m < A.M ? ld_stream(r + m) : 0.0f;
+    }
+}
+
+// sample b's models (b M + q, q < count) into shared memory
+template <int WARP>
+__device__ __forceinline__ void load_seg_models(const MotionSegArgs &A, int b, int count, WarpModel *mod)
+{
+    constexpr int K = model_dims(WARP);
+    for (int q = threadIdx.x; q < count; q += blockDim.x) {
+        WarpModel M{};
+#pragma unroll
+        for (int k = 0; k < K; ++k) M.m[k] = A.O.params[((int64_t)b * count + q) * K + k];
+        if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = A.O.cx; M.m[5] = A.O.cy; }
+        mod[q] = M;
+    }
+    __syncthreads();
+}
+
+template <int WARP>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const MotionSegArgs A)
+{
+    __shared__ WarpModel mod[kMaxCandidates];
+    const int b = blockIdx.y, M = A.M, J = A.J;
+    load_seg_models<WARP>(A, b, M * J, mod);
+    int64_t first = A.O.offsets[b], last = A.O.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > A.O.n) last = A.O.n;
+    const int Wc = A.O.C.Wc;
+    const int64_t npix = (int64_t)A.O.C.Hc * Wc;
+    float *acc = A.O.acc + (int64_t)b * M * J * npix * 4;
+    unsigned oob = 0;   // as in motion_obj_event_kernel: a kept finite event lies inside the canvas
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i < last; i += kBatch * stride) {
+        Event<WARP> e[kBatch];
+        float w[kBatch][kMaxSegModels];
+        int ne = 0;
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int64_t q = i + k * stride;
+            if (q < last) {
+                e[k].x = ld_stream(A.O.x + q); e[k].y = ld_stream(A.O.y + q);
+                e[k].t = ld_stream(A.O.t + q); e[k].p = ld_stream(A.O.p + q);
+                load_seg_weights(A, q, w[k]);
+                ne = k + 1;
+            }
+        }
+#pragma unroll
+        for (int m = 0; m < kMaxSegModels; ++m) {
+            if (m >= M) break;
+            for (int j = 0; j < J; ++j) {
+                const WarpModel Mo = mod[m * J + j];
+                float *accq = acc + (int64_t)(m * J + j) * npix * 4;
+#pragma unroll
+                for (int k = 0; k < kBatch; ++k) {
+                    if (k >= ne) continue;
+                    Event<WARP> ek = e[k];
+                    ek.p = __fmul_rn(e[k].p, w[k][m]);   // the splat weight p w, formed in f32
+                    Taps T;
+                    float jx[4], jy[4];
+                    if (model_taps<WARP, false>(A.O.C, ek, Mo, oob, T, jx, jy))
+                        red_add4(accq + ((int64_t)T.y0 * Wc + T.x0) * 4, T.ti);
+                }
+            }
+        }
+    }
+}
+
+template <int WARP>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_grad_kernel(const MotionSegArgs A)
+{
+    constexpr int K = model_dims(WARP);
+    const int b = blockIdx.y, m = blockIdx.z, M = A.M;
+    const int64_t z = (int64_t)b * M + m;
+    int64_t first = A.O.offsets[b], last = A.O.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > A.O.n) last = A.O.n;
+    const int64_t npix = (int64_t)A.O.C.Hc * A.O.C.Wc;
+    WarpModel Mo{};
+#pragma unroll
+    for (int k = 0; k < K; ++k) Mo.m[k] = A.O.params[z * K + k];
+    if (!is_linvel(WARP) && !is_rotation(WARP)) { Mo.m[4] = A.O.cx; Mo.m[5] = A.O.cy; }
+    const float *Wb = A.O.Wimg + z * npix;
+    // W_bm leaves out the variance's constant -2 g mean(G) / P of dF/dI (the tap differences of the parameter gradient
+    // cancel it, see flow_obj_coef_kernel); the weight gradient takes it back: dF/dI = W_bm + c0
+    double c0 = 0.0;
+    if (A.grad_w && A.gsums) c0 = 2.0 * (double)A.grad_f[z] * A.gsums[8 * z + 4] / ((double)npix * (double)npix);
+    double u[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) u[k] = 0.0;
+    unsigned oob = 0;
+    auto one = [&](int64_t i, float xe, float ye, float te, float pe, float we) {
+        Event<WARP> e;
+        e.x = xe; e.y = ye; e.t = te; e.p = 1.0f;   // the footprint does not depend on the weight
+        Taps T;
+        float jx[4], jy[4];
+        double gw = 0.0;
+        if (model_taps<WARP, true>(A.O.C, e, Mo, oob, T, jx, jy)) {
+            const int64_t r0 = (int64_t)T.y0 * A.O.C.Wc, r1 = (int64_t)T.y1 * A.O.C.Wc;
+            const double w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0),
+                         w11 = __ldg(Wb + r1 + T.x1);
+            const double dx = T.dx, dy = T.dy, ox = 1.0 - dx, oy = 1.0 - dy;
+            const float wmf = __fmul_rn(pe, we);
+            if (wmf != 0.0f) {   // splat_taps drops a zero weight: no term, as in motion_obj_event_kernel
+                const double wm = wmf;
+                const double sx = oy * (w01 - w00) + dy * (w11 - w10);
+                const double sy = ox * (w10 - w00) + dx * (w11 - w01);
+#pragma unroll
+                for (int k = 0; k < K; ++k) u[k] += wm * ((double)jx[k] * sx + (double)jy[k] * sy);
+            }
+            gw = (double)pe * (oy * (ox * w00 + dx * w01) + dy * (ox * w10 + dx * w11) + c0);
+        }
+        if (A.grad_w) A.grad_w[i * M + m] = (float)gw;
+    };
+    const float *wcol = A.weights + m;
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
+        float ex[kBatch], ey[kBatch], et[kBatch], ep[kBatch], ew[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int64_t q = i + k * stride;
+            ex[k] = ld_stream(A.O.x + q); ey[k] = ld_stream(A.O.y + q);
+            et[k] = ld_stream(A.O.t + q); ep[k] = ld_stream(A.O.p + q);
+            ew[k] = __ldg(wcol + q * M);
+        }
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) one(i + k * stride, ex[k], ey[k], et[k], ep[k], ew[k]);
+    }
+    for (; i < last; i += stride)
+        one(i, ld_stream(A.O.x + i), ld_stream(A.O.y + i), ld_stream(A.O.t + i), ld_stream(A.O.p + i), __ldg(wcol + i * M));
+    // CTA reduction, one f64 atomic per component and CTA
+    __shared__ double part[kFlowObjThreads / 32][K];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        double v = u[k];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) part[wid][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        double s = 0.0;
+        for (int w = 0; w < kFlowObjThreads / 32; ++w) s += part[w][threadIdx.x];
+        atomicAdd(A.O.grad + z * K + threadIdx.x, s);
+    }
+}
+
+template <int WARP>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_assign_kernel(const MotionSegArgs A)
+{
+    __shared__ WarpModel mod[kMaxSegModels];
+    const int b = blockIdx.y, M = A.M;
+    load_seg_models<WARP>(A, b, M, mod);
+    int64_t first = A.O.offsets[b], last = A.O.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > A.O.n) last = A.O.n;
+    const int Wc = A.O.C.Wc;
+    const int64_t npix = (int64_t)A.O.C.Hc * Wc;
+    const float *Gs = A.G + (int64_t)b * M * npix;
+    unsigned oob = 0;
+    auto one = [&](int64_t i, float xe, float ye, float te) {
+        double c[kMaxSegModels], s = 0.0;
+#pragma unroll
+        for (int m = 0; m < kMaxSegModels; ++m) {
+            c[m] = 0.0;
+            if (m >= M) continue;
+            Event<WARP> e;
+            e.x = xe; e.y = ye; e.t = te; e.p = 1.0f;
+            Taps T;
+            float jx[4], jy[4];
+            if (model_taps<WARP, false>(A.O.C, e, mod[m], oob, T, jx, jy)) {
+                const float *G = Gs + m * npix;
+                const int64_t r0 = (int64_t)T.y0 * Wc, r1 = (int64_t)T.y1 * Wc;
+                const double v = (double)T.ti.x * __ldg(G + r0 + T.x0) + (double)T.ti.y * __ldg(G + r0 + T.x1) +
+                                 (double)T.ti.z * __ldg(G + r1 + T.x0) + (double)T.ti.w * __ldg(G + r1 + T.x1);
+                c[m] = v < 0.0 ? 0.0 : v;   // a NaN stays NaN
+            }
+            s += c[m];
+        }
+        const double den = s + M * A.eps;
+        float *row = A.w_out + i * M;
+#pragma unroll
+        for (int m = 0; m < kMaxSegModels; ++m)
+            if (m < M) row[m] = den == 0.0 ? 1.0f / (float)M : (float)((c[m] + A.eps) / den);
+    };
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
+        float ex[kBatch], ey[kBatch], et[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            ex[k] = ld_stream(A.O.x + i + k * stride); ey[k] = ld_stream(A.O.y + i + k * stride);
+            et[k] = ld_stream(A.O.t + i + k * stride);
+        }
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) one(i + k * stride, ex[k], ey[k], et[k]);
+    }
+    for (; i < last; i += stride) one(i, ld_stream(A.O.x + i), ld_stream(A.O.y + i), ld_stream(A.O.t + i));
+}
+
+enum { SEG_CAND, SEG_GRAD, SEG_ASSIGN };
+
+template <int WARP>
+static void launch_motion_seg_warp(int pass, const MotionSegArgs &A, dim3 grid, cudaStream_t st)
+{
+    if (pass == SEG_CAND) motion_seg_cand_kernel<WARP><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else if (pass == SEG_GRAD) motion_seg_grad_kernel<WARP><<<grid, kFlowObjThreads, 0, st>>>(A);
+    else motion_seg_assign_kernel<WARP><<<grid, kFlowObjThreads, 0, st>>>(A);
+}
+
+static void launch_motion_seg(int warp, int pass, const MotionSegArgs &A, int batch, cudaStream_t st)
+{
+    dim3 grid = flow_obj_grid(A.O.n, batch);
+    if (pass == SEG_GRAD) grid.z = A.M;
+    if (warp == EVK_WARP_LINVEL) launch_motion_seg_warp<WARP_LINVEL_F32>(pass, A, grid, st);
+    else if (warp == EVK_WARP_ROTATION) launch_motion_seg_warp<WARP_ROTATION_F32>(pass, A, grid, st);
+    else launch_motion_seg_warp<WARP_XYZTHETA_F32>(pass, A, grid, st);
+}
+
+// shared argument checks and set-up of the segmentation entries: M models per sample, J candidates per model (0: the
+// differentiable entries, batch M canvases with the backward's images; else batch M J forward-only canvases)
+static int motion_seg_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const float *weights,
+                            int n_models, const int64_t *offsets, int batch, int64_t n, int warp, const double *params, int K,
+                            double cx, double cy, int H, int W, double sigma, int objective, void *workspace,
+                            size_t workspace_bytes, MotionSegArgs &A, BatchObjWorkspace &ws, BlurTaps &taps, int n_cand = 0)
+{
+    if (n_models < 1 || n_models > kMaxSegModels) {
+        set_error("%s: bad n_models %d (1 <= n_models <= %d)", who, n_models, kMaxSegModels);
+        return EVK_E_ARG;
+    }
+    if (!n_cand && (int64_t)batch * n_models > 65535) {
+        set_error("%s: bad arguments (batch * n_models <= 65535 canvases)", who);
+        return EVK_E_ARG;
+    }
+    if (n_cand && (n_cand < 1 || n_models * n_cand > kMaxCandidates || (int64_t)batch * n_models * n_cand > 65535)) {
+        set_error("%s: bad arguments (1 <= n_cand, n_models * n_cand <= %d, batch * n_models * n_cand <= 65535)", who,
+                  kMaxCandidates);
+        return EVK_E_ARG;
+    }
+    if (n > 0 && !weights) { set_error("%s: null weights", who); return EVK_E_ARG; }
+    A = MotionSegArgs{};
+    const int rc = n_cand ? motion_obj_setup(who, x, y, t, p, offsets, batch, n, warp, params, K, cx, cy, H, W, sigma, objective,
+                                             workspace, workspace_bytes, A.O, ws, taps, true, n_models * n_cand)
+                          : motion_obj_setup(who, x, y, t, p, offsets, batch < 0 ? batch : batch * n_models, n, warp, params, K,
+                                             cx, cy, H, W, sigma, objective, workspace, workspace_bytes, A.O, ws, taps);
+    if (rc) return rc;
+    A.weights = weights;
+    A.M = n_models;
+    A.J = n_cand ? n_cand : 1;
+    A.wvec4 = n_models % 4 == 0 && ((uintptr_t)weights & 15) == 0;
+    return EVK_OK;
+}
+
 // ---- dense-flow average-timestamp (Zhu) loss over a batch of samples (evk_flow_timestamp_objective_f32 / _grad_f32) --
 // Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by flow[b] with the flow objective's warp and keep
 // rule (flow_obj_warp), then the average-timestamp images of events_to_timestamp_image_torch (image.py:286-353) on the
@@ -2977,6 +3272,151 @@ int evk_cmax_motion_candidates_f32(const float *x, const float *y, const float *
     }
     // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
     batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, ws.Wimg, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_cmax_motion_segment_workspace_bytes(int batch, int n_models, int H, int W)
+{
+    if (batch < 0 || n_models < 1 || n_models > evk::kMaxSegModels || H < 2 || W < 2) return 0;
+    return evk::batch_obj_carve(nullptr, batch * n_models, H, W, (size_t)(H + 1) * (W + 1), nullptr);
+}
+
+int evk_cmax_motion_segment_f32(const float *x, const float *y, const float *t_rel, const float *p, const float *weights,
+                                int n_models, const int64_t *offsets, int batch, int64_t n_events, int warp, const double *params,
+                                int K, double cx, double cy, int H, int W, double sigma, int objective, double obj_param,
+                                double *f_out, float *iwe_out, void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    MotionSegArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_seg_setup("evk_cmax_motion_segment_f32", x, y, t_rel, p, weights, n_models, offsets, batch, n_events, warp,
+                              params, K, cx, cy, H, W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !iwe_out)) { set_error("evk_cmax_motion_segment_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_models;
+    // nonfinite stays zero, as in evk_cmax_motion_objective_f32
+    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)canvases * npix * 4 * sizeof(float), st));
+    A.O.acc = ws.acc;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_seg(warp, SEG_CAND, A, batch, st);
+    }
+    batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, iwe_out, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_cmax_motion_segment_grad_f32(const float *x, const float *y, const float *t_rel, const float *p, const float *weights,
+                                     int n_models, const int64_t *offsets, int batch, int64_t n_events, int warp,
+                                     const double *params, int K, double cx, double cy, int H, int W, double sigma, int objective,
+                                     double obj_param, const float *iwe, const float *grad_f, double *grad_params,
+                                     float *grad_weights, void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    MotionSegArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_seg_setup("evk_cmax_motion_segment_grad_f32", x, y, t_rel, p, weights, n_models, offsets, batch, n_events,
+                              warp, params, K, cx, cy, H, W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!iwe || !grad_f || !grad_params)) { set_error("evk_cmax_motion_segment_grad_f32: null array"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_models;
+    EVK_CUDA(cudaMemsetAsync(grad_params, 0, (size_t)canvases * K * sizeof(double), st));
+    batch_obj_backward_W(ws, iwe, Hc, Wc, taps, canvases, objective, obj_param, grad_f, st);
+    if (grad_weights && objective == OBJ_VARIANCE) {
+        // the mean of every G_bm (ws.G, just recomputed) for the constant term of the variance's dF/dI
+        EVK_CUDA(cudaMemsetAsync(ws.gsums, 0, (size_t)canvases * 8 * sizeof(double), st));
+        EVK_CUDA(cudaMemsetAsync(ws.gmax, 0, (size_t)canvases * sizeof(unsigned), st));
+        prof_count(1);
+        cmax_model_stats_kernel<<<dim3((npix + 255) / 256, 1, canvases), 256, 0, st>>>(ws.G, iwe, npix, objective, obj_param, ws.gsums,
+                                                                                        ws.gmax, nullptr, nullptr);
+        A.gsums = ws.gsums;
+    }
+    A.O.Wimg = ws.Wimg;
+    A.O.grad = grad_params;
+    A.grad_f = grad_f;
+    A.grad_w = grad_weights;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_seg(warp, SEG_GRAD, A, batch, st);
+    }
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_cmax_motion_segment_candidates_workspace_bytes(int batch, int n_models, int n_cand, int H, int W)
+{
+    if (batch < 0 || n_models < 1 || n_models > evk::kMaxSegModels || n_cand < 1 || n_models * n_cand > evk::kMaxCandidates ||
+        H < 2 || W < 2)
+        return 0;
+    return evk::batch_obj_carve(nullptr, batch * n_models * n_cand, H, W, (size_t)(H + 1) * (W + 1), nullptr, false);
+}
+
+int evk_cmax_motion_segment_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p, const float *weights,
+                                           int n_models, const int64_t *offsets, int batch, int64_t n_events, int warp,
+                                           const double *cand, int n_cand, int K, double cx, double cy, int H, int W,
+                                           double blur_sigma, int objective, double obj_param, double *f_out, void *workspace,
+                                           size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    MotionSegArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = motion_seg_setup("evk_cmax_motion_segment_candidates_f32", x, y, t_rel, p, weights, n_models, offsets, batch, n_events,
+                              warp, cand, K, cx, cy, H, W, blur_sigma, objective, workspace, workspace_bytes, A, ws, taps,
+                              n_cand < 1 ? -1 : n_cand);
+    if (rc) return rc;
+    if (batch > 0 && !f_out) { set_error("evk_cmax_motion_segment_candidates_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_models * n_cand;
+    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)canvases * npix * 4 * sizeof(float), st));
+    A.O.acc = ws.acc;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_seg(warp, SEG_CAND, A, batch, st);
+    }
+    batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, ws.Wimg, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_cmax_motion_segment_assign_f32(const float *x, const float *y, const float *t_rel, int n_models, const int64_t *offsets,
+                                       int batch, int64_t n_events, int warp, const double *params, int K, double cx, double cy,
+                                       int H, int W, const float *iwe, double sigma, double eps, float *weights_out,
+                                       void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_cmax_motion_segment_assign_f32";
+    MotionSegArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    // no polarity and no weights enter the assignment: x stands in for both in the shared checks
+    int rc = motion_seg_setup(who, x, y, t_rel, x, x, n_models, offsets, batch, n_events, warp, params, K, cx, cy, H, W, sigma,
+                              OBJ_VARIANCE, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (!(eps >= 0.0) || !isfinite(eps)) { set_error("%s: eps must be finite and >= 0", who); return EVK_E_ARG; }
+    if (batch > 0 && (!iwe || (n_events > 0 && !weights_out))) { set_error("%s: null array", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    batch_obj_blur(ws, iwe, H + 1, W + 1, taps, batch * n_models, st);
+    A.G = ws.G;
+    A.eps = eps;
+    A.w_out = weights_out;
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        launch_motion_seg(warp, SEG_ASSIGN, A, batch, st);
+    }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }

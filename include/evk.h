@@ -555,6 +555,60 @@ int evk_cmax_motion_candidates_f32(const float *x, const float *y, const float *
                                    double blur_sigma, int objective, double obj_param, double *f_out,
                                    void *workspace, size_t workspace_bytes, void *stream);
 
+/* Motion segmentation by motion compensation (Stoffregen, Gallego, Drummond, Kleeman, Scaramuzza, ICCV 2019):
+ * n_models = M motion models per sample (1 <= M <= 8) and a soft membership weights[e][m] (n_events x M floats,
+ * row-major, in DEVICE memory) of every event in every model.  Samples, t_rel, warp models, keep rule, canvas,
+ * blur, objectives and argument checks are those of evk_cmax_motion_objective_f32.  Image (b, m) is the IWE of
+ * sample b's events warped by params[b][m] (params: [batch][M][K] doubles on the device), every event splatted with
+ * the f32 product p[e] * weights[e][m]: exactly the taps of evk_cmax_motion_objective_f32 run on p * weights[:, m]
+ * and params[:, m].  f[b][m] is that image's objective; at M = 1 with weights 1 the entries compute what the motion
+ * objective computes.  batch * M <= 65535 canvases.
+ *   f_out  : [batch][M] doubles;  iwe_out: [batch][M][H+1][W+1] floats, which the backward and the assignment take
+ * evk_cmax_motion_segment_grad_f32 (grad_f [batch][M] floats on the device) writes grad_params [batch][M][K] doubles,
+ * the derivative of evk_cmax_motion_objective_grad_f32 per (b, m) with the event weights p * weights[e][m], and, when
+ * grad_weights is not NULL, grad_weights [n_events][M] floats = sum_{b,m} grad_f[b][m] df[b][m] / dweights[e][m]:
+ *   p[e] sum_taps k_tap dF/dI(tap)   (k the bilinear fractions of the event under params[b][m]; 0 when it is not
+ *   kept).  The footprint comes from the unweighted taps, so an event of weight 0 (or p = 0) still has a weight
+ *   gradient.  Only the rows of events inside a sample are written (the caller zeroes the others), so that a batch
+ *   may run as several calls on chunks of its samples; samples must not overlap.
+ * evk_cmax_motion_segment_candidates_f32 scores n_cand parameter vectors per model in one pass over the events:
+ * f_out[b][m][j] is the f[b][m] of evk_cmax_motion_segment_f32 with params[b][m] = cand[b][m][j]
+ * (cand: [batch][M][n_cand][K] doubles on the device; M * n_cand <= 32, batch * M * n_cand <= 65535).
+ * evk_cmax_motion_segment_assign_f32 is the E-step: with G_bm the blurred iwe[b][m] (blur_sigma),
+ *   c[e][m] = max(0, sum_taps k_tap G_bm(tap))  (k the polarity- and weight-free bilinear fractions under
+ *   params[b][m]; 0 when the event is not kept under model m), then
+ *   weights_out[e][m] = (c[e][m] + eps) / (sum_i c[e][i] + M eps)   (eps >= 0)
+ * A row whose c are all 0 with eps = 0 is 1/M; a non-finite c makes its own row non-finite.  As for grad_weights,
+ * only the rows of events inside a sample are written (motion_segmentation_assign_torch sets the others to 1/M).
+ * workspace: evk_cmax_motion_segment_workspace_bytes(batch, M, H, W) bytes for the forward, the backward and the
+ * assignment; evk_cmax_motion_segment_candidates_workspace_bytes(batch, M, n_cand, H, W) for the candidates.  Both
+ * 256-byte aligned; the queries return 0 for arguments the entries reject.  Every argument is checked before any
+ * CUDA call; no call synchronises, and each launches the same kernels whatever the batch. */
+size_t evk_cmax_motion_segment_workspace_bytes(int batch, int n_models, int H, int W);
+int evk_cmax_motion_segment_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                const float *weights, int n_models, const int64_t *offsets, int batch,
+                                int64_t n_events, int warp, const double *params, int K, double cx, double cy,
+                                int H, int W, double blur_sigma, int objective, double obj_param, double *f_out,
+                                float *iwe_out, void *workspace, size_t workspace_bytes, void *stream);
+int evk_cmax_motion_segment_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                     const float *weights, int n_models, const int64_t *offsets, int batch,
+                                     int64_t n_events, int warp, const double *params, int K, double cx, double cy,
+                                     int H, int W, double blur_sigma, int objective, double obj_param, const float *iwe,
+                                     const float *grad_f, double *grad_params, float *grad_weights,
+                                     void *workspace, size_t workspace_bytes, void *stream);
+size_t evk_cmax_motion_segment_candidates_workspace_bytes(int batch, int n_models, int n_cand, int H, int W);
+int evk_cmax_motion_segment_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                           const float *weights, int n_models, const int64_t *offsets, int batch,
+                                           int64_t n_events, int warp, const double *cand, int n_cand, int K,
+                                           double cx, double cy, int H, int W, double blur_sigma, int objective,
+                                           double obj_param, double *f_out, void *workspace,
+                                           size_t workspace_bytes, void *stream);
+int evk_cmax_motion_segment_assign_f32(const float *x, const float *y, const float *t_rel, int n_models,
+                                       const int64_t *offsets, int batch, int64_t n_events, int warp,
+                                       const double *params, int K, double cx, double cy, int H, int W,
+                                       const float *iwe, double blur_sigma, double eps, float *weights_out,
+                                       void *workspace, size_t workspace_bytes, void *stream);
+
 /* Dense-flow average-timestamp loss (Zhu et al., CVPR'19) over a batch of samples, as a differentiable loss:
  * warp_events_flow_torch (lib/transforms/optic_flow.py:5-46), then the timestamp images of
  * events_to_timestamp_image_torch (lib/representations/image.py:286-353) on the canvas of motion_compensate
