@@ -592,12 +592,41 @@ __global__ void __launch_bounds__(256) cmax_model_batch_kernel(const CmaxArgs A,
 // f64; no reduction per event whatever K is.
 constexpr int kGradThreads = 512;
 
+// The slopes of the bilinear interpolant of four gathered values q00 (y0, x0), q01 (y0, x1), q10 (y1, x0), q11 (y1, x1)
+// at the fractions (dx, dy), in the caller's type R (f32 in the flow passes, f64 in the model passes).
+template <class R>
+__device__ __forceinline__ void tap_slopes(R ox, R oy, R dx, R dy, R q00, R q01, R q10, R q11, R &sx, R &sy)
+{
+    sx = oy * (q01 - q00) + dy * (q11 - q10);
+    sy = ox * (q10 - q00) + dx * (q11 - q01);
+}
+
+// CTA reduction of every thread's u[K] (THREADS threads): warp shuffles, the warp sums in shared memory, then one f64
+// atomic per component and CTA into dst[K]
+template <int K, int THREADS>
+__device__ __forceinline__ void cta_add(const double (&u)[K], double *dst)
+{
+    __shared__ double part[THREADS / 32][K];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        double v = u[k];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) part[wid][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        double s = 0.0;
+        for (int w = 0; w < THREADS / 32; ++w) s += part[w][threadIdx.x];
+        atomicAdd(dst + threadIdx.x, s);
+    }
+}
+
 template <int WARP>
 __global__ void __launch_bounds__(kGradThreads, 1) cmax_grad_pass_kernel(const CmaxArgs A, const float *__restrict__ W, double *U)
 {
     constexpr int K = model_dims(WARP);
     extern __shared__ __align__(16) float sW[];
-    __shared__ double part[kGradThreads / 32][K];
     const int npix = A.Hc * A.Wc;
     for (int j = threadIdx.x; j < npix; j += kGradThreads) sW[j] = W[j];
     __syncthreads();
@@ -612,8 +641,8 @@ __global__ void __launch_bounds__(kGradThreads, 1) cmax_grad_pass_kernel(const C
         const int r0 = T.y0 * A.Wc, r1 = T.y1 * A.Wc;
         const double w00 = sW[r0 + T.x0], w01 = sW[r0 + T.x1], w10 = sW[r1 + T.x0], w11 = sW[r1 + T.x1];
         const double dx = T.dx, dy = T.dy, ox = 1.0 - dx, oy = 1.0 - dy, wm = T.wm;
-        const double sx = oy * (w01 - w00) + dy * (w11 - w10);
-        const double sy = ox * (w10 - w00) + dx * (w11 - w01);
+        double sx, sy;
+        tap_slopes(ox, oy, dx, dy, w00, w01, w10, w11, sx, sy);
 #pragma unroll
         for (int k = 0; k < K; ++k) u[k] += wm * ((double)jx[k] * sx + (double)jy[k] * sy);
     };
@@ -627,20 +656,7 @@ __global__ void __launch_bounds__(kGradThreads, 1) cmax_grad_pass_kernel(const C
         for (int k = 0; k < 4; ++k) one(ev[k]);
     }
     for (; i < A.n; i += stride) one(load_event<WARP>(A, i));
-    // CTA reduction, one f64 atomic per component and CTA
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-        double v = u[k];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) part[wid][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < K) {
-        double s = 0.0;
-        for (int w = 0; w < kGradThreads / 32; ++w) s += part[w][threadIdx.x];
-        atomicAdd(U + threadIdx.x, s);
-    }
+    cta_add<K, kGradThreads>(u, U);
 }
 
 // ---- image-space tail (43.6 K pixels; negligible next to the event pass) ------------------
@@ -1531,22 +1547,146 @@ __global__ void __launch_bounds__(256) cmax_planar_kernel(const float *__restric
 //   backward: W = g_b G(C_b) per sample (C = df/dG), then per event the four taps of W (L2 gathers) give df/dx', df/dy';
 //             times d they are spread over the event's four grid_sample taps: two v4 reductions into the 2x2-block
 //             flow gradient [B][2][H][W][4] of evk_warp_flow_grad_f32.
-struct FlowObjArgs {
-    CmaxArgs C;                  // canvas (Hc, Wc) for splat_taps
+//
+// ---- what every batched event pass shares (dense flow, parametric motion, segmentation, timestamp losses) ----------
+// The event arrays the batched passes read.  Sample b is events [offsets[b], offsets[b+1]), clipped to [0, n).
+struct EventSource {
     const float *x, *y, *t, *p;  // t relative to the sample's t0
+    const float *tau;            // the timestamp losses: the normalised stamp of every event
     const int64_t *offsets;
     int64_t n;
-    const float *flow;           // [B][2][H][W]
-    int H, W;
-    float *acc;                  // forward: [B][Hc][Wc][4]; backward: [B][2][H][W][4]
-    unsigned *nonfinite;         // [B] forward: set when an event's warped position is not finite
-    const float *Wimg;           // backward: [B][Hc][Wc]
 };
+
+__device__ __forceinline__ void sample_range(const EventSource &E, int b, int64_t &first, int64_t &last)
+{
+    first = E.offsets[b];
+    last = E.offsets[b + 1];
+    if (first < 0) first = 0;
+    if (last > E.n) last = E.n;
+}
+
+// The record of one event that a pass reads, and its loaders
+struct EvXYT { float x, y, t; };
+struct EvXYTP { float x, y, t, p; };
+struct EvXYTUP { float x, y, t, tau, p; };
+struct EvXYTPW { float x, y, t, p, w; };
+
+__device__ __forceinline__ EvXYT load_xyt(const EventSource &E, int64_t i)
+{
+    return {ld_stream(E.x + i), ld_stream(E.y + i), ld_stream(E.t + i)};
+}
+__device__ __forceinline__ EvXYTP load_xytp(const EventSource &E, int64_t i)
+{
+    return {ld_stream(E.x + i), ld_stream(E.y + i), ld_stream(E.t + i), ld_stream(E.p + i)};
+}
+__device__ __forceinline__ EvXYTUP load_xytup(const EventSource &E, int64_t i)
+{
+    return {ld_stream(E.x + i), ld_stream(E.y + i), ld_stream(E.t + i), ld_stream(E.tau + i), ld_stream(E.p + i)};
+}
 
 constexpr int kFlowObjThreads = 256;
 
+// The event loop of a single-model pass over [first, last) on the (slices, batch) grid: kBatch records loaded per thread
+// before any is used (see kBatch), then body(i, record) for each; the tail one event at a time.
+template <class Load, class Body>
+__device__ __forceinline__ void for_each_event(int64_t first, int64_t last, Load load, Body body)
+{
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
+    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
+        decltype(load(i)) e[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) e[k] = load(i + k * stride);
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) body(i + k * stride, e[k]);
+    }
+    for (; i < last; i += stride) body(i, load(i));
+}
+
+// The event loop of a multi-model pass: every batch is kBatch masked loads (the records past `last` keep their default
+// value), then body(records, ne) with the ne records loaded, which runs every model over them.
+template <class Load, class Body>
+__device__ __forceinline__ void for_each_event_batch(int64_t first, int64_t last, Load load, Body body)
+{
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    for (int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x; i < last; i += kBatch * stride) {
+        decltype(load(i)) e[kBatch];
+        int ne = 0;
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int64_t q = i + k * stride;
+            if (q < last) {
+                e[k] = load(q);
+                ne = k + 1;
+            }
+        }
+        body(e, ne);
+    }
+}
+
+// Model `index` of params [..][K] into M as model_taps reads it (xyztheta also takes the fixed centre), and `count`
+// consecutive models from `first` into shared memory for the whole CTA.  M is filled in place: a model returned by value
+// costs the linvel forward pass two registers.
+template <int WARP>
+__device__ __forceinline__ void load_model(const double *params, int64_t index, double cx, double cy, WarpModel &M)
+{
+    constexpr int K = model_dims(WARP);
+    M = WarpModel{};
+#pragma unroll
+    for (int k = 0; k < K; ++k) M.m[k] = params[index * K + k];
+    if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = cx; M.m[5] = cy; }
+}
+
+template <int WARP>
+__device__ __forceinline__ void load_models(const double *params, int64_t first, int count, double cx, double cy, WarpModel *mod)
+{
+    for (int q = threadIdx.x; q < count; q += kFlowObjThreads) {
+        WarpModel M;
+        load_model<WARP>(params, first + q, cx, cy, M);
+        mod[q] = M;
+    }
+    __syncthreads();
+}
+
+// an event of the (f32) model passes, splatted with weight p
+template <int WARP>
+__device__ __forceinline__ Event<WARP> model_event(float x, float y, float t, float p)
+{
+    Event<WARP> e;
+    e.x = x; e.y = y; e.t = t; e.p = p;
+    return e;
+}
+
+// The accumulator of the timestamp losses.  Polarity image s of an event: 0 for p > 0, 1 for p <= 0, -1 for a NaN p,
+// which is in neither image (evk_tsimg.cu).
+__device__ __forceinline__ int ts_polarity(float p) { return p > 0.0f ? 0 : p <= 0.0f ? 1 : -1; }
+
+// One event's taps into the sample's [2][Hc][Wc][8]: the 32-byte block {S taps, C taps} at the footprint's anchor in image
+// s, tsimg_scatter_kernel's taps tau (1-dx)(1-dy) .. and (1-dx)(1-dy) ..
+__device__ __forceinline__ void ts_block_add(float *acc, int64_t npix, int Wc, int s, const Taps &T, float tau)
+{
+    const float dx = T.dx, dy = T.dy;
+    const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+    const float tl = __fmul_rn(tau, ox), tr = __fmul_rn(tau, dx);
+    float *blk = acc + ((s ? npix : 0) + (int64_t)T.y0 * Wc + T.x0) * 8;
+    red_add4(blk, make_float4(__fmul_rn(tl, oy), __fmul_rn(tr, oy), __fmul_rn(tl, dy), __fmul_rn(tr, dy)));
+    red_add4(blk + 4, make_float4(__fmul_rn(ox, oy), __fmul_rn(dx, oy), __fmul_rn(ox, dy), __fmul_rn(dx, dy)));
+}
+
+// ---- the dense-flow passes ----
+struct FlowArgs {
+    CmaxArgs C;            // canvas (Hc, Wc) for splat_taps
+    EventSource E;
+    const float *flow;     // [B][2][H][W]
+    int H, W;
+    float *acc;            // forward: the sample's blocks ([B][Hc][Wc][4] or [B][2][Hc][Wc][8]); backward: [B][2][H][W][4]
+    unsigned *nonfinite;   // [B] forward: set when an event's warped position is not finite
+    const float *Wimg;     // contrast backward: [B][Hc][Wc]
+    const float2 *ab;      // timestamp backward: (A, B) [B][2][Hc][Wc]
+};
+
 // The warp and the keep rule of one event of sample b; false for events that contribute nothing.
-__device__ __forceinline__ bool flow_obj_warp(const FlowObjArgs &A, const float *flow, float xe, float ye, float d, float p,
+__device__ __forceinline__ bool flow_obj_warp(const FlowArgs &A, const float *flow, float xe, float ye, float d, float p,
                                               FlowSample &s, Taps &T, bool &nonfinite)
 {
     s = flow_sample<false>(flow, nullptr, A.H, A.W, xe, ye);
@@ -1559,7 +1699,7 @@ __device__ __forceinline__ bool flow_obj_warp(const FlowObjArgs &A, const float 
 
 // The backward of the flow losses: an event's df/dflow = (gu, gv) times the weights of its four grid_sample taps, added to
 // the 2x2-block flow gradient acc [2][H][W][4] of its sample; taps outside the field get nothing.
-__device__ __forceinline__ void flow_obj_spread(const FlowObjArgs &A, float *acc, const FlowSample &s, float gu, float gv)
+__device__ __forceinline__ void flow_obj_spread(const FlowArgs &A, float *acc, const FlowSample &s, float gu, float gv)
 {
     if (!s.sampled || (gu == 0.0f && gv == 0.0f)) return;
     const int64_t plane4 = (int64_t)A.H * A.W * 4;
@@ -1582,12 +1722,12 @@ __device__ __forceinline__ void flow_obj_spread(const FlowObjArgs &A, float *acc
 }
 
 template <bool GRAD>
-__device__ __forceinline__ void flow_obj_event(const FlowObjArgs &A, const float *flow, float *acc, const float *Wb,
-                                               float xe, float ye, float d, float p, bool &nonfinite)
+__device__ __forceinline__ void flow_obj_event(const FlowArgs &A, const float *flow, float *acc, const float *Wb, const EvXYTP &e,
+                                               bool &nonfinite)
 {
     FlowSample s;
     Taps T;
-    if (!flow_obj_warp(A, flow, xe, ye, d, p, s, T, nonfinite)) return;
+    if (!flow_obj_warp(A, flow, e.x, e.y, e.t, e.p, s, T, nonfinite)) return;
     if (!GRAD) {
         red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
         return;
@@ -1596,38 +1736,24 @@ __device__ __forceinline__ void flow_obj_event(const FlowObjArgs &A, const float
     const int r0 = T.y0 * A.C.Wc, r1 = T.y1 * A.C.Wc;
     const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0), w11 = __ldg(Wb + r1 + T.x1);
     const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
-    const float sx = T.wm * (oy * (w01 - w00) + T.dy * (w11 - w10));
-    const float sy = T.wm * (ox * (w10 - w00) + T.dx * (w11 - w01));
-    flow_obj_spread(A, acc, s, sx * d, sy * d);
+    float sx, sy;
+    tap_slopes(ox, oy, T.dx, T.dy, w00, w01, w10, w11, sx, sy);
+    flow_obj_spread(A, acc, s, T.wm * sx * e.t, T.wm * sy * e.t);
 }
 
 template <bool GRAD>
-__global__ void __launch_bounds__(kFlowObjThreads) flow_obj_event_kernel(const FlowObjArgs A)
+__global__ void __launch_bounds__(kFlowObjThreads) flow_obj_event_kernel(const FlowArgs A)
 {
     const int b = blockIdx.y;
-    int64_t first = A.offsets[b], last = A.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > A.n) last = A.n;
+    int64_t first, last;
+    sample_range(A.E, b, first, last);
     const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
     const float *flow = A.flow + (int64_t)b * 2 * A.H * A.W;
     float *acc = A.acc + (GRAD ? (int64_t)b * 2 * A.H * A.W * 4 : (int64_t)b * npix * 4);
     const float *Wb = GRAD ? A.Wimg + (int64_t)b * npix : nullptr;
     bool nonfinite = false;
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
-        float ex[kBatch], ey[kBatch], et[kBatch], ep[kBatch];
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            ex[k] = ld_stream(A.x + i + k * stride); ey[k] = ld_stream(A.y + i + k * stride);
-            et[k] = ld_stream(A.t + i + k * stride); ep[k] = ld_stream(A.p + i + k * stride);
-        }
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) flow_obj_event<GRAD>(A, flow, acc, Wb, ex[k], ey[k], et[k], ep[k], nonfinite);
-    }
-    for (; i < last; i += stride)
-        flow_obj_event<GRAD>(A, flow, acc, Wb, ld_stream(A.x + i), ld_stream(A.y + i), ld_stream(A.t + i), ld_stream(A.p + i),
-                             nonfinite);
+    for_each_event(first, last, [&](int64_t i) { return load_xytp(A.E, i); },
+                   [&](int64_t, const EvXYTP &e) { flow_obj_event<GRAD>(A, flow, acc, Wb, e, nonfinite); });
     if (!GRAD && nonfinite) A.nonfinite[b] = 1u;
 }
 
@@ -1763,28 +1889,42 @@ static int batch_obj_check(const char *who, const char *wrt, int batch, int H, i
     return EVK_OK;
 }
 
-// shared argument checks and set-up of the two flow entry points
-static int flow_obj_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
-                          int batch, int64_t n, const float *flow, int H, int W, double sigma, int objective, void *workspace,
-                          size_t workspace_bytes, FlowObjArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
+// Shared argument checks and set-up of the dense-flow entries.  `images` per sample: 1 for the contrast losses, 2 for the
+// timestamp losses (one per polarity; they also need tau), so that the tail's 65535 images allow 65535 or 32767 samples.
+// acc_blocks: 16-byte accumulator blocks per image (batch_obj_carve).
+static int flow_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
+                      const int64_t *offsets, int batch, int64_t n, const float *flow, int H, int W, double sigma, int objective,
+                      int images, size_t acc_blocks, void *workspace, size_t workspace_bytes, FlowArgs &A, BatchObjWorkspace &ws,
+                      BlurTaps &taps)
 {
     if (int rc = check_sigma(who, sigma)) return rc;
-    if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
-        (n > 0 && (!x || !y || !t || !p))) {
-        set_error("%s: bad arguments (0 <= batch <= 65535, H, W >= 2)", who);
+    const int max_batch = 65535 / images;
+    if (batch < 0 || batch > max_batch || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
+        (n > 0 && (!x || !y || !t || (images == 2 && !tau) || !p))) {
+        set_error("%s: bad arguments (0 <= batch <= %d, H, W >= 2)", who, max_batch);
         return EVK_E_ARG;
     }
-    int rc = batch_obj_check(who, "flow", batch, H, W, sigma, objective, flow_obj_acc_blocks(H, W), workspace, workspace_bytes, ws, taps);
+    int rc = batch_obj_check(who, "flow", images * batch, H, W, sigma, objective, acc_blocks, workspace, workspace_bytes, ws, taps);
     if (rc) return rc;
-    A = FlowObjArgs{};
+    A = FlowArgs{};
     A.C.Hc = H + 1; A.C.Wc = W + 1;
-    A.x = x; A.y = y; A.t = t; A.p = p; A.offsets = offsets; A.n = n;
+    A.E = EventSource{x, y, t, p, tau, offsets, n};
     A.flow = flow; A.H = H; A.W = W;
+    A.acc = ws.acc;
+    A.nonfinite = ws.nonfinite;
     return EVK_OK;
 }
 
-// (slices, batch) grid of an event pass: about 2K events per CTA, at most ~8 CTAs per SM over the whole batch
-static dim3 flow_obj_grid(int64_t n, int batch)
+// Zero the counters and the accumulators of `canvases` canvases of npix pixels, `floats` floats per pixel, before a forward
+// event pass (batch_obj_carve puts them back to back)
+static cudaError_t batch_obj_zero(const BatchObjWorkspace &ws, int64_t canvases, int npix, int floats, cudaStream_t st)
+{
+    return cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)canvases * npix * floats * sizeof(float),
+                           st);
+}
+
+// (slices, batch) grid of every batched event pass: about 2K events per CTA, at most ~8 CTAs per SM over the whole batch
+static dim3 batch_grid(int64_t n, int batch)
 {
     const int64_t per = n / batch;
     int64_t slices = (per + 2047) / 2048;
@@ -1843,221 +1983,18 @@ static void batch_obj_backward_W(const BatchObjWorkspace &ws, const float *iwe, 
 //             the event's Jacobian (model_taps<..., true>), summed in f64 per thread as cmax_grad_pass_kernel does; a CTA
 //             reduction and one f64 atomic per component and CTA into grad [B][K] -- no reduction per event, and no
 //             canvas-size limit (W is not held in shared memory).
-struct MotionObjArgs {
-    CmaxArgs C;                  // canvas (Hc, Wc) and bounds mask (Hm, Wm) for model_taps; p_scale 1, t_ref 0
-    const float *x, *y, *t, *p;  // t relative to the sample's t0
-    const int64_t *offsets;
-    int64_t n;
-    const double *params;        // [B][K] on the device
-    double cx, cy;               // the centre of xyztheta
-    float *acc;                  // forward: [B][Hc][Wc][4]
-    const float *Wimg;           // backward: [B][Hc][Wc]
-    double *grad;                // backward: [B][K]
-};
-
-template <int WARP, bool GRAD>
-__global__ void __launch_bounds__(kFlowObjThreads) motion_obj_event_kernel(const MotionObjArgs A)
-{
-    constexpr int K = model_dims(WARP);
-    const int b = blockIdx.y;
-    int64_t first = A.offsets[b], last = A.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > A.n) last = A.n;
-    const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
-    WarpModel M{};
-#pragma unroll
-    for (int k = 0; k < K; ++k) M.m[k] = A.params[(int64_t)b * K + k];
-    if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = A.cx; M.m[5] = A.cy; }
-    float *acc = GRAD ? nullptr : A.acc + b * npix * 4;
-    const float *Wb = GRAD ? A.Wimg + b * npix : nullptr;
-    double u[K];
-#pragma unroll
-    for (int k = 0; k < K; ++k) u[k] = 0.0;
-    unsigned oob = 0;   // a kept finite event lies inside the canvas; a non-finite one contributes nothing
-    auto one = [&](float xe, float ye, float te, float pe) {
-        Event<WARP> e;
-        e.x = xe; e.y = ye; e.t = te; e.p = pe;
-        Taps T;
-        float jx[4], jy[4];
-        if (!model_taps<WARP, GRAD>(A.C, e, M, oob, T, jx, jy)) return;
-        if (!GRAD) {
-            red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
-            return;
-        }
-        const int64_t r0 = (int64_t)T.y0 * A.C.Wc, r1 = (int64_t)T.y1 * A.C.Wc;
-        const double w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0), w11 = __ldg(Wb + r1 + T.x1);
-        const double dx = T.dx, dy = T.dy, ox = 1.0 - dx, oy = 1.0 - dy, wm = T.wm;
-        const double sx = oy * (w01 - w00) + dy * (w11 - w10);
-        const double sy = ox * (w10 - w00) + dx * (w11 - w01);
-#pragma unroll
-        for (int k = 0; k < K; ++k) u[k] += wm * ((double)jx[k] * sx + (double)jy[k] * sy);
-    };
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
-        float ex[kBatch], ey[kBatch], et[kBatch], ep[kBatch];
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            ex[k] = ld_stream(A.x + i + k * stride); ey[k] = ld_stream(A.y + i + k * stride);
-            et[k] = ld_stream(A.t + i + k * stride); ep[k] = ld_stream(A.p + i + k * stride);
-        }
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) one(ex[k], ey[k], et[k], ep[k]);
-    }
-    for (; i < last; i += stride) one(ld_stream(A.x + i), ld_stream(A.y + i), ld_stream(A.t + i), ld_stream(A.p + i));
-    if (!GRAD) return;
-    // CTA reduction, one f64 atomic per component and CTA
-    __shared__ double part[kFlowObjThreads / 32][K];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-        double v = u[k];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) part[wid][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < K) {
-        double s = 0.0;
-        for (int w = 0; w < kFlowObjThreads / 32; ++w) s += part[w][threadIdx.x];
-        atomicAdd(A.grad + (int64_t)b * K + threadIdx.x, s);
-    }
-}
-
-static int motion_obj_dims(int warp)
-{
-    return warp == EVK_WARP_LINVEL ? 2 : warp == EVK_WARP_ROTATION ? 3 : warp == EVK_WARP_XYZTHETA ? 4 : 0;
-}
-
-// shared argument checks and set-up of the two motion entry points
-static int motion_obj_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
-                            int batch, int64_t n, int warp, const double *params, int K, double cx, double cy, int H, int W,
-                            double sigma, int objective, void *workspace, size_t workspace_bytes, MotionObjArgs &A,
-                            BatchObjWorkspace &ws, BlurTaps &taps, bool candidates = false, int n_cand = 1)
-{
-    if (int rc = check_sigma(who, sigma)) return rc;
-    if (batch < 0 || batch > 65535 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
-        (n > 0 && (!x || !y || !t || !p))) {
-        set_error("%s: bad arguments (0 <= batch <= 65535, H, W >= 2)", who);
-        return EVK_E_ARG;
-    }
-    const int dims = motion_obj_dims(warp);
-    if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
-    if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
-    // the differentiable entries: one canvas per sample; the candidates entry: one forward-only canvas per sample and
-    // candidate (the tail's grid takes at most 65535 canvases)
-    if (candidates && (n_cand < 1 || n_cand > kMaxCandidates || (int64_t)batch * n_cand > 65535)) {
-        set_error("%s: bad arguments (1 <= n_cand <= %d, batch * n_cand <= 65535)", who, kMaxCandidates);
-        return EVK_E_ARG;
-    }
-    const int canvases = candidates ? batch * n_cand : batch;
-    int rc = batch_obj_check(who, "parameters", canvases, H, W, sigma, objective, (size_t)(H + 1) * (W + 1), workspace,
-                             workspace_bytes, ws, taps, !candidates);
-    if (rc) return rc;
-    A = MotionObjArgs{};
-    A.C.Hm = H; A.C.Wm = W; A.C.Hc = H + 1; A.C.Wc = W + 1;
-    A.C.p_scale = 1.0;
-    A.x = x; A.y = y; A.t = t; A.p = p; A.offsets = offsets; A.n = n;
-    A.params = params; A.cx = cx; A.cy = cy;
-    return EVK_OK;
-}
-
-template <bool GRAD>
-static void launch_motion_obj_events(int warp, const MotionObjArgs &A, int batch, cudaStream_t st)
-{
-    const dim3 grid = flow_obj_grid(A.n, batch);
-    if (warp == EVK_WARP_LINVEL) motion_obj_event_kernel<WARP_LINVEL_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else if (warp == EVK_WARP_ROTATION) motion_obj_event_kernel<WARP_ROTATION_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else motion_obj_event_kernel<WARP_XYZTHETA_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
-}
-
-// ---- many parameter vectors per sample in one event pass (evk_cmax_motion_candidates_f32) -------------------------
-// The grid search of grid_search_initial (events_cmax.py:241-311) and the line search of a batched quasi-Newton fit score
-// n_cand parameter vectors of every sample.  On the (slices, batch) grid of the other motion passes, each CTA takes its
-// sample's n_cand x K candidates into shared memory, reads each event ONCE (16 B) and splats it through model_taps under
-// every candidate: one v4 reduction per kept event and candidate into the candidate's 2x2-block image, canvas
-// z = b n_cand + j of [batch][n_cand][Hc][Wc][4].  batch_obj_forward_tail then scores the batch x n_cand canvases exactly
-// as it scores the samples of evk_cmax_motion_objective_f32.
-struct MotionCandArgs {
-    MotionObjArgs M;   // events, samples and canvas; M.params = the candidates [B][n_cand][K]; M.acc = the canvases' blocks
-    int n_cand;
-};
-
-template <int WARP>
-__global__ void __launch_bounds__(kFlowObjThreads) motion_obj_cand_kernel(const MotionCandArgs A)
-{
-    constexpr int K = model_dims(WARP);
-    __shared__ WarpModel cand[kMaxCandidates];
-    const int b = blockIdx.y, J = A.n_cand;
-    for (int j = threadIdx.x; j < J; j += kFlowObjThreads) {
-        WarpModel M{};
-#pragma unroll
-        for (int k = 0; k < K; ++k) M.m[k] = A.M.params[((int64_t)b * J + j) * K + k];
-        if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = A.M.cx; M.m[5] = A.M.cy; }
-        cand[j] = M;
-    }
-    __syncthreads();
-    int64_t first = A.M.offsets[b], last = A.M.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > A.M.n) last = A.M.n;
-    const int Wc = A.M.C.Wc;
-    const int64_t npix = (int64_t)A.M.C.Hc * Wc;
-    float *acc = A.M.acc + (int64_t)b * J * npix * 4;
-    unsigned oob = 0;   // as in motion_obj_event_kernel: a kept finite event lies inside the canvas
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i < last; i += kBatch * stride) {
-        Event<WARP> e[kBatch];
-        int ne = 0;
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            const int64_t q = i + k * stride;
-            if (q < last) {
-                e[k].x = ld_stream(A.M.x + q); e[k].y = ld_stream(A.M.y + q);
-                e[k].t = ld_stream(A.M.t + q); e[k].p = ld_stream(A.M.p + q);
-                ne = k + 1;
-            }
-        }
-        for (int j = 0; j < J; ++j) {
-            const WarpModel M = cand[j];
-            float *accj = acc + j * npix * 4;
-#pragma unroll
-            for (int k = 0; k < kBatch; ++k) {
-                Taps T;
-                float jx[4], jy[4];
-                if (k < ne && model_taps<WARP, false>(A.M.C, e[k], M, oob, T, jx, jy))
-                    red_add4(accj + ((int64_t)T.y0 * Wc + T.x0) * 4, T.ti);
-            }
-        }
-    }
-}
-
-static void launch_motion_cand_events(int warp, const MotionCandArgs &A, int batch, cudaStream_t st)
-{
-    const dim3 grid = flow_obj_grid(A.M.n, batch);
-    if (warp == EVK_WARP_LINVEL) motion_obj_cand_kernel<WARP_LINVEL_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else if (warp == EVK_WARP_ROTATION) motion_obj_cand_kernel<WARP_ROTATION_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else motion_obj_cand_kernel<WARP_XYZTHETA_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
-}
-
-// ---- motion segmentation by motion compensation (evk_cmax_motion_segment_*) ----------------------------------------
-// Stoffregen, Gallego, Drummond, Kleeman, Scaramuzza (ICCV 2019): M motion models per sample and a soft membership
-// w[e][m] of every event in every model.  Image (b, m) is the IWE of sample b's events warped by params[b][m], each
-// event splatted with the f32 weight p_e w[e][m] through model_taps -- exactly the taps of the motion objective run on
-// p * w[:, m] -- and canvas z = b M + m (candidates: (b M + m) J + j) goes through the same image tail.
-//   forward / candidates: motion_seg_cand_kernel on the (slices, batch) grid, the sample's M x J models in shared
-//             memory; each event is read once (16 B and its row of M weights) and costs one v4 reduction per kept
-//             event and model / candidate.
-//   backward: motion_seg_grad_kernel on (slices, batch, M): per event the unweighted taps of model m (so that an event
-//             of weight 0 still has its footprint), four gathers of W_bm, the parameter gradient of
-//             motion_obj_event_kernel<.., true> with wm = p w[e][m], and optionally dF/dw[e][m] = p sum_taps k W_bm.
-//   assignment (E-step): motion_seg_assign_kernel, per event and model c = max(0, sum_taps k G_bm) with the
-//             polarity- and weight-free bilinear fractions k, then w'[e][m] = (c_m + eps) / (sum c + M eps).
-constexpr int kMaxSegModels = 8;
-
-struct MotionSegArgs {
-    MotionObjArgs O;         // events, samples, canvas; O.params [B][M][J][K]; O.acc; O.Wimg [B][M]; O.grad [B][M][K]
-    const float *weights;    // [n][M]
+struct ModelArgs {
+    CmaxArgs C;              // canvas (Hc, Wc) and bounds mask (Hm, Wm) for model_taps; p_scale 1, t_ref 0
+    EventSource E;
+    const double *params;    // [B][M][J][K] on the device (M models per sample when segmenting, J candidates per model)
+    double cx, cy;           // the centre of xyztheta
     int M, J;
+    float *acc;              // forward: the canvases' blocks
+    const float *Wimg;       // contrast backward: W of every canvas [B][M][Hc][Wc]
+    const float2 *ab;        // timestamp backward: (A, B) [B][2][Hc][Wc]
+    double *grad;            // backward: [B][M][K]
+    // segmentation
+    const float *weights;    // [n][M]
     int wvec4;               // the weight rows load as float4s (M a multiple of 4, 16-byte aligned)
     const float *grad_f;     // backward: [B][M]
     const double *gsums;     // backward with the variance: the stats of every G_bm (sum(G) in [4])
@@ -2067,7 +2004,111 @@ struct MotionSegArgs {
     float *w_out;            // assignment: [n][M]
 };
 
-__device__ __forceinline__ void load_seg_weights(const MotionSegArgs &A, int64_t i, float (&w)[kMaxSegModels])
+template <int WARP, bool GRAD>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_obj_event_kernel(const ModelArgs A)
+{
+    constexpr int K = model_dims(WARP);
+    const int b = blockIdx.y;
+    int64_t first, last;
+    sample_range(A.E, b, first, last);
+    const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
+    WarpModel M;
+    load_model<WARP>(A.params, b, A.cx, A.cy, M);
+    float *acc = GRAD ? nullptr : A.acc + b * npix * 4;
+    const float *Wb = GRAD ? A.Wimg + b * npix : nullptr;
+    double u[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) u[k] = 0.0;
+    unsigned oob = 0;   // a kept finite event lies inside the canvas; a non-finite one contributes nothing
+    for_each_event(first, last, [&](int64_t i) { return load_xytp(A.E, i); }, [&](int64_t, const EvXYTP &e) {
+        Taps T;
+        float jx[4], jy[4];
+        if (!model_taps<WARP, GRAD>(A.C, model_event<WARP>(e.x, e.y, e.t, e.p), M, oob, T, jx, jy)) return;
+        if (!GRAD) {
+            red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
+            return;
+        }
+        const int64_t r0 = (int64_t)T.y0 * A.C.Wc, r1 = (int64_t)T.y1 * A.C.Wc;
+        const double w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0), w11 = __ldg(Wb + r1 + T.x1);
+        const double dx = T.dx, dy = T.dy, ox = 1.0 - dx, oy = 1.0 - dy, wm = T.wm;
+        double sx, sy;
+        tap_slopes(ox, oy, dx, dy, w00, w01, w10, w11, sx, sy);
+#pragma unroll
+        for (int k = 0; k < K; ++k) u[k] += wm * ((double)jx[k] * sx + (double)jy[k] * sy);
+    });
+    if (GRAD) cta_add<K, kFlowObjThreads>(u, A.grad + (int64_t)b * K);
+}
+
+static int motion_obj_dims(int warp)
+{
+    return warp == EVK_WARP_LINVEL ? 2 : warp == EVK_WARP_ROTATION ? 3 : warp == EVK_WARP_XYZTHETA ? 4 : 0;
+}
+
+// Shared argument checks and set-up of the model entries.  `images` per sample: 1 for the contrast losses, 2 for the
+// timestamp losses (one per polarity; they also need tau), so that the tail's 65535 images allow 65535 or 32767 samples.
+// n_cand 0: the differentiable entries, one set of images per sample; else a forward-only set per sample and candidate.
+// acc_blocks: 16-byte accumulator blocks per image (batch_obj_carve).
+static int model_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
+                       const int64_t *offsets, int batch, int64_t n, int warp, const double *params, int K, double cx, double cy,
+                       int H, int W, double sigma, int objective, int images, size_t acc_blocks, int n_cand, void *workspace,
+                       size_t workspace_bytes, ModelArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
+{
+    if (int rc = check_sigma(who, sigma)) return rc;
+    const int max_batch = 65535 / images;
+    if (batch < 0 || batch > max_batch || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
+        (n > 0 && (!x || !y || !t || (images == 2 && !tau) || !p))) {
+        set_error("%s: bad arguments (0 <= batch <= %d, H, W >= 2)", who, max_batch);
+        return EVK_E_ARG;
+    }
+    const int dims = motion_obj_dims(warp);
+    if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
+    if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
+    if (n_cand && (n_cand < 1 || n_cand > kMaxCandidates || (int64_t)batch * n_cand > max_batch)) {
+        set_error("%s: bad arguments (1 <= n_cand <= %d, batch * n_cand <= %d)", who, kMaxCandidates, max_batch);
+        return EVK_E_ARG;
+    }
+    int rc = batch_obj_check(who, "parameters", images * batch * (n_cand ? n_cand : 1), H, W, sigma, objective, acc_blocks,
+                             workspace, workspace_bytes, ws, taps, !n_cand);
+    if (rc) return rc;
+    A = ModelArgs{};
+    A.C.Hm = H; A.C.Wm = W; A.C.Hc = H + 1; A.C.Wc = W + 1;
+    A.C.p_scale = 1.0;
+    A.E = EventSource{x, y, t, p, tau, offsets, n};
+    A.params = params; A.cx = cx; A.cy = cy;
+    A.M = 1;
+    A.J = n_cand ? n_cand : 1;
+    A.acc = ws.acc;
+    return EVK_OK;
+}
+
+// f(std::integral_constant<int, WARP>) for the f32 kernel WARP of a model warp (model_setup has checked it)
+template <class F>
+static void with_model_warp(int warp, F f)
+{
+    if (warp == EVK_WARP_LINVEL) f(std::integral_constant<int, WARP_LINVEL_F32>{});
+    else if (warp == EVK_WARP_ROTATION) f(std::integral_constant<int, WARP_ROTATION_F32>{});
+    else f(std::integral_constant<int, WARP_XYZTHETA_F32>{});
+}
+
+// ---- motion segmentation by motion compensation (evk_cmax_motion_segment_*) ----------------------------------------
+// Stoffregen, Gallego, Drummond, Kleeman, Scaramuzza (ICCV 2019): M motion models per sample and a soft membership
+// w[e][m] of every event in every model.  Image (b, m) is the IWE of sample b's events warped by params[b][m], each
+// event splatted with the f32 weight p_e w[e][m] through model_taps -- exactly the taps of the motion objective run on
+// p * w[:, m] -- and canvas z = b M + m (candidates: (b M + m) J + j) goes through the same image tail.
+//   forward / candidates: motion_seg_cand_kernel on the (slices, batch) grid, the sample's M x J models in shared
+//             memory; each event is read once (16 B and its row of M weights) and costs one v4 reduction per kept
+//             event and model / candidate.  Its unweighted instantiation (M = 1, no weight rows, splat weight p) is the
+//             event pass of evk_cmax_motion_candidates_f32: n_cand parameter vectors of every sample (the grid search of
+//             grid_search_initial, events_cmax.py:241-311, and the line search of a batched quasi-Newton fit), canvas
+//             z = b n_cand + j, scored by batch_obj_forward_tail as the samples of evk_cmax_motion_objective_f32.
+//   backward: motion_seg_grad_kernel on (slices, batch, M): per event the unweighted taps of model m (so that an event
+//             of weight 0 still has its footprint), four gathers of W_bm, the parameter gradient of
+//             motion_obj_event_kernel<.., true> with wm = p w[e][m], and optionally dF/dw[e][m] = p sum_taps k W_bm.
+//   assignment (E-step): motion_seg_assign_kernel, per event and model c = max(0, sum_taps k G_bm) with the
+//             polarity- and weight-free bilinear fractions k, then w'[e][m] = (c_m + eps) / (sum c + M eps).
+constexpr int kMaxSegModels = 8;
+
+__device__ __forceinline__ void load_seg_weights(const ModelArgs &A, int64_t i, float (&w)[kMaxSegModels])
 {
     const float *r = A.weights + i * A.M;
     if (A.wvec4) {
@@ -2083,50 +2124,32 @@ __device__ __forceinline__ void load_seg_weights(const MotionSegArgs &A, int64_t
     }
 }
 
-// sample b's models (b M + q, q < count) into shared memory
-template <int WARP>
-__device__ __forceinline__ void load_seg_models(const MotionSegArgs &A, int b, int count, WarpModel *mod)
-{
-    constexpr int K = model_dims(WARP);
-    for (int q = threadIdx.x; q < count; q += blockDim.x) {
-        WarpModel M{};
-#pragma unroll
-        for (int k = 0; k < K; ++k) M.m[k] = A.O.params[((int64_t)b * count + q) * K + k];
-        if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = A.O.cx; M.m[5] = A.O.cy; }
-        mod[q] = M;
-    }
-    __syncthreads();
-}
+// what motion_seg_cand_kernel reads of an event: x, y, t, p and, weighted, its row of M weights
+struct SegEvent {
+    EvXYTP e;
+    float w[kMaxSegModels];
+};
 
-template <int WARP>
-__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const MotionSegArgs A)
+// WEIGHTED: the segmentation's M x J models with the weight rows; else one model (M = 1) of J candidates, splat weight p
+template <int WARP, bool WEIGHTED>
+__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const ModelArgs A)
 {
     __shared__ WarpModel mod[kMaxCandidates];
-    const int b = blockIdx.y, M = A.M, J = A.J;
-    load_seg_models<WARP>(A, b, M * J, mod);
-    int64_t first = A.O.offsets[b], last = A.O.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > A.O.n) last = A.O.n;
-    const int Wc = A.O.C.Wc;
-    const int64_t npix = (int64_t)A.O.C.Hc * Wc;
-    float *acc = A.O.acc + (int64_t)b * M * J * npix * 4;
+    const int b = blockIdx.y, M = WEIGHTED ? A.M : 1, J = A.J;
+    load_models<WARP>(A.params, (int64_t)b * M * J, M * J, A.cx, A.cy, mod);
+    int64_t first, last;
+    sample_range(A.E, b, first, last);
+    const int Wc = A.C.Wc;
+    const int64_t npix = (int64_t)A.C.Hc * Wc;
+    float *acc = A.acc + (int64_t)b * M * J * npix * 4;
     unsigned oob = 0;   // as in motion_obj_event_kernel: a kept finite event lies inside the canvas
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i < last; i += kBatch * stride) {
-        Event<WARP> e[kBatch];
-        float w[kBatch][kMaxSegModels];
-        int ne = 0;
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            const int64_t q = i + k * stride;
-            if (q < last) {
-                e[k].x = ld_stream(A.O.x + q); e[k].y = ld_stream(A.O.y + q);
-                e[k].t = ld_stream(A.O.t + q); e[k].p = ld_stream(A.O.p + q);
-                load_seg_weights(A, q, w[k]);
-                ne = k + 1;
-            }
-        }
+    auto load = [&](int64_t q) {
+        SegEvent r;
+        r.e = load_xytp(A.E, q);
+        if (WEIGHTED) load_seg_weights(A, q, r.w);
+        return r;
+    };
+    for_each_event_batch(first, last, load, [&](const SegEvent (&e)[kBatch], int ne) {
 #pragma unroll
         for (int m = 0; m < kMaxSegModels; ++m) {
             if (m >= M) break;
@@ -2136,33 +2159,30 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const 
 #pragma unroll
                 for (int k = 0; k < kBatch; ++k) {
                     if (k >= ne) continue;
-                    Event<WARP> ek = e[k];
-                    ek.p = __fmul_rn(e[k].p, w[k][m]);   // the splat weight p w, formed in f32
+                    const EvXYTP &ek = e[k].e;
+                    const float p = WEIGHTED ? __fmul_rn(ek.p, e[k].w[m]) : ek.p;   // the splat weight p w, formed in f32
                     Taps T;
                     float jx[4], jy[4];
-                    if (model_taps<WARP, false>(A.O.C, ek, Mo, oob, T, jx, jy))
+                    if (model_taps<WARP, false>(A.C, model_event<WARP>(ek.x, ek.y, ek.t, p), Mo, oob, T, jx, jy))
                         red_add4(accq + ((int64_t)T.y0 * Wc + T.x0) * 4, T.ti);
                 }
             }
         }
-    }
+    });
 }
 
 template <int WARP>
-__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_grad_kernel(const MotionSegArgs A)
+__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_grad_kernel(const ModelArgs A)
 {
     constexpr int K = model_dims(WARP);
     const int b = blockIdx.y, m = blockIdx.z, M = A.M;
     const int64_t z = (int64_t)b * M + m;
-    int64_t first = A.O.offsets[b], last = A.O.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > A.O.n) last = A.O.n;
-    const int64_t npix = (int64_t)A.O.C.Hc * A.O.C.Wc;
-    WarpModel Mo{};
-#pragma unroll
-    for (int k = 0; k < K; ++k) Mo.m[k] = A.O.params[z * K + k];
-    if (!is_linvel(WARP) && !is_rotation(WARP)) { Mo.m[4] = A.O.cx; Mo.m[5] = A.O.cy; }
-    const float *Wb = A.O.Wimg + z * npix;
+    int64_t first, last;
+    sample_range(A.E, b, first, last);
+    const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
+    WarpModel Mo;
+    load_model<WARP>(A.params, z, A.cx, A.cy, Mo);
+    const float *Wb = A.Wimg + z * npix;
     // W_bm leaves out the variance's constant -2 g mean(G) / P of dF/dI (the tap differences of the parameter gradient
     // cancel it, see flow_obj_coef_kernel); the weight gradient takes it back: dF/dI = W_bm + c0
     double c0 = 0.0;
@@ -2171,87 +2191,57 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_grad_kernel(const 
 #pragma unroll
     for (int k = 0; k < K; ++k) u[k] = 0.0;
     unsigned oob = 0;
-    auto one = [&](int64_t i, float xe, float ye, float te, float pe, float we) {
-        Event<WARP> e;
-        e.x = xe; e.y = ye; e.t = te; e.p = 1.0f;   // the footprint does not depend on the weight
+    const float *wcol = A.weights + m;
+    auto load = [&](int64_t q) {
+        const EvXYTP e = load_xytp(A.E, q);
+        return EvXYTPW{e.x, e.y, e.t, e.p, __ldg(wcol + q * M)};
+    };
+    for_each_event(first, last, load, [&](int64_t i, const EvXYTPW &e) {
         Taps T;
         float jx[4], jy[4];
         double gw = 0.0;
-        if (model_taps<WARP, true>(A.O.C, e, Mo, oob, T, jx, jy)) {
-            const int64_t r0 = (int64_t)T.y0 * A.O.C.Wc, r1 = (int64_t)T.y1 * A.O.C.Wc;
+        // the footprint does not depend on the weight
+        if (model_taps<WARP, true>(A.C, model_event<WARP>(e.x, e.y, e.t, 1.0f), Mo, oob, T, jx, jy)) {
+            const int64_t r0 = (int64_t)T.y0 * A.C.Wc, r1 = (int64_t)T.y1 * A.C.Wc;
             const double w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0),
                          w11 = __ldg(Wb + r1 + T.x1);
             const double dx = T.dx, dy = T.dy, ox = 1.0 - dx, oy = 1.0 - dy;
-            const float wmf = __fmul_rn(pe, we);
+            const float wmf = __fmul_rn(e.p, e.w);
             if (wmf != 0.0f) {   // splat_taps drops a zero weight: no term, as in motion_obj_event_kernel
                 const double wm = wmf;
-                const double sx = oy * (w01 - w00) + dy * (w11 - w10);
-                const double sy = ox * (w10 - w00) + dx * (w11 - w01);
+                double sx, sy;
+                tap_slopes(ox, oy, dx, dy, w00, w01, w10, w11, sx, sy);
 #pragma unroll
                 for (int k = 0; k < K; ++k) u[k] += wm * ((double)jx[k] * sx + (double)jy[k] * sy);
             }
-            gw = (double)pe * (oy * (ox * w00 + dx * w01) + dy * (ox * w10 + dx * w11) + c0);
+            gw = (double)e.p * (oy * (ox * w00 + dx * w01) + dy * (ox * w10 + dx * w11) + c0);
         }
         if (A.grad_w) A.grad_w[i * M + m] = (float)gw;
-    };
-    const float *wcol = A.weights + m;
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
-        float ex[kBatch], ey[kBatch], et[kBatch], ep[kBatch], ew[kBatch];
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            const int64_t q = i + k * stride;
-            ex[k] = ld_stream(A.O.x + q); ey[k] = ld_stream(A.O.y + q);
-            et[k] = ld_stream(A.O.t + q); ep[k] = ld_stream(A.O.p + q);
-            ew[k] = __ldg(wcol + q * M);
-        }
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) one(i + k * stride, ex[k], ey[k], et[k], ep[k], ew[k]);
-    }
-    for (; i < last; i += stride)
-        one(i, ld_stream(A.O.x + i), ld_stream(A.O.y + i), ld_stream(A.O.t + i), ld_stream(A.O.p + i), __ldg(wcol + i * M));
-    // CTA reduction, one f64 atomic per component and CTA
-    __shared__ double part[kFlowObjThreads / 32][K];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-        double v = u[k];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) part[wid][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < K) {
-        double s = 0.0;
-        for (int w = 0; w < kFlowObjThreads / 32; ++w) s += part[w][threadIdx.x];
-        atomicAdd(A.O.grad + z * K + threadIdx.x, s);
-    }
+    });
+    cta_add<K, kFlowObjThreads>(u, A.grad + z * K);
 }
 
 template <int WARP>
-__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_assign_kernel(const MotionSegArgs A)
+__global__ void __launch_bounds__(kFlowObjThreads) motion_seg_assign_kernel(const ModelArgs A)
 {
     __shared__ WarpModel mod[kMaxSegModels];
     const int b = blockIdx.y, M = A.M;
-    load_seg_models<WARP>(A, b, M, mod);
-    int64_t first = A.O.offsets[b], last = A.O.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > A.O.n) last = A.O.n;
-    const int Wc = A.O.C.Wc;
-    const int64_t npix = (int64_t)A.O.C.Hc * Wc;
+    load_models<WARP>(A.params, (int64_t)b * M, M, A.cx, A.cy, mod);
+    int64_t first, last;
+    sample_range(A.E, b, first, last);
+    const int Wc = A.C.Wc;
+    const int64_t npix = (int64_t)A.C.Hc * Wc;
     const float *Gs = A.G + (int64_t)b * M * npix;
     unsigned oob = 0;
-    auto one = [&](int64_t i, float xe, float ye, float te) {
+    for_each_event(first, last, [&](int64_t q) { return load_xyt(A.E, q); }, [&](int64_t i, const EvXYT &e) {
         double c[kMaxSegModels], s = 0.0;
 #pragma unroll
         for (int m = 0; m < kMaxSegModels; ++m) {
             c[m] = 0.0;
             if (m >= M) continue;
-            Event<WARP> e;
-            e.x = xe; e.y = ye; e.t = te; e.p = 1.0f;
             Taps T;
             float jx[4], jy[4];
-            if (model_taps<WARP, false>(A.O.C, e, mod[m], oob, T, jx, jy)) {
+            if (model_taps<WARP, false>(A.C, model_event<WARP>(e.x, e.y, e.t, 1.0f), mod[m], oob, T, jx, jy)) {
                 const float *G = Gs + m * npix;
                 const int64_t r0 = (int64_t)T.y0 * Wc, r1 = (int64_t)T.y1 * Wc;
                 const double v = (double)T.ti.x * __ldg(G + r0 + T.x0) + (double)T.ti.y * __ldg(G + r0 + T.x1) +
@@ -2265,39 +2255,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_assign_kernel(cons
 #pragma unroll
         for (int m = 0; m < kMaxSegModels; ++m)
             if (m < M) row[m] = den == 0.0 ? 1.0f / (float)M : (float)((c[m] + A.eps) / den);
-    };
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
-        float ex[kBatch], ey[kBatch], et[kBatch];
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            ex[k] = ld_stream(A.O.x + i + k * stride); ey[k] = ld_stream(A.O.y + i + k * stride);
-            et[k] = ld_stream(A.O.t + i + k * stride);
-        }
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) one(i + k * stride, ex[k], ey[k], et[k]);
-    }
-    for (; i < last; i += stride) one(i, ld_stream(A.O.x + i), ld_stream(A.O.y + i), ld_stream(A.O.t + i));
-}
-
-enum { SEG_CAND, SEG_GRAD, SEG_ASSIGN };
-
-template <int WARP>
-static void launch_motion_seg_warp(int pass, const MotionSegArgs &A, dim3 grid, cudaStream_t st)
-{
-    if (pass == SEG_CAND) motion_seg_cand_kernel<WARP><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else if (pass == SEG_GRAD) motion_seg_grad_kernel<WARP><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else motion_seg_assign_kernel<WARP><<<grid, kFlowObjThreads, 0, st>>>(A);
-}
-
-static void launch_motion_seg(int warp, int pass, const MotionSegArgs &A, int batch, cudaStream_t st)
-{
-    dim3 grid = flow_obj_grid(A.O.n, batch);
-    if (pass == SEG_GRAD) grid.z = A.M;
-    if (warp == EVK_WARP_LINVEL) launch_motion_seg_warp<WARP_LINVEL_F32>(pass, A, grid, st);
-    else if (warp == EVK_WARP_ROTATION) launch_motion_seg_warp<WARP_ROTATION_F32>(pass, A, grid, st);
-    else launch_motion_seg_warp<WARP_XYZTHETA_F32>(pass, A, grid, st);
+    });
 }
 
 // shared argument checks and set-up of the segmentation entries: M models per sample, J candidates per model (0: the
@@ -2305,7 +2263,7 @@ static void launch_motion_seg(int warp, int pass, const MotionSegArgs &A, int ba
 static int motion_seg_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const float *weights,
                             int n_models, const int64_t *offsets, int batch, int64_t n, int warp, const double *params, int K,
                             double cx, double cy, int H, int W, double sigma, int objective, void *workspace,
-                            size_t workspace_bytes, MotionSegArgs &A, BatchObjWorkspace &ws, BlurTaps &taps, int n_cand = 0)
+                            size_t workspace_bytes, ModelArgs &A, BatchObjWorkspace &ws, BlurTaps &taps, int n_cand = 0)
 {
     if (n_models < 1 || n_models > kMaxSegModels) {
         set_error("%s: bad n_models %d (1 <= n_models <= %d)", who, n_models, kMaxSegModels);
@@ -2321,11 +2279,9 @@ static int motion_seg_setup(const char *who, const float *x, const float *y, con
         return EVK_E_ARG;
     }
     if (n > 0 && !weights) { set_error("%s: null weights", who); return EVK_E_ARG; }
-    A = MotionSegArgs{};
-    const int rc = n_cand ? motion_obj_setup(who, x, y, t, p, offsets, batch, n, warp, params, K, cx, cy, H, W, sigma, objective,
-                                             workspace, workspace_bytes, A.O, ws, taps, true, n_models * n_cand)
-                          : motion_obj_setup(who, x, y, t, p, offsets, batch < 0 ? batch : batch * n_models, n, warp, params, K,
-                                             cx, cy, H, W, sigma, objective, workspace, workspace_bytes, A.O, ws, taps);
+    const int rc = model_setup(who, x, y, t, nullptr, p, offsets, n_cand || batch < 0 ? batch : batch * n_models, n, warp, params, K,
+                               cx, cy, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), n_models * n_cand, workspace,
+                               workspace_bytes, A, ws, taps);
     if (rc) return rc;
     A.weights = weights;
     A.M = n_models;
@@ -2345,74 +2301,50 @@ static int motion_seg_setup(const char *who, const float *x, const float *y, con
 //   backward: U_s = G(2 g_b G_s) (f64 adjoint blur); (A_s, B_s) = (U_s / C_s, -U_s T_s / C_s) as f32 pairs
 //             [B][2][Hc][Wc][2]; per kept event the four pairs of its polarity give dF/dk = tau A + B per tap, then
 //             df/dx', df/dy' through the tap weights as in flow_obj_event, spread by flow_obj_spread.
-struct FlowTsArgs {
-    FlowObjArgs F;     // warp, keep rule and samples; F.acc: forward [B][2][Hc][Wc][8], backward the flow-gradient blocks
-    const float *tau;  // the normalised stamp of every event
-    const float2 *ab;  // backward: (A, B) [B][2][Hc][Wc]
-};
-
 // one 32-byte block per canvas pixel and polarity; the backward's flow-gradient blocks ([2][H][W] per sample) are fewer
 static size_t flow_ts_acc_blocks(int H, int W) { return (size_t)2 * (H + 1) * (W + 1); }
 
 template <bool GRAD>
-__device__ __forceinline__ void flow_ts_event(const FlowTsArgs &A, const float *flow, float *acc, const float2 *ab, float xe,
-                                              float ye, float d, float tau, float p, bool &nonfinite)
+__device__ __forceinline__ void flow_ts_event(const FlowArgs &A, const float *flow, float *acc, const float2 *ab, const EvXYTUP &e,
+                                              bool &nonfinite)
 {
     FlowSample s;
     Taps T;
-    if (!flow_obj_warp(A.F, flow, xe, ye, d, 1.0f, s, T, nonfinite)) return;
-    const bool pos = p > 0.0f;
-    if (!pos && !(p <= 0.0f)) return;   // NaN polarity: in neither image (evk_tsimg.cu)
-    const int Wc = A.F.C.Wc;
-    const int64_t plane = (int64_t)A.F.C.Hc * Wc;
-    const float dx = T.dx, dy = T.dy;
-    const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+    if (!flow_obj_warp(A, flow, e.x, e.y, e.t, 1.0f, s, T, nonfinite)) return;
+    const int pol = ts_polarity(e.p);
+    if (pol < 0) return;
+    const int Wc = A.C.Wc;
+    const int64_t plane = (int64_t)A.C.Hc * Wc;
     if (!GRAD) {
-        // tsimg_scatter_kernel's taps: tau (1-dx)(1-dy) .. and (1-dx)(1-dy) ..
-        const float tl = __fmul_rn(tau, ox), tr = __fmul_rn(tau, dx);
-        float *blk = acc + ((pos ? 0 : plane) + (int64_t)T.y0 * Wc + T.x0) * 8;
-        red_add4(blk, make_float4(__fmul_rn(tl, oy), __fmul_rn(tr, oy), __fmul_rn(tl, dy), __fmul_rn(tr, dy)));
-        red_add4(blk + 4, make_float4(__fmul_rn(ox, oy), __fmul_rn(dx, oy), __fmul_rn(ox, dy), __fmul_rn(dx, dy)));
+        ts_block_add(acc, plane, Wc, pol, T, e.tau);
         return;
     }
-    if (!pos) ab += plane;
+    if (pol) ab += plane;
+    const float dx = T.dx, dy = T.dy;
+    const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
     const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
     const float2 a00 = __ldg(ab + r0 + T.x0), a01 = __ldg(ab + r0 + T.x1), a10 = __ldg(ab + r1 + T.x0), a11 = __ldg(ab + r1 + T.x1);
+    const float tau = e.tau;
     const float q00 = tau * a00.x + a00.y, q01 = tau * a01.x + a01.y, q10 = tau * a10.x + a10.y, q11 = tau * a11.x + a11.y;
-    const float sx = oy * (q01 - q00) + dy * (q11 - q10);
-    const float sy = ox * (q10 - q00) + dx * (q11 - q01);
-    flow_obj_spread(A.F, acc, s, sx * d, sy * d);
+    float sx, sy;
+    tap_slopes(ox, oy, dx, dy, q00, q01, q10, q11, sx, sy);
+    flow_obj_spread(A, acc, s, sx * e.t, sy * e.t);
 }
 
 template <bool GRAD>
-__global__ void __launch_bounds__(kFlowObjThreads) flow_ts_event_kernel(const FlowTsArgs A)
+__global__ void __launch_bounds__(kFlowObjThreads) flow_ts_event_kernel(const FlowArgs A)
 {
     const int b = blockIdx.y;
-    int64_t first = A.F.offsets[b], last = A.F.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > A.F.n) last = A.F.n;
-    const int64_t npix = (int64_t)A.F.C.Hc * A.F.C.Wc;
-    const float *flow = A.F.flow + (int64_t)b * 2 * A.F.H * A.F.W;
-    float *acc = A.F.acc + (GRAD ? (int64_t)b * 2 * A.F.H * A.F.W * 4 : (int64_t)b * 2 * npix * 8);
+    int64_t first, last;
+    sample_range(A.E, b, first, last);
+    const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
+    const float *flow = A.flow + (int64_t)b * 2 * A.H * A.W;
+    float *acc = A.acc + (GRAD ? (int64_t)b * 2 * A.H * A.W * 4 : (int64_t)b * 2 * npix * 8);
     const float2 *ab = GRAD ? A.ab + (int64_t)b * 2 * npix : nullptr;
     bool nonfinite = false;
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
-        float ex[kBatch], ey[kBatch], et[kBatch], eu[kBatch], ep[kBatch];
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            ex[k] = ld_stream(A.F.x + i + k * stride); ey[k] = ld_stream(A.F.y + i + k * stride);
-            et[k] = ld_stream(A.F.t + i + k * stride); eu[k] = ld_stream(A.tau + i + k * stride);
-            ep[k] = ld_stream(A.F.p + i + k * stride);
-        }
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) flow_ts_event<GRAD>(A, flow, acc, ab, ex[k], ey[k], et[k], eu[k], ep[k], nonfinite);
-    }
-    for (; i < last; i += stride)
-        flow_ts_event<GRAD>(A, flow, acc, ab, ld_stream(A.F.x + i), ld_stream(A.F.y + i), ld_stream(A.F.t + i),
-                            ld_stream(A.tau + i), ld_stream(A.F.p + i), nonfinite);
-    if (!GRAD && nonfinite) A.F.nonfinite[b] = 1u;
+    for_each_event(first, last, [&](int64_t i) { return load_xytup(A.E, i); },
+                   [&](int64_t, const EvXYTUP &e) { flow_ts_event<GRAD>(A, flow, acc, ab, e, nonfinite); });
+    if (!GRAD && nonfinite) A.nonfinite[b] = 1u;
 }
 
 // blocks -> T and C of every image z = 2b + s (blockIdx.z), tsimg_fold_kernel's arithmetic (the count starts at one, so its
@@ -2498,28 +2430,6 @@ static const float2 *ts_obj_backward_ab(const BatchObjWorkspace &ws, const float
     return ab;
 }
 
-// shared argument checks and set-up of the two timestamp entry points (those of flow_obj_setup, for 2B images)
-static int flow_ts_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
-                         const int64_t *offsets, int batch, int64_t n, const float *flow, int H, int W, double sigma,
-                         void *workspace, size_t workspace_bytes, FlowTsArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
-{
-    if (int rc = check_sigma(who, sigma)) return rc;
-    if (batch < 0 || batch > 32767 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
-        (n > 0 && (!x || !y || !t || !tau || !p))) {
-        set_error("%s: bad arguments (0 <= batch <= 32767, H, W >= 2)", who);
-        return EVK_E_ARG;
-    }
-    int rc = batch_obj_check(who, "flow", 2 * batch, H, W, sigma, OBJ_SOS, flow_ts_acc_blocks(H, W), workspace, workspace_bytes,
-                             ws, taps);
-    if (rc) return rc;
-    A = FlowTsArgs{};
-    A.F.C.Hc = H + 1; A.F.C.Wc = W + 1;
-    A.F.x = x; A.F.y = y; A.F.t = t; A.F.p = p; A.F.offsets = offsets; A.F.n = n;
-    A.F.flow = flow; A.F.H = H; A.F.W = W;
-    A.tau = tau;
-    return EVK_OK;
-}
-
 // ---- parametric average-timestamp (Zhu) loss over a batch of samples (evk_motion_timestamp_objective_f32 / _grad_f32) --
 // Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by its own model params[b] through model_taps
 // (linvel, rotation or xyztheta, f32, as the motion contrast loss warps), with weight 1: an event contributes iff its splat
@@ -2531,92 +2441,47 @@ static int flow_ts_setup(const char *who, const float *x, const float *y, const 
 //             df/dx', df/dy' through the tap weights, contracted with the Jacobian rows of model_taps<..., true> and summed
 //             in f64 per thread; a CTA reduction and one f64 atomic per component and CTA into grad [B][K], as in
 //             motion_obj_event_kernel.
-struct MotionTsArgs {
-    MotionObjArgs M;   // warp, keep rule, samples and parameters; M.acc: forward [B][2][Hc][Wc][8]; M.grad: backward [B][K]
-    const float *tau;  // the normalised stamp of every event
-    const float2 *ab;  // backward: (A, B) [B][2][Hc][Wc]
-};
-
 template <int WARP, bool GRAD>
-__global__ void __launch_bounds__(kFlowObjThreads) motion_ts_event_kernel(const MotionTsArgs A)
+__global__ void __launch_bounds__(kFlowObjThreads) motion_ts_event_kernel(const ModelArgs A)
 {
     constexpr int K = model_dims(WARP);
     const int b = blockIdx.y;
-    int64_t first = A.M.offsets[b], last = A.M.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > A.M.n) last = A.M.n;
-    const int Wc = A.M.C.Wc;
-    const int64_t npix = (int64_t)A.M.C.Hc * Wc;
-    WarpModel M{};
-#pragma unroll
-    for (int k = 0; k < K; ++k) M.m[k] = A.M.params[(int64_t)b * K + k];
-    if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = A.M.cx; M.m[5] = A.M.cy; }
-    float *acc = GRAD ? nullptr : A.M.acc + b * 2 * npix * 8;
+    int64_t first, last;
+    sample_range(A.E, b, first, last);
+    const int Wc = A.C.Wc;
+    const int64_t npix = (int64_t)A.C.Hc * Wc;
+    WarpModel M;
+    load_model<WARP>(A.params, b, A.cx, A.cy, M);
+    float *acc = GRAD ? nullptr : A.acc + b * 2 * npix * 8;
     const float2 *ab = GRAD ? A.ab + b * 2 * npix : nullptr;
     double u[K];
 #pragma unroll
     for (int k = 0; k < K; ++k) u[k] = 0.0;
     unsigned oob = 0;   // a contributing event lies inside the canvas; a non-finite one contributes nothing
-    auto one = [&](float xe, float ye, float te, float ue, float pe) {
-        const bool pos = pe > 0.0f;
-        if (!pos && !(pe <= 0.0f)) return;   // NaN polarity: in neither image (evk_tsimg.cu)
-        Event<WARP> e;
-        e.x = xe; e.y = ye; e.t = te; e.p = 1.0f;
+    for_each_event(first, last, [&](int64_t i) { return load_xytup(A.E, i); }, [&](int64_t, const EvXYTUP &e) {
+        const int pol = ts_polarity(e.p);
+        if (pol < 0) return;
         Taps T;
         float jx[4], jy[4];
-        if (!model_taps<WARP, GRAD>(A.M.C, e, M, oob, T, jx, jy)) return;
-        const float dx = T.dx, dy = T.dy;
-        const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+        if (!model_taps<WARP, GRAD>(A.C, model_event<WARP>(e.x, e.y, e.t, 1.0f), M, oob, T, jx, jy)) return;
         if (!GRAD) {
-            // tsimg_scatter_kernel's taps: tau (1-dx)(1-dy) .. and (1-dx)(1-dy) ..
-            const float tl = __fmul_rn(ue, ox), tr = __fmul_rn(ue, dx);
-            float *blk = acc + ((pos ? 0 : npix) + (int64_t)T.y0 * Wc + T.x0) * 8;
-            red_add4(blk, make_float4(__fmul_rn(tl, oy), __fmul_rn(tr, oy), __fmul_rn(tl, dy), __fmul_rn(tr, dy)));
-            red_add4(blk + 4, make_float4(__fmul_rn(ox, oy), __fmul_rn(dx, oy), __fmul_rn(ox, dy), __fmul_rn(dx, dy)));
+            ts_block_add(acc, npix, Wc, pol, T, e.tau);
             return;
         }
-        const float2 *abs_ = pos ? ab : ab + npix;
+        const float dx = T.dx, dy = T.dy;
+        const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+        const float2 *abs_ = pol ? ab + npix : ab;
         const int64_t r0 = (int64_t)T.y0 * Wc, r1 = (int64_t)T.y1 * Wc;
         const float2 a00 = __ldg(abs_ + r0 + T.x0), a01 = __ldg(abs_ + r0 + T.x1), a10 = __ldg(abs_ + r1 + T.x0),
                      a11 = __ldg(abs_ + r1 + T.x1);
-        const double tau = ue;
+        const double tau = e.tau;
         const double q00 = tau * a00.x + a00.y, q01 = tau * a01.x + a01.y, q10 = tau * a10.x + a10.y, q11 = tau * a11.x + a11.y;
-        const double sx = (double)oy * (q01 - q00) + (double)dy * (q11 - q10);
-        const double sy = (double)ox * (q10 - q00) + (double)dx * (q11 - q01);
+        double sx, sy;
+        tap_slopes<double>(ox, oy, dx, dy, q00, q01, q10, q11, sx, sy);
 #pragma unroll
         for (int k = 0; k < K; ++k) u[k] += (double)jx[k] * sx + (double)jy[k] * sy;
-    };
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i + (kBatch - 1) * stride < last; i += kBatch * stride) {
-        float ex[kBatch], ey[kBatch], et[kBatch], eu[kBatch], ep[kBatch];
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            ex[k] = ld_stream(A.M.x + i + k * stride); ey[k] = ld_stream(A.M.y + i + k * stride);
-            et[k] = ld_stream(A.M.t + i + k * stride); eu[k] = ld_stream(A.tau + i + k * stride);
-            ep[k] = ld_stream(A.M.p + i + k * stride);
-        }
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) one(ex[k], ey[k], et[k], eu[k], ep[k]);
-    }
-    for (; i < last; i += stride)
-        one(ld_stream(A.M.x + i), ld_stream(A.M.y + i), ld_stream(A.M.t + i), ld_stream(A.tau + i), ld_stream(A.M.p + i));
-    if (!GRAD) return;
-    // CTA reduction, one f64 atomic per component and CTA
-    __shared__ double part[kFlowObjThreads / 32][K];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-        double v = u[k];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) part[wid][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < K) {
-        double s = 0.0;
-        for (int w = 0; w < kFlowObjThreads / 32; ++w) s += part[w][threadIdx.x];
-        atomicAdd(A.M.grad + (int64_t)b * K + threadIdx.x, s);
-    }
+    });
+    if (GRAD) cta_add<K, kFlowObjThreads>(u, A.grad + (int64_t)b * K);
 }
 
 // the candidates entry's workspace for `images` = 2 batch n_cand images: the forward-only carve (no f64 adjoint images;
@@ -2630,53 +2495,6 @@ static size_t motion_ts_cand_bytes(int images, int H, int W)
     return motion_ts_cand_head(images, H, W) + align_up((size_t)images * (H + 1) * (W + 1) * sizeof(float), 256);
 }
 
-// shared argument checks and set-up of the parametric timestamp entry points (those of motion_obj_setup, for 2B images;
-// with `candidates`, for 2 B n_cand forward-only images)
-static int motion_ts_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
-                           const int64_t *offsets, int batch, int64_t n, int warp, const double *params, int K, double cx,
-                           double cy, int H, int W, double sigma, void *workspace, size_t workspace_bytes, MotionTsArgs &A,
-                           BatchObjWorkspace &ws, BlurTaps &taps, bool candidates = false, int n_cand = 1)
-{
-    if (int rc = check_sigma(who, sigma)) return rc;
-    if (batch < 0 || batch > 32767 || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
-        (n > 0 && (!x || !y || !t || !tau || !p))) {
-        set_error("%s: bad arguments (0 <= batch <= 32767, H, W >= 2)", who);
-        return EVK_E_ARG;
-    }
-    const int dims = motion_obj_dims(warp);
-    if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
-    if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
-    // the tail's grid takes at most 65535 images, two per sample and candidate
-    if (candidates && (n_cand < 1 || n_cand > kMaxCandidates || (int64_t)batch * n_cand > 32767)) {
-        set_error("%s: bad arguments (1 <= n_cand <= %d, batch * n_cand <= 32767)", who, kMaxCandidates);
-        return EVK_E_ARG;
-    }
-    const int images = 2 * batch * (candidates ? n_cand : 1);
-    int rc = batch_obj_check(who, "parameters", images, H, W, sigma, OBJ_SOS, flow_ts_acc_blocks(H, W), workspace,
-                             workspace_bytes, ws, taps, !candidates);
-    if (rc) return rc;
-    if (candidates && workspace_bytes < motion_ts_cand_bytes(images, H, W)) {
-        set_error("%s: 256-byte aligned workspace of %zu bytes required", who, motion_ts_cand_bytes(images, H, W));
-        return EVK_E_WORKSPACE;
-    }
-    A = MotionTsArgs{};
-    A.M.C.Hm = H; A.M.C.Wm = W; A.M.C.Hc = H + 1; A.M.C.Wc = W + 1;
-    A.M.C.p_scale = 1.0;
-    A.M.x = x; A.M.y = y; A.M.t = t; A.M.p = p; A.M.offsets = offsets; A.M.n = n;
-    A.M.params = params; A.M.cx = cx; A.M.cy = cy;
-    A.tau = tau;
-    return EVK_OK;
-}
-
-template <bool GRAD>
-static void launch_motion_ts_events(int warp, const MotionTsArgs &A, int batch, cudaStream_t st)
-{
-    const dim3 grid = flow_obj_grid(A.M.n, batch);
-    if (warp == EVK_WARP_LINVEL) motion_ts_event_kernel<WARP_LINVEL_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else if (warp == EVK_WARP_ROTATION) motion_ts_event_kernel<WARP_ROTATION_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else motion_ts_event_kernel<WARP_XYZTHETA_F32, GRAD><<<grid, kFlowObjThreads, 0, st>>>(A);
-}
-
 // ---- many parameter vectors per sample in one event pass (evk_motion_timestamp_candidates_f32) --------------------
 // The grid search and the line search of a batched fit of the timestamp loss score n_cand parameter vectors of every
 // sample.  On the (slices, batch) grid, each CTA takes its sample's n_cand x K candidates into shared memory, reads each
@@ -2684,51 +2502,34 @@ static void launch_motion_ts_events(int warp, const MotionTsArgs &A, int batch, 
 // motion_ts_event_kernel's forward into the 32-byte {S, C} block of its polarity, image pair z = 2 (b n_cand + j) + s of
 // [batch][n_cand][2][Hc][Wc][8].  ts_obj_forward_tail then treats the batch x n_cand pairs as the samples of
 // evk_motion_timestamp_objective_f32, so f comes out in [batch][n_cand] order.
-struct MotionTsCandArgs {
-    MotionTsArgs T;    // events, stamps, samples and canvas; T.M.params = the candidates [B][n_cand][K]; T.M.acc = the blocks
-    int n_cand;
+template <int WARP>
+struct TsCandEvent {
+    Event<WARP> e;   // splat weight 1
+    float tau;
+    int pol = -1;    // ts_polarity; -1 also past the end of the sample
 };
 
 template <int WARP>
-__global__ void __launch_bounds__(kFlowObjThreads) motion_ts_cand_kernel(const MotionTsCandArgs A)
+__global__ void __launch_bounds__(kFlowObjThreads) motion_ts_cand_kernel(const ModelArgs A)
 {
-    constexpr int K = model_dims(WARP);
     __shared__ WarpModel cand[kMaxCandidates];
-    const MotionObjArgs &M0 = A.T.M;
-    const int b = blockIdx.y, J = A.n_cand;
-    for (int j = threadIdx.x; j < J; j += kFlowObjThreads) {
-        WarpModel M{};
-#pragma unroll
-        for (int k = 0; k < K; ++k) M.m[k] = M0.params[((int64_t)b * J + j) * K + k];
-        if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = M0.cx; M.m[5] = M0.cy; }
-        cand[j] = M;
-    }
-    __syncthreads();
-    int64_t first = M0.offsets[b], last = M0.offsets[b + 1];
-    if (first < 0) first = 0;
-    if (last > M0.n) last = M0.n;
-    const int Wc = M0.C.Wc;
-    const int64_t npix = (int64_t)M0.C.Hc * Wc;
-    float *acc = M0.acc + (int64_t)b * J * 2 * npix * 8;
+    const int b = blockIdx.y, J = A.J;
+    load_models<WARP>(A.params, (int64_t)b * J, J, A.cx, A.cy, cand);
+    int64_t first, last;
+    sample_range(A.E, b, first, last);
+    const int Wc = A.C.Wc;
+    const int64_t npix = (int64_t)A.C.Hc * Wc;
+    float *acc = A.acc + (int64_t)b * J * 2 * npix * 8;
     unsigned oob = 0;   // as in motion_ts_event_kernel: a contributing event lies inside the canvas
-    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
-    int64_t i = first + (int64_t)blockIdx.x * kFlowObjThreads + threadIdx.x;
-    for (; i < last; i += kBatch * stride) {
-        Event<WARP> e[kBatch];
-        float eu[kBatch];
-        int64_t plane[kBatch];   // 0 for a positive event, npix for a negative one, -1 for none (NaN polarity, past the end)
-#pragma unroll
-        for (int k = 0; k < kBatch; ++k) {
-            const int64_t q = i + k * stride;
-            plane[k] = -1;
-            if (q < last) {
-                e[k].x = ld_stream(M0.x + q); e[k].y = ld_stream(M0.y + q); e[k].t = ld_stream(M0.t + q); e[k].p = 1.0f;
-                eu[k] = ld_stream(A.T.tau + q);
-                const float pe = ld_stream(M0.p + q);
-                if (pe > 0.0f) plane[k] = 0;
-                else if (pe <= 0.0f) plane[k] = npix;   // NaN polarity: in neither image (evk_tsimg.cu)
-            }
-        }
+    auto load = [&](int64_t q) {
+        const EvXYTUP r = load_xytup(A.E, q);
+        TsCandEvent<WARP> c;
+        c.e = model_event<WARP>(r.x, r.y, r.t, 1.0f);
+        c.tau = r.tau;
+        c.pol = ts_polarity(r.p);
+        return c;
+    };
+    for_each_event_batch(first, last, load, [&](const TsCandEvent<WARP> (&e)[kBatch], int) {
         for (int j = 0; j < J; ++j) {
             const WarpModel M = cand[j];
             float *accj = acc + (int64_t)j * 2 * npix * 8;
@@ -2736,25 +2537,11 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_ts_cand_kernel(const M
             for (int k = 0; k < kBatch; ++k) {
                 Taps T;
                 float jx[4], jy[4];
-                if (plane[k] < 0 || !model_taps<WARP, false>(M0.C, e[k], M, oob, T, jx, jy)) continue;
-                const float dx = T.dx, dy = T.dy;
-                const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
-                // tsimg_scatter_kernel's taps, as motion_ts_event_kernel forms them
-                const float tl = __fmul_rn(eu[k], ox), tr = __fmul_rn(eu[k], dx);
-                float *blk = accj + (plane[k] + (int64_t)T.y0 * Wc + T.x0) * 8;
-                red_add4(blk, make_float4(__fmul_rn(tl, oy), __fmul_rn(tr, oy), __fmul_rn(tl, dy), __fmul_rn(tr, dy)));
-                red_add4(blk + 4, make_float4(__fmul_rn(ox, oy), __fmul_rn(dx, oy), __fmul_rn(ox, dy), __fmul_rn(dx, dy)));
+                if (e[k].pol < 0 || !model_taps<WARP, false>(A.C, e[k].e, M, oob, T, jx, jy)) continue;
+                ts_block_add(accj, npix, Wc, e[k].pol, T, e[k].tau);
             }
         }
-    }
-}
-
-static void launch_motion_ts_cand_events(int warp, const MotionTsCandArgs &A, int batch, cudaStream_t st)
-{
-    const dim3 grid = flow_obj_grid(A.T.M.n, batch);
-    if (warp == EVK_WARP_LINVEL) motion_ts_cand_kernel<WARP_LINVEL_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else if (warp == EVK_WARP_ROTATION) motion_ts_cand_kernel<WARP_ROTATION_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
-    else motion_ts_cand_kernel<WARP_XYZTHETA_F32><<<grid, kFlowObjThreads, 0, st>>>(A);
+    });
 }
 
 }  // namespace evk
@@ -3119,23 +2906,21 @@ int evk_cmax_flow_objective_f32(const float *x, const float *y, const float *t_r
                                 void *stream)
 {
     using namespace evk;
-    FlowObjArgs A;
+    FlowArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = flow_obj_setup("evk_cmax_flow_objective_f32", x, y, t_rel, p, offsets, batch, n_events, flow, H, W, sigma, objective,
-                            workspace, workspace_bytes, A, ws, taps);
+    int rc = flow_setup("evk_cmax_flow_objective_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, flow, H, W, sigma,
+                        objective, 1, flow_obj_acc_blocks(H, W), workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!f_out || !iwe_out)) { set_error("evk_cmax_flow_objective_f32: null output"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc;
-    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)batch * npix * 4 * sizeof(float), st));
-    A.acc = ws.acc;
-    A.nonfinite = ws.nonfinite;
+    EVK_CUDA(batch_obj_zero(ws, batch, npix, 4, st));
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        flow_obj_event_kernel<false><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        flow_obj_event_kernel<false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
     }
     batch_obj_forward_tail(ws, Hc, Wc, taps, batch, objective, obj_param, iwe_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
@@ -3148,11 +2933,11 @@ int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float
                                      size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    FlowObjArgs A;
+    FlowArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = flow_obj_setup("evk_cmax_flow_objective_grad_f32", x, y, t_rel, p, offsets, batch, n_events, flow, H, W, sigma,
-                            objective, workspace, workspace_bytes, A, ws, taps);
+    int rc = flow_setup("evk_cmax_flow_objective_grad_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, flow, H, W, sigma,
+                        objective, 1, flow_obj_acc_blocks(H, W), workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!iwe || !grad_f || !grad_flow)) { set_error("evk_cmax_flow_objective_grad_f32: null array"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
@@ -3162,12 +2947,11 @@ int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float
     EVK_CUDA(cudaMemsetAsync(ws.acc, 0, (size_t)planes * H * W * 4 * sizeof(float), st));
     // W = G(g_b C_b): recompute G from the saved IWE, the coefficient image, its blur
     batch_obj_backward_W(ws, iwe, Hc, Wc, taps, batch, objective, obj_param, grad_f, st);
-    A.acc = ws.acc;
     A.Wimg = ws.Wimg;
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        flow_obj_event_kernel<true><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        flow_obj_event_kernel<true><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
     }
     prof_count(1);
     flow_obj_grad_fold_kernel<<<grid_simple(planes * H * W, 256), 256, 0, st>>>(ws.acc, grad_flow, planes, H, W);
@@ -3187,23 +2971,24 @@ int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t
                                   void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    MotionObjArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = motion_obj_setup("evk_cmax_motion_objective_f32", x, y, t_rel, p, offsets, batch, n_events, warp, params, K, cx, cy,
-                              H, W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup("evk_cmax_motion_objective_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, warp, params, K, cx,
+                         cy, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), 0, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!f_out || !iwe_out)) { set_error("evk_cmax_motion_objective_f32: null output"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc;
     // nonfinite stays zero: a motion sample's non-finite events contribute nothing (model_taps), as in the single window
-    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)batch * npix * 4 * sizeof(float), st));
-    A.acc = ws.acc;
+    EVK_CUDA(batch_obj_zero(ws, batch, npix, 4, st));
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_obj_events<false>(warp, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_obj_event_kernel<wt.value, false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     batch_obj_forward_tail(ws, Hc, Wc, taps, batch, objective, obj_param, iwe_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
@@ -3217,11 +3002,11 @@ int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const flo
                                        void *stream)
 {
     using namespace evk;
-    MotionObjArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = motion_obj_setup("evk_cmax_motion_objective_grad_f32", x, y, t_rel, p, offsets, batch, n_events, warp, params, K, cx,
-                              cy, H, W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup("evk_cmax_motion_objective_grad_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, warp, params, K,
+                         cx, cy, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), 0, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!iwe || !grad_f || !grad_params)) { set_error("evk_cmax_motion_objective_grad_f32: null array"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
@@ -3233,7 +3018,9 @@ int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const flo
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_obj_events<true>(warp, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_obj_event_kernel<wt.value, true><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
@@ -3251,24 +3038,25 @@ int evk_cmax_motion_candidates_f32(const float *x, const float *y, const float *
                                    void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    MotionCandArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = motion_obj_setup("evk_cmax_motion_candidates_f32", x, y, t_rel, p, offsets, batch, n_events, warp, cand, K, cx, cy,
-                              H, W, blur_sigma, objective, workspace, workspace_bytes, A.M, ws, taps, true, n_cand);
+    int rc = model_setup("evk_cmax_motion_candidates_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, warp, cand, K, cx, cy,
+                         H, W, blur_sigma, objective, 1, (size_t)(H + 1) * (W + 1), n_cand < 1 ? -1 : n_cand, workspace,
+                         workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && !f_out) { set_error("evk_cmax_motion_candidates_f32: null output"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_cand;
     // nonfinite stays zero, as in evk_cmax_motion_objective_f32
-    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)canvases * npix * 4 * sizeof(float), st));
-    A.M.acc = ws.acc;
-    A.n_cand = n_cand;
+    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_cand_events(warp, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_seg_cand_kernel<wt.value, false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
     batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, ws.Wimg, f_out, st);
@@ -3288,7 +3076,7 @@ int evk_cmax_motion_segment_f32(const float *x, const float *y, const float *t_r
                                 double *f_out, float *iwe_out, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    MotionSegArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
     int rc = motion_seg_setup("evk_cmax_motion_segment_f32", x, y, t_rel, p, weights, n_models, offsets, batch, n_events, warp,
@@ -3299,12 +3087,13 @@ int evk_cmax_motion_segment_f32(const float *x, const float *y, const float *t_r
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_models;
     // nonfinite stays zero, as in evk_cmax_motion_objective_f32
-    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)canvases * npix * 4 * sizeof(float), st));
-    A.O.acc = ws.acc;
+    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_seg(warp, SEG_CAND, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_seg_cand_kernel<wt.value, true><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, iwe_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
@@ -3318,7 +3107,7 @@ int evk_cmax_motion_segment_grad_f32(const float *x, const float *y, const float
                                      float *grad_weights, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    MotionSegArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
     int rc = motion_seg_setup("evk_cmax_motion_segment_grad_f32", x, y, t_rel, p, weights, n_models, offsets, batch, n_events,
@@ -3339,14 +3128,16 @@ int evk_cmax_motion_segment_grad_f32(const float *x, const float *y, const float
                                                                                         ws.gmax, nullptr, nullptr);
         A.gsums = ws.gsums;
     }
-    A.O.Wimg = ws.Wimg;
-    A.O.grad = grad_params;
+    A.Wimg = ws.Wimg;
+    A.grad = grad_params;
     A.grad_f = grad_f;
     A.grad_w = grad_weights;
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_seg(warp, SEG_GRAD, A, batch, st);
+        dim3 grid = batch_grid(n_events, batch);
+        grid.z = n_models;
+        with_model_warp(warp, [&](auto wt) { motion_seg_grad_kernel<wt.value><<<grid, kFlowObjThreads, 0, st>>>(A); });
     }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
@@ -3367,7 +3158,7 @@ int evk_cmax_motion_segment_candidates_f32(const float *x, const float *y, const
                                            size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    MotionSegArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
     int rc = motion_seg_setup("evk_cmax_motion_segment_candidates_f32", x, y, t_rel, p, weights, n_models, offsets, batch, n_events,
@@ -3378,12 +3169,13 @@ int evk_cmax_motion_segment_candidates_f32(const float *x, const float *y, const
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_models * n_cand;
-    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)canvases * npix * 4 * sizeof(float), st));
-    A.O.acc = ws.acc;
+    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_seg(warp, SEG_CAND, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_seg_cand_kernel<wt.value, true><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, ws.Wimg, f_out, st);
     EVK_CUDA(cudaGetLastError());
@@ -3397,7 +3189,7 @@ int evk_cmax_motion_segment_assign_f32(const float *x, const float *y, const flo
 {
     using namespace evk;
     const char *who = "evk_cmax_motion_segment_assign_f32";
-    MotionSegArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
     // no polarity and no weights enter the assignment: x stands in for both in the shared checks
@@ -3415,7 +3207,9 @@ int evk_cmax_motion_segment_assign_f32(const float *x, const float *y, const flo
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_seg(warp, SEG_ASSIGN, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_seg_assign_kernel<wt.value><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
@@ -3433,23 +3227,21 @@ int evk_flow_timestamp_objective_f32(const float *x, const float *y, const float
                                      size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    FlowTsArgs A;
+    FlowArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = flow_ts_setup("evk_flow_timestamp_objective_f32", x, y, t_rel, tau, p, offsets, batch, n_events, flow, H, W, sigma,
-                           workspace, workspace_bytes, A, ws, taps);
+    int rc = flow_setup("evk_flow_timestamp_objective_f32", x, y, t_rel, tau, p, offsets, batch, n_events, flow, H, W, sigma, OBJ_SOS,
+                        2, flow_ts_acc_blocks(H, W), workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!f_out || !ts_out || !cnt_out)) { set_error("evk_flow_timestamp_objective_f32: null output"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch;
-    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)images * npix * 8 * sizeof(float), st));
-    A.F.acc = ws.acc;
-    A.F.nonfinite = ws.nonfinite;
+    EVK_CUDA(batch_obj_zero(ws, images, npix, 8, st));
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        flow_ts_event_kernel<false><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        flow_ts_event_kernel<false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
     }
     ts_obj_forward_tail(ws, Hc, Wc, taps, batch, ts_out, cnt_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
@@ -3462,11 +3254,11 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
                                           float *grad_flow, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    FlowTsArgs A;
+    FlowArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = flow_ts_setup("evk_flow_timestamp_objective_grad_f32", x, y, t_rel, tau, p, offsets, batch, n_events, flow, H, W,
-                           sigma, workspace, workspace_bytes, A, ws, taps);
+    int rc = flow_setup("evk_flow_timestamp_objective_grad_f32", x, y, t_rel, tau, p, offsets, batch, n_events, flow, H, W, sigma,
+                        OBJ_SOS, 2, flow_ts_acc_blocks(H, W), workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!ts_img || !cnt_img || !grad_f || !grad_flow)) {
         set_error("evk_flow_timestamp_objective_grad_f32: null array");
@@ -3476,12 +3268,11 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int images = 2 * batch;
     EVK_CUDA(cudaMemsetAsync(ws.acc, 0, (size_t)images * H * W * 4 * sizeof(float), st));
-    A.F.acc = ws.acc;
     A.ab = ts_obj_backward_ab(ws, ts_img, cnt_img, H + 1, W + 1, taps, batch, grad_f, st);
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        flow_ts_event_kernel<true><<<flow_obj_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        flow_ts_event_kernel<true><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
     }
     prof_count(1);
     flow_obj_grad_fold_kernel<<<grid_simple((int64_t)images * H * W, 256), 256, 0, st>>>(ws.acc, grad_flow, images, H, W);
@@ -3501,23 +3292,24 @@ int evk_motion_timestamp_objective_f32(const float *x, const float *y, const flo
                                        float *cnt_out, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    MotionTsArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = motion_ts_setup("evk_motion_timestamp_objective_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp, params,
-                             K, cx, cy, H, W, sigma, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup("evk_motion_timestamp_objective_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp, params, K, cx,
+                         cy, H, W, sigma, OBJ_SOS, 2, flow_ts_acc_blocks(H, W), 0, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!f_out || !ts_out || !cnt_out)) { set_error("evk_motion_timestamp_objective_f32: null output"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch;
     // nonfinite stays zero: a non-finite event contributes nothing (model_taps), as in the motion contrast loss
-    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)images * npix * 8 * sizeof(float), st));
-    A.M.acc = ws.acc;
+    EVK_CUDA(batch_obj_zero(ws, images, npix, 8, st));
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_ts_events<false>(warp, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_ts_event_kernel<wt.value, false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     ts_obj_forward_tail(ws, Hc, Wc, taps, batch, ts_out, cnt_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
@@ -3531,11 +3323,11 @@ int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, cons
                                             size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    MotionTsArgs A;
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = motion_ts_setup("evk_motion_timestamp_objective_grad_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp,
-                             params, K, cx, cy, H, W, sigma, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup("evk_motion_timestamp_objective_grad_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp, params, K,
+                         cx, cy, H, W, sigma, OBJ_SOS, 2, flow_ts_acc_blocks(H, W), 0, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!ts_img || !cnt_img || !grad_f || !grad_params)) {
         set_error("evk_motion_timestamp_objective_grad_f32: null array");
@@ -3545,11 +3337,13 @@ int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, cons
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     EVK_CUDA(cudaMemsetAsync(grad_params, 0, (size_t)batch * K * sizeof(double), st));
     A.ab = ts_obj_backward_ab(ws, ts_img, cnt_img, H + 1, W + 1, taps, batch, grad_f, st);
-    A.M.grad = grad_params;
+    A.grad = grad_params;
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_ts_events<true>(warp, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_ts_event_kernel<wt.value, true><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
@@ -3567,24 +3361,30 @@ int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const fl
                                         void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    MotionTsCandArgs A;
+    const char *who = "evk_motion_timestamp_candidates_f32";
+    ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = motion_ts_setup("evk_motion_timestamp_candidates_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp, cand,
-                             K, cx, cy, H, W, blur_sigma, workspace, workspace_bytes, A.T, ws, taps, true, n_cand);
+    int rc = model_setup(who, x, y, t_rel, tau, p, offsets, batch, n_events, warp, cand, K, cx, cy, H, W, blur_sigma, OBJ_SOS, 2,
+                         flow_ts_acc_blocks(H, W), n_cand < 1 ? -1 : n_cand, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
-    if (batch > 0 && !f_out) { set_error("evk_motion_timestamp_candidates_f32: null output"); return EVK_E_ARG; }
+    const int images = 2 * batch * n_cand;
+    if (workspace_bytes < motion_ts_cand_bytes(images, H, W)) {
+        set_error("%s: 256-byte aligned workspace of %zu bytes required", who, motion_ts_cand_bytes(images, H, W));
+        return EVK_E_WORKSPACE;
+    }
+    if (batch > 0 && !f_out) { set_error("%s: null output", who); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch * n_cand;
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc;
     // nonfinite stays zero, as in evk_motion_timestamp_objective_f32
-    EVK_CUDA(cudaMemsetAsync(ws.nonfinite, 0, (size_t)((char *)ws.acc - (char *)ws.nonfinite) + (size_t)images * npix * 8 * sizeof(float), st));
-    A.T.M.acc = ws.acc;
-    A.n_cand = n_cand;
+    EVK_CUDA(batch_obj_zero(ws, images, npix, 8, st));
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        launch_motion_ts_cand_events(warp, A, batch, st);
+        with_model_warp(warp, [&](auto wt) {
+            motion_ts_cand_kernel<wt.value><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
     }
     float *cnt = reinterpret_cast<float *>(static_cast<char *>(workspace) + motion_ts_cand_head(images, H, W));
     ts_obj_forward_tail(ws, Hc, Wc, taps, batch * n_cand, ws.Wimg, cnt, f_out, st);
