@@ -4,7 +4,8 @@ differentiable losses of the dense flow (`flow_objective`, and the average-times
 `flow_timestamp_objective`) and of the parametric models (`motion_objective`, and the average-timestamp
 loss of `motion_timestamp_objective`), the batched fits of one motion per window to the contrast loss
 (`motion_fit`) and to the average-timestamp loss (`motion_timestamp_fit`), and the segmentation of every
-window into several motions (`motion_segmentation`).
+window into several motions (`motion_segmentation`).  The batched losses share their event preparation, argument
+checks and loops over chunks of windows (`_batched`).
 
 Everything public in the ten modules is re-exported here, so `from event_utils_b200.contrast_max
 import linvel_warp, variance_objective, optimize_contrast` works the way the same import from the

@@ -1,0 +1,237 @@
+"""The plumbing the batched losses share (flow_objective, flow_timestamp_objective, motion_objective,
+motion_timestamp_objective, motion_fit, motion_timestamp_fit, motion_segmentation): the events of a batch as the kernels
+take them, the checks of the arguments the public functions have in common, and the two loops that run an entry over
+chunks of windows -- the candidates passes (_chunked_candidates) and a fit's forward and gradient (_chunked_objective).
+The chunk rule itself is fit_window_chunk.
+"""
+import torch
+
+from .. import _lib
+from ..representations import _events as E
+from .warps import linvel_warp, pure_rotation_warp, xyztheta_warp
+
+OBJECTIVES = {"variance": _lib.OBJ_VARIANCE, "sos": _lib.OBJ_SOS, "soe": _lib.OBJ_SOE, "sosa": _lib.OBJ_SOSA}
+DEFAULT_PARAM = {"sosa": 3.0}   # sosa_objective(p=3)
+_WARPS = ((linvel_warp, _lib.WARP_LINVEL), (pure_rotation_warp, _lib.WARP_ROTATION), (xyztheta_warp, _lib.WARP_XYZTHETA))
+MAX_CANDIDATES = 32   # parameter vectors per window and pass over the events
+
+
+def _check_objective(objective, wrt):
+    if objective not in OBJECTIVES:
+        if objective in ("moa", "isoa"):
+            raise ValueError("objective %r is piecewise constant in the %s and has no gradient; use one of %s"
+                             % (objective, wrt, sorted(OBJECTIVES)))
+        raise ValueError("unknown objective %r (one of %s)" % (objective, sorted(OBJECTIVES)))
+
+
+def _warp_code(warpfunc, who):
+    warp = next((code for cls, code in _WARPS if type(warpfunc) is cls), None)
+    if warp is None:
+        raise ValueError("%s supports the models linvel_warp, pure_rotation_warp and xyztheta_warp, got %s"
+                         % (who, type(warpfunc).__name__))
+    return warp
+
+
+def _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W):
+    """the scalar arguments the motion entries share: (warp code, (cx, cy), H, W, objective code, sigma, obj_param)"""
+    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
+    param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
+    return warp, centre, H, W, OBJECTIVES[objective], float(blur_sigma), param
+
+
+def _ts_model(warp, warpfunc, blur_sigma, H, W):
+    """the scalar arguments the motion timestamp entries share: (warp code, (cx, cy), H, W, sigma)"""
+    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
+    return warp, centre, H, W, float(blur_sigma)
+
+
+def _float_tensor(v, name):
+    v = E.as_tensor(v)
+    if not v.is_floating_point():
+        raise ValueError("%s must be a floating-point tensor, got %s" % (name, v.dtype))
+    return v
+
+
+def _params_tensor(params, warpfunc):
+    """params as a (B,K) float tensor ((K,) is one sample)"""
+    params = _float_tensor(params, "params")
+    if params.dim() == 1:
+        params = params.unsqueeze(0)
+    if params.dim() != 2 or params.shape[1] != warpfunc.dims:
+        raise ValueError("params must have shape (B,%d) or (%d,) for %s, got %s"
+                         % (warpfunc.dims, warpfunc.dims, type(warpfunc).__name__, tuple(params.shape)))
+    return params
+
+
+def _candidates_tensor(candidates, warpfunc):
+    """candidates as a (B,J,K) float tensor"""
+    cand = _float_tensor(candidates, "candidates")
+    if cand.dim() != 3 or cand.shape[2] != warpfunc.dims or cand.shape[1] < 1:
+        raise ValueError("candidates must have shape (B,J,%d) with J >= 1 for %s, got %s"
+                         % (warpfunc.dims, type(warpfunc).__name__, tuple(cand.shape)))
+    return cand
+
+
+def _window_count(batch_end_indices):
+    if batch_end_indices is None:
+        return 1
+    if isinstance(batch_end_indices, torch.Tensor):
+        return batch_end_indices.reshape(-1).shape[0]
+    return len(batch_end_indices)
+
+
+def _check_window_count(batch_end_indices, B, what):
+    """_batch_events' check of the sample count, for the functions that make it before any CUDA call"""
+    if batch_end_indices is not None and _window_count(batch_end_indices) != B:
+        raise ValueError("%d samples of events for a batch of %d %s" % (_window_count(batch_end_indices), B, what))
+
+
+def _event_tensors(xs, ys, ts, ps, t0, who, wrt):
+    """the events as flat tensors; they and t0 are data and must not require grad"""
+    xs, ys, ts, ps = (E.as_tensor(a).reshape(-1) for a in (xs, ys, ts, ps))
+    if any(a.requires_grad for a in (xs, ys, ts, ps)) or (isinstance(t0, torch.Tensor) and t0.requires_grad):
+        raise ValueError("%s differentiates with respect to %s only; the events and t0 must not require grad (detach them)"
+                         % (who, wrt))
+    n = xs.shape[0]
+    if not (ys.shape[0] == ts.shape[0] == ps.shape[0] == n):
+        raise ValueError("xs, ys, ts, ps must have the same length")
+    return xs, ys, ts, ps
+
+
+def _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what, stamps=False):
+    """The events of a batch of B samples on `dev` as the batched kernels take them: x, y, p f32, t_rel = t - t0_b
+    formed in ts' dtype then cast to f32 (t0 None: each sample's last stamp), and the B+1 int64 sample offsets.
+    With `stamps`, also the stamps on `dev` in that dtype and the sample index of every event."""
+    n = xs.shape[0]
+    with torch.cuda.device(dev):
+        if batch_end_indices is None:
+            ends = torch.full((1,), n, dtype=torch.int64, device=dev)
+        elif isinstance(batch_end_indices, torch.Tensor):
+            ends = batch_end_indices.reshape(-1).to(device=dev, dtype=torch.int64)
+        else:
+            ends = torch.tensor([int(e) for e in batch_end_indices], dtype=torch.int64).to(dev)
+        if ends.shape[0] != B:
+            raise ValueError("%d samples of events for a batch of %d %s" % (ends.shape[0], B, what))
+        offsets = torch.cat((torch.zeros(1, dtype=torch.int64, device=dev), ends))
+        x, y, p = (E.to_device(a, dev).to(torch.float32).contiguous() for a in (xs, ys, ps))
+        t = E.to_device(ts, dev)
+        rt = torch.result_type(t, 1.0)
+        t = t.to(rt)
+        if n == 0:
+            t_rel = torch.empty(0, dtype=torch.float32, device=dev)
+            sample = torch.empty(0, dtype=torch.int64, device=dev)
+        else:
+            if t0 is None:
+                t0b = t[(ends - 1).clamp(0, n - 1)]                     # each sample's last event (as warp_events_flow_torch)
+            else:
+                t0b = torch.as_tensor(t0, dtype=rt).to(dev).reshape(-1).expand(B)
+            # the sample of each event: windows are contiguous, [ends[b-1], ends[b])
+            sample = torch.searchsorted(ends, torch.arange(n, device=dev), right=True).clamp_(max=B - 1)
+            t_rel = (t - t0b.to(rt)[sample]).to(torch.float32).contiguous()
+    if stamps:
+        return x, y, t_rel, p, offsets, t, sample
+    return x, y, t_rel, p, offsets
+
+
+def _normalised_stamps(t, sample, offsets, reverse):
+    """tau of every event as f32: (t - t_first_b) / (t_last_b - t_first_b + 1e-6) of its sample b, or
+    (-t + t_last_b) / (...) (image.py:324-327), in t's dtype, as device tensor ops (no host read-back).  t: the stamps
+    in a float dtype, sample: each event's sample index, offsets: the B+1 sample offsets."""
+    n = t.shape[0]
+    if n == 0:
+        return torch.empty(0, dtype=torch.float32, device=t.device)
+    t_first = t[offsets[:-1].clamp(0, n - 1)]
+    t_last = t[(offsets[1:] - 1).clamp(0, n - 1)]
+    den = ((t_last - t_first) + 1e-6)[sample]
+    num = (-t + t_last[sample]) if reverse else (t - t_first[sample])
+    return (num / den).to(torch.float32).contiguous()
+
+
+def _timestamp_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what, reverse):
+    """_batch_events for the average-timestamp losses: x, y, t_rel, tau (_normalised_stamps), p, offsets"""
+    x, y, t_rel, p, offsets, t, sample = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what, stamps=True)
+    with torch.cuda.device(dev):
+        tau = _normalised_stamps(t, sample, offsets, reverse)
+    return x, y, t_rel, tau, p, offsets
+
+
+def fit_window_chunk(B, per_window_bytes, budget, cap):
+    """Windows per call of a fit's forward and gradient entries: at most `cap` (the entries' batch limit) and at most
+    as many as fit `budget` bytes of workspace and images, but at least one"""
+    return max(1, min(B, budget // per_window_bytes, cap))
+
+
+def _pointers(tensors):
+    return tuple(_lib.ptr(a) for a in tensors)
+
+
+def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget, cap, M=None):
+    """f (B,J) f64 of the prepared device events under the device candidates c64 (B,J,K) f64 through the entry
+    `stem`_f32, in passes of at most MAX_CANDIDATES candidate images per window over chunks of windows whose workspace
+    (`stem`_workspace_bytes) fits `budget` and whose images number at most `cap`.  `events` are the arrays in front of
+    the offsets and `scalars` the arguments behind W.  With M, the entry scores M models per window: the last of
+    `events` is the memberships, c64 is (B,M,J,K) and f (B,M,J)."""
+    warp, (cx, cy), H, W = model
+    J, K = c64.shape[-2:]
+    B = c64.shape[0]
+    ms = () if M is None else (M,)
+    L = _lib.lib()
+    entry, workspace_bytes = getattr(L, stem + "_f32"), getattr(L, stem + "_workspace_bytes")
+    dev = events[0].device
+    f = torch.empty(c64.shape[:-1], dtype=torch.float64, device=dev)
+    if B == 0:
+        return f
+    jc = min(J, MAX_CANDIDATES // (M or 1))
+    wb = fit_window_chunk(B, workspace_bytes(1, *ms, jc, H, W), budget, cap // ((M or 1) * jc))
+    ws = _lib.scratch(key, workspace_bytes(wb, *ms, jc, H, W), dev)
+    front = _pointers(events) + ms
+    for b0 in range(0, B, wb):
+        b1 = min(B, b0 + wb)
+        for j0 in range(0, J, jc):
+            j1 = min(J, j0 + jc)
+            c = c64[b0:b1, ..., j0:j1, :].contiguous()
+            out = torch.empty(c.shape[:-1], dtype=torch.float64, device=dev)
+            _lib.check(entry(*front, _lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], warp, _lib.ptr(c), j1 - j0, K,
+                             cx, cy, H, W, *scalars, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream()))
+            f[b0:b1, ..., j0:j1] = out
+    return f
+
+
+def _chunked_objective(stem, key, events, offsets, model, scalars, images, budget, cap, M=None, gradient=True):
+    """fg: (B,K) f64 params -> (f (B,) f64, g (B,K) f64) of the prepared device events through the entries `stem`_f32 /
+    `stem`_grad_f32 (grad_f = 1), in chunks of at most `cap` windows whose workspace (`stem`_workspace_bytes) and images
+    fit `budget` (fit_window_chunk); the windows are independent, so a chunk changes no value's arithmetic.  `events`
+    are the arrays in front of the offsets, `scalars` the arguments behind W and `images` the canvases per window of
+    each image the forward hands to the gradient.  With M, the entries score M models per window: the last of `events`
+    is the memberships (they get no gradient), params is (B*M,K), f (B*M,) and g (B*M,K).  Without `gradient`, g is
+    None and the gradient entry is not called."""
+    warp, (cx, cy), H, W = model
+    ms, no_weight_gradient = ((), ()) if M is None else ((M,), (None,))
+    rows = M or 1
+    L = _lib.lib()
+    forward, grad, workspace_bytes = (getattr(L, stem + s) for s in ("_f32", "_grad_f32", "_workspace_bytes"))
+    dev = events[0].device
+    front = _pointers(events) + ms
+
+    def fg(params):
+        K = params.shape[1]
+        B = params.shape[0] // rows
+        prm = params.contiguous()
+        f = torch.empty(B * rows, dtype=torch.float64, device=dev)
+        g = torch.empty((B * rows, K), dtype=torch.float64, device=dev) if gradient else None
+        wb = fit_window_chunk(B, workspace_bytes(1, *ms, H, W) + 4 * sum(images) * (H + 1) * (W + 1), budget, cap)
+        kept = [torch.empty((wb * c, H + 1, W + 1), dtype=torch.float32, device=dev) for c in images]
+        imgs = _pointers(kept)
+        ones = torch.ones(wb * rows, dtype=torch.float32, device=dev)
+        ws = _lib.scratch(key, workspace_bytes(wb, *ms, H, W), dev)
+        for b0 in range(0, B, wb):
+            b1 = min(B, b0 + wb)
+            r0, r1 = b0 * rows, b1 * rows
+            ev = front + (_lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], warp, _lib.ptr(prm[r0:r1]), K, cx, cy, H, W,
+                          *scalars)
+            _lib.check(forward(*ev, _lib.ptr(f[r0:r1]), *imgs, _lib.ptr(ws), ws.numel(), _lib.stream()))
+            if gradient:
+                _lib.check(grad(*ev, *imgs, _lib.ptr(ones), _lib.ptr(g[r0:r1]), *no_weight_gradient, _lib.ptr(ws),
+                                ws.numel(), _lib.stream()))
+        return f, g
+    return fg

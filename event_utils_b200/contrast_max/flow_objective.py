@@ -6,13 +6,9 @@ reference's motion_compensate does (lib/visualization/draw_flow.py:15-26) and sc
 lib/contrast_max/objectives.py.  One call evaluates a whole batch on the GPU (evk_cmax_flow_objective_f32) and its
 backward gives the exact gradient of the returned f with respect to the flow (evk_cmax_flow_objective_grad_f32).
 """
-import torch
-
 from .. import _lib
 from ..representations import _events as E
-
-OBJECTIVES = {"variance": _lib.OBJ_VARIANCE, "sos": _lib.OBJ_SOS, "soe": _lib.OBJ_SOE, "sosa": _lib.OBJ_SOSA}
-DEFAULT_PARAM = {"sosa": 3.0}   # sosa_objective(p=3)
+from ._batched import DEFAULT_PARAM, OBJECTIVES, _batch_events, _check_objective, _event_tensors
 
 
 def flow_contrast_objective_torch(xs, ys, ts, ps, flow, t0=None, objective="variance", blur_sigma=1.0, obj_param=None,
@@ -59,58 +55,3 @@ def _flow_batch(flow):
     if flow.dim() != 4 or flow.shape[1] != 2:
         raise ValueError("flow must have shape (B,2,H,W) or (2,H,W), got %s" % (tuple(flow.shape),))
     return flow
-
-
-def _check_objective(objective, wrt):
-    if objective not in OBJECTIVES:
-        if objective in ("moa", "isoa"):
-            raise ValueError("objective %r is piecewise constant in the %s and has no gradient; use one of %s"
-                             % (objective, wrt, sorted(OBJECTIVES)))
-        raise ValueError("unknown objective %r (one of %s)" % (objective, sorted(OBJECTIVES)))
-
-
-def _event_tensors(xs, ys, ts, ps, t0, who, wrt):
-    """the events as flat tensors; they and t0 are data and must not require grad"""
-    xs, ys, ts, ps = (E.as_tensor(a).reshape(-1) for a in (xs, ys, ts, ps))
-    if any(a.requires_grad for a in (xs, ys, ts, ps)) or (isinstance(t0, torch.Tensor) and t0.requires_grad):
-        raise ValueError("%s differentiates with respect to %s only; the events and t0 must not require grad (detach them)"
-                         % (who, wrt))
-    n = xs.shape[0]
-    if not (ys.shape[0] == ts.shape[0] == ps.shape[0] == n):
-        raise ValueError("xs, ys, ts, ps must have the same length")
-    return xs, ys, ts, ps
-
-
-def _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, what, stamps=False):
-    """The events of a batch of B samples on `dev` as the batched kernels take them: x, y, p f32, t_rel = t - t0_b
-    formed in ts' dtype then cast to f32 (t0 None: each sample's last stamp), and the B+1 int64 sample offsets.
-    With `stamps`, also the stamps on `dev` in that dtype and the sample index of every event."""
-    n = xs.shape[0]
-    with torch.cuda.device(dev):
-        if batch_end_indices is None:
-            ends = torch.full((1,), n, dtype=torch.int64, device=dev)
-        elif isinstance(batch_end_indices, torch.Tensor):
-            ends = batch_end_indices.reshape(-1).to(device=dev, dtype=torch.int64)
-        else:
-            ends = torch.tensor([int(e) for e in batch_end_indices], dtype=torch.int64).to(dev)
-        if ends.shape[0] != B:
-            raise ValueError("%d samples of events for a batch of %d %s" % (ends.shape[0], B, what))
-        offsets = torch.cat((torch.zeros(1, dtype=torch.int64, device=dev), ends))
-        x, y, p = (E.to_device(a, dev).to(torch.float32).contiguous() for a in (xs, ys, ps))
-        t = E.to_device(ts, dev)
-        rt = torch.result_type(t, 1.0)
-        t = t.to(rt)
-        if n == 0:
-            t_rel = torch.empty(0, dtype=torch.float32, device=dev)
-            sample = torch.empty(0, dtype=torch.int64, device=dev)
-        else:
-            if t0 is None:
-                t0b = t[(ends - 1).clamp(0, n - 1)]                     # each sample's last event (as warp_events_flow_torch)
-            else:
-                t0b = torch.as_tensor(t0, dtype=rt).to(dev).reshape(-1).expand(B)
-            # the sample of each event: windows are contiguous, [ends[b-1], ends[b])
-            sample = torch.searchsorted(ends, torch.arange(n, device=dev), right=True).clamp_(max=B - 1)
-            t_rel = (t - t0b.to(rt)[sample]).to(torch.float32).contiguous()
-    if stamps:
-        return x, y, t_rel, p, offsets, t, sample
-    return x, y, t_rel, p, offsets

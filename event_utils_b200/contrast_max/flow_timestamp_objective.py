@@ -7,11 +7,11 @@ and sum their squares (zhu_timestamp_objective, lib/contrast_max/objectives.py:5
 batch on the GPU (evk_flow_timestamp_objective_f32) and its backward gives the exact gradient with respect to the flow
 (evk_flow_timestamp_objective_grad_f32).
 """
-import torch
-
 from .. import _lib
 from ..representations import _events as E
-from .flow_objective import _batch_events, _event_tensors, _flow_batch
+from ._batched import _normalised_stamps  # noqa: F401  (reached under this module's name as well)
+from ._batched import _check_window_count, _event_tensors, _timestamp_events
+from .flow_objective import _flow_batch
 
 
 def flow_timestamp_objective_torch(xs, ys, ts, ps, flow, t0=None, blur_sigma=2.0, timestamp_reverse=False,
@@ -48,30 +48,11 @@ def flow_timestamp_objective_torch(xs, ys, ts, ps, flow, t0=None, blur_sigma=2.0
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "flow_timestamp_objective_torch", "the flow")
     flow = _flow_batch(flow)
     B, H, W = flow.shape[0], flow.shape[2], flow.shape[3]
-    if batch_end_indices is not None:
-        n_samples = (batch_end_indices.reshape(-1).shape[0] if isinstance(batch_end_indices, torch.Tensor)
-                     else len(batch_end_indices))
-        if n_samples != B:
-            raise ValueError("%d samples of events for a batch of %d flows" % (n_samples, B))
+    _check_window_count(batch_end_indices, B, "flows")
     _lib.lib()
     dev = E.compute_device(flow, xs, ys, ts, ps)
-    x, y, t_rel, p, offsets, t, sample = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "flows", stamps=True)
-    with torch.cuda.device(dev):
-        tau = _normalised_stamps(t, sample, offsets, timestamp_reverse)
+    x, y, t_rel, tau, p, offsets = _timestamp_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "flows", timestamp_reverse)
     from ..autograd import FlowTimestampObjective
     f = FlowTimestampObjective.apply(flow, x, y, t_rel, tau, p, offsets, float(blur_sigma))
     return f.to(device=flow.device, dtype=flow.dtype)
 
-
-def _normalised_stamps(t, sample, offsets, reverse):
-    """tau of every event as f32: (t - t_first_b) / (t_last_b - t_first_b + 1e-6) of its sample b, or
-    (-t + t_last_b) / (...) (image.py:324-327), in t's dtype, as device tensor ops (no host read-back).  t: the stamps
-    in a float dtype, sample: each event's sample index, offsets: the B+1 sample offsets."""
-    n = t.shape[0]
-    if n == 0:
-        return torch.empty(0, dtype=torch.float32, device=t.device)
-    t_first = t[offsets[:-1].clamp(0, n - 1)]
-    t_last = t[(offsets[1:] - 1).clamp(0, n - 1)]
-    den = ((t_last - t_first) + 1e-6)[sample]
-    num = (-t + t_last[sample]) if reverse else (t - t_first[sample])
-    return (num / den).to(torch.float32).contiguous()

@@ -15,8 +15,9 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from .flow_objective import _batch_events, _check_objective, _event_tensors
-from .motion_objective import _candidates, _model, _warp_code
+from ._batched import fit_window_chunk  # noqa: F401  (a public name of this module)
+from ._batched import _batch_events, _check_objective, _chunked_objective, _event_tensors, _model, _warp_code, _window_count
+from .motion_objective import _candidates
 
 MotionFit = collections.namedtuple("MotionFit", "params f status iterations")
 MotionFit.__doc__ = """motion_contrast_fit_torch's result: params (B,K) f64, f (B,) f64, status (B,) int8, iterations (B,) int32"""
@@ -91,11 +92,15 @@ def _fit_arguments(who, blur_sigma, line_search_steps, x0, param_ranges):
     sigmas = [float(s) for s in (blur_sigma if isinstance(blur_sigma, (list, tuple)) else [blur_sigma])]
     if not sigmas:
         raise ValueError("blur_sigma must be a number or a non-empty sequence")
-    if not 1 <= int(line_search_steps) <= 32:
-        raise ValueError("line_search_steps must be in 1..32, got %r" % (line_search_steps,))
+    _check_line_search_steps(line_search_steps)
     if x0 is None and param_ranges is None:
         raise ValueError("%s needs x0 or param_ranges" % who)
     return sigmas
+
+
+def _check_line_search_steps(line_search_steps):
+    if not 1 <= int(line_search_steps) <= 32:
+        raise ValueError("line_search_steps must be in 1..32, got %r" % (line_search_steps,))
 
 
 def _fit_stages(stage, sigmas, B, K, dev, x0, param_ranges, num_samples_per_param, grid_levels, log_scale, param_scale,
@@ -131,14 +136,6 @@ def _fit_stages(stage, sigmas, B, K, dev, x0, param_ranges, num_samples_per_para
     return MotionFit(xk, f, status, iters)
 
 
-def _window_count(batch_end_indices):
-    if batch_end_indices is None:
-        return 1
-    if isinstance(batch_end_indices, torch.Tensor):
-        return batch_end_indices.reshape(-1).shape[0]
-    return len(batch_end_indices)
-
-
 def _per_window(v, B, shape, name, dev):
     """v of `shape` or (B,)+shape as a (B,)+shape f64 tensor on dev (a host value is copied without a host wait)"""
     t = v if isinstance(v, torch.Tensor) else torch.from_numpy(np.array(v, dtype=np.float64))
@@ -163,12 +160,6 @@ def _to_device(t, dev):
     return t.to(dev)
 
 
-def fit_window_chunk(B, per_window_bytes, budget, cap):
-    """Windows per call of a fit's forward and gradient entries: at most `cap` (the entries' batch limit) and at most
-    as many as fit `budget` bytes of workspace and images, but at least one"""
-    return max(1, min(B, budget // per_window_bytes, cap))
-
-
 # One forward + gradient call of motion_contrast_fit_torch takes at most this many windows (the entries' batch limit)
 # and at most as many as fit FIT_WORKSPACE_BYTES of workspace and images; larger batches run in chunks of windows.
 FIT_MAX_WINDOWS = 65535
@@ -178,30 +169,9 @@ FIT_WORKSPACE_BYTES = 4 << 30
 def _objective_and_gradient(x, y, t_rel, p, offsets, opts):
     """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_cmax_motion_objective_f32 / _grad_f32 (grad_f = 1), in
     chunks of windows (fit_window_chunk); the windows are independent, so a chunk changes no value's arithmetic"""
-    warp, (cx, cy), H, W, objective, sigma, param = opts
-    L = _lib.lib()
-    dev = x.device
-
-    def fg(params):
-        B, K = params.shape
-        prm = params.contiguous()
-        f = torch.empty(B, dtype=torch.float64, device=dev)
-        g = torch.empty((B, K), dtype=torch.float64, device=dev)
-        per_window = L.evk_cmax_motion_objective_workspace_bytes(1, H, W) + 4 * (H + 1) * (W + 1)
-        wb = fit_window_chunk(B, per_window, FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS)
-        iwe = torch.empty((wb, H + 1, W + 1), dtype=torch.float32, device=dev)
-        ones = torch.ones(wb, dtype=torch.float32, device=dev)
-        ws = _lib.scratch("motion_objective", L.evk_cmax_motion_objective_workspace_bytes(wb, H, W), dev)
-        for b0 in range(0, B, wb):
-            b1 = min(B, b0 + wb)
-            ev = (_lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(offsets[b0:]), b1 - b0, x.shape[0], warp,
-                  _lib.ptr(prm[b0:b1]), K, cx, cy, H, W, sigma, objective, param)
-            _lib.check(L.evk_cmax_motion_objective_f32(*ev, _lib.ptr(f[b0:b1]), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(),
-                                                       _lib.stream()))
-            _lib.check(L.evk_cmax_motion_objective_grad_f32(*ev, _lib.ptr(iwe), _lib.ptr(ones), _lib.ptr(g[b0:b1]),
-                                                            _lib.ptr(ws), ws.numel(), _lib.stream()))
-        return f, g
-    return fg
+    warp, centre, H, W, objective, sigma, param = opts
+    return _chunked_objective("evk_cmax_motion_objective", "motion_objective", (x, y, t_rel, p), offsets, (warp, centre, H, W),
+                              (sigma, objective, param), (1,), FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS)
 
 
 def _grid_axes(ranges, num_samples_per_param, log_scale):

@@ -11,10 +11,9 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from .flow_objective import DEFAULT_PARAM, OBJECTIVES, _batch_events, _check_objective, _event_tensors
-from .warps import linvel_warp, pure_rotation_warp, xyztheta_warp
-
-_WARPS = ((linvel_warp, _lib.WARP_LINVEL), (pure_rotation_warp, _lib.WARP_ROTATION), (xyztheta_warp, _lib.WARP_XYZTHETA))
+from ._batched import MAX_CANDIDATES  # noqa: F401  (a public name of this module)
+from ._batched import (_batch_events, _candidates_tensor, _check_objective, _chunked_candidates, _event_tensors, _model,
+                       _params_tensor, _warp_code)
 
 
 def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, objective="variance", blur_sigma=1.0,
@@ -54,31 +53,20 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
     warp = _warp_code(warpfunc, "motion_contrast_objective_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_contrast_objective_torch", "params")
-    params = E.as_tensor(params)
-    if not params.is_floating_point():
-        raise ValueError("params must be a floating-point tensor, got %s" % params.dtype)
-    if params.dim() == 1:
-        params = params.unsqueeze(0)
-    if params.dim() != 2 or params.shape[1] != warpfunc.dims:
-        raise ValueError("params must have shape (B,%d) or (%d,) for %s, got %s"
-                         % (warpfunc.dims, warpfunc.dims, type(warpfunc).__name__, tuple(params.shape)))
+    params = _params_tensor(params, warpfunc)
     B = params.shape[0]
     H, W = int(img_size[0]), int(img_size[1])
     _lib.lib()
     dev = E.compute_device(params, xs, ys, ts, ps)
     x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "parameter vectors")
     from ..autograd import MotionObjective
-    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
-    param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
-    f = MotionObjective.apply(params, x, y, t_rel, p, offsets,
-                              (warp, centre, H, W, OBJECTIVES[objective], float(blur_sigma), param))
+    f = MotionObjective.apply(params, x, y, t_rel, p, offsets, _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W))
     return f.to(device=params.device, dtype=params.dtype)
 
 
 # The workspace of one evk_cmax_motion_candidates_f32 call stays below this many bytes: larger batches of windows run in
 # chunks (28 bytes per canvas pixel and candidate: 4 GiB hold 109 windows x 32 candidates at 180x240).
 CANDIDATES_WORKSPACE_BYTES = 4 << 30
-MAX_CANDIDATES = 32   # parameter vectors per window and pass over the events
 
 
 def motion_contrast_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=None, objective="variance", blur_sigma=1.0,
@@ -97,12 +85,7 @@ def motion_contrast_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=No
     warp = _warp_code(warpfunc, "motion_contrast_candidates_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_contrast_candidates_torch", "nothing")
-    cand = E.as_tensor(candidates)
-    if not cand.is_floating_point():
-        raise ValueError("candidates must be a floating-point tensor, got %s" % cand.dtype)
-    if cand.dim() != 3 or cand.shape[2] != warpfunc.dims or cand.shape[1] < 1:
-        raise ValueError("candidates must have shape (B,J,%d) with J >= 1 for %s, got %s"
-                         % (warpfunc.dims, type(warpfunc).__name__, tuple(cand.shape)))
+    cand = _candidates_tensor(candidates, warpfunc)
     B = cand.shape[0]
     H, W = int(img_size[0]), int(img_size[1])
     _lib.lib()
@@ -114,44 +97,9 @@ def motion_contrast_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=No
     return f.to(cand.device)
 
 
-def _warp_code(warpfunc, who):
-    warp = next((code for cls, code in _WARPS if type(warpfunc) is cls), None)
-    if warp is None:
-        raise ValueError("%s supports the models linvel_warp, pure_rotation_warp and xyztheta_warp, got %s"
-                         % (who, type(warpfunc).__name__))
-    return warp
-
-
-def _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W):
-    """the scalar arguments the motion entries share: (warp code, (cx, cy), H, W, objective code, sigma, obj_param)"""
-    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
-    param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
-    return warp, centre, H, W, OBJECTIVES[objective], float(blur_sigma), param
-
-
 def _candidates(x, y, t_rel, p, offsets, c64, opts):
     """f (B,J) f64 of the prepared device events under the device candidates c64 (B,J,K) f64, in passes of at most
     MAX_CANDIDATES candidates over chunks of windows whose workspace fits CANDIDATES_WORKSPACE_BYTES"""
-    warp, (cx, cy), H, W, objective, sigma, param = opts
-    B, J, K = c64.shape
-    L = _lib.lib()
-    dev = x.device
-    f = torch.empty((B, J), dtype=torch.float64, device=dev)
-    if B == 0:
-        return f
-    jc = min(J, MAX_CANDIDATES)
-    per_window = L.evk_cmax_motion_candidates_workspace_bytes(1, jc, H, W)
-    wb = max(1, min(B, CANDIDATES_WORKSPACE_BYTES // per_window, 65535 // jc))
-    ws = _lib.scratch("motion_candidates", L.evk_cmax_motion_candidates_workspace_bytes(wb, jc, H, W), dev)
-    for b0 in range(0, B, wb):
-        b1 = min(B, b0 + wb)
-        for j0 in range(0, J, MAX_CANDIDATES):
-            j1 = min(J, j0 + MAX_CANDIDATES)
-            c = c64[b0:b1, j0:j1].contiguous()
-            out = torch.empty((b1 - b0, j1 - j0), dtype=torch.float64, device=dev)
-            _lib.check(L.evk_cmax_motion_candidates_f32(
-                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(offsets[b0:]), b1 - b0, x.shape[0], warp,
-                _lib.ptr(c), j1 - j0, K, cx, cy, H, W, sigma, objective, param, _lib.ptr(out), _lib.ptr(ws), ws.numel(),
-                _lib.stream()))
-            f[b0:b1, j0:j1] = out
-    return f
+    warp, centre, H, W, objective, sigma, param = opts
+    return _chunked_candidates("evk_cmax_motion_candidates", "motion_candidates", (x, y, t_rel, p), offsets, c64,
+                               (warp, centre, H, W), (sigma, objective, param), CANDIDATES_WORKSPACE_BYTES, 65535)

@@ -17,9 +17,9 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from .flow_objective import _batch_events, _check_objective, _event_tensors
-from .motion_fit import (FIT_WORKSPACE_BYTES, _batched_bfgs, _per_window, _window_count, fit_window_chunk)
-from .motion_objective import _model, _warp_code
+from ._batched import (_batch_events, _check_objective, _chunked_candidates, _chunked_objective, _event_tensors,
+                       _float_tensor, _model, _warp_code, _window_count, fit_window_chunk)
+from .motion_fit import FIT_WORKSPACE_BYTES, _batched_bfgs, _check_line_search_steps, _per_window
 
 MAX_MODELS = 8            # motion models per window
 MAX_CANVASES = 65535      # images per call of an entry (the image tail's grid limit)
@@ -82,9 +82,7 @@ def motion_segmentation_candidates_torch(xs, ys, ts, ps, candidates, weights, wa
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_segmentation_candidates_torch", "nothing")
     weights = _weights_tensor(weights, xs.shape[0])
     M = weights.shape[1]
-    cand = E.as_tensor(candidates)
-    if not cand.is_floating_point():
-        raise ValueError("candidates must be a floating-point tensor, got %s" % cand.dtype)
+    cand = _float_tensor(candidates, "candidates")
     if cand.dim() != 4 or cand.shape[1] != M or cand.shape[2] < 1 or cand.shape[3] != warpfunc.dims:
         raise ValueError("candidates must have shape (B,%d,J,%d) with J >= 1 for %d models of %s, got %s"
                          % (M, warpfunc.dims, M, type(warpfunc).__name__, tuple(cand.shape)))
@@ -119,9 +117,7 @@ def motion_segmentation_assign_torch(xs, ys, ts, ps, params, warpfunc, weights, 
     weights = _weights_tensor(weights, xs.shape[0])
     M = weights.shape[1]
     params = _models_tensor(params, "params", M, warpfunc, batch_end_indices)
-    eps = float(eps)
-    if not eps >= 0.0 or eps == float("inf"):
-        raise ValueError("eps must be finite and >= 0, got %r" % (eps,))
+    eps = _check_eps(eps)
     B = params.shape[0]
     H, W = int(img_size[0]), int(img_size[1])
     _lib.lib()
@@ -160,11 +156,8 @@ def motion_segmentation_fit_torch(xs, ys, ts, ps, warpfunc, x0, batch_end_indice
     warp = _warp_code(warpfunc, "motion_segmentation_fit_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_segmentation_fit_torch", "nothing")
-    if not 1 <= int(line_search_steps) <= 32:
-        raise ValueError("line_search_steps must be in 1..32, got %r" % (line_search_steps,))
-    eps = float(eps)
-    if not eps >= 0.0 or eps == float("inf"):
-        raise ValueError("eps must be finite and >= 0, got %r" % (eps,))
+    _check_line_search_steps(line_search_steps)
+    eps = _check_eps(eps)
     K = warpfunc.dims
     B = _window_count(batch_end_indices)
     x0 = E.as_tensor(x0)
@@ -203,10 +196,15 @@ def motion_segmentation_fit_torch(xs, ys, ts, ps, warpfunc, x0, batch_end_indice
     return MotionSegmentation(xk.reshape(B, M, K), w, f.reshape(B, M), status.reshape(B, M), iters.reshape(B, M))
 
 
+def _check_eps(eps):
+    eps = float(eps)
+    if not eps >= 0.0 or eps == float("inf"):
+        raise ValueError("eps must be finite and >= 0, got %r" % (eps,))
+    return eps
+
+
 def _weights_tensor(weights, n):
-    weights = E.as_tensor(weights)
-    if not weights.is_floating_point():
-        raise ValueError("weights must be a floating-point tensor, got %s" % weights.dtype)
+    weights = _float_tensor(weights, "weights")
     if weights.dim() != 2 or weights.shape[0] != n or not 1 <= weights.shape[1] <= MAX_MODELS:
         raise ValueError("weights must have shape (N,M) with N = %d events and 1 <= M <= %d, got %s"
                          % (n, MAX_MODELS, tuple(weights.shape)))
@@ -215,9 +213,7 @@ def _weights_tensor(weights, n):
 
 def _models_tensor(params, name, M, warpfunc, batch_end_indices):
     """params as a (B,M,K) tensor ((M,K) is every window's)"""
-    params = E.as_tensor(params)
-    if not params.is_floating_point():
-        raise ValueError("%s must be a floating-point tensor, got %s" % (name, params.dtype))
+    params = _float_tensor(params, name)
     K = warpfunc.dims
     if params.dim() == 2 and tuple(params.shape) == (M, K):
         params = params.unsqueeze(0).expand(_window_count(batch_end_indices), M, K)
@@ -234,29 +230,10 @@ def _device_weights(weights, dev):
 def _segment_candidates(x, y, t_rel, p, w, offsets, c64, opts):
     """f (B,M,J) f64 of the prepared device events and memberships under the device candidates c64 (B,M,J,K) f64, in
     passes of at most 32 // M candidates over chunks of windows"""
-    warp, (cx, cy), H, W, objective, sigma, param = opts
-    B, M, J, K = c64.shape
-    L = _lib.lib()
-    dev = x.device
-    f = torch.empty((B, M, J), dtype=torch.float64, device=dev)
-    if B == 0:
-        return f
-    jc = min(J, 32 // M)
-    per_window = L.evk_cmax_motion_segment_candidates_workspace_bytes(1, M, jc, H, W)
-    wb = fit_window_chunk(B, per_window, SEGMENT_CANDIDATES_WORKSPACE_BYTES, MAX_CANVASES // (M * jc))
-    ws = _lib.scratch("motion_segment_candidates", L.evk_cmax_motion_segment_candidates_workspace_bytes(wb, M, jc, H, W), dev)
-    for b0 in range(0, B, wb):
-        b1 = min(B, b0 + wb)
-        for j0 in range(0, J, jc):
-            j1 = min(J, j0 + jc)
-            c = c64[b0:b1, :, j0:j1].contiguous()
-            out = torch.empty((b1 - b0, M, j1 - j0), dtype=torch.float64, device=dev)
-            _lib.check(L.evk_cmax_motion_segment_candidates_f32(
-                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(w), M, _lib.ptr(offsets[b0:]), b1 - b0,
-                x.shape[0], warp, _lib.ptr(c), j1 - j0, K, cx, cy, H, W, sigma, objective, param, _lib.ptr(out),
-                _lib.ptr(ws), ws.numel(), _lib.stream()))
-            f[b0:b1, :, j0:j1] = out
-    return f
+    warp, centre, H, W, objective, sigma, param = opts
+    return _chunked_candidates("evk_cmax_motion_segment_candidates", "motion_segment_candidates", (x, y, t_rel, p, w), offsets,
+                               c64, (warp, centre, H, W), (sigma, objective, param), SEGMENT_CANDIDATES_WORKSPACE_BYTES,
+                               MAX_CANVASES, M=c64.shape[1])
 
 
 def _segment_chunk(B, M, H, W):
@@ -269,31 +246,9 @@ def _segment_chunk(B, M, H, W):
 def _segment_objective_and_gradient(x, y, t_rel, p, w, offsets, M, opts, gradient=True):
     """(B*M,K) f64 params -> (f (B*M,) f64, g (B*M,K) f64) at the held memberships w, through
     evk_cmax_motion_segment_f32 / _grad_f32 (grad_f = 1) in chunks of windows (no weight gradient)"""
-    warp, (cx, cy), H, W, objective, sigma, param = opts
-    L = _lib.lib()
-    dev = x.device
-
-    def fg(params):
-        BM, K = params.shape
-        B = BM // M
-        prm = params.contiguous()
-        f = torch.empty(BM, dtype=torch.float64, device=dev)
-        g = torch.empty((BM, K), dtype=torch.float64, device=dev) if gradient else None
-        wb = _segment_chunk(B, M, H, W)
-        iwe = torch.empty((wb * M, H + 1, W + 1), dtype=torch.float32, device=dev)
-        ones = torch.ones(wb * M, dtype=torch.float32, device=dev)
-        ws = _lib.scratch("motion_segment", L.evk_cmax_motion_segment_workspace_bytes(wb, M, H, W), dev)
-        for b0 in range(0, B, wb):
-            b1 = min(B, b0 + wb)
-            ev = (_lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(p), _lib.ptr(w), M, _lib.ptr(offsets[b0:]), b1 - b0,
-                  x.shape[0], warp, _lib.ptr(prm[b0 * M:b1 * M]), K, cx, cy, H, W, sigma, objective, param)
-            _lib.check(L.evk_cmax_motion_segment_f32(*ev, _lib.ptr(f[b0 * M:b1 * M]), _lib.ptr(iwe), _lib.ptr(ws), ws.numel(),
-                                                     _lib.stream()))
-            if gradient:
-                _lib.check(L.evk_cmax_motion_segment_grad_f32(*ev, _lib.ptr(iwe), _lib.ptr(ones), _lib.ptr(g[b0 * M:b1 * M]),
-                                                              None, _lib.ptr(ws), ws.numel(), _lib.stream()))
-        return f, g
-    return fg
+    warp, centre, H, W, objective, sigma, param = opts
+    return _chunked_objective("evk_cmax_motion_segment", "motion_segment", (x, y, t_rel, p, w), offsets, (warp, centre, H, W),
+                              (sigma, objective, param), (M,), FIT_WORKSPACE_BYTES, MAX_CANVASES // M, M=M, gradient=gradient)
 
 
 def _assign(x, y, t_rel, p, w, offsets, p64, opts, eps):

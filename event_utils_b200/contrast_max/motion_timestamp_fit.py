@@ -10,11 +10,9 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from .flow_objective import _batch_events, _event_tensors
-from .flow_timestamp_objective import _normalised_stamps
-from .motion_fit import FIT_WORKSPACE_BYTES, _check_per_window, _fit_arguments, _fit_stages, _window_count, fit_window_chunk
-from .motion_objective import _warp_code
-from .motion_timestamp_objective import _ts_candidates, _ts_model
+from ._batched import _chunked_objective, _event_tensors, _timestamp_events, _ts_model, _warp_code, _window_count
+from .motion_fit import FIT_WORKSPACE_BYTES, _check_per_window, _fit_arguments, _fit_stages
+from .motion_timestamp_objective import _ts_candidates
 
 # One forward + gradient call of motion_timestamp_fit_torch takes at most this many windows (the entries' batch limit:
 # two tail images per window) and at most as many as fit motion_fit.FIT_WORKSPACE_BYTES
@@ -63,9 +61,8 @@ def motion_timestamp_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None,
     H, W = int(img_size[0]), int(img_size[1])
     _lib.lib()
     dev = E.compute_device(*(a for a in (x0, param_ranges, bounds, xs, ys, ts, ps) if isinstance(a, torch.Tensor)))
-    x, y, t_rel, p, offsets, t, sample = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows", stamps=True)
+    x, y, t_rel, tau, p, offsets = _timestamp_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows", timestamp_reverse)
     with torch.cuda.device(dev):
-        tau = _normalised_stamps(t, sample, offsets, timestamp_reverse)
 
         def stage(sigma):
             opts = _ts_model(warp, warpfunc, sigma, H, W)
@@ -80,28 +77,6 @@ def _objective_and_gradient(x, y, t_rel, tau, p, offsets, opts):
     """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_motion_timestamp_objective_f32 / _grad_f32 (grad_f = 1),
     in chunks of at most TIMESTAMP_FIT_MAX_WINDOWS windows whose workspace and images fit FIT_WORKSPACE_BYTES; the windows
     are independent, so a chunk changes no value's arithmetic"""
-    warp, (cx, cy), H, W, sigma = opts
-    L = _lib.lib()
-    dev = x.device
-
-    def fg(params):
-        B, K = params.shape
-        prm = params.contiguous()
-        f = torch.empty(B, dtype=torch.float64, device=dev)
-        g = torch.empty((B, K), dtype=torch.float64, device=dev)
-        per_window = L.evk_motion_timestamp_objective_workspace_bytes(1, H, W) + 16 * (H + 1) * (W + 1)
-        wb = fit_window_chunk(B, per_window, FIT_WORKSPACE_BYTES, TIMESTAMP_FIT_MAX_WINDOWS)
-        T = torch.empty((wb, 2, H + 1, W + 1), dtype=torch.float32, device=dev)
-        C = torch.empty_like(T)
-        ones = torch.ones(wb, dtype=torch.float32, device=dev)
-        ws = _lib.scratch("motion_timestamp_objective", L.evk_motion_timestamp_objective_workspace_bytes(wb, H, W), dev)
-        for b0 in range(0, B, wb):
-            b1 = min(B, b0 + wb)
-            ev = (_lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets[b0:]), b1 - b0,
-                  x.shape[0], warp, _lib.ptr(prm[b0:b1]), K, cx, cy, H, W, sigma)
-            _lib.check(L.evk_motion_timestamp_objective_f32(*ev, _lib.ptr(f[b0:b1]), _lib.ptr(T), _lib.ptr(C), _lib.ptr(ws),
-                                                            ws.numel(), _lib.stream()))
-            _lib.check(L.evk_motion_timestamp_objective_grad_f32(*ev, _lib.ptr(T), _lib.ptr(C), _lib.ptr(ones),
-                                                                 _lib.ptr(g[b0:b1]), _lib.ptr(ws), ws.numel(), _lib.stream()))
-        return f, g
-    return fg
+    warp, centre, H, W, sigma = opts
+    return _chunked_objective("evk_motion_timestamp_objective", "motion_timestamp_objective", (x, y, t_rel, tau, p), offsets,
+                              (warp, centre, H, W), (sigma,), (2, 2), FIT_WORKSPACE_BYTES, TIMESTAMP_FIT_MAX_WINDOWS)

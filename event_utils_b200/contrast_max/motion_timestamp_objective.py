@@ -12,9 +12,8 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from .flow_objective import _batch_events, _event_tensors
-from .flow_timestamp_objective import _normalised_stamps
-from .motion_objective import _WARPS, MAX_CANDIDATES, _warp_code
+from ._batched import (_candidates_tensor, _check_window_count, _chunked_candidates, _event_tensors, _params_tensor,
+                       _timestamp_events, _ts_model, _warp_code)
 
 
 def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, blur_sigma=2.0, timestamp_reverse=False,
@@ -54,35 +53,18 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
            f32 and stores the images in f32, so the gradient is accurate to f32 rounding whatever params' dtype.  With
            every input already on the GPU neither the forward nor the backward synchronises with the host.
     """
-    warp = next((code for cls, code in _WARPS if type(warpfunc) is cls), None)
-    if warp is None:
-        raise ValueError("motion_timestamp_objective_torch supports the models linvel_warp, pure_rotation_warp and "
-                         "xyztheta_warp, got %s" % type(warpfunc).__name__)
+    warp = _warp_code(warpfunc, "motion_timestamp_objective_torch")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_timestamp_objective_torch", "params")
-    params = E.as_tensor(params)
-    if not params.is_floating_point():
-        raise ValueError("params must be a floating-point tensor, got %s" % params.dtype)
-    if params.dim() == 1:
-        params = params.unsqueeze(0)
-    if params.dim() != 2 or params.shape[1] != warpfunc.dims:
-        raise ValueError("params must have shape (B,%d) or (%d,) for %s, got %s"
-                         % (warpfunc.dims, warpfunc.dims, type(warpfunc).__name__, tuple(params.shape)))
+    params = _params_tensor(params, warpfunc)
     B = params.shape[0]
-    if batch_end_indices is not None:
-        n_samples = (batch_end_indices.reshape(-1).shape[0] if isinstance(batch_end_indices, torch.Tensor)
-                     else len(batch_end_indices))
-        if n_samples != B:
-            raise ValueError("%d samples of events for a batch of %d parameter vectors" % (n_samples, B))
+    _check_window_count(batch_end_indices, B, "parameter vectors")
     H, W = int(img_size[0]), int(img_size[1])
     _lib.lib()
     dev = E.compute_device(params, xs, ys, ts, ps)
-    x, y, t_rel, p, offsets, t, sample = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "parameter vectors",
-                                                       stamps=True)
-    with torch.cuda.device(dev):
-        tau = _normalised_stamps(t, sample, offsets, timestamp_reverse)
+    x, y, t_rel, tau, p, offsets = _timestamp_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "parameter vectors",
+                                                     timestamp_reverse)
     from ..autograd import MotionTimestampObjective
-    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
-    f = MotionTimestampObjective.apply(params, x, y, t_rel, tau, p, offsets, (warp, centre, H, W, float(blur_sigma)))
+    f = MotionTimestampObjective.apply(params, x, y, t_rel, tau, p, offsets, _ts_model(warp, warpfunc, blur_sigma, H, W))
     return f.to(device=params.device, dtype=params.dtype)
 
 
@@ -106,54 +88,22 @@ def motion_timestamp_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=N
     """
     warp = _warp_code(warpfunc, "motion_timestamp_candidates_torch")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_timestamp_candidates_torch", "nothing")
-    cand = E.as_tensor(candidates)
-    if not cand.is_floating_point():
-        raise ValueError("candidates must be a floating-point tensor, got %s" % cand.dtype)
-    if cand.dim() != 3 or cand.shape[2] != warpfunc.dims or cand.shape[1] < 1:
-        raise ValueError("candidates must have shape (B,J,%d) with J >= 1 for %s, got %s"
-                         % (warpfunc.dims, type(warpfunc).__name__, tuple(cand.shape)))
+    cand = _candidates_tensor(candidates, warpfunc)
     B = cand.shape[0]
     H, W = int(img_size[0]), int(img_size[1])
     _lib.lib()
     dev = E.compute_device(cand, xs, ys, ts, ps)
-    x, y, t_rel, p, offsets, t, sample = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "candidate sets",
-                                                       stamps=True)
+    x, y, t_rel, tau, p, offsets = _timestamp_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "candidate sets",
+                                                     timestamp_reverse)
     with torch.cuda.device(dev):
-        tau = _normalised_stamps(t, sample, offsets, timestamp_reverse)
         c64 = cand.detach().to(device=dev, dtype=torch.float64)
         f = _ts_candidates(x, y, t_rel, tau, p, offsets, c64, _ts_model(warp, warpfunc, blur_sigma, H, W))
     return f.to(cand.device)
 
 
-def _ts_model(warp, warpfunc, blur_sigma, H, W):
-    """the scalar arguments the motion timestamp entries share: (warp code, (cx, cy), H, W, sigma)"""
-    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
-    return warp, centre, H, W, float(blur_sigma)
-
-
 def _ts_candidates(x, y, t_rel, tau, p, offsets, c64, opts):
     """f (B,J) f64 of the prepared device events under the device candidates c64 (B,J,K) f64, in passes of at most
     MAX_CANDIDATES candidates over chunks of windows whose workspace fits TIMESTAMP_CANDIDATES_WORKSPACE_BYTES"""
-    warp, (cx, cy), H, W, sigma = opts
-    B, J, K = c64.shape
-    L = _lib.lib()
-    dev = x.device
-    f = torch.empty((B, J), dtype=torch.float64, device=dev)
-    if B == 0:
-        return f
-    jc = min(J, MAX_CANDIDATES)
-    per_window = L.evk_motion_timestamp_candidates_workspace_bytes(1, jc, H, W)
-    wb = max(1, min(B, TIMESTAMP_CANDIDATES_WORKSPACE_BYTES // per_window, 32767 // jc))
-    ws = _lib.scratch("motion_timestamp_candidates", L.evk_motion_timestamp_candidates_workspace_bytes(wb, jc, H, W), dev)
-    for b0 in range(0, B, wb):
-        b1 = min(B, b0 + wb)
-        for j0 in range(0, J, MAX_CANDIDATES):
-            j1 = min(J, j0 + MAX_CANDIDATES)
-            c = c64[b0:b1, j0:j1].contiguous()
-            out = torch.empty((b1 - b0, j1 - j0), dtype=torch.float64, device=dev)
-            _lib.check(L.evk_motion_timestamp_candidates_f32(
-                _lib.ptr(x), _lib.ptr(y), _lib.ptr(t_rel), _lib.ptr(tau), _lib.ptr(p), _lib.ptr(offsets[b0:]), b1 - b0,
-                x.shape[0], warp, _lib.ptr(c), j1 - j0, K, cx, cy, H, W, sigma, _lib.ptr(out), _lib.ptr(ws), ws.numel(),
-                _lib.stream()))
-            f[b0:b1, j0:j1] = out
-    return f
+    warp, centre, H, W, sigma = opts
+    return _chunked_candidates("evk_motion_timestamp_candidates", "motion_timestamp_candidates", (x, y, t_rel, tau, p),
+                               offsets, c64, (warp, centre, H, W), (sigma,), TIMESTAMP_CANDIDATES_WORKSPACE_BYTES, 32767)

@@ -26,8 +26,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from event_utils_b200.contrast_max import (linvel_warp, motion_contrast_fit_torch, motion_contrast_objective_torch,  # noqa: E402
                                            pure_rotation_warp, xyztheta_warp)
 from event_utils_b200.contrast_max.motion_fit import _grid_search  # noqa: E402
-from event_utils_b200.contrast_max.motion_objective import _candidates, _model  # noqa: E402
-from event_utils_b200.contrast_max.flow_objective import _batch_events  # noqa: E402
+from event_utils_b200.contrast_max.motion_objective import _candidates  # noqa: E402
+from event_utils_b200.contrast_max._batched import _batch_events, _model  # noqa: E402
 
 CENTRE = (120.0, 90.0)
 

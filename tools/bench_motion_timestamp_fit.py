@@ -27,10 +27,9 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from bench_motion_fit import SCALE, WARPS, _code, recovered, timed, truths_of, windows  # noqa: E402
 from event_utils_b200.contrast_max import (motion_timestamp_candidates_torch, motion_timestamp_fit_torch,  # noqa: E402
                                            motion_timestamp_objective_torch)
-from event_utils_b200.contrast_max.flow_objective import _batch_events  # noqa: E402
-from event_utils_b200.contrast_max.flow_timestamp_objective import _normalised_stamps  # noqa: E402
+from event_utils_b200.contrast_max._batched import _timestamp_events, _ts_model  # noqa: E402
 from event_utils_b200.contrast_max.motion_fit import _grid_search  # noqa: E402
-from event_utils_b200.contrast_max.motion_timestamp_objective import _ts_candidates, _ts_model  # noqa: E402
+from event_utils_b200.contrast_max.motion_timestamp_objective import _ts_candidates  # noqa: E402
 
 SIGMA = 2.0
 ROWS = [
@@ -84,8 +83,7 @@ def run_row(row, scipy_windows):
     if "x0" in kw:
         start = kw["x0"]
     else:
-        xd, yd, td, pd, off, ts, sample = _batch_events(*ev, None, ends_d, B, ev[0].device, "windows", stamps=True)
-        tau = _normalised_stamps(ts, sample, off, False)
+        xd, yd, td, tau, pd, off = _timestamp_events(*ev, None, ends_d, B, ev[0].device, "windows", False)
         opts = _ts_model(_code(kind), warp, SIGMA, 180, 240)
         ranges = kw["param_ranges"].to(torch.float64).unsqueeze(0).expand(B, -1, -1).contiguous()
         start = _grid_search(lambda c: _ts_candidates(xd, yd, td, tau, pd, off, c, opts), ranges, kw["num_samples_per_param"],

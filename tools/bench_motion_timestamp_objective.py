@@ -25,7 +25,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from event_utils_b200 import _lib  # noqa: E402
 from event_utils_b200.contrast_max import (motion_timestamp_objective_torch, pure_rotation_warp, xyztheta_warp,  # noqa: E402
                                            zhu_timestamp_objective)
-from event_utils_b200.contrast_max.flow_timestamp_objective import _normalised_stamps  # noqa: E402
+from event_utils_b200.contrast_max._batched import _normalised_stamps  # noqa: E402
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from bench_cmax_motion_objective import card  # noqa: E402
