@@ -15,6 +15,7 @@ Which inputs get a gradient (as in the reference; the others get None):
     events_to_neg_pos_voxel_torch    ts (voxel_grid.py:155-182)
     flow_contrast_objective_torch    flow only (contrast_max/flow_objective.py; the events are data)
     flow_timestamp_objective_torch   flow only (contrast_max/flow_timestamp_objective.py; the events are data)
+    grid_flow_contrast_objective_torch  the node grid only (contrast_max/grid_flow.py; the events are data)
     motion_contrast_objective_torch  params only (contrast_max/motion_objective.py; the events are data)
     motion_segmentation_objective_torch  params and weights (contrast_max/motion_segmentation.py; the events are data)
     motion_timestamp_objective_torch params only (contrast_max/motion_timestamp_objective.py; the events are data)
@@ -179,18 +180,20 @@ class WarpFlow(torch.autograd.Function):
 
 def _loss_entry(L, entry, events, offsets, d):
     """The arguments every entry of a batched loss starts with, and its scratch.  entry = (stem, scratch key, (M,) for
-    a multi-model loss, the arguments in front of and behind the differentiable input d, (H, W))."""
-    stem, key, ms, pre, post, (H, W) = entry
+    a multi-model loss, the arguments in front of and behind the differentiable input d, (H, W), the arguments the
+    workspace query takes in front of (H, W) besides the batch and M)."""
+    stem, key, ms, pre, post, (H, W), query = entry
     B = d.shape[0]
     lead = tuple(_lib.ptr(a) for a in events) + ms + (_lib.ptr(offsets), B, events[0].shape[0]) + pre + (_lib.ptr(d),) + post
-    ws = _lib.scratch(key, getattr(L, stem + "_workspace_bytes")(B, *ms, H, W), d.device)
+    ws = _lib.scratch(key, getattr(L, stem + "_workspace_bytes")(B, *ms, *query, H, W), d.device)
     return lead, ws
 
 
-def _loss_forward(ctx, stem, key, inp, dtype, pre, post, size, events, offsets, images, weights=None):
+def _loss_forward(ctx, stem, key, inp, dtype, pre, post, size, events, offsets, images, weights=None, query=()):
     """The forward the batched losses share: f (B,) f64 of `stem`_f32 from inp in `dtype` on the events' device and the
     prepared device events.  `images` are the canvases per sample of each image the entry hands to `stem`_grad_f32.
-    With the memberships `weights` (N,M), as f32 the last of the event arrays, the loss has M models: f is (B,M)."""
+    With the memberships `weights` (N,M), as f32 the last of the event arrays, the loss has M models: f is (B,M).
+    `query`: the arguments `stem`_workspace_bytes takes between the batch and (H, W)."""
     dev = events[0].device
     L = _lib.lib()
     with torch.cuda.device(dev):
@@ -202,7 +205,7 @@ def _loss_forward(ctx, stem, key, inp, dtype, pre, post, size, events, offsets, 
         B, (H, W) = d.shape[0], size
         f = torch.empty((B,) + ms, dtype=torch.float64, device=dev)
         imgs = [torch.empty((B, c, H + 1, W + 1), dtype=torch.float32, device=dev) for c in images]
-        ctx.entry = (stem, key, ms, pre, post, size)
+        ctx.entry = (stem, key, ms, pre, post, size, query)
         lead, ws = _loss_entry(L, ctx.entry, events, offsets, d)
         _lib.check(getattr(L, stem + "_f32")(*lead, _lib.ptr(f), *(_lib.ptr(i) for i in imgs), _lib.ptr(ws), ws.numel(),
                                              _lib.stream()))
@@ -242,6 +245,26 @@ class FlowObjective(torch.autograd.Function):
         H, W = flow.shape[2:]
         return _loss_forward(ctx, "evk_cmax_flow_objective", "flow_objective", flow, torch.float32, (),
                              (H, W, sigma, objective, param), (H, W), (x, y, t_rel, p), offsets, (1,))
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return _loss_backward(ctx, g)[:1] + (None,) * 6
+
+
+class GridFlowObjective(torch.autograd.Function):
+    """The batched grid-flow contrast objective of contrast_max/grid_flow.py (the dense-flow objective with the flow
+    bilinearly interpolated from a gh x gw grid of nodes): f (B,) f64 from grid_flow (B,2,gh,gw) and the prepared device
+    events.  Only the nodes get a gradient: the exact derivative of f, one pass over the events
+    (evk_cmax_grid_flow_objective_grad_f32).  opts = (H, W, objective, sigma, obj_param)."""
+
+    @staticmethod
+    def forward(ctx, grid_flow, x, y, t_rel, p, offsets, opts):
+        H, W, objective, sigma, param = opts
+        gh, gw = grid_flow.shape[2:]
+        return _loss_forward(ctx, "evk_cmax_grid_flow_objective", "grid_flow_objective", grid_flow, torch.float32, (),
+                             (gh, gw, H, W, sigma, objective, param), (H, W), (x, y, t_rel, p), offsets, (1,),
+                             query=(gh, gw))
 
     @staticmethod
     @once_differentiable

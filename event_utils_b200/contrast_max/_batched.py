@@ -14,6 +14,7 @@ OBJECTIVES = {"variance": _lib.OBJ_VARIANCE, "sos": _lib.OBJ_SOS, "soe": _lib.OB
 DEFAULT_PARAM = {"sosa": 3.0}   # sosa_objective(p=3)
 _WARPS = ((linvel_warp, _lib.WARP_LINVEL), (pure_rotation_warp, _lib.WARP_ROTATION), (xyztheta_warp, _lib.WARP_XYZTHETA))
 MAX_CANDIDATES = 32   # parameter vectors per window and pass over the events
+MAX_GRID_CANDIDATE_NODES = 12288   # candidates times nodes of a grid-flow candidates pass (the grids a CTA holds)
 
 
 def _check_objective(objective, wrt):
@@ -165,14 +166,25 @@ def _pointers(tensors):
     return tuple(_lib.ptr(a) for a in tensors)
 
 
+def _model_layout(model, K):
+    """the arguments of a motion entry in front of its parameter pointer, between the parameter count and (H, W), and
+    those its workspace query takes in front of (H, W): model = (warp, (cx, cy), H, W).  A grid-flow entry takes
+    model = ("grid", (gh, gw), H, W): its grids of K = 2 gh gw floats are followed by gh, gw, which its query takes too."""
+    kind, extra, H, W = model
+    if kind == "grid":
+        return (), (), extra, extra, H, W
+    cx, cy = extra
+    return (kind,), (K, cx, cy), (), (), H, W
+
+
 def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget, cap, M=None):
-    """f (B,J) f64 of the prepared device events under the device candidates c64 (B,J,K) f64 through the entry
-    `stem`_f32, in passes of at most MAX_CANDIDATES candidate images per window over chunks of windows whose workspace
+    """f (B,J) f64 of the prepared device events under the device candidates c64 (B,J,K) through the entry `stem`_f32,
+    in passes of at most MAX_CANDIDATES candidate images per window over chunks of windows whose workspace
     (`stem`_workspace_bytes) fits `budget` and whose images number at most `cap`.  `events` are the arrays in front of
-    the offsets and `scalars` the arguments behind W.  With M, the entry scores M models per window: the last of
-    `events` is the memberships, c64 is (B,M,J,K) and f (B,M,J)."""
-    warp, (cx, cy), H, W = model
+    the offsets and `scalars` the arguments behind W; model is _model_layout's.  With M, the entry scores M models per
+    window: the last of `events` is the memberships, c64 is (B,M,J,K) and f (B,M,J)."""
     J, K = c64.shape[-2:]
+    pre, mid, grid, query, H, W = _model_layout(model, K)
     B = c64.shape[0]
     ms = () if M is None else (M,)
     L = _lib.lib()
@@ -182,8 +194,10 @@ def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget,
     if B == 0:
         return f
     jc = min(J, MAX_CANDIDATES // (M or 1))
-    wb = fit_window_chunk(B, workspace_bytes(1, *ms, jc, H, W), budget, cap // ((M or 1) * jc))
-    ws = _lib.scratch(key, workspace_bytes(wb, *ms, jc, H, W), dev)
+    if grid:
+        jc = max(1, min(jc, MAX_GRID_CANDIDATE_NODES // (grid[0] * grid[1])))
+    wb = fit_window_chunk(B, workspace_bytes(1, *ms, jc, *query, H, W), budget, cap // ((M or 1) * jc))
+    ws = _lib.scratch(key, workspace_bytes(wb, *ms, jc, *query, H, W), dev)
     front = _pointers(events) + ms
     for b0 in range(0, B, wb):
         b1 = min(B, b0 + wb)
@@ -191,8 +205,8 @@ def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget,
             j1 = min(J, j0 + jc)
             c = c64[b0:b1, ..., j0:j1, :].contiguous()
             out = torch.empty(c.shape[:-1], dtype=torch.float64, device=dev)
-            _lib.check(entry(*front, _lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], warp, _lib.ptr(c), j1 - j0, K,
-                             cx, cy, H, W, *scalars, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream()))
+            _lib.check(entry(*front, _lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], *pre, _lib.ptr(c), j1 - j0,
+                             *mid, *grid, H, W, *scalars, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream()))
             f[b0:b1, ..., j0:j1] = out
     return f
 
@@ -201,11 +215,11 @@ def _chunked_objective(stem, key, events, offsets, model, scalars, images, budge
     """fg: (B,K) f64 params -> (f (B,) f64, g (B,K) f64) of the prepared device events through the entries `stem`_f32 /
     `stem`_grad_f32 (grad_f = 1), in chunks of at most `cap` windows whose workspace (`stem`_workspace_bytes) and images
     fit `budget` (fit_window_chunk); the windows are independent, so a chunk changes no value's arithmetic.  `events`
-    are the arrays in front of the offsets, `scalars` the arguments behind W and `images` the canvases per window of
-    each image the forward hands to the gradient.  With M, the entries score M models per window: the last of `events`
-    is the memberships (they get no gradient), params is (B*M,K), f (B*M,) and g (B*M,K).  Without `gradient`, g is
-    None and the gradient entry is not called."""
-    warp, (cx, cy), H, W = model
+    are the arrays in front of the offsets, `scalars` the arguments behind W, model is _model_layout's and `images` the
+    canvases per window of each image the forward hands to the gradient.  With M, the entries score M models per window:
+    the last of `events` is the memberships (they get no gradient), params is (B*M,K), f (B*M,) and g (B*M,K).  Without
+    `gradient`, g is None and the gradient entry is not called.  A grid-flow entry takes the parameters (the nodes) and
+    returns their gradient in f32."""
     ms, no_weight_gradient = ((), ()) if M is None else ((M,), (None,))
     rows = M or 1
     L = _lib.lib()
@@ -216,22 +230,24 @@ def _chunked_objective(stem, key, events, offsets, model, scalars, images, budge
     def fg(params):
         K = params.shape[1]
         B = params.shape[0] // rows
-        prm = params.contiguous()
+        pre, mid, grid, query, H, W = _model_layout(model, K)
+        dtype = torch.float32 if grid else torch.float64
+        prm = params.to(dtype).contiguous()
         f = torch.empty(B * rows, dtype=torch.float64, device=dev)
-        g = torch.empty((B * rows, K), dtype=torch.float64, device=dev) if gradient else None
-        wb = fit_window_chunk(B, workspace_bytes(1, *ms, H, W) + 4 * sum(images) * (H + 1) * (W + 1), budget, cap)
+        g = torch.empty((B * rows, K), dtype=dtype, device=dev) if gradient else None
+        wb = fit_window_chunk(B, workspace_bytes(1, *ms, *query, H, W) + 4 * sum(images) * (H + 1) * (W + 1), budget, cap)
         kept = [torch.empty((wb * c, H + 1, W + 1), dtype=torch.float32, device=dev) for c in images]
         imgs = _pointers(kept)
         ones = torch.ones(wb * rows, dtype=torch.float32, device=dev)
-        ws = _lib.scratch(key, workspace_bytes(wb, *ms, H, W), dev)
+        ws = _lib.scratch(key, workspace_bytes(wb, *ms, *query, H, W), dev)
         for b0 in range(0, B, wb):
             b1 = min(B, b0 + wb)
             r0, r1 = b0 * rows, b1 * rows
-            ev = front + (_lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], warp, _lib.ptr(prm[r0:r1]), K, cx, cy, H, W,
+            ev = front + (_lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], *pre, _lib.ptr(prm[r0:r1]), *mid, *grid, H, W,
                           *scalars)
             _lib.check(forward(*ev, _lib.ptr(f[r0:r1]), *imgs, _lib.ptr(ws), ws.numel(), _lib.stream()))
             if gradient:
                 _lib.check(grad(*ev, *imgs, _lib.ptr(ones), _lib.ptr(g[r0:r1]), *no_weight_gradient, _lib.ptr(ws),
                                 ws.numel(), _lib.stream()))
-        return f, g
+        return f, (g.to(torch.float64) if g is not None else None)
     return fg

@@ -1685,16 +1685,24 @@ struct FlowArgs {
     const float2 *ab;      // timestamp backward: (A, B) [B][2][Hc][Wc]
 };
 
+// The warp by the flow (u, v) at the event, the keep rule and the taps of one event; false for events that contribute
+// nothing.  Shared by the dense-flow and the grid-flow passes.
+__device__ __forceinline__ bool flow_obj_keep(const FlowArgs &A, float xe, float ye, float u, float v, float d, float p, Taps &T,
+                                              bool &nonfinite)
+{
+    const float xw = __fadd_rn(xe, __fmul_rn(u, d)), yw = __fadd_rn(ye, __fmul_rn(v, d));
+    if (!isfinite(xw) || !isfinite(yw)) { nonfinite = true; return false; }
+    if (!(xw >= 0.0f && xw < (float)A.W && yw >= 0.0f && yw < (float)A.H)) return false;
+    unsigned oob = 0;   // a kept event's footprint lies inside the canvas
+    return splat_taps<false>(A.C, xw, yw, p, 0.0f, true, oob, T);
+}
+
 // The warp and the keep rule of one event of sample b; false for events that contribute nothing.
 __device__ __forceinline__ bool flow_obj_warp(const FlowArgs &A, const float *flow, float xe, float ye, float d, float p,
                                               FlowSample &s, Taps &T, bool &nonfinite)
 {
     s = flow_sample<false>(flow, nullptr, A.H, A.W, xe, ye);
-    const float xw = __fadd_rn(xe, __fmul_rn(s.u, d)), yw = __fadd_rn(ye, __fmul_rn(s.v, d));
-    if (!isfinite(xw) || !isfinite(yw)) { nonfinite = true; return false; }
-    if (!(xw >= 0.0f && xw < (float)A.W && yw >= 0.0f && yw < (float)A.H)) return false;
-    unsigned oob = 0;   // a kept event's footprint lies inside the canvas
-    return splat_taps<false>(A.C, xw, yw, p, 0.0f, true, oob, T);
+    return flow_obj_keep(A, xe, ye, s.u, s.v, d, p, T, nonfinite);
 }
 
 // The backward of the flow losses: an event's df/dflow = (gu, gv) times the weights of its four grid_sample taps, added to
@@ -1971,6 +1979,277 @@ static void batch_obj_backward_W(const BatchObjWorkspace &ws, const float *iwe, 
     flow_obj_coef_kernel<<<g, 256, 0, st>>>(ws.G, npix, objective, obj_param, grad_f, ws.w);
     if (do_blur) cmax_blur_d_axis0_kernel<<<g, 256, 0, st>>>(ws.w, ws.wt, Hc, Wc, taps);
     cmax_blur_d_axis1_store_kernel<<<g, 256, 0, st>>>(ws.wt, ws.w, Hc, Wc, taps, do_blur, ws.Wimg);
+}
+
+// ---- grid-parametrised flow objective over a batch of samples (evk_cmax_grid_flow_*) --------------------------------
+// The dense-flow objective with the flow of sample b given on a gh x gw grid of nodes (align_corners: node (i, j) at pixel
+// (j (W-1)/(gw-1), i (H-1)/(gh-1))): an event at (x, y) takes the bilinear interpolation of the nodes at
+// (x (gw-1)/(W-1), y (gh-1)/(H-1)), zero outside the node grid; then flow_obj_keep, the splat and the tail of the flow
+// objective (optic_flow.py:37-44, draw_flow.py:15-26).  The grid of the event passes is (slices, batch), as for the
+// flow objective, and every CTA holds its sample's nodes in dynamic shared memory as {u, v} pairs:
+//   forward / candidates: grid_flow_cand_kernel.  Per event one 16-byte record, the node cell and its four weights once
+//             (they do not depend on the candidate), then per candidate j four 8-byte node gathers from shared memory,
+//             the warp and one v4 reduction into canvas z = b J + j, scored by batch_obj_forward_tail.
+//   backward: batch_obj_backward_W, then grid_flow_grad_kernel: per event the four gathers of W_b give df/dx', df/dy'
+//             (as in flow_obj_event); times t_rel and the four node weights they go to a per-CTA f64 accumulator
+//             [2][gh][gw] in shared memory.  Coarse grids send a whole warp to a few node cells, and shared f32 / f64
+//             adds are CAS loops on sm_90a, so the lanes of a warp with the same cell first sum their eight values
+//             (match.any, then a shuffle tree over the peers) and one lane per cell adds them.  At the end one f64
+//             atomic per node component and CTA into [B][2][gh][gw] (in the workspace), then a cast to the f32 output:
+//             no L2 reduction per event and no per-pixel gradient blocks.
+constexpr int kMaxGridNodes = 4096;        // gh gw of the forward and backward
+constexpr int kMaxGridCandNodes = 12288;   // n_cand gh gw of the candidates pass (96 KB of f32 nodes)
+
+struct GridArgs {
+    FlowArgs F;            // canvas, events, H, W, acc, nonfinite, Wimg
+    const float *grid;     // [B][J][2][gh][gw]
+    int gh, gw, J;
+    float rx, ry;          // (gw-1)/(W-1), (gh-1)/(H-1) in f32
+    double *grad;          // backward: [B][2][gh][gw]
+};
+
+// The node cell of an event: the shared-memory indices o[k] of the four taps nw, ne, sw, se and their bilinear weights
+// (0 for a tap outside the node grid), the arithmetic of flow_sample at the node coordinates.  `cell` is -1 when no tap
+// lies inside the grid (or the coordinates are not finite: u = v = 0, as for the dense flow).
+struct NodeSample {
+    int o[4];
+    float w[4];
+    unsigned inside;   // bit k: tap k lies inside the node grid
+    int cell;
+};
+
+__device__ __forceinline__ NodeSample node_sample(const GridArgs &A, float xe, float ye)
+{
+    NodeSample s;
+    s.cell = -1;
+    s.inside = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { s.o[k] = 0; s.w[k] = 0.0f; }
+    const float ix = __fmul_rn(xe, A.rx), iy = __fmul_rn(ye, A.ry);
+    if (!(fabsf(ix) < 1.0e9f && fabsf(iy) < 1.0e9f)) return s;
+    const float fx = floorf(ix), fy = floorf(iy);
+    const int x0 = (int)fx, y0 = (int)fy;
+    const float xs = fx + 1.0f, ys = fy + 1.0f;
+    const float w[4] = {__fmul_rn(__fsub_rn(xs, ix), __fsub_rn(ys, iy)), __fmul_rn(__fsub_rn(ix, fx), __fsub_rn(ys, iy)),
+                        __fmul_rn(__fsub_rn(xs, ix), __fsub_rn(iy, fy)), __fmul_rn(__fsub_rn(ix, fx), __fsub_rn(iy, fy))};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int xx = x0 + (k & 1), yy = y0 + (k >> 1);
+        if ((unsigned)xx < (unsigned)A.gw && (unsigned)yy < (unsigned)A.gh) {
+            s.o[k] = yy * A.gw + xx;
+            s.w[k] = w[k];
+            s.inside |= 1u << k;
+        }
+    }
+    if (s.inside) s.cell = (y0 + 1) * (A.gw + 1) + (x0 + 1);   // x0, y0 >= -1 when a tap is inside
+    return s;
+}
+
+// the flow of one candidate's nodes at an event, in flow_sample's order of terms (a tap outside the grid reads 0)
+__device__ __forceinline__ void node_flow(const float2 *nodes, const NodeSample &s, float &u, float &v)
+{
+    u = 0.0f; v = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float2 q = s.inside >> k & 1u ? nodes[s.o[k]] : make_float2(0.0f, 0.0f);
+        u = __fadd_rn(u, __fmul_rn(q.x, s.w[k]));
+        v = __fadd_rn(v, __fmul_rn(q.y, s.w[k]));
+    }
+}
+
+// the J grids of sample b, [J][2][gh][gw] in global memory, as [J][gh gw] {u, v} pairs in shared memory
+__device__ __forceinline__ void load_nodes(const GridArgs &A, int b, float2 *nodes)
+{
+    const int G = A.gh * A.gw, J = A.J;
+    const float *src = A.grid + (int64_t)b * J * 2 * G;
+    for (int q = threadIdx.x; q < J * G; q += kFlowObjThreads) {
+        const int j = q / G, k = q - j * G;
+        nodes[q] = make_float2(__ldg(src + (2 * j) * G + k), __ldg(src + (2 * j + 1) * G + k));
+    }
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(kFlowObjThreads) grid_flow_cand_kernel(const GridArgs A)
+{
+    extern __shared__ float2 grid_nodes[];   // [J][gh gw]
+    const int b = blockIdx.y, J = A.J, G = A.gh * A.gw;
+    load_nodes(A, b, grid_nodes);
+    int64_t first, last;
+    sample_range(A.F.E, b, first, last);
+    const int Wc = A.F.C.Wc;
+    const int64_t npix = (int64_t)A.F.C.Hc * Wc;
+    float *acc = A.F.acc + (int64_t)b * J * npix * 4;
+    unsigned nonfinite = 0;   // bit j: candidate j warped an event to a non-finite position (J <= 32)
+    for_each_event(first, last, [&](int64_t i) { return load_xytp(A.F.E, i); }, [&](int64_t, const EvXYTP &e) {
+        const NodeSample s = node_sample(A, e.x, e.y);
+        for (int j = 0; j < J; ++j) {
+            float u, v;
+            node_flow(grid_nodes + j * G, s, u, v);
+            Taps T;
+            bool nf = false;
+            if (flow_obj_keep(A.F, e.x, e.y, u, v, e.t, e.p, T, nf))
+                red_add4(acc + ((int64_t)j * npix + (int64_t)T.y0 * Wc + T.x0) * 4, T.ti);
+            if (nf) nonfinite |= 1u << j;
+        }
+    });
+    for (int j = 0; j < J; ++j)
+        if (nonfinite >> j & 1u) A.F.nonfinite[(int64_t)b * J + j] = 1u;
+}
+
+// v[0..7] summed over the lanes of the warp that share `key` (all 32 lanes call this); the lowest lane of each key holds
+// the sum and gets true.  A shuffle tree over each key's peers (the lanes of rank 2^r k add the next peer's partial sum).
+__device__ __forceinline__ bool warp_key_sum(int key, float (&v)[8])
+{
+    const unsigned full = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    const unsigned peers = __match_any_sync(full, key);
+    unsigned rank = __popc(peers & ((1u << lane) - 1u));
+    unsigned rest = peers & (0xfffffffeu << lane);   // the peers above this lane
+    while (__any_sync(full, rest != 0u)) {
+        const int next = __ffs(rest);
+        float t[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) t[k] = __shfl_sync(full, v[k], (next - 1) & 31);
+        if (next) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] += t[k];
+        }
+        rest &= __ballot_sync(full, !(rank & 1u));
+        rank >>= 1;
+    }
+    return lane == __ffs(peers) - 1;
+}
+
+__global__ void __launch_bounds__(kFlowObjThreads) grid_flow_grad_kernel(const GridArgs A)
+{
+    extern __shared__ double grid_acc[];   // [2][gh gw] f64, then the nodes as [gh gw] {u, v}
+    const int b = blockIdx.y, G = A.gh * A.gw;
+    float2 *nodes = reinterpret_cast<float2 *>(grid_acc + 2 * G);
+    for (int q = threadIdx.x; q < 2 * G; q += kFlowObjThreads) grid_acc[q] = 0.0;
+    load_nodes(A, b, nodes);   // and the barrier
+    int64_t first, last;
+    sample_range(A.F.E, b, first, last);
+    const int Wc = A.F.C.Wc;
+    const float *Wb = A.F.Wimg + (int64_t)b * A.F.C.Hc * Wc;
+    const int lane = threadIdx.x & 31;
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    // warp-uniform trip count (warp_key_sum needs every lane): kBatch records per lane, masked past `last`
+    for (int64_t i0 = first + (int64_t)blockIdx.x * kFlowObjThreads + (threadIdx.x - lane); i0 < last; i0 += kBatch * stride) {
+        EvXYTP e[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int64_t q = i0 + k * stride + lane;
+            e[k] = q < last ? load_xytp(A.F.E, q) : EvXYTP{0.0f, 0.0f, 0.0f, 0.0f};
+            if (!(q < last)) e[k].x = __int_as_float(0x7fc00000);   // a NaN position: no cell, no term
+        }
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const NodeSample s = node_sample(A, e[k].x, e[k].y);
+            float val[8];
+#pragma unroll
+            for (int q = 0; q < 8; ++q) val[q] = 0.0f;
+            int key = -1 - lane;   // a lane without a term is alone with its key
+            float u, v;
+            node_flow(nodes, s, u, v);
+            Taps T;
+            bool nf = false;
+            if (s.cell >= 0 && flow_obj_keep(A.F, e[k].x, e[k].y, u, v, e[k].t, e[k].p, T, nf)) {
+                // df/dx' and df/dy' through the four bilinear taps of the IWE, as in flow_obj_event
+                const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
+                const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0),
+                            w11 = __ldg(Wb + r1 + T.x1);
+                const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
+                float sx, sy;
+                tap_slopes(ox, oy, T.dx, T.dy, w00, w01, w10, w11, sx, sy);
+                const float gu = T.wm * sx * e[k].t, gv = T.wm * sy * e[k].t;
+                if (gu != 0.0f || gv != 0.0f) {
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        if (s.inside >> q & 1u) { val[q] = gu * s.w[q]; val[4 + q] = gv * s.w[q]; }
+                    }
+                    key = s.cell;
+                }
+            }
+            if (warp_key_sum(key, val) && key >= 0) {
+                // the peers share the leader's cell and so its taps inside the grid
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    if (!(s.inside >> q & 1u)) continue;
+                    if (val[q] != 0.0f) atomicAdd(grid_acc + s.o[q], (double)val[q]);
+                    if (val[4 + q] != 0.0f) atomicAdd(grid_acc + G + s.o[q], (double)val[4 + q]);
+                }
+            }
+        }
+    }
+    __syncthreads();
+    double *dst = A.grad + (int64_t)b * 2 * G;
+    for (int q = threadIdx.x; q < 2 * G; q += kFlowObjThreads)
+        if (grid_acc[q] != 0.0) atomicAdd(dst + q, grid_acc[q]);
+}
+
+// [B][2][gh][gw] f64 sums -> the f32 gradient
+__global__ void __launch_bounds__(256) grid_flow_grad_cast_kernel(const double *__restrict__ g, float *__restrict__ out, int64_t n)
+{
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = (float)g[i];
+}
+
+// Shared argument checks and set-up of the grid-flow entries.  n_cand 0: the differentiable entries (one canvas per
+// sample, gh gw <= kMaxGridNodes); else n_cand forward-only canvases per sample (n_cand <= kMaxCandidates,
+// n_cand gh gw <= kMaxGridCandNodes, batch n_cand <= 65535).
+static int grid_flow_limits(int batch, int n_cand, int gh, int gw, int H, int W)
+{
+    if (batch < 0 || H < 2 || W < 2 || gh < 2 || gw < 2 || gh > H || gw > W) return 0;
+    const int64_t G = (int64_t)gh * gw;
+    if (!n_cand) return batch <= 65535 && G <= kMaxGridNodes;
+    return n_cand >= 1 && n_cand <= kMaxCandidates && (int64_t)n_cand * G <= kMaxGridCandNodes && (int64_t)batch * n_cand <= 65535;
+}
+
+static int grid_flow_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
+                           int batch, int64_t n, const float *grid, int n_cand, int gh, int gw, int H, int W, double sigma,
+                           int objective, void *workspace, size_t workspace_bytes, GridArgs &A, BatchObjWorkspace &ws,
+                           BlurTaps &taps)
+{
+    if (int rc = check_sigma(who, sigma)) return rc;
+    if (!grid_flow_limits(batch, n_cand, gh, gw, H, W) || n < 0 || (batch > 0 && (!offsets || !grid)) ||
+        (n > 0 && (!x || !y || !t || !p))) {
+        set_error("%s: bad arguments (2 <= gh <= H, 2 <= gw <= W, gh gw <= %d; candidates: 1 <= n_cand <= %d, n_cand gh gw "
+                  "<= %d, batch n_cand <= 65535; else batch <= 65535)", who, kMaxGridNodes, kMaxCandidates, kMaxGridCandNodes);
+        return EVK_E_ARG;
+    }
+    const int J = n_cand ? n_cand : 1;
+    int rc = batch_obj_check(who, "flow", batch * J, H, W, sigma, objective, (size_t)(H + 1) * (W + 1), workspace, workspace_bytes,
+                             ws, taps, !n_cand);
+    if (rc) return rc;
+    A = GridArgs{};
+    A.F.C.Hc = H + 1; A.F.C.Wc = W + 1;
+    A.F.E = EventSource{x, y, t, p, nullptr, offsets, n};
+    A.F.H = H; A.F.W = W;
+    A.F.acc = ws.acc;
+    A.F.nonfinite = ws.nonfinite;
+    A.grid = grid;
+    A.gh = gh; A.gw = gw; A.J = J;
+    A.rx = (float)(gw - 1) / (float)(W - 1);
+    A.ry = (float)(gh - 1) / (float)(H - 1);
+    return EVK_OK;
+}
+
+// forward and candidates: zero, the event pass, the tail into iwe_out (the candidates: ws.Wimg)
+static int grid_flow_forward(const GridArgs &A, const BatchObjWorkspace &ws, const BlurTaps &taps, int batch, int objective,
+                             double obj_param, float *iwe_out, double *f_out, cudaStream_t st)
+{
+    const int Hc = A.F.C.Hc, Wc = A.F.C.Wc, npix = Hc * Wc, canvases = batch * A.J;
+    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
+    if (A.F.E.n > 0) {
+        const size_t smem = (size_t)A.J * A.gh * A.gw * sizeof(float2);
+        EVK_CUDA(cudaFuncSetAttribute(grid_flow_cand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ProfScope prof(st);
+        prof_count(1);
+        grid_flow_cand_kernel<<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(A);
+    }
+    batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, iwe_out, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
 }
 
 // ---- parametric motion objective over a batch of samples (evk_cmax_motion_objective_f32 / _grad_f32) ---------------
@@ -2957,6 +3236,92 @@ int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float
     flow_obj_grad_fold_kernel<<<grid_simple(planes * H * W, 256), 256, 0, st>>>(ws.acc, grad_flow, planes, H, W);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
+}
+
+size_t evk_cmax_grid_flow_objective_workspace_bytes(int batch, int gh, int gw, int H, int W)
+{
+    if (!evk::grid_flow_limits(batch, 0, gh, gw, H, W)) return 0;
+    return evk::batch_obj_carve(nullptr, batch, H, W, (size_t)(H + 1) * (W + 1), nullptr);
+}
+
+int evk_cmax_grid_flow_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                     int batch, int64_t n_events, const float *grid_flow, int gh, int gw, int H, int W,
+                                     double sigma, int objective, double obj_param, double *f_out, float *iwe_out,
+                                     void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    GridArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = grid_flow_setup("evk_cmax_grid_flow_objective_f32", x, y, t_rel, p, offsets, batch, n_events, grid_flow, 0, gh, gw, H,
+                             W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !iwe_out)) { set_error("evk_cmax_grid_flow_objective_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    return grid_flow_forward(A, ws, taps, batch, objective, obj_param, iwe_out, f_out, static_cast<cudaStream_t>(stream));
+}
+
+int evk_cmax_grid_flow_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                          const int64_t *offsets, int batch, int64_t n_events, const float *grid_flow, int gh,
+                                          int gw, int H, int W, double sigma, int objective, double obj_param, const float *iwe,
+                                          const float *grad_f, float *grad_grid, void *workspace, size_t workspace_bytes,
+                                          void *stream)
+{
+    using namespace evk;
+    GridArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = grid_flow_setup("evk_cmax_grid_flow_objective_grad_f32", x, y, t_rel, p, offsets, batch, n_events, grid_flow, 0, gh,
+                             gw, H, W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!iwe || !grad_f || !grad_grid)) {
+        set_error("evk_cmax_grid_flow_objective_grad_f32: null array");
+        return EVK_E_ARG;
+    }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int64_t nodes = (int64_t)batch * 2 * gh * gw;
+    // the f64 node sums live in the accumulator, which the backward has no other use for ((H+1)(W+1) 16 B >= 2 gh gw 8 B)
+    A.grad = reinterpret_cast<double *>(ws.acc);
+    EVK_CUDA(cudaMemsetAsync(A.grad, 0, (size_t)nodes * sizeof(double), st));
+    batch_obj_backward_W(ws, iwe, H + 1, W + 1, taps, batch, objective, obj_param, grad_f, st);
+    A.F.Wimg = ws.Wimg;
+    if (n_events > 0) {
+        const size_t smem = (size_t)gh * gw * (2 * sizeof(double) + sizeof(float2));
+        EVK_CUDA(cudaFuncSetAttribute(grid_flow_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ProfScope prof(st);
+        prof_count(1);
+        grid_flow_grad_kernel<<<batch_grid(n_events, batch), kFlowObjThreads, smem, st>>>(A);
+    }
+    prof_count(1);
+    grid_flow_grad_cast_kernel<<<grid_simple(nodes, 256), 256, 0, st>>>(A.grad, grad_grid, nodes);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_cmax_grid_flow_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
+{
+    if (!evk::grid_flow_limits(batch, n_cand, gh, gw, H, W)) return 0;
+    return evk::batch_obj_carve(nullptr, batch * n_cand, H, W, (size_t)(H + 1) * (W + 1), nullptr, false);
+}
+
+int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                      int batch, int64_t n_events, const float *cand, int n_cand, int gh, int gw, int H, int W,
+                                      double blur_sigma, int objective, double obj_param, double *f_out, void *workspace,
+                                      size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    GridArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = grid_flow_setup("evk_cmax_grid_flow_candidates_f32", x, y, t_rel, p, offsets, batch, n_events, cand,
+                             n_cand < 1 ? -1 : n_cand, gh, gw, H, W, blur_sigma, objective, workspace, workspace_bytes, A, ws,
+                             taps);
+    if (rc) return rc;
+    if (batch > 0 && !f_out) { set_error("evk_cmax_grid_flow_candidates_f32: null output"); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
+    return grid_flow_forward(A, ws, taps, batch, objective, obj_param, ws.Wimg, f_out, static_cast<cudaStream_t>(stream));
 }
 
 size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W)

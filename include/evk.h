@@ -499,6 +499,52 @@ int evk_cmax_flow_objective_grad_f32(const float *x, const float *y, const float
                                      const float *iwe, const float *grad_f, float *grad_flow,
                                      void *workspace, size_t workspace_bytes, void *stream);
 
+/* The dense-flow contrast objective with the flow of every sample given on a coarse grid of nodes (tile-based flow,
+ * Shiba et al., ECCV 2022).  grid_flow: [batch][2][gh][gw] f32 on the device, 2 <= gh <= H, 2 <= gw <= W,
+ * gh * gw <= 4096.  Node (i, j) sits at pixel (j (W-1)/(gw-1), i (H-1)/(gh-1)) (align_corners), and an event at
+ * (x, y) takes the flow (u, v) = bilinear interpolation of grid_flow[b] at (x rx, y ry), rx = (gw-1)/(W-1) and
+ * ry = (gh-1)/(H-1) rounded to f32, products in f32; a node tap outside the grid contributes 0 (zero padding, as the
+ * grid_sample of optic_flow.py:37-44).  Everything after that is evk_cmax_flow_objective_f32: x' = x + u t_rel,
+ * y' = y + v t_rel in f32, kept iff 0 <= x' < W and 0 <= y' < H, the bilinear IWE on the (H+1)x(W+1) canvas
+ * (draw_flow.py:15-26), the blur, the four objectives (EVK_OBJ_MOA / EVK_OBJ_ISOA: EVK_E_UNSUPPORTED) and a NaN f for
+ * a sample with a non-finite x' or y'.  For events at integer pixels inside the sensor, f equals the dense-flow f of
+ * the flow that bilinear upsampling with align_corners makes of the nodes, to f32 rounding; at gh = H, gw = W the grid
+ * is the dense flow.
+ *   f_out: batch doubles;  iwe_out: [batch][H+1][W+1] floats, which the backward takes as `iwe`
+ * evk_cmax_grid_flow_objective_grad_f32 writes grad_grid [batch][2][gh][gw] floats = grad_f[b] df_b/dgrid_flow[b]:
+ * df/dx' and df/dy' of evk_cmax_flow_objective_grad_f32, times t_rel, spread over the event's four node taps with
+ * their bilinear weights, summed per CTA in shared memory and across CTAs in f64, then rounded to f32.
+ * workspace: evk_cmax_grid_flow_objective_workspace_bytes(batch, gh, gw, H, W) bytes, 256-byte aligned, for either
+ * call; 0 for arguments the entries reject.  batch <= 65535.  Neither call synchronises, and both launch the same
+ * kernels whatever the batch. */
+size_t evk_cmax_grid_flow_objective_workspace_bytes(int batch, int gh, int gw, int H, int W);
+int evk_cmax_grid_flow_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                     const int64_t *offsets, int batch, int64_t n_events, const float *grid_flow,
+                                     int gh, int gw, int H, int W, double blur_sigma, int objective, double obj_param,
+                                     double *f_out, float *iwe_out, void *workspace, size_t workspace_bytes,
+                                     void *stream);
+int evk_cmax_grid_flow_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                          const int64_t *offsets, int batch, int64_t n_events,
+                                          const float *grid_flow, int gh, int gw, int H, int W, double blur_sigma,
+                                          int objective, double obj_param, const float *iwe, const float *grad_f,
+                                          float *grad_grid, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Many node grids per sample in one pass over the events (a batched line search of a grid-flow fit):
+ * f_out[b][j] is exactly the f_b of evk_cmax_grid_flow_objective_f32 with grid_flow[b] = cand[b][j].
+ *   cand : [batch][n_cand][2][gh][gw] floats on the device, 1 <= n_cand <= 32, n_cand * gh * gw <= 12288 (the
+ *          candidate grids of a sample fit in shared memory), batch * n_cand <= 65535
+ *   f_out: [batch][n_cand] doubles
+ * Every event is read once; its node cell and weights are computed once and used for every candidate.  All limits are
+ * checked before any CUDA call.  Forward only.  workspace: evk_cmax_grid_flow_candidates_workspace_bytes(batch,
+ * n_cand, gh, gw, H, W) bytes, 256-byte aligned; 0 for arguments the entry rejects.  The call does not synchronise
+ * and launches the same kernels whatever batch and n_cand. */
+size_t evk_cmax_grid_flow_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W);
+int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                      const int64_t *offsets, int batch, int64_t n_events, const float *cand,
+                                      int n_cand, int gh, int gw, int H, int W, double blur_sigma, int objective,
+                                      double obj_param, double *f_out, void *workspace, size_t workspace_bytes,
+                                      void *stream);
+
 /* Parametric contrast maximisation over a batch of samples, as a differentiable loss: per sample the f32
  * fast-mode evaluation of evk_cmax_warp_objective_f32 / evk_cmax_linvel_objective_f32 with Hm = Hs = H,
  * Wm = Ws = W, p_scale 1 and no flags (get_iwe, lib/contrast_max/objectives.py:184-192).  Sample b is the
