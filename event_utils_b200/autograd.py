@@ -16,6 +16,7 @@ Which inputs get a gradient (as in the reference; the others get None):
     flow_contrast_objective_torch    flow only (contrast_max/flow_objective.py; the events are data)
     flow_timestamp_objective_torch   flow only (contrast_max/flow_timestamp_objective.py; the events are data)
     grid_flow_contrast_objective_torch  the node grid only (contrast_max/grid_flow.py; the events are data)
+    grid_flow_timestamp_objective_torch  the node grid only (contrast_max/grid_flow_timestamp.py; the events are data)
     motion_contrast_objective_torch  params only (contrast_max/motion_objective.py; the events are data)
     motion_segmentation_objective_torch  params and weights (contrast_max/motion_segmentation.py; the events are data)
     motion_timestamp_objective_torch params only (contrast_max/motion_timestamp_objective.py; the events are data)
@@ -283,6 +284,27 @@ class FlowTimestampObjective(torch.autograd.Function):
         H, W = flow.shape[2:]
         return _loss_forward(ctx, "evk_flow_timestamp_objective", "flow_timestamp_objective", flow, torch.float32, (),
                              (H, W, sigma), (H, W), (x, y, t_rel, tau, p), offsets, (2, 2))
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return _loss_backward(ctx, g)[:1] + (None,) * 7
+
+
+class GridFlowTimestampObjective(torch.autograd.Function):
+    """The batched grid-flow average-timestamp loss of contrast_max/grid_flow_timestamp.py (the dense-flow timestamp loss
+    with the flow bilinearly interpolated from a gh x gw grid of nodes): f (B,) f64 from grid_flow (B,2,gh,gw) and the
+    prepared device events with their normalised stamps tau.  Only the nodes get a gradient: the exact derivative of f,
+    one pass over the events (evk_grid_flow_timestamp_objective_grad_f32).  The forward keeps the timestamp and count
+    images.  opts = (H, W, sigma)."""
+
+    @staticmethod
+    def forward(ctx, grid_flow, x, y, t_rel, tau, p, offsets, opts):
+        H, W, sigma = opts
+        gh, gw = grid_flow.shape[2:]
+        return _loss_forward(ctx, "evk_grid_flow_timestamp_objective", "grid_flow_timestamp_objective", grid_flow,
+                             torch.float32, (), (gh, gw, H, W, sigma), (H, W), (x, y, t_rel, tau, p), offsets, (2, 2),
+                             query=(gh, gw))
 
     @staticmethod
     @once_differentiable

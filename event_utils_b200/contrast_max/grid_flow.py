@@ -18,8 +18,8 @@ from ..representations import _events as E
 from ._batched import MAX_GRID_CANDIDATE_NODES  # noqa: F401  (a public name of this module)
 from ._batched import (DEFAULT_PARAM, OBJECTIVES, _batch_events, _check_objective, _chunked_candidates, _chunked_objective,
                        _event_tensors, _float_tensor, _window_count)
-from .motion_fit import (FIT_MAX_WINDOWS, FIT_WORKSPACE_BYTES, _batched_bfgs, _check_line_search_steps, _per_window,
-                         motion_contrast_fit_torch)
+from .motion_fit import (FIT_MAX_WINDOWS, FIT_WORKSPACE_BYTES, _batched_bfgs, _check_line_search_steps, _check_per_window,
+                         _per_window, motion_contrast_fit_torch)
 from .motion_objective import CANDIDATES_WORKSPACE_BYTES
 from .warps import linvel_warp
 
@@ -174,20 +174,52 @@ def grid_flow_fit_torch(xs, ys, ts, ps, img_size, grid_shapes=((3, 4), (6, 8), (
     _check_objective(objective, "flow")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "grid_flow_fit_torch", "nothing")
     H, W = int(img_size[0]), int(img_size[1])
+
+    def global_fit(sigma):
+        return motion_contrast_fit_torch(xs, ys, ts, ps, linvel_warp(), batch_end_indices, t0, objective, sigma, obj_param,
+                                         (H, W), param_ranges=param_ranges, num_samples_per_param=num_samples_per_param,
+                                         grid_levels=grid_levels, log_scale=log_scale, max_iter=max_iter,
+                                         line_search_steps=line_search_steps, ftol=ftol, gtol=gtol).params
+
+    def events(B, dev):
+        return _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows")
+
+    def loss(ev, grid, sigma):
+        x, y, t_rel, p, offsets = ev
+        scalars = _scalars(objective, sigma, obj_param)
+        return (_chunked_objective("evk_cmax_grid_flow_objective", "grid_flow_objective", ev[:4], offsets, ("grid", grid, H, W),
+                                   scalars, (1,), FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS),
+                lambda c: _candidates(x, y, t_rel, p, offsets, c, grid, H, W, scalars))
+    return GridFlowFit(*_grid_fit("grid_flow_fit_torch", (xs, ys, ts, ps), (H, W), grid_shapes, smoothness, charbonnier_eps,
+                                  batch_end_indices, blur_sigma, x0, param_ranges, None, num_samples_per_param, param_scale,
+                                  max_iter, line_search_steps, ftol, gtol, global_fit, events, loss))
+
+
+def _grid_fit(who, tensors, size, grid_shapes, smoothness, charbonnier_eps, batch_end_indices, blur_sigma, x0, param_ranges,
+              bounds, num_samples_per_param, param_scale, max_iter, line_search_steps, ftol, gtol, global_fit, events, loss,
+              bound_to_ranges=False):
+    """The coarse-to-fine fit of F = f + smoothness R that grid_flow_fit_torch and grid_flow_timestamp_fit_torch share:
+    the argument checks (before any CUDA call), the start, and the BFGS stages per grid shape and blur.
+    tensors: the inputs that choose the device;  global_fit(sigma) -> (B,2) linvel params (vx, vy) of the global fit at
+    the first blur, the start without x0;  events(B, dev) -> the prepared device events;  loss(events, (gh, gw), sigma)
+    -> (fg of f, candidates of f on f32 node grids).  bounds ((2,2) or (B,2,2)): [lo, hi] of u and of v at every node;
+    without it, bound_to_ranges confines a fit started from the global fit to the flow range -param_ranges implies,
+    widened by one level-0 grid step and stretched to contain the start.  Returns (flow, F, f, status, iterations)."""
+    H, W = size
     shapes = [(int(a), int(b)) for a, b in grid_shapes]
     if not shapes:
         raise ValueError("grid_shapes must name at least one (gh, gw)")
     for gh, gw in shapes:
         _check_grid_shape(gh, gw, H, W, MAX_GRID_NODES)
         if 2 * gh * gw > MAX_FIT_PARAMETERS:
-            raise ValueError("grid_flow_fit_torch keeps a dense inverse Hessian of K = 2 gh gw <= %d parameters per window; "
-                             "a %d x %d grid has K = %d" % (MAX_FIT_PARAMETERS, gh, gw, 2 * gh * gw))
+            raise ValueError("%s keeps a dense inverse Hessian of K = 2 gh gw <= %d parameters per window; "
+                             "a %d x %d grid has K = %d" % (who, MAX_FIT_PARAMETERS, gh, gw, 2 * gh * gw))
     sigmas = [float(s) for s in (blur_sigma if isinstance(blur_sigma, (list, tuple)) else [blur_sigma])]
     if not sigmas:
         raise ValueError("blur_sigma must be a number or a non-empty sequence")
     _check_line_search_steps(line_search_steps)
     if x0 is None and param_ranges is None:
-        raise ValueError("grid_flow_fit_torch needs x0 or param_ranges")
+        raise ValueError("%s needs x0 or param_ranges" % who)
     if float(smoothness) < 0 or not float(charbonnier_eps) > 0:
         raise ValueError("smoothness must be >= 0 and charbonnier_eps > 0")
     B = _window_count(batch_end_indices)
@@ -196,48 +228,58 @@ def grid_flow_fit_torch(xs, ys, ts, ps, img_size, grid_shapes=((3, 4), (6, 8), (
         got = tuple(x0.shape) if isinstance(x0, torch.Tensor) else tuple(torch.as_tensor(x0).shape)
         if got not in ((2, gh0, gw0), (B, 2, gh0, gw0)):
             raise ValueError("x0 must have shape %s or %s, got %s" % ((2, gh0, gw0), (B, 2, gh0, gw0), got))
+    if bounds is not None:
+        _check_per_window(bounds, B, (2, 2), "bounds")
     lam, eps = float(smoothness), float(charbonnier_eps)
     _lib.lib()
-    dev = E.compute_device(*(a for a in (x0, param_ranges, xs, ys, ts, ps) if isinstance(a, torch.Tensor)))
+    dev = E.compute_device(*(a for a in (x0, param_ranges, bounds) + tuple(tensors) if isinstance(a, torch.Tensor)))
+    box = None
     if x0 is None:
-        lin = motion_contrast_fit_torch(xs, ys, ts, ps, linvel_warp(), batch_end_indices, t0, objective, sigmas[0], obj_param,
-                                        (H, W), param_ranges=param_ranges, num_samples_per_param=num_samples_per_param,
-                                        grid_levels=grid_levels, log_scale=log_scale, max_iter=max_iter,
-                                        line_search_steps=line_search_steps, ftol=ftol, gtol=gtol)
+        params = global_fit(sigmas[0])
         with torch.cuda.device(dev):
-            flow = (-lin.params).view(B, 2, 1, 1).expand(B, 2, gh0, gw0).contiguous()
+            flow = (-params).view(B, 2, 1, 1).expand(B, 2, gh0, gw0).contiguous()
+            r = _per_window(param_ranges, B, (2, 2), "param_ranges", dev)
+            step = (r[..., 1] - r[..., 0]) / (num_samples_per_param - 1)
             if param_scale is None:
-                r = _per_window(param_ranges, B, (2, 2), "param_ranges", dev)
-                param_scale = ((r[..., 1] - r[..., 0]) / (num_samples_per_param - 1)).amax(1)
+                param_scale = step.amax(1)
+            if bounds is None and bound_to_ranges:
+                # u = -vx, v = -vy: the ranges' edges swap; one grid step beyond them, and the start inside
+                box = torch.stack((torch.minimum(-r[..., 1] - step, -params), torch.maximum(-r[..., 0] + step, -params)), -1)
     else:
         flow = _per_window(x0, B, (2, gh0, gw0), "x0", dev)
-    x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows")
+    if bounds is not None:
+        box = _per_window(bounds, B, (2, 2), "bounds", dev)
+    ev = events(B, dev)
     with torch.cuda.device(dev):
         scale = torch.as_tensor(1.0 if param_scale is None else param_scale, dtype=torch.float64, device=dev)
         iters = torch.zeros(B, dtype=torch.int32, device=dev)
-        status = f = contrast = None
+        status = f = None
         for gh, gw in shapes:
             if tuple(flow.shape[2:]) != (gh, gw):
                 flow = torch.nn.functional.interpolate(flow, (gh, gw), mode="bilinear", align_corners=True)
             K = 2 * gh * gw
             sc = scale.reshape(-1, 1).expand(B, K)
+            lim = None
+            if box is not None:
+                # every node of component c in [lo_c, hi_c]: the clamp moves a start outside the box onto it, and undoes
+                # the rounding of the upsampling
+                lim = box.unsqueeze(2).expand(B, 2, gh * gw, 2).reshape(B, K, 2)
+                flow = torch.minimum(torch.maximum(flow, box[..., 0, None, None]), box[..., 1, None, None])
             xk = flow.reshape(B, K)
             for sigma in sigmas:
-                fg, candidates = _stage(x, y, t_rel, p, offsets, (gh, gw), H, W,
-                                                _scalars(objective, sigma, obj_param), lam, eps)
-                xk, f, status, it = _batched_bfgs(fg, candidates, xk, sc, max_iter, line_search_steps, ftol, gtol,
+                fg, candidates = _stage(*loss(ev, (gh, gw), sigma), (gh, gw), lam, eps)
+                xk, f, status, it = _batched_bfgs(fg, candidates, xk, sc, max_iter, line_search_steps, ftol, gtol, lim,
                                                   unit_first_step=True)
                 iters += it
             flow = xk.reshape(B, 2, gh, gw)
-        contrast = f - lam * charbonnier_smoothness(flow, eps)[0]
-    return GridFlowFit(flow, f, contrast, status, iters)
+        rest = f - lam * charbonnier_smoothness(flow, eps)[0]
+    return flow, f, rest, status, iters
 
 
-def _stage(x, y, t_rel, p, offsets, grid, H, W, scalars, lam, eps):
-    """fg and candidates of F = f + lam R on the (gh, gw) grid, for _batched_bfgs"""
+def _stage(obj, cand, grid, lam, eps):
+    """fg and candidates of F = f + lam R on the (gh, gw) grid, for _batched_bfgs: obj (B,K) nodes -> (f, g) of the loss,
+    cand (B,J,K) f32 node grids -> (B,J) f"""
     gh, gw = grid
-    obj = _chunked_objective("evk_cmax_grid_flow_objective", "grid_flow_objective", (x, y, t_rel, p), offsets,
-                             ("grid", grid, H, W), scalars, (1,), FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS)
 
     def fg(xk):
         f, g = obj(xk)
@@ -246,7 +288,7 @@ def _stage(x, y, t_rel, p, offsets, grid, H, W, scalars, lam, eps):
 
     def candidates(pts):
         B, J, K = pts.shape
-        f = _candidates(x, y, t_rel, p, offsets, pts.to(torch.float32), grid, H, W, scalars)
+        f = cand(pts.to(torch.float32))
         R = charbonnier_smoothness(pts.reshape(B, J, 2, gh, gw), eps)[0]
         return f + lam * R
 

@@ -1997,7 +1997,10 @@ static void batch_obj_backward_W(const BatchObjWorkspace &ws, const float *iwe, 
 //             (match.any, then a shuffle tree over the peers) and one lane per cell adds them.  At the end one f64
 //             atomic per node component and CTA into [B][2][gh][gw] (in the workspace), then a cast to the f32 output:
 //             no L2 reduction per event and no per-pixel gradient blocks.
-constexpr int kMaxGridNodes = 4096;        // gh gw of the forward and backward
+// The grid-flow average-timestamp loss (evk_grid_flow_timestamp_*) runs the same passes with TS = true: a 20-byte record
+// per event, weight 1, the two v4 reductions of ts_block_add into image pair z = 2 (b J + j) + s and ts_obj_forward_tail;
+// its backward gathers the (A, B) pairs of ts_obj_backward_ab instead of W_b, as flow_ts_event does.
+constexpr int kMaxGridNodes = 4096;       // gh gw of the forward and backward
 constexpr int kMaxGridCandNodes = 12288;   // n_cand gh gw of the candidates pass (96 KB of f32 nodes)
 
 struct GridArgs {
@@ -2069,6 +2072,15 @@ __device__ __forceinline__ void load_nodes(const GridArgs &A, int b, float2 *nod
     __syncthreads();
 }
 
+// the record of one event that a grid-flow pass reads: 16 bytes for the contrast loss, 20 for the timestamp loss (TS)
+template <bool TS>
+__device__ __forceinline__ auto load_grid_event(const EventSource &E, int64_t i)
+{
+    if constexpr (TS) return load_xytup(E, i);
+    else return load_xytp(E, i);
+}
+
+template <bool TS>
 __global__ void __launch_bounds__(kFlowObjThreads) grid_flow_cand_kernel(const GridArgs A)
 {
     extern __shared__ float2 grid_nodes[];   // [J][gh gw]
@@ -2078,17 +2090,23 @@ __global__ void __launch_bounds__(kFlowObjThreads) grid_flow_cand_kernel(const G
     sample_range(A.F.E, b, first, last);
     const int Wc = A.F.C.Wc;
     const int64_t npix = (int64_t)A.F.C.Hc * Wc;
-    float *acc = A.F.acc + (int64_t)b * J * npix * 4;
+    float *acc = A.F.acc + (int64_t)b * J * npix * (TS ? 2 * 8 : 4);   // per canvas: one IWE block or two {S, C} blocks
     unsigned nonfinite = 0;   // bit j: candidate j warped an event to a non-finite position (J <= 32)
-    for_each_event(first, last, [&](int64_t i) { return load_xytp(A.F.E, i); }, [&](int64_t, const EvXYTP &e) {
+    for_each_event(first, last, [&](int64_t i) { return load_grid_event<TS>(A.F.E, i); }, [&](int64_t, const auto &e) {
         const NodeSample s = node_sample(A, e.x, e.y);
         for (int j = 0; j < J; ++j) {
             float u, v;
             node_flow(grid_nodes + j * G, s, u, v);
             Taps T;
             bool nf = false;
-            if (flow_obj_keep(A.F, e.x, e.y, u, v, e.t, e.p, T, nf))
+            if constexpr (TS) {
+                // weight 1; a NaN p is dropped after the non-finite check, as in flow_ts_event
+                const int pol = ts_polarity(e.p);
+                if (flow_obj_keep(A.F, e.x, e.y, u, v, e.t, 1.0f, T, nf) && pol >= 0)
+                    ts_block_add(acc + (int64_t)j * 2 * npix * 8, npix, Wc, pol, T, e.tau);
+            } else if (flow_obj_keep(A.F, e.x, e.y, u, v, e.t, e.p, T, nf)) {
                 red_add4(acc + ((int64_t)j * npix + (int64_t)T.y0 * Wc + T.x0) * 4, T.ti);
+            }
             if (nf) nonfinite |= 1u << j;
         }
     });
@@ -2120,8 +2138,40 @@ __device__ __forceinline__ bool warp_key_sum(int key, float (&v)[8])
     return lane == __ffs(peers) - 1;
 }
 
+// One event's node terms: (gu, gv) = df/d(u, v) times the four node weights of s into val (u taps, then v taps), keyed
+// by the node cell.  Untouched when both are zero.
+__device__ __forceinline__ void node_terms(const NodeSample &s, float gu, float gv, float (&val)[8], int &key)
+{
+    if (gu != 0.0f || gv != 0.0f) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (s.inside >> q & 1u) { val[q] = gu * s.w[q]; val[4 + q] = gv * s.w[q]; }
+        }
+        key = s.cell;
+    }
+}
+
+// The terms of the lanes of the warp with the same key summed (warp_key_sum) and added by one lane per node cell to the
+// CTA's f64 accumulator acc [2][G] in shared memory.  All 32 lanes call this; a lane without a term has its own key.
+__device__ __forceinline__ void node_grad_flush(double *acc, int G, const NodeSample &s, int key, float (&val)[8])
+{
+    if (warp_key_sum(key, val) && key >= 0) {
+        // the peers share the leader's cell and so its taps inside the grid
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (!(s.inside >> q & 1u)) continue;
+            if (val[q] != 0.0f) atomicAdd(acc + s.o[q], (double)val[q]);
+            if (val[4 + q] != 0.0f) atomicAdd(acc + G + s.o[q], (double)val[4 + q]);
+        }
+    }
+}
+
+// The node-gradient pass of both grid-flow losses.  The event loop is written out rather than taken from a lambda-driven
+// helper such as for_each_event: that form costs the contrast pass 3 registers.
+template <bool TS>
 __global__ void __launch_bounds__(kFlowObjThreads) grid_flow_grad_kernel(const GridArgs A)
 {
+    using Ev = decltype(load_grid_event<TS>(A.F.E, 0));
     extern __shared__ double grid_acc[];   // [2][gh gw] f64, then the nodes as [gh gw] {u, v}
     const int b = blockIdx.y, G = A.gh * A.gw;
     float2 *nodes = reinterpret_cast<float2 *>(grid_acc + 2 * G);
@@ -2130,21 +2180,24 @@ __global__ void __launch_bounds__(kFlowObjThreads) grid_flow_grad_kernel(const G
     int64_t first, last;
     sample_range(A.F.E, b, first, last);
     const int Wc = A.F.C.Wc;
-    const float *Wb = A.F.Wimg + (int64_t)b * A.F.C.Hc * Wc;
+    const int64_t npix = (int64_t)A.F.C.Hc * Wc;
+    const float *Wb = TS ? nullptr : A.F.Wimg + b * npix;        // contrast: W_b
+    const float2 *ab = TS ? A.F.ab + b * 2 * npix : nullptr;     // timestamp: the (A, B) pairs of both polarities
     const int lane = threadIdx.x & 31;
     const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
     // warp-uniform trip count (warp_key_sum needs every lane): kBatch records per lane, masked past `last`
     for (int64_t i0 = first + (int64_t)blockIdx.x * kFlowObjThreads + (threadIdx.x - lane); i0 < last; i0 += kBatch * stride) {
-        EvXYTP e[kBatch];
+        Ev ev[kBatch];
 #pragma unroll
         for (int k = 0; k < kBatch; ++k) {
             const int64_t q = i0 + k * stride + lane;
-            e[k] = q < last ? load_xytp(A.F.E, q) : EvXYTP{0.0f, 0.0f, 0.0f, 0.0f};
-            if (!(q < last)) e[k].x = __int_as_float(0x7fc00000);   // a NaN position: no cell, no term
+            ev[k] = q < last ? load_grid_event<TS>(A.F.E, q) : Ev{};
+            if (!(q < last)) ev[k].x = __int_as_float(0x7fc00000);   // a NaN position: no cell, no term
         }
 #pragma unroll
         for (int k = 0; k < kBatch; ++k) {
-            const NodeSample s = node_sample(A, e[k].x, e[k].y);
+            const Ev &e = ev[k];
+            const NodeSample s = node_sample(A, e.x, e.y);
             float val[8];
 #pragma unroll
             for (int q = 0; q < 8; ++q) val[q] = 0.0f;
@@ -2153,7 +2206,24 @@ __global__ void __launch_bounds__(kFlowObjThreads) grid_flow_grad_kernel(const G
             node_flow(nodes, s, u, v);
             Taps T;
             bool nf = false;
-            if (s.cell >= 0 && flow_obj_keep(A.F, e[k].x, e[k].y, u, v, e[k].t, e[k].p, T, nf)) {
+            if constexpr (TS) {
+                // weight 1 and a NaN p dropped, as in flow_ts_event; dF/dk = tau A + B per tap of the event's polarity
+                const int pol = ts_polarity(e.p);
+                if (s.cell >= 0 && flow_obj_keep(A.F, e.x, e.y, u, v, e.t, 1.0f, T, nf) && pol >= 0) {
+                    const float2 *abs_ = pol ? ab + npix : ab;
+                    const float dx = T.dx, dy = T.dy;
+                    const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+                    const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
+                    const float2 a00 = __ldg(abs_ + r0 + T.x0), a01 = __ldg(abs_ + r0 + T.x1), a10 = __ldg(abs_ + r1 + T.x0),
+                                 a11 = __ldg(abs_ + r1 + T.x1);
+                    const float tau = e.tau;
+                    const float q00 = tau * a00.x + a00.y, q01 = tau * a01.x + a01.y, q10 = tau * a10.x + a10.y,
+                                q11 = tau * a11.x + a11.y;
+                    float sx, sy;
+                    tap_slopes(ox, oy, dx, dy, q00, q01, q10, q11, sx, sy);
+                    node_terms(s, sx * e.t, sy * e.t, val, key);
+                }
+            } else if (s.cell >= 0 && flow_obj_keep(A.F, e.x, e.y, u, v, e.t, e.p, T, nf)) {
                 // df/dx' and df/dy' through the four bilinear taps of the IWE, as in flow_obj_event
                 const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
                 const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0),
@@ -2161,24 +2231,9 @@ __global__ void __launch_bounds__(kFlowObjThreads) grid_flow_grad_kernel(const G
                 const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
                 float sx, sy;
                 tap_slopes(ox, oy, T.dx, T.dy, w00, w01, w10, w11, sx, sy);
-                const float gu = T.wm * sx * e[k].t, gv = T.wm * sy * e[k].t;
-                if (gu != 0.0f || gv != 0.0f) {
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        if (s.inside >> q & 1u) { val[q] = gu * s.w[q]; val[4 + q] = gv * s.w[q]; }
-                    }
-                    key = s.cell;
-                }
+                node_terms(s, T.wm * sx * e.t, T.wm * sy * e.t, val, key);
             }
-            if (warp_key_sum(key, val) && key >= 0) {
-                // the peers share the leader's cell and so its taps inside the grid
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    if (!(s.inside >> q & 1u)) continue;
-                    if (val[q] != 0.0f) atomicAdd(grid_acc + s.o[q], (double)val[q]);
-                    if (val[4 + q] != 0.0f) atomicAdd(grid_acc + G + s.o[q], (double)val[4 + q]);
-                }
-            }
+            node_grad_flush(grid_acc, G, s, key, val);
         }
     }
     __syncthreads();
@@ -2196,34 +2251,38 @@ __global__ void __launch_bounds__(256) grid_flow_grad_cast_kernel(const double *
 
 // Shared argument checks and set-up of the grid-flow entries.  n_cand 0: the differentiable entries (one canvas per
 // sample, gh gw <= kMaxGridNodes); else n_cand forward-only canvases per sample (n_cand <= kMaxCandidates,
-// n_cand gh gw <= kMaxGridCandNodes, batch n_cand <= 65535).
-static int grid_flow_limits(int batch, int n_cand, int gh, int gw, int H, int W)
+// n_cand gh gw <= kMaxGridCandNodes).  `images` tail images per canvas (1 for the contrast loss, 2 for the timestamp loss,
+// one per polarity), and at most 65535 images: batch (n_cand) <= 65535 / images.
+static int grid_flow_limits(int batch, int n_cand, int gh, int gw, int H, int W, int images = 1)
 {
     if (batch < 0 || H < 2 || W < 2 || gh < 2 || gw < 2 || gh > H || gw > W) return 0;
-    const int64_t G = (int64_t)gh * gw;
-    if (!n_cand) return batch <= 65535 && G <= kMaxGridNodes;
-    return n_cand >= 1 && n_cand <= kMaxCandidates && (int64_t)n_cand * G <= kMaxGridCandNodes && (int64_t)batch * n_cand <= 65535;
+    const int64_t G = (int64_t)gh * gw, canvases = 65535 / images;
+    if (!n_cand) return batch <= canvases && G <= kMaxGridNodes;
+    return n_cand >= 1 && n_cand <= kMaxCandidates && (int64_t)n_cand * G <= kMaxGridCandNodes && (int64_t)batch * n_cand <= canvases;
 }
 
-static int grid_flow_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const int64_t *offsets,
-                           int batch, int64_t n, const float *grid, int n_cand, int gh, int gw, int H, int W, double sigma,
-                           int objective, void *workspace, size_t workspace_bytes, GridArgs &A, BatchObjWorkspace &ws,
-                           BlurTaps &taps)
+// tau: the timestamp loss's normalised stamps (images 2, with its objective OBJ_SOS and acc_blocks flow_ts_acc_blocks);
+// acc_blocks: 16-byte accumulator blocks per image (batch_obj_carve)
+static int grid_flow_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
+                           const int64_t *offsets, int batch, int64_t n, const float *grid, int n_cand, int gh, int gw, int H, int W,
+                           double sigma, int objective, int images, size_t acc_blocks, void *workspace, size_t workspace_bytes,
+                           GridArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
 {
     if (int rc = check_sigma(who, sigma)) return rc;
-    if (!grid_flow_limits(batch, n_cand, gh, gw, H, W) || n < 0 || (batch > 0 && (!offsets || !grid)) ||
-        (n > 0 && (!x || !y || !t || !p))) {
+    if (!grid_flow_limits(batch, n_cand, gh, gw, H, W, images) || n < 0 || (batch > 0 && (!offsets || !grid)) ||
+        (n > 0 && (!x || !y || !t || (images == 2 && !tau) || !p))) {
         set_error("%s: bad arguments (2 <= gh <= H, 2 <= gw <= W, gh gw <= %d; candidates: 1 <= n_cand <= %d, n_cand gh gw "
-                  "<= %d, batch n_cand <= 65535; else batch <= 65535)", who, kMaxGridNodes, kMaxCandidates, kMaxGridCandNodes);
+                  "<= %d, batch n_cand <= %d; else batch <= %d)", who, kMaxGridNodes, kMaxCandidates, kMaxGridCandNodes,
+                  65535 / images, 65535 / images);
         return EVK_E_ARG;
     }
     const int J = n_cand ? n_cand : 1;
-    int rc = batch_obj_check(who, "flow", batch * J, H, W, sigma, objective, (size_t)(H + 1) * (W + 1), workspace, workspace_bytes,
-                             ws, taps, !n_cand);
+    int rc = batch_obj_check(who, "flow", images * batch * J, H, W, sigma, objective, acc_blocks, workspace, workspace_bytes, ws,
+                             taps, !n_cand);
     if (rc) return rc;
     A = GridArgs{};
     A.F.C.Hc = H + 1; A.F.C.Wc = W + 1;
-    A.F.E = EventSource{x, y, t, p, nullptr, offsets, n};
+    A.F.E = EventSource{x, y, t, p, tau, offsets, n};
     A.F.H = H; A.F.W = W;
     A.F.acc = ws.acc;
     A.F.nonfinite = ws.nonfinite;
@@ -2234,20 +2293,47 @@ static int grid_flow_setup(const char *who, const float *x, const float *y, cons
     return EVK_OK;
 }
 
-// forward and candidates: zero, the event pass, the tail into iwe_out (the candidates: ws.Wimg)
+// forward and candidates, before the tail: zero the counters and the accumulators of the batch J canvases, the event pass
+template <bool TS>
+static int grid_flow_event_pass(const GridArgs &A, const BatchObjWorkspace &ws, int batch, cudaStream_t st)
+{
+    const int npix = A.F.C.Hc * A.F.C.Wc, canvases = batch * A.J;
+    EVK_CUDA(batch_obj_zero(ws, (TS ? 2 : 1) * (int64_t)canvases, npix, TS ? 8 : 4, st));
+    if (A.F.E.n > 0) {
+        const size_t smem = (size_t)A.J * A.gh * A.gw * sizeof(float2);
+        EVK_CUDA(cudaFuncSetAttribute(grid_flow_cand_kernel<TS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ProfScope prof(st);
+        prof_count(1);
+        grid_flow_cand_kernel<TS><<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(A);
+    }
+    return EVK_OK;
+}
+
+// forward and candidates of the contrast loss: the event pass, the tail into iwe_out (the candidates: ws.Wimg)
 static int grid_flow_forward(const GridArgs &A, const BatchObjWorkspace &ws, const BlurTaps &taps, int batch, int objective,
                              double obj_param, float *iwe_out, double *f_out, cudaStream_t st)
 {
-    const int Hc = A.F.C.Hc, Wc = A.F.C.Wc, npix = Hc * Wc, canvases = batch * A.J;
-    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
+    if (int rc = grid_flow_event_pass<false>(A, ws, batch, st)) return rc;
+    batch_obj_forward_tail(ws, A.F.C.Hc, A.F.C.Wc, taps, batch * A.J, objective, obj_param, iwe_out, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+// backward, after the image-space half (which set A.F.Wimg or A.F.ab): the node pass into the f64 sums A.grad (zeroed by
+// the caller), then their cast to grad_grid
+template <bool TS>
+static int grid_flow_node_grad(const GridArgs &A, int batch, float *grad_grid, cudaStream_t st)
+{
+    const int64_t nodes = (int64_t)batch * 2 * A.gh * A.gw;
     if (A.F.E.n > 0) {
-        const size_t smem = (size_t)A.J * A.gh * A.gw * sizeof(float2);
-        EVK_CUDA(cudaFuncSetAttribute(grid_flow_cand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const size_t smem = (size_t)A.gh * A.gw * (2 * sizeof(double) + sizeof(float2));
+        EVK_CUDA(cudaFuncSetAttribute(grid_flow_grad_kernel<TS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ProfScope prof(st);
         prof_count(1);
-        grid_flow_cand_kernel<<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(A);
+        grid_flow_grad_kernel<TS><<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(A);
     }
-    batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, iwe_out, f_out, st);
+    prof_count(1);
+    grid_flow_grad_cast_kernel<<<grid_simple(nodes, 256), 256, 0, st>>>(A.grad, grad_grid, nodes);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }
@@ -3253,8 +3339,8 @@ int evk_cmax_grid_flow_objective_f32(const float *x, const float *y, const float
     GridArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = grid_flow_setup("evk_cmax_grid_flow_objective_f32", x, y, t_rel, p, offsets, batch, n_events, grid_flow, 0, gh, gw, H,
-                             W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    int rc = grid_flow_setup("evk_cmax_grid_flow_objective_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, grid_flow, 0,
+                             gh, gw, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!f_out || !iwe_out)) { set_error("evk_cmax_grid_flow_objective_f32: null output"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
@@ -3271,8 +3357,9 @@ int evk_cmax_grid_flow_objective_grad_f32(const float *x, const float *y, const 
     GridArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = grid_flow_setup("evk_cmax_grid_flow_objective_grad_f32", x, y, t_rel, p, offsets, batch, n_events, grid_flow, 0, gh,
-                             gw, H, W, sigma, objective, workspace, workspace_bytes, A, ws, taps);
+    int rc = grid_flow_setup("evk_cmax_grid_flow_objective_grad_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, grid_flow,
+                             0, gh, gw, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), workspace, workspace_bytes, A, ws,
+                             taps);
     if (rc) return rc;
     if (batch > 0 && (!iwe || !grad_f || !grad_grid)) {
         set_error("evk_cmax_grid_flow_objective_grad_f32: null array");
@@ -3286,17 +3373,7 @@ int evk_cmax_grid_flow_objective_grad_f32(const float *x, const float *y, const 
     EVK_CUDA(cudaMemsetAsync(A.grad, 0, (size_t)nodes * sizeof(double), st));
     batch_obj_backward_W(ws, iwe, H + 1, W + 1, taps, batch, objective, obj_param, grad_f, st);
     A.F.Wimg = ws.Wimg;
-    if (n_events > 0) {
-        const size_t smem = (size_t)gh * gw * (2 * sizeof(double) + sizeof(float2));
-        EVK_CUDA(cudaFuncSetAttribute(grid_flow_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ProfScope prof(st);
-        prof_count(1);
-        grid_flow_grad_kernel<<<batch_grid(n_events, batch), kFlowObjThreads, smem, st>>>(A);
-    }
-    prof_count(1);
-    grid_flow_grad_cast_kernel<<<grid_simple(nodes, 256), 256, 0, st>>>(A.grad, grad_grid, nodes);
-    EVK_CUDA(cudaGetLastError());
-    return EVK_OK;
+    return grid_flow_node_grad<false>(A, batch, grad_grid, st);
 }
 
 size_t evk_cmax_grid_flow_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
@@ -3314,9 +3391,9 @@ int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const floa
     GridArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = grid_flow_setup("evk_cmax_grid_flow_candidates_f32", x, y, t_rel, p, offsets, batch, n_events, cand,
-                             n_cand < 1 ? -1 : n_cand, gh, gw, H, W, blur_sigma, objective, workspace, workspace_bytes, A, ws,
-                             taps);
+    int rc = grid_flow_setup("evk_cmax_grid_flow_candidates_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, cand,
+                             n_cand < 1 ? -1 : n_cand, gh, gw, H, W, blur_sigma, objective, 1, (size_t)(H + 1) * (W + 1), workspace,
+                             workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && !f_out) { set_error("evk_cmax_grid_flow_candidates_f32: null output"); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
@@ -3753,6 +3830,94 @@ int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const fl
     }
     float *cnt = reinterpret_cast<float *>(static_cast<char *>(workspace) + motion_ts_cand_head(images, H, W));
     ts_obj_forward_tail(ws, Hc, Wc, taps, batch * n_cand, ws.Wimg, cnt, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_grid_flow_timestamp_objective_workspace_bytes(int batch, int gh, int gw, int H, int W)
+{
+    if (!evk::grid_flow_limits(batch, 0, gh, gw, H, W, 2)) return 0;
+    return evk::batch_obj_carve(nullptr, 2 * batch, H, W, evk::flow_ts_acc_blocks(H, W), nullptr);
+}
+
+int evk_grid_flow_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                          const int64_t *offsets, int batch, int64_t n_events, const float *grid_flow, int gh,
+                                          int gw, int H, int W, double sigma, double *f_out, float *ts_out, float *cnt_out,
+                                          void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_grid_flow_timestamp_objective_f32";
+    GridArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = grid_flow_setup(who, x, y, t_rel, tau, p, offsets, batch, n_events, grid_flow, 0, gh, gw, H, W, sigma, OBJ_SOS, 2,
+                             flow_ts_acc_blocks(H, W), workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !ts_out || !cnt_out)) { set_error("%s: null output", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if ((rc = grid_flow_event_pass<true>(A, ws, batch, st))) return rc;
+    ts_obj_forward_tail(ws, H + 1, W + 1, taps, batch, ts_out, cnt_out, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_grid_flow_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                               const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                               const float *grid_flow, int gh, int gw, int H, int W, double sigma,
+                                               const float *ts_img, const float *cnt_img, const float *grad_f, float *grad_grid,
+                                               void *workspace, size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_grid_flow_timestamp_objective_grad_f32";
+    GridArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = grid_flow_setup(who, x, y, t_rel, tau, p, offsets, batch, n_events, grid_flow, 0, gh, gw, H, W, sigma, OBJ_SOS, 2,
+                             flow_ts_acc_blocks(H, W), workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!ts_img || !cnt_img || !grad_f || !grad_grid)) { set_error("%s: null array", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // the f64 node sums live in the accumulator, which the backward has no other use for (ts_obj_backward_ab writes
+    // ws.Wimg and ws.wt): 2 batch 2 (H+1)(W+1) 16 B >= batch 2 gh gw 8 B
+    A.grad = reinterpret_cast<double *>(ws.acc);
+    EVK_CUDA(cudaMemsetAsync(A.grad, 0, (size_t)batch * 2 * gh * gw * sizeof(double), st));
+    A.F.ab = ts_obj_backward_ab(ws, ts_img, cnt_img, H + 1, W + 1, taps, batch, grad_f, st);
+    return grid_flow_node_grad<true>(A, batch, grad_grid, st);
+}
+
+size_t evk_grid_flow_timestamp_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
+{
+    if (!evk::grid_flow_limits(batch, n_cand, gh, gw, H, W, 2)) return 0;
+    return evk::motion_ts_cand_bytes(2 * batch * n_cand, H, W);
+}
+
+int evk_grid_flow_timestamp_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                           const int64_t *offsets, int batch, int64_t n_events, const float *cand, int n_cand,
+                                           int gh, int gw, int H, int W, double blur_sigma, double *f_out, void *workspace,
+                                           size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_grid_flow_timestamp_candidates_f32";
+    GridArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = grid_flow_setup(who, x, y, t_rel, tau, p, offsets, batch, n_events, cand, n_cand < 1 ? -1 : n_cand, gh, gw, H, W,
+                             blur_sigma, OBJ_SOS, 2, flow_ts_acc_blocks(H, W), workspace, workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    const int images = 2 * batch * n_cand;
+    if (workspace_bytes < motion_ts_cand_bytes(images, H, W)) {
+        set_error("%s: 256-byte aligned workspace of %zu bytes required", who, motion_ts_cand_bytes(images, H, W));
+        return EVK_E_WORKSPACE;
+    }
+    if (batch > 0 && !f_out) { set_error("%s: null output", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if ((rc = grid_flow_event_pass<true>(A, ws, batch, st))) return rc;
+    // T goes to ws.Wimg and C behind the forward-only carve, as in evk_motion_timestamp_candidates_f32
+    float *cnt = reinterpret_cast<float *>(static_cast<char *>(workspace) + motion_ts_cand_head(images, H, W));
+    ts_obj_forward_tail(ws, H + 1, W + 1, taps, batch * n_cand, ws.Wimg, cnt, f_out, st);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }

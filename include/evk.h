@@ -744,6 +744,51 @@ int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const fl
                                         double blur_sigma, double *f_out, void *workspace, size_t workspace_bytes,
                                         void *stream);
 
+/* The dense-flow average-timestamp loss with the flow of every sample given on a coarse grid of nodes: the node grid,
+ * its interpolation and limits of evk_cmax_grid_flow_objective_f32 (grid_flow: [batch][2][gh][gw] f32 on the device,
+ * 2 <= gh <= H, 2 <= gw <= W, gh * gw <= 4096; align_corners nodes, f32 ratios rx, ry, zero for node taps outside the
+ * grid), then everything of evk_flow_timestamp_objective_f32 at the interpolated flow: x' = x + u t_rel,
+ * y' = y + v t_rel in f32, kept iff 0 <= x' < W and 0 <= y' < H, a NaN f for a sample with a non-finite x' or y', a
+ * NaN p dropped, the T and C images per polarity, the blur and f_b = sum G(T_+)^2 + sum G(T_-)^2.  For events at
+ * integer pixels inside the sensor, f equals the dense-flow f of the flow that bilinear upsampling with align_corners
+ * makes of the nodes, to f32 rounding; at gh = H, gw = W the grid is the dense flow.
+ *   f_out: batch doubles;  ts_out, cnt_out: [batch][2][H+1][W+1] floats, which the backward takes as ts_img, cnt_img.
+ *   0 <= batch <= 32767.
+ * evk_grid_flow_timestamp_objective_grad_f32 writes grad_grid [batch][2][gh][gw] floats = grad_f[b] df_b/dgrid_flow[b]:
+ * df/dx' and df/dy' of evk_flow_timestamp_objective_grad_f32, times t_rel, spread over the event's four node taps with
+ * their bilinear weights, summed per CTA in shared memory and across CTAs in f64, then rounded to f32.
+ * workspace: evk_grid_flow_timestamp_objective_workspace_bytes(batch, gh, gw, H, W) bytes, 256-byte aligned, for
+ * either call; 0 for arguments the entries reject.  All limits and the blur-sigma rule are checked before any CUDA
+ * call.  Neither call synchronises, and both launch the same kernels whatever the batch. */
+size_t evk_grid_flow_timestamp_objective_workspace_bytes(int batch, int gh, int gw, int H, int W);
+int evk_grid_flow_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                          const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                          const float *grid_flow, int gh, int gw, int H, int W, double blur_sigma,
+                                          double *f_out, float *ts_out, float *cnt_out, void *workspace,
+                                          size_t workspace_bytes, void *stream);
+int evk_grid_flow_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                               const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                               const float *grid_flow, int gh, int gw, int H, int W, double blur_sigma,
+                                               const float *ts_img, const float *cnt_img, const float *grad_f,
+                                               float *grad_grid, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Many node grids per sample in one pass over the events, for the grid-flow average-timestamp loss (a batched line
+ * search of a grid-flow fit): f_out[b][j] is exactly the f_b of evk_grid_flow_timestamp_objective_f32 with
+ * grid_flow[b] = cand[b][j].  A non-finite warped position makes only that candidate's f NaN.
+ *   cand : [batch][n_cand][2][gh][gw] floats on the device, 1 <= n_cand <= 32, n_cand * gh * gw <= 12288,
+ *          batch * n_cand <= 32767
+ *   f_out: [batch][n_cand] doubles
+ * Every event is read once; its node cell and weights are computed once and used for every candidate.  All limits are
+ * checked before any CUDA call.  Forward only.  workspace: evk_grid_flow_timestamp_candidates_workspace_bytes(batch,
+ * n_cand, gh, gw, H, W) bytes (about 96 bytes per canvas pixel and candidate), 256-byte aligned; 0 for arguments the
+ * entry rejects.  The call does not synchronise and launches the same kernels whatever batch and n_cand. */
+size_t evk_grid_flow_timestamp_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W);
+int evk_grid_flow_timestamp_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                           const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                           const float *cand, int n_cand, int gh, int gw, int H, int W,
+                                           double blur_sigma, double *f_out, void *workspace, size_t workspace_bytes,
+                                           void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * RobustNorm (row f4): clamp a tensor between two of its order statistics and rescale it.  Replaces
  * RobustNorm.__call__ / .percentile, lib/data_loaders/data_augmentation.py:82-130 (two kthvalue sorts),
