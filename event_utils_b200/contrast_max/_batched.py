@@ -8,11 +8,13 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from .warps import linvel_warp, pure_rotation_warp, xyztheta_warp
+from .warps import affine_warp, homography_warp, linvel_warp, pure_rotation_warp, xyztheta_warp
 
 OBJECTIVES = {"variance": _lib.OBJ_VARIANCE, "sos": _lib.OBJ_SOS, "soe": _lib.OBJ_SOE, "sosa": _lib.OBJ_SOSA}
 DEFAULT_PARAM = {"sosa": 3.0}   # sosa_objective(p=3)
-_WARPS = ((linvel_warp, _lib.WARP_LINVEL), (pure_rotation_warp, _lib.WARP_ROTATION), (xyztheta_warp, _lib.WARP_XYZTHETA))
+_WARPS = ((linvel_warp, _lib.WARP_LINVEL), (pure_rotation_warp, _lib.WARP_ROTATION), (xyztheta_warp, _lib.WARP_XYZTHETA),
+          (affine_warp, _lib.WARP_AFFINE), (homography_warp, _lib.WARP_HOMOGRAPHY))
+_CENTRED = (_lib.WARP_XYZTHETA, _lib.WARP_AFFINE, _lib.WARP_HOMOGRAPHY)   # the models about a fixed centre (cx, cy)
 MAX_CANDIDATES = 32   # parameter vectors per window and pass over the events
 MAX_GRID_CANDIDATE_NODES = 12288   # candidates times nodes of a grid-flow candidates pass (the grids a CTA holds)
 
@@ -28,21 +30,21 @@ def _check_objective(objective, wrt):
 def _warp_code(warpfunc, who):
     warp = next((code for cls, code in _WARPS if type(warpfunc) is cls), None)
     if warp is None:
-        raise ValueError("%s supports the models linvel_warp, pure_rotation_warp and xyztheta_warp, got %s"
-                         % (who, type(warpfunc).__name__))
+        raise ValueError("%s supports the models linvel_warp, pure_rotation_warp and xyztheta_warp and the planar models "
+                         "affine_warp and homography_warp, got %s" % (who, type(warpfunc).__name__))
     return warp
 
 
 def _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W):
     """the scalar arguments the motion entries share: (warp code, (cx, cy), H, W, objective code, sigma, obj_param)"""
-    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
+    centre = tuple(float(c) for c in warpfunc.center) if warp in _CENTRED else (0.0, 0.0)
     param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
     return warp, centre, H, W, OBJECTIVES[objective], float(blur_sigma), param
 
 
 def _ts_model(warp, warpfunc, blur_sigma, H, W):
     """the scalar arguments the motion timestamp entries share: (warp code, (cx, cy), H, W, sigma)"""
-    centre = tuple(float(c) for c in warpfunc.center) if warp == _lib.WARP_XYZTHETA else (0.0, 0.0)
+    centre = tuple(float(c) for c in warpfunc.center) if warp in _CENTRED else (0.0, 0.0)
     return warp, centre, H, W, float(blur_sigma)
 
 

@@ -26,6 +26,9 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
         linvel_warp         (vx, vy)              x' = x - d vx,  y' = y - d vy               (warps.py:51-61)
         pure_rotation_warp  (cx, cy, omega)       rotation about (cx, cy) by omega d
         xyztheta_warp       (hx, hy, hz, theta)   about warpfunc.center
+        affine_warp         (hx, hy, a11, a12, a21, a22)            about warpfunc.center (warps.py has the formulas)
+        homography_warp     (hx, hy, a11, a12, a21, a22, g1, g2)    about warpfunc.center; an event past the horizon
+                                                                    (w <= 0) is not kept
     An event is kept iff 0 < x' <= W and 0 < y' <= H with (H, W) = img_size (events_bounds_mask, event_util.py:26-27; a
     NaN position compares false and is kept, then contributes nothing, as in the single-window evaluation) and is splatted
     bilinearly on the (H+1, W+1) canvas (events_to_image_drv, image.py:179-217).  Then G = gaussian_filter(IWE,
@@ -41,7 +44,7 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
     @param xs, ys, ts, ps the concatenated events, (N,) tensors or arrays; they are data, not differentiable
     @param params (B,K) or (K,) for one sample, K = warpfunc.dims, any float dtype; the only differentiable input
            (expanded views work)
-    @param warpfunc an instance of linvel_warp, pure_rotation_warp or xyztheta_warp
+    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp or homography_warp
     @param t0 None (each sample's last timestamp, get_iwe's ts[-1]), a number, or B values
     @param batch_end_indices the cumulative end indices of BaseVoxelDataset.collate_fn
            (lib/data_loaders/base_dataset.py:513-539), a list or an int64 tensor; None means one sample of all events

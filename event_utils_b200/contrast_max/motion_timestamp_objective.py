@@ -27,6 +27,7 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
              linvel_warp         (vx, vy)              x' = x - d vx,  y' = y - d vy               (warps.py:51-61)
              pure_rotation_warp  (cx, cy, omega)       rotation about (cx, cy) by omega d
              xyztheta_warp       (hx, hy, hz, theta)   about warpfunc.center
+             affine_warp, homography_warp           about warpfunc.center (warps.py; past the horizon: not kept)
       2. tau = (t - t_first_b) / (t_last_b - t_first_b + 1e-6), or (-t + t_last_b) / (...) with timestamp_reverse
          (image.py:324-327), formed in ts' dtype, then f32, as flow_timestamp_objective_torch forms it.
       3. An event contributes iff its f32 x', y' are finite, 0 < x' < W and 0 < y' < H with (H, W) = img_size: those are
@@ -43,7 +44,7 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
     @param xs, ys, ts, ps the concatenated events, (N,) tensors or arrays; they are data, not differentiable
     @param params (B,K) or (K,) for one sample, K = warpfunc.dims, any float dtype; the only differentiable input
            (expanded views work)
-    @param warpfunc an instance of linvel_warp, pure_rotation_warp or xyztheta_warp
+    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp or homography_warp
     @param t0 None (each sample's last timestamp, zhu_timestamp_objective's ts[-1]), a number, or B values
     @param img_size (H, W): the bounds of step 3 and the canvas (H+1, W+1)
     @param batch_end_indices the cumulative end indices of BaseVoxelDataset.collate_fn

@@ -121,3 +121,90 @@ class xyztheta_warp(warp_function):
         jx = np.stack((-dt, nothing, -(dt * u), dt * v))
         jy = np.stack((nothing, -dt, -(dt * v), -(dt * u)))
         return xw, yw, jx, jy
+
+
+class affine_warp(warp_function):
+    """6-DoF affine motion in its first-order form about a fixed centre, params = (hx, hy, a11, a12, a21, a22): the
+    image-plane velocity of a point at (u, v) = (x - cx, y - cy) is (hx + a11 u + a12 v, hy + a21 u + a22 v).  It is the
+    usual model for tracking an object or a patch that shears or scales unevenly.
+        sx = (hx + a11 u) + a12 v,      sy = (hy + a22 v) + a21 u
+        x' = x - dt sx,                 y' = y - dt sy
+        d x'/dp = (-dt, 0, -dt u, -dt v, 0, 0)      d y'/dp = (0, -dt, 0, 0, -dt u, -dt v)
+    f64 numpy in the order written.  The batched losses, fits and segmentation evaluate it natively on the GPU; the
+    reference-API objectives (variance_objective, get_iwe, ...) take it through this warp() (fused_kind None).
+
+    xyztheta_warp(hx, hy, hz, theta) is affine_warp(hx, hy, hz, -theta, theta, hz) bit for bit with the same centre
+    (a + (-b) v is a - b v in IEEE arithmetic), so a 4-DoF fit embedded that way is the starting point of an affine
+    fit.  A grid search over K = 6 parameters scores num_samples_per_param ** 6 points per window (15625 at 5 samples
+    per parameter): start from an embedded 4-DoF fit instead."""
+
+    def __init__(self, center=(120.0, 90.0)):
+        super().__init__('affine_warp', 6)
+        self.center = (float(center[0]), float(center[1]))
+
+    def model(self, params):
+        """the parameter block of the batched GPU evaluation: the 6 parameters, then the centre"""
+        return [float(v) for v in params[:6]] + list(self.center)
+
+    def warp(self, xs, ys, ts, ps, t0, params, compute_grad=False):
+        hx, hy, a11, a12, a21, a22 = (float(v) for v in params[:6])
+        cx, cy = self.center
+        dt = ts - t0
+        u, v = xs - cx, ys - cy
+        sx, sy = (hx + a11 * u) + a12 * v, (hy + a22 * v) + a21 * u
+        xw, yw = xs - dt * sx, ys - dt * sy
+        if not compute_grad:
+            return xw, yw, None, None
+        nothing = np.zeros_like(dt, dtype=np.float64)
+        du, dv = dt * u, dt * v
+        jx = np.stack((-dt, nothing, -du, -dv, nothing, nothing))
+        jy = np.stack((nothing, -dt, nothing, nothing, -du, -dv))
+        return xw, yw, jx, jy
+
+
+class homography_warp(warp_function):
+    """8-DoF homography in its first-order form about a fixed centre, params = (hx, hy, a11, a12, a21, a22, g1, g2): the
+    generator A = [[a11, a12, hx], [a21, a22, hy], [g1, g2, 0]] acts on (u, v, 1) = (x - cx, y - cy, 1), and a33 = 0
+    fixes the scale, so the 8 values are a chart of the homography's Lie algebra.  It is the motion of a planar scene
+    (or of any scene under a rotating camera, Gallego et al., CVPR 2018).  The warp undoes the motion during dt:
+        sx, sy as affine_warp,   nx = u - dt sx,   ny = v - dt sy
+        q = dt ((g1 u) + (g2 v)),   w = 1 - q
+        x' = (x - dt sx) + nx q / w,      y' = (y - dt sy) + ny q / w          (= cx + nx / w, cy + ny / w)
+        d x'/d(hx, .., a22) = affine_warp's row / w,   d x'/d(g1, g2) = (nx dt u, nx dt v) / w^2   (y' with ny)
+    f64 numpy in the order written.  An event with w <= 0 has crossed the horizon: the batched losses drop it like an
+    event off the canvas (no contribution, no gradient); this warp() returns its formula unchanged, which the reference
+    API's bounds mask then judges.  The batched losses, fits and segmentation evaluate the model natively on the GPU;
+    the reference-API objectives take it through this warp() (fused_kind None).
+
+    With g1 = g2 = 0 (w = 1) this is affine_warp bit for bit, so an affine fit -- or a 4-DoF fit embedded as
+    (hx, hy, hz, -theta, theta, hz), see affine_warp -- extended by g = (0, 0) is the starting point of a homography
+    fit.  A grid search over K = 8 parameters scores num_samples_per_param ** 8 points per window (390625 at 5 samples
+    per parameter): start from an embedded fit instead."""
+
+    def __init__(self, center=(120.0, 90.0)):
+        super().__init__('homography_warp', 8)
+        self.center = (float(center[0]), float(center[1]))
+
+    def model(self, params):
+        """the parameter block of the batched GPU evaluation: the 8 parameters, then the centre"""
+        return [float(v) for v in params[:8]] + list(self.center)
+
+    def warp(self, xs, ys, ts, ps, t0, params, compute_grad=False):
+        hx, hy, a11, a12, a21, a22, g1, g2 = (float(v) for v in params[:8])
+        cx, cy = self.center
+        dt = ts - t0
+        u, v = xs - cx, ys - cy
+        sx, sy = (hx + a11 * u) + a12 * v, (hy + a22 * v) + a21 * u
+        mx, my = dt * sx, dt * sy
+        nx, ny = u - mx, v - my
+        q = dt * (g1 * u + g2 * v)
+        w = 1.0 - q
+        with np.errstate(divide="ignore", invalid="ignore"):
+            xw, yw = (xs - mx) + nx * q / w, (ys - my) + ny * q / w
+            if not compute_grad:
+                return xw, yw, None, None
+            nothing = np.zeros_like(dt, dtype=np.float64)
+            du, dv, w2 = dt * u, dt * v, w * w
+            jx = np.stack((-dt / w, nothing, -du / w, -dv / w, nothing, nothing, nx * du / w2, nx * dv / w2))
+            jy = np.stack((nothing, -dt / w, nothing, nothing, -du / w, -dv / w, ny * du / w2, ny * dv / w2))
+        return xw, yw, jx, jy

@@ -61,9 +61,12 @@ struct BlurTaps {
 
 // Parameters of the rotation / 4-DoF motion models (host order of evk_cmax_warp_objective_*):
 //   rotation  {cx, cy, omega}                  xyztheta  {hx, hy, hz, theta, cx, cy}
-struct WarpModel {
-    double m[6];
+// The batched passes hold ModelOf<WARP> (below), which is this block for every model of up to 4 parameters.
+template <int N>
+struct ModelParams {
+    double m[N];
 };
+using WarpModel = ModelParams<6>;
 
 struct CmaxArgs {
     const void *x, *y, *t, *p;
@@ -85,12 +88,26 @@ struct CmaxArgs {
 };
 
 enum { WARP_LINVEL_F64 = 0, WARP_LINVEL_F32 = 1, WARP_FLOW_F32 = 2,
-       WARP_ROTATION_F64 = 3, WARP_ROTATION_F32 = 4, WARP_XYZTHETA_F64 = 5, WARP_XYZTHETA_F32 = 6 };
+       WARP_ROTATION_F64 = 3, WARP_ROTATION_F32 = 4, WARP_XYZTHETA_F64 = 5, WARP_XYZTHETA_F32 = 6,
+       WARP_AFFINE_F32 = 7, WARP_HOMOGRAPHY_F32 = 8 };
 
 __host__ __device__ constexpr bool is_model_warp(int w) { return w >= WARP_ROTATION_F64; }
 __host__ __device__ constexpr bool is_rotation(int w) { return w == WARP_ROTATION_F64 || w == WARP_ROTATION_F32; }
 __host__ __device__ constexpr bool is_linvel(int w) { return w == WARP_LINVEL_F64 || w == WARP_LINVEL_F32; }
-__host__ __device__ constexpr int model_dims(int w) { return is_linvel(w) ? 2 : is_rotation(w) ? 3 : 4; }
+__host__ __device__ constexpr bool is_planar(int w) { return w == WARP_AFFINE_F32 || w == WARP_HOMOGRAPHY_F32; }
+__host__ __device__ constexpr int model_dims(int w)
+{
+    return is_linvel(w) ? 2 : is_rotation(w) ? 3 : w == WARP_AFFINE_F32 ? 6 : w == WARP_HOMOGRAPHY_F32 ? 8 : 4;
+}
+// length of the Jacobian rows model_taps fills (at least 4: the smaller models keep the rows they always had)
+__host__ __device__ constexpr int jac_dims(int w) { return model_dims(w) > 4 ? model_dims(w) : 4; }
+
+// The parameter block of a model as model_taps reads it: the K parameters, then the fixed centre (cx, cy) of xyztheta
+// and the planar models.  At least 6 doubles (WarpModel, the block of the single-window entries and of every model of
+// up to 4 parameters); the planar models take K + 2, so that the smaller models keep their registers and shared memory.
+__host__ __device__ constexpr int model_slots(int w) { return model_dims(w) + 2 > 6 ? model_dims(w) + 2 : 6; }
+template <int WARP>
+using ModelOf = ModelParams<model_slots(WARP)>;
 
 // bilinear splat of weight w (and derivative weight a) at (xf, yf) on the canvas:
 // image.py:199-207 (IWE) and :131-135 (derivative images) with w1 = [a;0], w2 = [0;a].
@@ -273,6 +290,16 @@ __device__ __forceinline__ void ld_vec16(const double *p, double (&v)[2])
 //     dy'/d(hx, hy, hz, theta) = (0, -dt, -dt v, -dt u)
 //   linvel (vx, vy), warps.py:51-61 (the batched motion objective; the single-window linvel entries keep their own
 //   fused pass, cmax_event):  x' = x - dt vx,  y' = y - dt vy,  dx'/d(vx, vy) = (-dt, 0),  dy'/d(vx, vy) = (0, -dt)
+//   affine (hx, hy, a11, a12, a21, a22) about the fixed centre (cx, cy), the batched passes only (f32):
+//     sx = (hx + a11 u) + a12 v,  sy = (hy + a22 v) + a21 u,  x' = x - dt sx,  y' = y - dt sy
+//     dx'/dp = (-dt, 0, -dt u, -dt v, 0, 0)      dy'/dp = (0, -dt, 0, 0, -dt u, -dt v)
+//   homography (hx, hy, a11, a12, a21, a22, g1, g2): the first-order warp of the generator
+//   [[a11, a12, hx], [a21, a22, hy], [g1, g2, 0]] on (u, v, 1), the batched passes only (f32):
+//     nx = u - dt sx,  ny = v - dt sy,  q = dt ((g1 u) + (g2 v)),  w = 1 - q
+//     x' = (x - dt sx) + nx q / w,  y' = (y - dt sy) + ny q / w        (= cx + nx / w, cy + ny / w)
+//     dx'/d(hx .. a22) = affine's row / w,  dx'/d(g1, g2) = (nx dt u, nx dt v) / w^2  (y' likewise with ny)
+//     An event with w <= 0 or a non-finite w has crossed the horizon and is not kept.  With g1 = g2 = 0, w is 1 and
+//     the warp and Jacobian are affine's bit for bit; affine at (hx, hy, hz, -theta, theta, hz) is xyztheta's.
 // in the order written (no FMA: the library builds with -fmad=false), f64 in parity mode, f32 in fast mode.
 // THE one place that turns an event into its bilinear footprint for these models: warp, bounds mask
 // (event_util.py:26-27), f64 -> f32 cast (image.py:180-183) and splat_taps -- the IWE pass and the gradient
@@ -281,8 +308,8 @@ __device__ __forceinline__ void sin_cos(double a, double *s, double *c) { sincos
 __device__ __forceinline__ void sin_cos(float a, float *s, float *c) { sincosf(a, s, c); }
 
 template <int WARP, bool JAC>
-__device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> &e, const WarpModel &M, unsigned &oob, Taps &T,
-                                           float (&jx)[4], float (&jy)[4])
+__device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> &e, const ModelOf<WARP> &M, unsigned &oob,
+                                           Taps &T, float (&jx)[jac_dims(WARP)], float (&jy)[jac_dims(WARP)])
 {
     using R = typename EvT<WARP>::type;
     R p = e.p;
@@ -312,6 +339,35 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
             jy[0] = (float)s; jy[1] = (float)((R)1 - c); jy[2] = (float)(-(d * rx));
             jx[3] = jy[3] = 0.0f;
         }
+    } else if constexpr (is_planar(WARP)) {
+        constexpr int K = model_dims(WARP);
+        const R hx = (R)M.m[0], hy = (R)M.m[1], a11 = (R)M.m[2], a12 = (R)M.m[3], a21 = (R)M.m[4], a22 = (R)M.m[5];
+        const R cx = (R)M.m[K], cy = (R)M.m[K + 1];
+        const R u = e.x - cx, v = e.y - cy;
+        const R sx = (hx + a11 * u) + a12 * v, sy = (hy + a22 * v) + a21 * u;
+        const R mx = d * sx, my = d * sy;
+        xw = e.x - mx;
+        yw = e.y - my;
+        const R du = d * u, dv = d * v;
+        if constexpr (WARP == WARP_HOMOGRAPHY_F32) {
+            const R g1 = (R)M.m[6], g2 = (R)M.m[7];
+            const R nx = u - mx, ny = v - my;
+            const R q = d * (g1 * u + g2 * v);
+            const R w = (R)1 - q;
+            if (!(w > (R)0) || isinf(w)) return false;   // past the horizon: not kept, like an event off the canvas
+            xw = xw + nx * q / w;
+            yw = yw + ny * q / w;
+            if (JAC) {
+                const R w2 = w * w;
+                jx[0] = -d / w; jx[1] = 0.0f; jx[2] = -du / w; jx[3] = -dv / w; jx[4] = 0.0f; jx[5] = 0.0f;
+                jy[0] = 0.0f; jy[1] = -d / w; jy[2] = 0.0f; jy[3] = 0.0f; jy[4] = -du / w; jy[5] = -dv / w;
+                jx[6] = nx * du / w2; jx[7] = nx * dv / w2;
+                jy[6] = ny * du / w2; jy[7] = ny * dv / w2;
+            }
+        } else if (JAC) {
+            jx[0] = -d; jx[1] = 0.0f; jx[2] = -du; jx[3] = -dv; jx[4] = 0.0f; jx[5] = 0.0f;
+            jy[0] = 0.0f; jy[1] = -d; jy[2] = 0.0f; jy[3] = 0.0f; jy[4] = -du; jy[5] = -dv;
+        }
     } else {
         const R hx = (R)M.m[0], hy = (R)M.m[1], hz = (R)M.m[2], th = (R)M.m[3], cx = (R)M.m[4], cy = (R)M.m[5];
         const R u = e.x - cx, v = e.y - cy;
@@ -334,7 +390,7 @@ __device__ __forceinline__ void model_splat(const CmaxArgs &A, float *acc, const
                                             unsigned *simg)
 {
     Taps T;
-    float jx[4], jy[4];
+    float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
     if (!model_taps<WARP, false>(A, e, M, oob, T, jx, jy)) return;
     if (ONCHIP && fabsf(T.wm) <= 1.0f) {
         const int r0 = T.y0 * A.Wc, r1 = T.y1 * A.Wc;
@@ -636,7 +692,7 @@ __global__ void __launch_bounds__(kGradThreads, 1) cmax_grad_pass_kernel(const C
     unsigned oob = 0;   // counted by pass 1
     auto one = [&](const Event<WARP> &e) {
         Taps T;
-        float jx[4], jy[4];
+        float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
         if (!model_taps<WARP, true>(A, e, A.model, oob, T, jx, jy)) return;
         const int r0 = T.y0 * A.Wc, r1 = T.y1 * A.Wc;
         const double w00 = sW[r0 + T.x0], w01 = sW[r0 + T.x1], w10 = sW[r1 + T.x0], w11 = sW[r1 + T.x1];
@@ -1624,24 +1680,25 @@ __device__ __forceinline__ void for_each_event_batch(int64_t first, int64_t last
     }
 }
 
-// Model `index` of params [..][K] into M as model_taps reads it (xyztheta also takes the fixed centre), and `count`
-// consecutive models from `first` into shared memory for the whole CTA.  M is filled in place: a model returned by value
-// costs the linvel forward pass two registers.
+// Model `index` of params [..][K] into M as model_taps reads it (xyztheta and the planar models also take the fixed
+// centre, behind their K parameters), and `count` consecutive models from `first` into shared memory for the whole CTA.
+// M is filled in place: a model returned by value costs the linvel forward pass two registers.
 template <int WARP>
-__device__ __forceinline__ void load_model(const double *params, int64_t index, double cx, double cy, WarpModel &M)
+__device__ __forceinline__ void load_model(const double *params, int64_t index, double cx, double cy, ModelOf<WARP> &M)
 {
     constexpr int K = model_dims(WARP);
-    M = WarpModel{};
+    M = ModelOf<WARP>{};
 #pragma unroll
     for (int k = 0; k < K; ++k) M.m[k] = params[index * K + k];
-    if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[4] = cx; M.m[5] = cy; }
+    if (!is_linvel(WARP) && !is_rotation(WARP)) { M.m[K] = cx; M.m[K + 1] = cy; }
 }
 
 template <int WARP>
-__device__ __forceinline__ void load_models(const double *params, int64_t first, int count, double cx, double cy, WarpModel *mod)
+__device__ __forceinline__ void load_models(const double *params, int64_t first, int count, double cx, double cy,
+                                            ModelOf<WARP> *mod)
 {
     for (int q = threadIdx.x; q < count; q += kFlowObjThreads) {
-        WarpModel M;
+        ModelOf<WARP> M;
         load_model<WARP>(params, first + q, cx, cy, M);
         mod[q] = M;
     }
@@ -2339,8 +2396,8 @@ static int grid_flow_node_grad(const GridArgs &A, int batch, float *grad_grid, c
 }
 
 // ---- parametric motion objective over a batch of samples (evk_cmax_motion_objective_f32 / _grad_f32) ---------------
-// Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by its own model params[b] -- linvel, rotation
-// or xyztheta through model_taps, with the bounds mask of event_util.py:26-27 at img_size = (H, W) and the splat of
+// Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by its own model params[b] -- linvel, rotation,
+// xyztheta, affine or homography through model_taps, with the bounds mask of event_util.py:26-27 at img_size = (H, W) and the splat of
 // image.py:179-217 on the (H+1)x(W+1) canvas -- then blurred and scored by the flow objective's image-space tail.  The
 // grid of both event passes is (slices, batch), as for the flow objective:
 //   forward:  one v4 reduction per kept event into the sample's 2x2-block image [B][Hc][Wc][4] (16 B per pixel)
@@ -2352,7 +2409,7 @@ struct ModelArgs {
     CmaxArgs C;              // canvas (Hc, Wc) and bounds mask (Hm, Wm) for model_taps; p_scale 1, t_ref 0
     EventSource E;
     const double *params;    // [B][M][J][K] on the device (M models per sample when segmenting, J candidates per model)
-    double cx, cy;           // the centre of xyztheta
+    double cx, cy;           // the centre of xyztheta and the planar models
     int M, J;
     float *acc;              // forward: the canvases' blocks
     const float *Wimg;       // contrast backward: W of every canvas [B][M][Hc][Wc]
@@ -2377,7 +2434,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_obj_event_kernel(const
     int64_t first, last;
     sample_range(A.E, b, first, last);
     const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
-    WarpModel M;
+    ModelOf<WARP> M;
     load_model<WARP>(A.params, b, A.cx, A.cy, M);
     float *acc = GRAD ? nullptr : A.acc + b * npix * 4;
     const float *Wb = GRAD ? A.Wimg + b * npix : nullptr;
@@ -2387,7 +2444,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_obj_event_kernel(const
     unsigned oob = 0;   // a kept finite event lies inside the canvas; a non-finite one contributes nothing
     for_each_event(first, last, [&](int64_t i) { return load_xytp(A.E, i); }, [&](int64_t, const EvXYTP &e) {
         Taps T;
-        float jx[4], jy[4];
+        float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
         if (!model_taps<WARP, GRAD>(A.C, model_event<WARP>(e.x, e.y, e.t, e.p), M, oob, T, jx, jy)) return;
         if (!GRAD) {
             red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
@@ -2406,7 +2463,14 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_obj_event_kernel(const
 
 static int motion_obj_dims(int warp)
 {
-    return warp == EVK_WARP_LINVEL ? 2 : warp == EVK_WARP_ROTATION ? 3 : warp == EVK_WARP_XYZTHETA ? 4 : 0;
+    switch (warp) {
+    case EVK_WARP_LINVEL: return 2;
+    case EVK_WARP_ROTATION: return 3;
+    case EVK_WARP_XYZTHETA: return 4;
+    case EVK_WARP_AFFINE: return 6;
+    case EVK_WARP_HOMOGRAPHY: return 8;
+    default: return 0;
+    }
 }
 
 // Shared argument checks and set-up of the model entries.  `images` per sample: 1 for the contrast losses, 2 for the
@@ -2452,6 +2516,8 @@ static void with_model_warp(int warp, F f)
 {
     if (warp == EVK_WARP_LINVEL) f(std::integral_constant<int, WARP_LINVEL_F32>{});
     else if (warp == EVK_WARP_ROTATION) f(std::integral_constant<int, WARP_ROTATION_F32>{});
+    else if (warp == EVK_WARP_AFFINE) f(std::integral_constant<int, WARP_AFFINE_F32>{});
+    else if (warp == EVK_WARP_HOMOGRAPHY) f(std::integral_constant<int, WARP_HOMOGRAPHY_F32>{});
     else f(std::integral_constant<int, WARP_XYZTHETA_F32>{});
 }
 
@@ -2499,7 +2565,7 @@ struct SegEvent {
 template <int WARP, bool WEIGHTED>
 __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const ModelArgs A)
 {
-    __shared__ WarpModel mod[kMaxCandidates];
+    __shared__ ModelOf<WARP> mod[kMaxCandidates];
     const int b = blockIdx.y, M = WEIGHTED ? A.M : 1, J = A.J;
     load_models<WARP>(A.params, (int64_t)b * M * J, M * J, A.cx, A.cy, mod);
     int64_t first, last;
@@ -2519,7 +2585,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const 
         for (int m = 0; m < kMaxSegModels; ++m) {
             if (m >= M) break;
             for (int j = 0; j < J; ++j) {
-                const WarpModel Mo = mod[m * J + j];
+                const ModelOf<WARP> Mo = mod[m * J + j];
                 float *accq = acc + (int64_t)(m * J + j) * npix * 4;
 #pragma unroll
                 for (int k = 0; k < kBatch; ++k) {
@@ -2527,7 +2593,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const 
                     const EvXYTP &ek = e[k].e;
                     const float p = WEIGHTED ? __fmul_rn(ek.p, e[k].w[m]) : ek.p;   // the splat weight p w, formed in f32
                     Taps T;
-                    float jx[4], jy[4];
+                    float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
                     if (model_taps<WARP, false>(A.C, model_event<WARP>(ek.x, ek.y, ek.t, p), Mo, oob, T, jx, jy))
                         red_add4(accq + ((int64_t)T.y0 * Wc + T.x0) * 4, T.ti);
                 }
@@ -2545,7 +2611,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_grad_kernel(const 
     int64_t first, last;
     sample_range(A.E, b, first, last);
     const int64_t npix = (int64_t)A.C.Hc * A.C.Wc;
-    WarpModel Mo;
+    ModelOf<WARP> Mo;
     load_model<WARP>(A.params, z, A.cx, A.cy, Mo);
     const float *Wb = A.Wimg + z * npix;
     // W_bm leaves out the variance's constant -2 g mean(G) / P of dF/dI (the tap differences of the parameter gradient
@@ -2563,7 +2629,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_grad_kernel(const 
     };
     for_each_event(first, last, load, [&](int64_t i, const EvXYTPW &e) {
         Taps T;
-        float jx[4], jy[4];
+        float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
         double gw = 0.0;
         // the footprint does not depend on the weight
         if (model_taps<WARP, true>(A.C, model_event<WARP>(e.x, e.y, e.t, 1.0f), Mo, oob, T, jx, jy)) {
@@ -2589,7 +2655,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_grad_kernel(const 
 template <int WARP>
 __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_assign_kernel(const ModelArgs A)
 {
-    __shared__ WarpModel mod[kMaxSegModels];
+    __shared__ ModelOf<WARP> mod[kMaxSegModels];
     const int b = blockIdx.y, M = A.M;
     load_models<WARP>(A.params, (int64_t)b * M, M, A.cx, A.cy, mod);
     int64_t first, last;
@@ -2605,7 +2671,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_assign_kernel(cons
             c[m] = 0.0;
             if (m >= M) continue;
             Taps T;
-            float jx[4], jy[4];
+            float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
             if (model_taps<WARP, false>(A.C, model_event<WARP>(e.x, e.y, e.t, 1.0f), mod[m], oob, T, jx, jy)) {
                 const float *G = Gs + m * npix;
                 const int64_t r0 = (int64_t)T.y0 * Wc, r1 = (int64_t)T.y1 * Wc;
@@ -2797,7 +2863,7 @@ static const float2 *ts_obj_backward_ab(const BatchObjWorkspace &ws, const float
 
 // ---- parametric average-timestamp (Zhu) loss over a batch of samples (evk_motion_timestamp_objective_f32 / _grad_f32) --
 // Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by its own model params[b] through model_taps
-// (linvel, rotation or xyztheta, f32, as the motion contrast loss warps), with weight 1: an event contributes iff its splat
+// (linvel, rotation, xyztheta, affine or homography, f32, as the motion contrast loss warps), with weight 1: an event contributes iff its splat
 // there is not zero (finite, 0 < x' < W, 0 < y' < H).  Then the images and f_b of the dense-flow timestamp loss above, on
 // the same 2B images z = 2b + s and through the same image-space halves (ts_obj_forward_tail, ts_obj_backward_ab):
 //   forward:  two v4 reductions per contributing event into the 32-byte block {S taps, C taps} of its polarity (the
@@ -2815,7 +2881,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_ts_event_kernel(const 
     sample_range(A.E, b, first, last);
     const int Wc = A.C.Wc;
     const int64_t npix = (int64_t)A.C.Hc * Wc;
-    WarpModel M;
+    ModelOf<WARP> M;
     load_model<WARP>(A.params, b, A.cx, A.cy, M);
     float *acc = GRAD ? nullptr : A.acc + b * 2 * npix * 8;
     const float2 *ab = GRAD ? A.ab + b * 2 * npix : nullptr;
@@ -2827,7 +2893,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_ts_event_kernel(const 
         const int pol = ts_polarity(e.p);
         if (pol < 0) return;
         Taps T;
-        float jx[4], jy[4];
+        float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
         if (!model_taps<WARP, GRAD>(A.C, model_event<WARP>(e.x, e.y, e.t, 1.0f), M, oob, T, jx, jy)) return;
         if (!GRAD) {
             ts_block_add(acc, npix, Wc, pol, T, e.tau);
@@ -2877,7 +2943,7 @@ struct TsCandEvent {
 template <int WARP>
 __global__ void __launch_bounds__(kFlowObjThreads) motion_ts_cand_kernel(const ModelArgs A)
 {
-    __shared__ WarpModel cand[kMaxCandidates];
+    __shared__ ModelOf<WARP> cand[kMaxCandidates];
     const int b = blockIdx.y, J = A.J;
     load_models<WARP>(A.params, (int64_t)b * J, J, A.cx, A.cy, cand);
     int64_t first, last;
@@ -2896,12 +2962,12 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_ts_cand_kernel(const M
     };
     for_each_event_batch(first, last, load, [&](const TsCandEvent<WARP> (&e)[kBatch], int) {
         for (int j = 0; j < J; ++j) {
-            const WarpModel M = cand[j];
+            const ModelOf<WARP> M = cand[j];
             float *accj = acc + (int64_t)j * 2 * npix * 8;
 #pragma unroll
             for (int k = 0; k < kBatch; ++k) {
                 Taps T;
-                float jx[4], jy[4];
+                float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
                 if (e[k].pol < 0 || !model_taps<WARP, false>(A.C, e[k].e, M, oob, T, jx, jy)) continue;
                 ts_block_add(accj, npix, Wc, e[k].pol, T, e[k].tau);
             }

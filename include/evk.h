@@ -552,7 +552,16 @@ int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const floa
  * parameters params[b] (K doubles, in DEVICE memory) with the model `warp`:
  *   EVK_WARP_LINVEL    (vx, vy)                K = 2   x' = x - t_rel vx (lib/contrast_max/warps.py:51-61)
  *   EVK_WARP_ROTATION  (cx, cy, omega)         K = 3
- *   EVK_WARP_XYZTHETA  (hx, hy, hz, theta)     K = 4   about the centre (cx, cy) given here (ignored otherwise)
+ *   EVK_WARP_XYZTHETA  (hx, hy, hz, theta)     K = 4   about the centre (cx, cy) given here
+ *   EVK_WARP_AFFINE    (hx, hy, a11, a12, a21, a22)            K = 6   about (cx, cy)
+ *   EVK_WARP_HOMOGRAPHY (hx, hy, a11, a12, a21, a22, g1, g2)   K = 8   about (cx, cy)
+ * (cx, cy) is the fixed centre of xyztheta, affine and homography and is ignored by the other models.  With
+ * d = t_rel, u = x - cx, v = y - cy, the two planar models are first order in d:
+ *   affine:      sx = (hx + a11 u) + a12 v,  sy = (hy + a22 v) + a21 u,  x' = x - d sx,  y' = y - d sy
+ *   homography:  sx, sy as affine, nx = u - d sx, ny = v - d sy, q = d ((g1 u) + (g2 v)), w = 1 - q,
+ *                x' = (x - d sx) + nx q / w,  y' = (y - d sy) + ny q / w
+ * An event whose w is <= 0 or not finite (past the homography's horizon) is not kept.  Affine at
+ * (hx, hy, hz, -theta, theta, hz) is xyztheta bit for bit, and homography at g1 = g2 = 0 is affine bit for bit.
  * in f32, in the order written.  An event is kept iff 0 < x' <= W and 0 < y' <= H (events_bounds_mask,
  * lib/util/event_util.py:26-27; NaN compares false and is kept, then contributes nothing) and splatted
  * bilinearly on the (H+1)x(W+1) canvas (events_to_image_drv, lib/representations/image.py:179-217).  Then
@@ -568,6 +577,8 @@ int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const floa
  * workspace: evk_cmax_motion_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
  * Neither call synchronises, and both launch the same kernels whatever the batch. */
 #define EVK_WARP_LINVEL 3
+#define EVK_WARP_AFFINE 4
+#define EVK_WARP_HOMOGRAPHY 5
 size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W);
 int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
                                   const int64_t *offsets, int batch, int64_t n_events, int warp,
@@ -693,8 +704,8 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
  * reference's zhu_timestamp_objective (lib/contrast_max/objectives.py:524-558), driven by its warp_function, with the
  * sign of a loss to minimise.  Sample b is the events [offsets[b], offsets[b+1]) (clipped to [0, n_events); end < start
  * is empty), warped by its own parameters params[b] (K doubles in DEVICE memory) with the model `warp` and its f32
- * arithmetic exactly as in evk_cmax_motion_objective_f32 (EVK_WARP_LINVEL / _ROTATION / _XYZTHETA; the centre (cx, cy)
- * of xyztheta).  An event contributes iff its splat in that loss is not zero: x', y' finite, 0 < x' < W and
+ * arithmetic exactly as in evk_cmax_motion_objective_f32 (EVK_WARP_LINVEL / _ROTATION / _XYZTHETA / _AFFINE /
+ * _HOMOGRAPHY; the centre (cx, cy) of xyztheta and the planar models).  An event contributes iff its splat in that loss is not zero: x', y' finite, 0 < x' < W and
  * 0 < y' < H (the bounds mask 0 < x' <= W, then the clip that gives x' = W zero weight).  A non-finite x' or y'
  * contributes nothing and does not poison the sample.  The reference instead zeroes the masked events and piles them
  * at (0, 0) as events with p = 0 and t = 0 (objectives.py:543-545).  tau and the images are those of

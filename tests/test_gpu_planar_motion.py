@@ -1,0 +1,495 @@
+"""The planar motion models (affine_warp, homography_warp) through every batched entry: the contrast and timestamp losses,
+their candidates passes, motion segmentation and its assignment, against the f64 references of
+tests/planar_motion_reference.py; the embeddings xyztheta -> affine -> homography bit for bit on the GPU; the horizon;
+and the fits' recovery of planar motions from the documented start."""
+import ctypes
+
+import numpy as np
+import pytest
+import torch
+
+import planar_motion_reference as P
+from conftest import assert_close_to_max
+
+pytestmark = pytest.mark.gpu
+
+H, W = 60, 80
+CENTRE = (40.0, 30.0)
+PARAMS = {"affine": [(20.0, -10.0, 3.0, -2.0, 1.5, -4.0), (-30.0, 15.0, -2.0, 4.0, -3.0, 1.0), (5.0, 5.0, 0.5, 3.0, -2.5, 2.0)],
+          "homography": [(20.0, -10.0, 3.0, -2.0, 1.5, -4.0, 0.05, -0.03), (-30.0, 15.0, -2.0, 4.0, -3.0, 1.0, -0.04, 0.06),
+                         (5.0, 5.0, 0.5, 3.0, -2.5, 2.0, 0.08, 0.02)]}
+
+
+def _warp(kind, centre=CENTRE):
+    from event_utils_b200.contrast_max import warps
+    return {"affine": warps.affine_warp, "homography": warps.homography_warp, "xyztheta": warps.xyztheta_warp}[kind](center=centre)
+
+
+def batch_stream(seed, sizes, h=H, w=W):
+    """concatenated windows; events in the sensor, d = t - t0 in [-0.1, 0] on a 2^-12 grid, tau in [0, 1]"""
+    rng = np.random.default_rng(seed)
+    n = sum(sizes)
+    x = (rng.random(n) * (w - 1)).astype(np.float32)
+    y = (rng.random(n) * (h - 1)).astype(np.float32)
+    p = (rng.integers(0, 2, n) * 2 - 1).astype(np.float32)
+    d = np.empty(n, np.float32)
+    off = np.concatenate(([0], np.cumsum(sizes))).astype(np.int64)
+    for b in range(len(sizes)):
+        d[off[b]:off[b + 1]] = -np.sort(rng.integers(0, 410, sizes[b]))[::-1] / 4096.0
+    tau = ((d + 0.1) / 0.1).astype(np.float32)
+    return x, y, d, tau, p, off
+
+
+def _cuda(*arrays):
+    return [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in arrays]
+
+
+def _ends(off):
+    return torch.from_numpy(off[1:]).cuda()
+
+
+def contrast(kind, x, y, d, p, off, params, sigma=1.0, name="variance", centre=CENTRE):
+    """(f (B,) f64 torch with autograd, params leaf) of motion_contrast_objective_torch, d reaching the kernel unchanged"""
+    from event_utils_b200.contrast_max import motion_contrast_objective_torch
+    prm = torch.tensor(np.asarray(params, np.float64), device="cuda", requires_grad=True)
+    f = motion_contrast_objective_torch(*_cuda(x, y, d, p), prm, _warp(kind, centre), t0=0.0, objective=name, blur_sigma=sigma,
+                                        img_size=(H, W), batch_end_indices=_ends(off))
+    return f, prm
+
+
+def entry(stem, kind, events, off, params, scalars, outs, M=None, centre=CENTRE):
+    """a forward C entry: events as device tensors, outs the shapes of its f64 f and f32 images; returns them"""
+    from event_utils_b200 import _lib
+    L = _lib.lib()
+    B = len(off) - 1
+    prm = torch.tensor(np.asarray(params, np.float64), device="cuda")
+    code = {"affine": _lib.WARP_AFFINE, "homography": _lib.WARP_HOMOGRAPHY, "xyztheta": _lib.WARP_XYZTHETA}[kind]
+    res = [torch.empty(s, dtype=torch.float64 if i == 0 else torch.float32, device="cuda") for i, s in enumerate(outs)]
+    ms = () if M is None else (M,)
+    ws = torch.empty(getattr(L, stem + "_workspace_bytes")(B, *ms, H, W), dtype=torch.uint8, device="cuda")
+    O = torch.from_numpy(off).cuda()
+    _lib.check(getattr(L, stem + "_f32")(*[a.data_ptr() for a in events], *ms, O.data_ptr(), B, events[0].shape[0], code,
+                                         prm.data_ptr(), prm.shape[-1], centre[0], centre[1], H, W, *scalars,
+                                         *[r.data_ptr() for r in res], ws.data_ptr(), ws.numel(), None))
+    torch.cuda.synchronize()
+    return [r.cpu() for r in res]
+
+
+def contrast_forward(kind, x, y, d, p, off, params, sigma=1.0, name="variance", centre=CENTRE):
+    B = len(off) - 1
+    return entry("evk_cmax_motion_objective", kind, _cuda(x, y, d, p), off, params, (sigma, {"variance": 0, "soe": 2}[name], 0.0),
+                 [(B,), (B, H + 1, W + 1)], centre=centre)
+
+
+def ts_forward(kind, x, y, d, tau, p, off, params, sigma=1.0, centre=CENTRE):
+    B = len(off) - 1
+    return entry("evk_motion_timestamp_objective", kind, _cuda(x, y, d, tau, p), off, params, (sigma,),
+                 [(B,), (B, 2, H + 1, W + 1), (B, 2, H + 1, W + 1)], centre=centre)
+
+
+def seg_forward(kind, x, y, d, p, w, off, params, sigma=1.0, centre=CENTRE):
+    B, M = len(off) - 1, w.shape[1]
+    return entry("evk_cmax_motion_segment", kind, _cuda(x, y, d, p, w), off, params, (sigma, 0, 0.0),
+                 [(B, M), (B, M, H + 1, W + 1)], M=M, centre=centre)
+
+
+def timestamp(kind, x, y, d, tau, p, off, params, sigma=1.0, centre=CENTRE):
+    """motion_timestamp_objective_torch with the stamps chosen so that its tau is the given one: ts = d, one window each"""
+    from event_utils_b200.contrast_max import motion_timestamp_objective_torch
+    prm = torch.tensor(np.asarray(params, np.float64), device="cuda", requires_grad=True)
+    f = motion_timestamp_objective_torch(*_cuda(x, y, d, p), prm, _warp(kind, centre), t0=0.0, blur_sigma=sigma, img_size=(H, W),
+                                         batch_end_indices=_ends(off))
+    return f, prm
+
+
+def _tau_of(d, off):
+    """the tau motion_timestamp_objective_torch forms from ts = d (tests/flow_timestamp_reference.tau_f32)"""
+    return P.tau_f32(d, off)
+
+
+SIZES = {1: [20000], 3: [15000, 0, 12000, 9000]}
+
+
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+@pytest.mark.parametrize("name", ["variance", "soe"])
+@pytest.mark.parametrize("batch", [1, 3])
+def test_contrast_loss_against_the_reference(kind, name, batch):
+    x, y, d, _, p, off = batch_stream(7 + batch, SIZES[batch])
+    params = PARAMS[kind][:1] if batch == 1 else [PARAMS[kind][0], PARAMS[kind][1], PARAMS[kind][1], PARAMS[kind][2]]
+    f, iwe = contrast_forward(kind, x, y, d, p, off, params, 1.0, name)
+    p64 = torch.tensor(params, dtype=torch.float64, requires_grad=True)
+    fr, iwer = P.contrast(kind, x, y, d, p, off, p64, 1.0, name, img_size=(H, W), centre=CENTRE)
+    for b in range(len(params)):
+        assert_close_to_max(iwe[b].numpy(), iwer[b].detach().numpy(), 1e-5, "iwe %d" % b)
+        assert abs(f[b].item() - fr[b].item()) <= 1e-5 * max(abs(fr[b].item()), 1e-30), (b, f[b], fr[b])
+    fg, prm = contrast(kind, x, y, d, p, off, params, 1.0, name)
+    g = torch.from_numpy(np.random.default_rng(5).standard_normal(len(params)))
+    (fg * g.cuda()).sum().backward()
+    (fr * g).sum().backward()
+    assert_close_to_max(prm.grad.cpu().numpy(), p64.grad.numpy(), 1e-4, "grad %s %s" % (kind, name))
+    # the candidates pass is the forward, value for value
+    from event_utils_b200.contrast_max import motion_contrast_candidates_torch
+    cand = torch.tensor(np.asarray(params, np.float64), device="cuda").unsqueeze(1).repeat(1, 3, 1)
+    fc = motion_contrast_candidates_torch(*_cuda(x, y, d, p), cand, _warp(kind), t0=0.0, objective=name, blur_sigma=1.0,
+                                          img_size=(H, W), batch_end_indices=_ends(off))
+    # f32 image sums in another order (atomics): equal to f32 rounding, bit for bit only on sparse footprints (below)
+    np.testing.assert_allclose(fc.cpu().numpy(), fg.detach().cpu().unsqueeze(1).repeat(1, 3).numpy(), rtol=1e-6, atol=0)
+
+
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+@pytest.mark.parametrize("batch", [1, 3])
+def test_timestamp_loss_against_the_reference(kind, batch):
+    x, y, d, _, p, off = batch_stream(17 + batch, SIZES[batch])
+    tau = _tau_of(d, off)
+    params = PARAMS[kind][:1] if batch == 1 else [PARAMS[kind][0], PARAMS[kind][1], PARAMS[kind][1], PARAMS[kind][2]]
+    f, T, C = ts_forward(kind, x, y, d, tau, p, off, params)
+    p64 = torch.tensor(params, dtype=torch.float64, requires_grad=True)
+    fr, Tr, Cr = P.timestamp(kind, x, y, d, tau, p, off, p64, 1.0, img_size=(H, W), centre=CENTRE)
+    for b in range(len(params)):
+        assert_close_to_max(T[b].numpy(), Tr[b].detach().numpy(), 1e-5, "T %d" % b)
+        assert_close_to_max(C[b].numpy(), Cr[b].detach().numpy(), 1e-5, "C %d" % b)
+        assert abs(f[b].item() - fr[b].item()) <= 1e-5 * max(abs(fr[b].item()), 1e-30), (b, f[b], fr[b])
+    fg, prm = timestamp(kind, x, y, d, tau, p, off, params)
+    np.testing.assert_allclose(fg.detach().cpu().numpy(), f.numpy(), rtol=1e-6, atol=0)
+    g = torch.from_numpy(np.random.default_rng(6).standard_normal(len(params)))
+    (fg * g.cuda()).sum().backward()
+    (fr * g).sum().backward()
+    assert_close_to_max(prm.grad.cpu().numpy(), p64.grad.numpy(), 1e-4, "ts grad %s" % kind)
+    from event_utils_b200.contrast_max import motion_timestamp_candidates_torch
+    cand = torch.tensor(np.asarray(params, np.float64), device="cuda").unsqueeze(1).repeat(1, 2, 1)
+    fc = motion_timestamp_candidates_torch(*_cuda(x, y, d, p), cand, _warp(kind), t0=0.0, blur_sigma=1.0, img_size=(H, W),
+                                           batch_end_indices=_ends(off))
+    np.testing.assert_allclose(fc.cpu().numpy(), f.unsqueeze(1).repeat(1, 2).numpy(), rtol=1e-6, atol=0)
+
+
+def _memberships(n, M, seed):
+    w = np.random.default_rng(seed).random((n, M)).astype(np.float32)
+    return (w / w.sum(1, keepdims=True)).astype(np.float32)
+
+
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+@pytest.mark.parametrize("batch", [1, 3])
+def test_segmentation_against_the_reference(kind, batch):
+    from event_utils_b200.contrast_max import (motion_segmentation_assign_torch, motion_segmentation_candidates_torch,
+                                               motion_segmentation_objective_torch)
+    x, y, d, _, p, off = batch_stream(27 + batch, [6000] if batch == 1 else [5000, 0, 4000, 3000])
+    M = 2
+    w = _memberships(x.shape[0], M, 3)
+    B = len(off) - 1
+    params = np.array([[PARAMS[kind][b % 3], PARAMS[kind][(b + 1) % 3]] for b in range(B)])
+    f, iwe = seg_forward(kind, x, y, d, p, w, off, params)
+    p64 = torch.tensor(params, dtype=torch.float64, requires_grad=True)
+    w64 = torch.tensor(w, dtype=torch.float64, requires_grad=True)
+    fr, iwer = P.segmentation(kind, x, y, d, p, w64, off, p64, 1.0, "variance", img_size=(H, W), centre=CENTRE)
+    for b in range(B):
+        for m in range(M):
+            assert_close_to_max(iwe[b, m].numpy(), iwer[b, m].detach().numpy(), 1e-5, "iwe %d %d" % (b, m))
+    np.testing.assert_allclose(f.numpy(), fr.detach().numpy(), rtol=1e-5, atol=1e-30)
+    prm = torch.tensor(params, device="cuda", requires_grad=True)
+    wt = torch.from_numpy(w).cuda().requires_grad_(True)
+    ev = _cuda(x, y, d, p)
+    fg = motion_segmentation_objective_torch(*ev, wt, prm, _warp(kind), t0=0.0, blur_sigma=1.0, img_size=(H, W),
+                                             batch_end_indices=_ends(off))
+    np.testing.assert_allclose(fg.detach().cpu().numpy(), f.numpy(), rtol=1e-6, atol=0)
+    g = torch.from_numpy(np.random.default_rng(8).standard_normal((B, M)))
+    (fg * g.cuda()).sum().backward()
+    (fr * g).sum().backward()
+    assert_close_to_max(prm.grad.cpu().numpy(), p64.grad.numpy(), 1e-4, "seg grad params")
+    assert_close_to_max(wt.grad.cpu().numpy(), w64.grad.numpy(), 1e-4, "seg grad weights")
+    cand = torch.tensor(params, device="cuda").unsqueeze(2).repeat(1, 1, 2, 1)
+    fc = motion_segmentation_candidates_torch(*ev, cand, wt.detach(), _warp(kind), t0=0.0, blur_sigma=1.0, img_size=(H, W),
+                                              batch_end_indices=_ends(off))
+    np.testing.assert_allclose(fc.cpu().numpy(), f.unsqueeze(2).repeat(1, 1, 2).numpy(), rtol=1e-6, atol=0)
+    wa = motion_segmentation_assign_torch(*ev, torch.tensor(params, device="cuda"), _warp(kind), torch.from_numpy(w).cuda(),
+                                          t0=0.0, blur_sigma=1.0, img_size=(H, W), batch_end_indices=_ends(off), eps=1e-6)
+    wr = P.assign(kind, x, y, d, off, params, iwe.numpy(), 1.0, 1e-6, img_size=(H, W), centre=CENTRE)
+    # to 1e-4 of the row sum: the torch function forms its own images, whose f32 sums meet in another order than those of
+    # the images the reference is given
+    np.testing.assert_allclose(wa.cpu().numpy(), wr, rtol=1e-5, atol=1e-4)
+
+
+def _embedded(hx, hy, hz, th):
+    return (hx, hy, hz, -th, th, hz)
+
+
+def sparse_footprints(xyz, seed, n=6000):
+    """Windows 0, 2, 3 of random events thinned so that under xyz[b] and xyz[3 - b] (the two models of the segmentation
+    below) every kept event's 2x2 footprint shares no pixel with another's (window 1 is empty).  Every image pixel then
+    receives at most one tap, so the images do not depend on the order of the f32 sums."""
+    from motion_objective_reference import warp_f32
+    rng = np.random.default_rng(seed)
+    xs, ys, ds, ps, ends = [], [], [], [], []
+    for b in range(4):
+        if b != 1:
+            x = (rng.random(n) * (W - 1)).astype(np.float32)
+            y = (rng.random(n) * (H - 1)).astype(np.float32)
+            d = (-np.sort(rng.integers(0, 410, n))[::-1] / 4096.0).astype(np.float32)
+            keep = np.ones(n, bool)
+            anchors = []
+            for prm in (xyz[b], xyz[3 - b]):
+                xw, yw = warp_f32("xyztheta", x, y, d, prm, CENTRE)
+                keep &= P.contributes(xw, yw, H, W)
+                anchors.append((np.floor(xw), np.floor(yw)))
+            taken = [np.zeros((H + 3, W + 3), bool) for _ in anchors]
+            pick = []
+            for e in np.flatnonzero(keep):
+                cells = [(int(ax[e]) + 1, int(ay[e]) + 1) for ax, ay in anchors]
+                if any(t[cy - 1:cy + 2, cx - 1:cx + 2].any() for t, (cx, cy) in zip(taken, cells)):
+                    continue
+                for t, (cx, cy) in zip(taken, cells):
+                    t[cy, cx] = True
+                pick.append(e)
+            pick = np.array(pick)
+            xs.append(x[pick]), ys.append(y[pick]), ds.append(d[pick])
+            ps.append((rng.integers(0, 2, pick.size) * 2 - 1).astype(np.float32))
+        ends.append(sum(a.size for a in xs))
+    off = np.array([0] + ends, np.int64)
+    return [np.concatenate(a) for a in (xs, ys, ds, ps)] + [off]
+
+
+def test_embeddings_bit_for_bit_end_to_end():
+    """affine at (hx, hy, hz, -theta, theta, hz) is xyztheta, and homography at g = 0 is affine: f and the images of every
+    forward and candidates pass equal, and the gradients map through the embedding"""
+    from event_utils_b200.contrast_max import (motion_contrast_candidates_torch, motion_segmentation_assign_torch,
+                                               motion_segmentation_candidates_torch, motion_timestamp_candidates_torch)
+    xyz = np.array([(20.0, -10.0, 3.0, 2.0), (-30.0, 15.0, -2.0, 4.0), (5.0, 5.0, 0.5, -3.0), (1.0, 2.0, -1.0, 0.5)])
+    x, y, d, p, off = sparse_footprints(xyz, seed=41)
+    tau = _tau_of(d, off)
+    chain = {"xyztheta": xyz, "affine": np.array([_embedded(*r) for r in xyz])}
+    chain["homography"] = np.concatenate((chain["affine"], np.zeros((4, 2))), axis=1)
+    w = _memberships(x.shape[0], 2, 5)
+    seg = {k: np.stack((v, v[::-1]), axis=1) for k, v in chain.items()}
+    out = {}
+    for kind, prm in chain.items():
+        ev = _cuda(x, y, d, p)
+        r = {"contrast": contrast_forward(kind, x, y, d, p, off, prm), "ts": ts_forward(kind, x, y, d, tau, p, off, prm),
+             "seg": seg_forward(kind, x, y, d, p, w, off, seg[kind])}
+        kw = dict(t0=0.0, blur_sigma=1.0, img_size=(H, W), batch_end_indices=_ends(off))
+        c = torch.tensor(prm, device="cuda").unsqueeze(1)
+        r["contrast_cand"] = [motion_contrast_candidates_torch(*ev, c, _warp(kind), **kw).cpu()]
+        r["ts_cand"] = [motion_timestamp_candidates_torch(*ev, c, _warp(kind), **kw).cpu()]
+        cs = torch.tensor(seg[kind], device="cuda").unsqueeze(2)
+        r["seg_cand"] = [motion_segmentation_candidates_torch(*ev, cs, torch.from_numpy(w).cuda(), _warp(kind), **kw).cpu()]
+        r["assign"] = [motion_segmentation_assign_torch(*ev, torch.tensor(seg[kind], device="cuda"), _warp(kind),
+                                                        torch.from_numpy(w).cuda(), eps=1e-6, **kw).cpu()]
+        fc, pc = contrast(kind, x, y, d, p, off, prm)
+        fc.sum().backward()
+        ft, pt = timestamp(kind, x, y, d, tau, p, off, prm)
+        ft.sum().backward()
+        r["grads"] = (pc.grad.cpu().numpy(), pt.grad.cpu().numpy())
+        out[kind] = r
+    for a, b in (("xyztheta", "affine"), ("affine", "homography")):
+        for key in ("contrast", "ts", "seg", "contrast_cand", "ts_cand", "seg_cand", "assign"):
+            for i, (u, v) in enumerate(zip(out[a][key], out[b][key])):
+                if key in ("contrast", "ts", "seg") and i == 0 or key.endswith("_cand"):
+                    # f: the tail's f64 block sums meet in f64 atomics, whose order is not fixed from call to call
+                    np.testing.assert_allclose(v.numpy(), u.numpy(), rtol=1e-12, atol=0, err_msg="%s %s %s" % (a, b, key))
+                else:
+                    assert torch.equal(u, v), (a, b, key, i)
+    for ga, gh, gx in zip(out["affine"]["grads"], out["homography"]["grads"], out["xyztheta"]["grads"]):
+        # within f64 summation-order rounding: the same per-event terms, summed in another grouping
+        np.testing.assert_allclose(gh[:, :6], ga, rtol=1e-9, atol=1e-9 * np.abs(ga).max())
+        mapped = np.stack((ga[:, 0], ga[:, 1], ga[:, 2] + ga[:, 5], ga[:, 4] - ga[:, 3]), axis=1)
+        np.testing.assert_allclose(mapped, gx, rtol=1e-9, atol=1e-9 * np.abs(gx).max())
+
+
+def test_events_past_the_horizon_add_nothing():
+    """g1 = 6: with d down to -0.1 the events left of u = -1/(6 |d|) have w <= 0.  They add nothing to f, the images or
+    the gradient: dropping them from the stream changes no value beyond summation order"""
+    x, y, d, _, p, off = batch_stream(51, [20000])
+    tau = _tau_of(d, off)
+    prm = [(5.0, -3.0, 0.5, 0.2, -0.1, 0.3, 6.0, 0.0)]
+    u = x.astype(np.float64) - CENTRE[0]
+    q = d.astype(np.float64) * 6.0 * u
+    past = 1 - q <= 0
+    assert 0.02 < past.mean() < 0.5, past.mean()
+    xw, yw = P.warp_f32("homography", x, y, d, prm[0], CENTRE)
+    assert not P.contributes(xw, yw, H, W)[past].any()
+    keep = ~past
+    # the kept events keep their stamps, so tau is taken from the whole window for both streams
+    xs, ys, ds, taus, ps = x[keep], y[keep], d[keep], tau[keep], p[keep]
+    offs = np.array([0, int(keep.sum())])
+    f_all, iwe_all = contrast_forward("homography", x, y, d, p, off, prm)
+    f_kept, iwe_kept = contrast_forward("homography", xs, ys, ds, ps, offs, prm)
+    np.testing.assert_allclose(iwe_all.numpy(), iwe_kept.numpy(), rtol=0, atol=1e-5 * iwe_all.abs().max().item())
+    np.testing.assert_allclose(f_all.numpy(), f_kept.numpy(), rtol=1e-6)
+    t_all = ts_forward("homography", x, y, d, tau, p, off, prm)
+    t_kept = ts_forward("homography", xs, ys, ds, taus, ps, offs, prm)
+    np.testing.assert_allclose(t_all[0].numpy(), t_kept[0].numpy(), rtol=1e-6)
+    np.testing.assert_allclose(t_all[1].numpy(), t_kept[1].numpy(), rtol=0, atol=1e-6)
+    ga = contrast("homography", x, y, d, p, off, prm)
+    ga[0].sum().backward()
+    gk = contrast("homography", xs, ys, ds, ps, offs, prm)
+    gk[0].sum().backward()
+    assert torch.isfinite(ga[1].grad).all()
+    assert_close_to_max(ga[1].grad.cpu().numpy(), gk[1].grad.cpu().numpy(), 1e-6, "horizon grad")
+    p64 = torch.tensor(prm, dtype=torch.float64, requires_grad=True)
+    fr, _ = P.contrast("homography", x, y, d, p, off, p64, 1.0, "variance", img_size=(H, W), centre=CENTRE)
+    fr.sum().backward()
+    assert_close_to_max(ga[1].grad.cpu().numpy(), p64.grad.numpy(), 1e-4, "horizon grad vs reference")
+
+
+def test_reference_api_get_iwe_takes_the_generic_path():
+    from event_utils_b200.contrast_max.objectives import get_iwe
+    rng = np.random.default_rng(61)
+    n = 30000
+    xs, ys = rng.uniform(40, 200, n), rng.uniform(30, 150, n)
+    ts, ps = np.sort(rng.uniform(0, 0.05, n)), rng.integers(0, 2, n) * 2.0 - 1
+    for kind, prm in (("affine", (20.0, -10.0, 3.0, -2.0, 1.5, -4.0)), ("homography", (20.0, -10.0, 3.0, -2.0, 1.5, -4.0, 0.004,
+                                                                                        -0.003))):
+        warp = _warp(kind, (120.0, 90.0))
+        iwe, _ = get_iwe(prm, xs, ys, ts, ps, warp, (180, 240))
+        ev = [torch.tensor(a, device="cuda") for a in (xs, ys, ts, ps)]
+        gpu = contrast_image(ev, prm, warp)
+        # f64 warp on the host against the f32 warp of the batched pass: the taps agree to f32 rounding of the positions
+        assert_close_to_max(np.asarray(iwe, np.float64), gpu, 1e-4, "get_iwe %s" % kind)
+
+
+def contrast_image(ev, prm, warp):
+    """the IWE of motion_contrast_objective_torch's forward at (180, 240), t0 = the last stamp"""
+    from event_utils_b200.contrast_max import _batched as B
+    from event_utils_b200 import _lib
+    L = _lib.lib()
+    x, y, t_rel, p, off = B._batch_events(*ev, None, None, 1, ev[0].device, "parameters")
+    prm64 = torch.tensor([prm], dtype=torch.float64, device="cuda")
+    f = torch.empty(1, dtype=torch.float64, device="cuda")
+    iwe = torch.empty((1, 181, 241), device="cuda")
+    ws = torch.empty(L.evk_cmax_motion_objective_workspace_bytes(1, 180, 240), dtype=torch.uint8, device="cuda")
+    code = B._warp_code(warp, "test")
+    _lib.check(L.evk_cmax_motion_objective_f32(x.data_ptr(), y.data_ptr(), t_rel.data_ptr(), p.data_ptr(), off.data_ptr(), 1,
+                                               x.shape[0], code, prm64.data_ptr(), len(prm), warp.center[0], warp.center[1], 180,
+                                               240, 0.0, 0, 0.0, f.data_ptr(), iwe.data_ptr(), ws.data_ptr(), ws.numel(), None))
+    return iwe[0].cpu().numpy().astype(np.float64)
+
+
+def test_no_host_round_trips_and_constant_launch_count():
+    from event_utils_b200 import _lib
+    from event_utils_b200.contrast_max import motion_contrast_objective_torch, motion_timestamp_objective_torch
+    L = _lib.lib()
+    for kind in ("affine", "homography"):
+        counts = []
+        for sizes in ([40000], [2500] * 16):
+            x, y, d, _, p, off = batch_stream(2, sizes)
+            params = np.tile(np.array([PARAMS[kind][0]]), (len(sizes), 1))
+            contrast(kind, x, y, d, p, off, params)[0].sum().backward()       # warm-up
+            timestamp(kind, x, y, d, None, p, off, params)[0].sum().backward()
+            prm = torch.tensor(params, device="cuda", requires_grad=True)
+            ev = _cuda(x, y, d, p)
+            ends = _ends(off)
+            torch.cuda.synchronize()
+            L.evk_prof_enable(1)
+            torch.cuda.set_sync_debug_mode("error")
+            try:
+                f = motion_contrast_objective_torch(*ev, prm, _warp(kind), objective="soe", img_size=(H, W), batch_end_indices=ends)
+                g = motion_timestamp_objective_torch(*ev, prm, _warp(kind), img_size=(H, W), batch_end_indices=ends)
+                (f.sum() + g.sum()).backward()
+            finally:
+                torch.cuda.set_sync_debug_mode(0)
+            ms, timed, launches = ctypes.c_double(), ctypes.c_longlong(), ctypes.c_longlong()
+            _lib.check(L.evk_prof_collect(ctypes.byref(ms), ctypes.byref(timed), ctypes.byref(launches)))
+            L.evk_prof_enable(0)
+            assert torch.isfinite(prm.grad).all()
+            counts.append(launches.value)
+        assert counts[0] == counts[1] and counts[0] > 0, counts
+
+
+# ---- recovery from the documented start -----------------------------------------------------------------------------
+_A = [(30.0, -20.0, 4.0, -3.0, 0.0, 0.0), (-25.0, 10.0, -3.0, 1.0, 4.0, 1.0), (10.0, 30.0, 2.0, 2.5, 1.0, -2.0),
+      (-15.0, -25.0, 0.0, -3.0, -0.5, 3.0)]
+TRUTHS = {"affine": _A,
+          "homography": [a + g for a, g in zip(_A, [(0.05, -0.04), (-0.06, 0.05), (0.04, 0.06), (-0.05, -0.05)])]}
+DURATION = 0.05
+
+
+def _planar_windows(kind, seed):
+    rng = np.random.default_rng(seed)
+    parts = [P.planar_scene(kind, tr, rng, duration=DURATION) for tr in TRUTHS[kind]]
+    ends = np.cumsum([a[0].size for a in parts])
+    return [np.concatenate(a) for a in zip(*parts)], ends
+
+
+def _displacement_error(kind, got, truth):
+    """largest difference, in px, between the warps of `got` and `truth` over the scene disc at d = -DURATION"""
+    g = np.linspace(-60, 60, 25)
+    u, v = np.meshgrid(g, g)
+    k = u ** 2 + v ** 2 <= 60 ** 2
+    xs, ys = 120.0 + u[k], 90.0 + v[k]
+    ts = np.zeros_like(xs)
+    w = _warp(kind, (120.0, 90.0))
+    a = w.warp(xs, ys, ts, ts, DURATION, got)
+    b = w.warp(xs, ys, ts, ts, DURATION, truth)
+    return float(np.hypot(a[0] - b[0], a[1] - b[1]).max())
+
+
+def _four_dof_start(truths):
+    """the projection of each truth on xyztheta's subspace: hz = (a11 + a22) / 2, theta = (a21 - a12) / 2"""
+    t = np.asarray(truths)
+    return np.stack((t[:, 0], t[:, 1], (t[:, 2] + t[:, 5]) / 2, (t[:, 4] - t[:, 3]) / 2), axis=1)
+
+
+# largest displacement error over the scene (px at the window's duration) of every recovered window; observed on an H100
+# (80 GB HBM3, 700 W), three runs.  The homography's projective part is pinned loosely by a 60 px scene over 0.05 s.
+RECOVERY_PX = {("contrast", "affine"): 1.0,       # observed 0.26-0.80 px (from 12-19 px at the 4-DoF fit)
+               ("contrast", "homography"): 5.0,   # observed 1.00-3.49 px (from 18-31 px)
+               ("timestamp", "affine"): 0.1,      # observed 0.019-0.030 px (from 7-14 px)
+               ("timestamp", "homography"): 5.0}  # observed 1.85-4.01 px (from 18-25 px)
+
+
+@pytest.mark.parametrize("loss", ["contrast", "timestamp"])
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+def test_fits_recover_planar_motion_from_the_embedded_four_dof_fit(loss, kind):
+    from event_utils_b200.contrast_max import motion_contrast_fit_torch, motion_timestamp_fit_torch
+    fit_fn = motion_contrast_fit_torch if loss == "contrast" else motion_timestamp_fit_torch
+    (x, y, t, p), ends = _planar_windows(kind, {"affine": 71, "homography": 72}[kind])
+    ev = [torch.from_numpy(x).float().cuda(), torch.from_numpy(y).float().cuda(), torch.from_numpy(t).cuda(),
+          torch.from_numpy(p).float().cuda()]
+    kw = dict(batch_end_indices=torch.tensor(ends, device="cuda"), blur_sigma=[4.0, 2.0, 1.0], max_iter=100)
+    four = fit_fn(*ev, _warp("xyztheta", (120.0, 90.0)), x0=torch.tensor(_four_dof_start(TRUTHS[kind]), device="cuda"), **kw)
+    start = torch.stack([torch.tensor(_embedded(*r)) for r in four.params.cpu().tolist()]).double()
+    if kind == "homography":
+        start = torch.cat((start, torch.zeros(start.shape[0], 2, dtype=torch.float64)), dim=1)
+    fit = fit_fn(*ev, _warp(kind, (120.0, 90.0)), x0=start.cuda(), **kw)
+    errs = [_displacement_error(kind, g, tr) for g, tr in zip(fit.params.cpu().numpy(), TRUTHS[kind])]
+    before = [_displacement_error(kind, np.concatenate((s, np.zeros(len(tr) - 6))), tr)
+              for s, tr in zip(start.numpy()[:, :6], TRUTHS[kind])]
+    print("%s %s: displacement error px %s (from the 4-DoF start %s)" % (loss, kind, np.round(errs, 3), np.round(before, 2)))
+    assert max(errs) <= RECOVERY_PX[(loss, kind)], (errs, before)
+    assert min(before) > 5.0      # the planar motion is visible: the 4-DoF fit cannot reach it
+
+
+# share of events whose argmax label is their object's; observed on an H100 (80 GB HBM3, 700 W): 0.9966, 0.9958, 0.9959
+LABEL_SHARE = 0.99
+
+
+def test_segmentation_fit_labels_two_affine_objects():
+    from event_utils_b200.contrast_max import motion_segmentation_fit_torch
+    rng = np.random.default_rng(91)
+    B = 4
+    xs, ys, ts, labels, ends, truths = [], [], [], [], [], []
+    for b in range(B):
+        tr = [(35.0, 10.0, 3.0, -2.0, 2.5, 1.0), (-30.0, -10.0, -2.0, 3.0, -1.5, -2.5)]
+        tr = [tuple(np.array(r) * rng.uniform(0.8, 1.2)) for r in tr]
+        parts = []
+        for s, cx in enumerate((65.0, 175.0)):
+            x, y, t, _ = P.planar_scene("affine", tr[s], rng, n_pts=150, per_pt=100, duration=DURATION, centre=(cx, 90.0),
+                                        radius=40.0, t_end=DURATION)
+            # the models share the window's centre c = (120, 90): about c, the motion of scene s is h' = h - A (c_s - c)
+            parts.append((x, y, t, np.full(x.size, s)))
+            tr[s] = tuple(np.array(tr[s][:2]) - np.array([[tr[s][2], tr[s][3]], [tr[s][4], tr[s][5]]]) @ np.array([cx - 120.0, 0.0])) \
+                + tuple(tr[s][2:])
+        x, y, t, lab = (np.concatenate(a) for a in zip(*parts))
+        order = np.argsort(t, kind="stable")
+        xs.append(x[order]), ys.append(y[order]), ts.append(t[order]), labels.append(lab[order])
+        ends.append(sum(len(a) for a in xs))
+        truths.append(tr)
+    x, y, t, lab = (np.concatenate(a) for a in (xs, ys, ts, labels))
+    ev = [torch.from_numpy(x).float().cuda(), torch.from_numpy(y).float().cuda(), torch.from_numpy(t).cuda(),
+          torch.ones(x.shape[0], device="cuda")]
+    truths = np.array(truths)
+    x0 = truths * (1 + rng.uniform(-0.15, 0.15, truths.shape))
+    fit = motion_segmentation_fit_torch(*ev, _warp("affine", (120.0, 90.0)), torch.tensor(x0, device="cuda"), t0=DURATION,
+                                        batch_end_indices=torch.tensor(ends, device="cuda"), blur_sigma=1.0, em_iters=8,
+                                        max_iter=20)
+    share = float((fit.weights.argmax(1).cpu().numpy() == lab).mean())
+    print("affine segmentation: label share %.4f" % share)
+    assert share >= LABEL_SHARE, share
