@@ -40,7 +40,7 @@ CMAX_ABS_POLARITY = 0x20
 CMAX_NO_CHANNEL_MIX = 0x40
 OBJ_VARIANCE, OBJ_SOS, OBJ_SOE, OBJ_MOA, OBJ_ISOA, OBJ_SOSA = range(6)
 WARP_ROTATION, WARP_XYZTHETA, WARP_LINVEL = 1, 2, 3
-WARP_AFFINE, WARP_HOMOGRAPHY = 4, 5      # the batched motion entries only (evk.h)
+WARP_AFFINE, WARP_HOMOGRAPHY, WARP_CAMERA_ROTATION = 4, 5, 6      # the batched motion entries only (evk.h)
 
 _lib = None
 _lock = threading.Lock()

@@ -316,11 +316,13 @@ class MotionObjective(torch.autograd.Function):
     """The batched parametric contrast objective of contrast_max/motion_objective.py (get_iwe, objectives.py:184-192, with
     the linvel, rotation or 4-DoF model, then an objective of objectives.py): f (B,) f64 from params (B,K) and the
     prepared device events.  Only the parameters get a gradient: the exact derivative of f, one pass over the events
-    (evk_cmax_motion_objective_grad_f32).  opts = (warp code, centre, H, W, objective, sigma, obj_param)."""
+    (evk_cmax_motion_objective_grad_f32).  opts = (warp code, centre, H, W, objective, sigma, obj_param); params are the
+    rows the entries take (contrast_max/_batched._rows), so K = 5 for the camera rotation."""
 
     @staticmethod
     def forward(ctx, params, x, y, t_rel, p, offsets, opts):
-        warp, (cx, cy), H, W, objective, sigma, param = opts
+        warp, centre, H, W, objective, sigma, param = opts
+        cx, cy = centre[:2]
         return _loss_forward(ctx, "evk_cmax_motion_objective", "motion_objective", params, torch.float64, (warp,),
                              (params.shape[-1], cx, cy, H, W, sigma, objective, param), (H, W), (x, y, t_rel, p), offsets, (1,))
 
@@ -334,11 +336,13 @@ class MotionSegmentationObjective(torch.autograd.Function):
     """The weighted multi-model contrast of contrast_max/motion_segmentation.py: f (B,M) f64 from params (B,M,K), the
     memberships weights (N,M) and the prepared device events.  The parameters and the memberships get gradients, one
     pass over the events for both (evk_cmax_motion_segment_grad_f32); the membership gradient only when weights
-    requires grad.  opts = (warp code, centre, H, W, objective, sigma, obj_param)."""
+    requires grad.  opts = (warp code, centre, H, W, objective, sigma, obj_param); params are the entries' rows
+    (_batched._rows)."""
 
     @staticmethod
     def forward(ctx, params, weights, x, y, t_rel, p, offsets, opts):
-        warp, (cx, cy), H, W, objective, sigma, param = opts
+        warp, centre, H, W, objective, sigma, param = opts
+        cx, cy = centre[:2]
         return _loss_forward(ctx, "evk_cmax_motion_segment", "motion_segment", params, torch.float64, (warp,),
                              (params.shape[-1], cx, cy, H, W, sigma, objective, param), (H, W), (x, y, t_rel, p), offsets,
                              (weights.shape[1],), weights)
@@ -354,11 +358,12 @@ class MotionTimestampObjective(torch.autograd.Function):
     (zhu_timestamp_objective, objectives.py:524-558, with the linvel, rotation or 4-DoF model): f (B,) f64 from params
     (B,K) and the prepared device events with their normalised stamps tau.  Only the parameters get a gradient: the exact
     derivative of f, one pass over the events (evk_motion_timestamp_objective_grad_f32).  The forward keeps the timestamp
-    and count images.  opts = (warp code, centre, H, W, sigma)."""
+    and count images.  opts = (warp code, centre, H, W, sigma); params are the entries' rows (_batched._rows)."""
 
     @staticmethod
     def forward(ctx, params, x, y, t_rel, tau, p, offsets, opts):
-        warp, (cx, cy), H, W, sigma = opts
+        warp, centre, H, W, sigma = opts
+        cx, cy = centre[:2]
         return _loss_forward(ctx, "evk_motion_timestamp_objective", "motion_timestamp_objective", params, torch.float64,
                              (warp,), (params.shape[-1], cx, cy, H, W, sigma), (H, W), (x, y, t_rel, tau, p), offsets, (2, 2))
 

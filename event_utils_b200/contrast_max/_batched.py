@@ -8,13 +8,15 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from .warps import affine_warp, homography_warp, linvel_warp, pure_rotation_warp, xyztheta_warp
+from .warps import affine_warp, camera_rotation_warp, homography_warp, linvel_warp, pure_rotation_warp, xyztheta_warp
 
 OBJECTIVES = {"variance": _lib.OBJ_VARIANCE, "sos": _lib.OBJ_SOS, "soe": _lib.OBJ_SOE, "sosa": _lib.OBJ_SOSA}
 DEFAULT_PARAM = {"sosa": 3.0}   # sosa_objective(p=3)
 _WARPS = ((linvel_warp, _lib.WARP_LINVEL), (pure_rotation_warp, _lib.WARP_ROTATION), (xyztheta_warp, _lib.WARP_XYZTHETA),
-          (affine_warp, _lib.WARP_AFFINE), (homography_warp, _lib.WARP_HOMOGRAPHY))
-_CENTRED = (_lib.WARP_XYZTHETA, _lib.WARP_AFFINE, _lib.WARP_HOMOGRAPHY)   # the models about a fixed centre (cx, cy)
+          (affine_warp, _lib.WARP_AFFINE), (homography_warp, _lib.WARP_HOMOGRAPHY),
+          (camera_rotation_warp, _lib.WARP_CAMERA_ROTATION))
+# the models about a fixed centre (cx, cy), the camera rotation's principal point
+_CENTRED = (_lib.WARP_XYZTHETA, _lib.WARP_AFFINE, _lib.WARP_HOMOGRAPHY, _lib.WARP_CAMERA_ROTATION)
 MAX_CANDIDATES = 32   # parameter vectors per window and pass over the events
 MAX_GRID_CANDIDATE_NODES = 12288   # candidates times nodes of a grid-flow candidates pass (the grids a CTA holds)
 
@@ -30,22 +32,41 @@ def _check_objective(objective, wrt):
 def _warp_code(warpfunc, who):
     warp = next((code for cls, code in _WARPS if type(warpfunc) is cls), None)
     if warp is None:
-        raise ValueError("%s supports the models linvel_warp, pure_rotation_warp and xyztheta_warp and the planar models "
-                         "affine_warp and homography_warp, got %s" % (who, type(warpfunc).__name__))
+        raise ValueError("%s supports the models linvel_warp, pure_rotation_warp and xyztheta_warp, the planar models "
+                         "affine_warp and homography_warp, and camera_rotation_warp, got %s" % (who, type(warpfunc).__name__))
     return warp
 
 
-def _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W):
-    """the scalar arguments the motion entries share: (warp code, (cx, cy), H, W, objective code, sigma, obj_param)"""
+def _centre(warp, warpfunc):
+    """the model's constants: (cx, cy), which the entries take behind K, followed for camera_rotation_warp by its focal
+    lengths (fx, fy), which _rows appends to every parameter row"""
     centre = tuple(float(c) for c in warpfunc.center) if warp in _CENTRED else (0.0, 0.0)
+    if warp == _lib.WARP_CAMERA_ROTATION:
+        centre += tuple(float(f) for f in warpfunc.focal)
+    return centre
+
+
+def _rows(params, centre):
+    """params (..., K) as the rows of the motion entries: for camera_rotation_warp (centre (cx, cy, fx, fy)) each row
+    (wx, wy, wz) becomes (wx, wy, wz, fx, fy), in f64.  Differentiable in params, so the focal-length columns of the
+    entries' gradient drop out through autograd; the two columns are fills on params' device, with no host round trip.
+    Any other model's params come back as they are."""
+    if len(centre) == 2:
+        return params
+    params = params.to(torch.float64)
+    return torch.cat([params] + [params.new_full(params.shape[:-1] + (1,), f) for f in centre[2:]], dim=-1)
+
+
+def _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W):
+    """the scalar arguments the motion entries share: (warp code, _centre, H, W, objective code, sigma, obj_param)"""
+    centre = _centre(warp, warpfunc)
     param = float(obj_param if obj_param is not None else DEFAULT_PARAM.get(objective, 0.0))
     return warp, centre, H, W, OBJECTIVES[objective], float(blur_sigma), param
 
 
 def _ts_model(warp, warpfunc, blur_sigma, H, W):
-    """the scalar arguments the motion timestamp entries share: (warp code, (cx, cy), H, W, sigma)"""
-    centre = tuple(float(c) for c in warpfunc.center) if warp in _CENTRED else (0.0, 0.0)
-    return warp, centre, H, W, float(blur_sigma)
+    """the scalar arguments the motion timestamp entries share: (warp code, _centre, H, W, sigma)"""
+    return warp, _centre(warp, warpfunc), H, W, float(blur_sigma)
 
 
 def _float_tensor(v, name):
@@ -170,13 +191,13 @@ def _pointers(tensors):
 
 def _model_layout(model, K):
     """the arguments of a motion entry in front of its parameter pointer, between the parameter count and (H, W), and
-    those its workspace query takes in front of (H, W): model = (warp, (cx, cy), H, W).  A grid-flow entry takes
-    model = ("grid", (gh, gw), H, W): its grids of K = 2 gh gw floats are followed by gh, gw, which its query takes too."""
+    those its workspace query takes in front of (H, W): model = (warp, _centre, H, W); K is the parameters per row
+    before _rows.  A grid-flow entry takes model = ("grid", (gh, gw), H, W): its grids of K = 2 gh gw floats are
+    followed by gh, gw, which its query takes too."""
     kind, extra, H, W = model
     if kind == "grid":
         return (), (), extra, extra, H, W
-    cx, cy = extra
-    return (kind,), (K, cx, cy), (), (), H, W
+    return (kind,), (K + len(extra) - 2, extra[0], extra[1]), (), (), H, W
 
 
 def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget, cap, M=None):
@@ -184,7 +205,8 @@ def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget,
     in passes of at most MAX_CANDIDATES candidate images per window over chunks of windows whose workspace
     (`stem`_workspace_bytes) fits `budget` and whose images number at most `cap`.  `events` are the arrays in front of
     the offsets and `scalars` the arguments behind W; model is _model_layout's.  With M, the entry scores M models per
-    window: the last of `events` is the memberships, c64 is (B,M,J,K) and f (B,M,J)."""
+    window: the last of `events` is the memberships, c64 is (B,M,J,K) and f (B,M,J).  camera_rotation_warp's candidates
+    reach the entry with their focal lengths (_rows)."""
     J, K = c64.shape[-2:]
     pre, mid, grid, query, H, W = _model_layout(model, K)
     B = c64.shape[0]
@@ -205,7 +227,7 @@ def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget,
         b1 = min(B, b0 + wb)
         for j0 in range(0, J, jc):
             j1 = min(J, j0 + jc)
-            c = c64[b0:b1, ..., j0:j1, :].contiguous()
+            c = _rows(c64[b0:b1, ..., j0:j1, :], model[1]).contiguous()
             out = torch.empty(c.shape[:-1], dtype=torch.float64, device=dev)
             _lib.check(entry(*front, _lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], *pre, _lib.ptr(c), j1 - j0,
                              *mid, *grid, H, W, *scalars, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream()))
@@ -221,7 +243,8 @@ def _chunked_objective(stem, key, events, offsets, model, scalars, images, budge
     canvases per window of each image the forward hands to the gradient.  With M, the entries score M models per window:
     the last of `events` is the memberships (they get no gradient), params is (B*M,K), f (B*M,) and g (B*M,K).  Without
     `gradient`, g is None and the gradient entry is not called.  A grid-flow entry takes the parameters (the nodes) and
-    returns their gradient in f32."""
+    returns their gradient in f32.  camera_rotation_warp's rows reach the entries with their focal lengths (_rows), and
+    g leaves out the entries' two focal-length columns."""
     ms, no_weight_gradient = ((), ()) if M is None else ((M,), (None,))
     rows = M or 1
     L = _lib.lib()
@@ -234,9 +257,9 @@ def _chunked_objective(stem, key, events, offsets, model, scalars, images, budge
         B = params.shape[0] // rows
         pre, mid, grid, query, H, W = _model_layout(model, K)
         dtype = torch.float32 if grid else torch.float64
-        prm = params.to(dtype).contiguous()
+        prm = _rows(params.to(dtype), model[1]).contiguous()
         f = torch.empty(B * rows, dtype=torch.float64, device=dev)
-        g = torch.empty((B * rows, K), dtype=dtype, device=dev) if gradient else None
+        g = torch.empty((B * rows, prm.shape[1]), dtype=dtype, device=dev) if gradient else None
         wb = fit_window_chunk(B, workspace_bytes(1, *ms, *query, H, W) + 4 * sum(images) * (H + 1) * (W + 1), budget, cap)
         kept = [torch.empty((wb * c, H + 1, W + 1), dtype=torch.float32, device=dev) for c in images]
         imgs = _pointers(kept)
@@ -251,5 +274,5 @@ def _chunked_objective(stem, key, events, offsets, model, scalars, images, budge
             if gradient:
                 _lib.check(grad(*ev, *imgs, _lib.ptr(ones), _lib.ptr(g[r0:r1]), *no_weight_gradient, _lib.ptr(ws),
                                 ws.numel(), _lib.stream()))
-        return f, (g.to(torch.float64) if g is not None else None)
+        return f, (g[:, :K].to(torch.float64) if g is not None else None)
     return fg

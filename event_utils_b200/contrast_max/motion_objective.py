@@ -13,7 +13,7 @@ from .. import _lib
 from ..representations import _events as E
 from ._batched import MAX_CANDIDATES  # noqa: F401  (a public name of this module)
 from ._batched import (_batch_events, _candidates_tensor, _check_objective, _chunked_candidates, _event_tensors, _model,
-                       _params_tensor, _warp_code)
+                       _params_tensor, _rows, _warp_code)
 
 
 def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, objective="variance", blur_sigma=1.0,
@@ -29,6 +29,8 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
         affine_warp         (hx, hy, a11, a12, a21, a22)            about warpfunc.center (warps.py has the formulas)
         homography_warp     (hx, hy, a11, a12, a21, a22, g1, g2)    about warpfunc.center; an event past the horizon
                                                                     (w <= 0) is not kept
+        camera_rotation_warp (wx, wy, wz)                           exact camera rotation with warpfunc's intrinsics;
+                                                                    an event behind the camera (Pz <= 0) is not kept
     An event is kept iff 0 < x' <= W and 0 < y' <= H with (H, W) = img_size (events_bounds_mask, event_util.py:26-27; a
     NaN position compares false and is kept, then contributes nothing, as in the single-window evaluation) and is splatted
     bilinearly on the (H+1, W+1) canvas (events_to_image_drv, image.py:179-217).  Then G = gaussian_filter(IWE,
@@ -44,7 +46,8 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
     @param xs, ys, ts, ps the concatenated events, (N,) tensors or arrays; they are data, not differentiable
     @param params (B,K) or (K,) for one sample, K = warpfunc.dims, any float dtype; the only differentiable input
            (expanded views work)
-    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp or homography_warp
+    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp, homography_warp or
+           camera_rotation_warp
     @param t0 None (each sample's last timestamp, get_iwe's ts[-1]), a number, or B values
     @param batch_end_indices the cumulative end indices of BaseVoxelDataset.collate_fn
            (lib/data_loaders/base_dataset.py:513-539), a list or an int64 tensor; None means one sample of all events
@@ -63,7 +66,8 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
     dev = E.compute_device(params, xs, ys, ts, ps)
     x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "parameter vectors")
     from ..autograd import MotionObjective
-    f = MotionObjective.apply(params, x, y, t_rel, p, offsets, _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W))
+    opts = _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W)
+    f = MotionObjective.apply(_rows(params, opts[1]), x, y, t_rel, p, offsets, opts)
     return f.to(device=params.device, dtype=params.dtype)
 
 

@@ -18,7 +18,7 @@ import torch
 from .. import _lib
 from ..representations import _events as E
 from ._batched import (_batch_events, _check_objective, _chunked_candidates, _chunked_objective, _event_tensors,
-                       _float_tensor, _model, _warp_code, _window_count, fit_window_chunk)
+                       _float_tensor, _model, _rows, _warp_code, _window_count, fit_window_chunk)
 from .motion_fit import FIT_WORKSPACE_BYTES, _batched_bfgs, _check_line_search_steps, _per_window
 
 MAX_MODELS = 8            # motion models per window
@@ -61,8 +61,8 @@ def motion_segmentation_objective_torch(xs, ys, ts, ps, weights, params, warpfun
     dev = E.compute_device(params, weights, xs, ys, ts, ps)
     x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "parameter sets")
     from ..autograd import MotionSegmentationObjective
-    f = MotionSegmentationObjective.apply(params, weights, x, y, t_rel, p, offsets,
-                                          _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W))
+    opts = _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W)
+    f = MotionSegmentationObjective.apply(_rows(params, opts[1]), weights, x, y, t_rel, p, offsets, opts)
     return f.to(device=params.device, dtype=params.dtype)
 
 
@@ -254,14 +254,16 @@ def _segment_objective_and_gradient(x, y, t_rel, p, w, offsets, M, opts, gradien
 def _assign(x, y, t_rel, p, w, offsets, p64, opts, eps):
     """the E-step on prepared device inputs: images of the memberships w under the models p64 (B,M,K) f64, then
     evk_cmax_motion_segment_assign_f32, in chunks of windows; rows outside every window are 1/M"""
-    warp, (cx, cy), H, W, _, sigma, _ = opts
-    B, M, K = p64.shape
+    warp, centre, H, W, _, sigma, _ = opts
+    cx, cy = centre[:2]
+    B, M, _ = p64.shape
     L = _lib.lib()
     dev = x.device
     out = torch.full((x.shape[0], M), 1.0 / M, dtype=torch.float32, device=dev)
     if B == 0:
         return out
-    prm = p64.contiguous()
+    prm = _rows(p64, centre).contiguous()
+    K = prm.shape[-1]
     wb = _segment_chunk(B, M, H, W)
     iwe = torch.empty((wb * M, H + 1, W + 1), dtype=torch.float32, device=dev)
     f = torch.empty(wb * M, dtype=torch.float64, device=dev)

@@ -13,7 +13,7 @@ import torch
 from .. import _lib
 from ..representations import _events as E
 from ._batched import (_candidates_tensor, _check_window_count, _chunked_candidates, _event_tensors, _params_tensor,
-                       _timestamp_events, _ts_model, _warp_code)
+                       _rows, _timestamp_events, _ts_model, _warp_code)
 
 
 def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, blur_sigma=2.0, timestamp_reverse=False,
@@ -28,6 +28,7 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
              pure_rotation_warp  (cx, cy, omega)       rotation about (cx, cy) by omega d
              xyztheta_warp       (hx, hy, hz, theta)   about warpfunc.center
              affine_warp, homography_warp           about warpfunc.center (warps.py; past the horizon: not kept)
+             camera_rotation_warp (wx, wy, wz)      exact camera rotation (warps.py; behind the camera: not kept)
       2. tau = (t - t_first_b) / (t_last_b - t_first_b + 1e-6), or (-t + t_last_b) / (...) with timestamp_reverse
          (image.py:324-327), formed in ts' dtype, then f32, as flow_timestamp_objective_torch forms it.
       3. An event contributes iff its f32 x', y' are finite, 0 < x' < W and 0 < y' < H with (H, W) = img_size: those are
@@ -44,7 +45,8 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
     @param xs, ys, ts, ps the concatenated events, (N,) tensors or arrays; they are data, not differentiable
     @param params (B,K) or (K,) for one sample, K = warpfunc.dims, any float dtype; the only differentiable input
            (expanded views work)
-    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp or homography_warp
+    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp, homography_warp or
+           camera_rotation_warp
     @param t0 None (each sample's last timestamp, zhu_timestamp_objective's ts[-1]), a number, or B values
     @param img_size (H, W): the bounds of step 3 and the canvas (H+1, W+1)
     @param batch_end_indices the cumulative end indices of BaseVoxelDataset.collate_fn
@@ -65,7 +67,8 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
     x, y, t_rel, tau, p, offsets = _timestamp_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "parameter vectors",
                                                      timestamp_reverse)
     from ..autograd import MotionTimestampObjective
-    f = MotionTimestampObjective.apply(params, x, y, t_rel, tau, p, offsets, _ts_model(warp, warpfunc, blur_sigma, H, W))
+    opts = _ts_model(warp, warpfunc, blur_sigma, H, W)
+    f = MotionTimestampObjective.apply(_rows(params, opts[1]), x, y, t_rel, tau, p, offsets, opts)
     return f.to(device=params.device, dtype=params.dtype)
 
 

@@ -208,3 +208,86 @@ class homography_warp(warp_function):
             jx = np.stack((-dt / w, nothing, -du / w, -dv / w, nothing, nothing, nx * du / w2, nx * dv / w2))
             jy = np.stack((nothing, -dt / w, nothing, nothing, -du / w, -dv / w, ny * du / w2, ny * dv / w2))
         return xw, yw, jx, jy
+
+
+def _intrinsics(camera_matrix):
+    """(fx, fy, cx, cy) of a 3x3 camera matrix without skew or of the four values themselves"""
+    k = np.asarray(camera_matrix, dtype=np.float64)
+    if k.shape == (3, 3):
+        if k[0, 1] != 0.0 or k[1, 0] != 0.0 or k[2, 0] != 0.0 or k[2, 1] != 0.0 or k[2, 2] != 1.0:
+            raise ValueError("camera_matrix must be [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] (no skew), got %s" % k.tolist())
+        k = np.array([k[0, 0], k[1, 1], k[0, 2], k[1, 2]])
+    elif k.shape != (4,):
+        raise ValueError("camera_matrix must be a 3x3 matrix or (fx, fy, cx, cy), got shape %s" % (k.shape,))
+    fx, fy, cx, cy = (float(v) for v in k)
+    if not (np.isfinite(k).all() and fx > 0.0 and fy > 0.0):
+        raise ValueError("the focal lengths must be finite and positive and the principal point finite, got fx=%r, "
+                         "fy=%r, cx=%r, cy=%r" % (fx, fy, cx, cy))
+    return fx, fy, cx, cy
+
+
+class camera_rotation_warp(warp_function):
+    """A rotating camera, exact in the rotation: params = (wx, wy, wz), the camera's angular velocity (rad/s) in its own
+    frame, with OpenCV's axes (x to the right, y down, z along the optical axis).  camera_matrix is the 3x3 K (no
+    skew) or (fx, fy, cx, cy); the events are pixel coordinates that have already been undistorted.  With dt = t - t0:
+        b = ((x - cx) / fx, (y - cy) / fy, 1),   theta = dt w,   phi = |theta|,   c = theta x b,   e = theta x c
+        P = exp([theta]x) b = (b + A c) + B e,   A = sin(phi) / phi,   B = (1 - cos(phi)) / phi^2
+        x' = cx + fx Px / Pz,   y' = cy + fy Py / Pz
+    with A = r cos(phi/2), B = r^2 / 2 and r = sin(phi/2) / (phi/2) (1 at phi = 0).  A camera whose orientation is
+    R(t0) exp([w]x dt) sees a static scene along the bearings exp(-[w]x dt) b(t0); the warp undoes that rotation.  So
+    with fx = fy, w = (0, 0, wz) is pure_rotation_warp(cx, cy, -wz).  With X = Px / Pz, Y = Py / Pz and the SO(3) left
+    Jacobian J_l = A I + B [theta]x + C theta theta^T, C = (phi - sin(phi)) / phi^3:
+        d x'/dw = -dt fx J_l^T (X Y, -(1 + X X), Y),      d y'/dw = -dt fy J_l^T (1 + Y Y, -X Y, -X)
+    f64 numpy, C from its series below phi = 1e-2.  An event with Pz <= 0 has rotated behind the camera: the batched
+    losses drop it like an event off the canvas (no contribution, no gradient); this warp() returns its formula
+    unchanged, which the reference API's bounds mask then judges.
+
+    The batched losses, their candidates passes, the fits and motion segmentation evaluate the model natively on the
+    GPU with K = 3 parameters: they append (fx, fy) to every row they hand the C entries (EVK_WARP_CAMERA_ROTATION,
+    whose rows are (wx, wy, wz, fx, fy) about the principal point center = (cx, cy)).  The reference-API objectives
+    take it through this warp() (fused_kind None).  homography_warp holds a rotation only to first order in dt w
+    (A = K [w]x K^-1), which misplaces the scene by about f phi^2 / 2 at the window's edge."""
+
+    def __init__(self, camera_matrix):
+        super().__init__('camera_rotation_warp', 3)
+        fx, fy, cx, cy = _intrinsics(camera_matrix)
+        self.focal = (fx, fy)
+        self.center = (cx, cy)
+
+    def model(self, params):
+        """the parameter block of the batched GPU evaluation: the angular velocity, the focal lengths (the row the C
+        entries take), then the principal point"""
+        return [float(v) for v in params[:3]] + list(self.focal) + list(self.center)
+
+    def warp(self, xs, ys, ts, ps, t0, params, compute_grad=False):
+        wx, wy, wz = (float(v) for v in params[:3])
+        fx, fy = self.focal
+        cx, cy = self.center
+        dt = ts - t0
+        bx, by = (xs - cx) / fx, (ys - cy) / fy
+        tx, ty, tz = dt * wx, dt * wy, dt * wz
+        p2 = (tx * tx + ty * ty) + tz * tz
+        phi = np.sqrt(p2)
+        half = 0.5 * phi
+        sh, ch = np.sin(half), np.cos(half)
+        r = np.where(phi > 0, sh / np.where(phi > 0, half, 1.0), 1.0)
+        A, B = r * ch, 0.5 * (r * r)
+        c0, c1, c2 = ty - tz * by, tz * bx - tx, tx * by - ty * bx
+        e0, e1, e2 = ty * c2 - tz * c1, tz * c0 - tx * c2, tx * c1 - ty * c0
+        Px, Py, Pz = (bx + A * c0) + B * e0, (by + A * c1) + B * e1, (1.0 + A * c2) + B * e2
+        with np.errstate(divide="ignore", invalid="ignore"):
+            xw, yw = cx + fx * Px / Pz, cy + fy * Py / Pz
+            if not compute_grad:
+                return xw, yw, None, None
+            X, Y = Px / Pz, Py / Pz
+            series = 1.0 / 6 - p2 * (1.0 / 120 - p2 * (1.0 / 5040))
+            C = np.where(phi < 1e-2, series, (phi - 2.0 * (sh * ch)) / np.where(phi < 1e-2, 1.0, p2 * phi))
+
+            def jlt(w0, w1, w2, s):
+                k0, k1, k2 = ty * w2 - tz * w1, tz * w0 - tx * w2, tx * w1 - ty * w0
+                q = C * ((tx * w0 + ty * w1) + tz * w2)
+                return np.stack((s * ((A * w0 - B * k0) + q * tx), s * ((A * w1 - B * k1) + q * ty),
+                                 s * ((A * w2 - B * k2) + q * tz)))
+            jx = jlt(X * Y, -(1.0 + X * X), Y, -(dt * fx))
+            jy = jlt(1.0 + Y * Y, -(X * Y), -X, -(dt * fy))
+        return xw, yw, jx, jy

@@ -89,22 +89,25 @@ struct CmaxArgs {
 
 enum { WARP_LINVEL_F64 = 0, WARP_LINVEL_F32 = 1, WARP_FLOW_F32 = 2,
        WARP_ROTATION_F64 = 3, WARP_ROTATION_F32 = 4, WARP_XYZTHETA_F64 = 5, WARP_XYZTHETA_F32 = 6,
-       WARP_AFFINE_F32 = 7, WARP_HOMOGRAPHY_F32 = 8 };
+       WARP_AFFINE_F32 = 7, WARP_HOMOGRAPHY_F32 = 8, WARP_CAMERA_ROTATION_F32 = 9 };
 
 __host__ __device__ constexpr bool is_model_warp(int w) { return w >= WARP_ROTATION_F64; }
 __host__ __device__ constexpr bool is_rotation(int w) { return w == WARP_ROTATION_F64 || w == WARP_ROTATION_F32; }
 __host__ __device__ constexpr bool is_linvel(int w) { return w == WARP_LINVEL_F64 || w == WARP_LINVEL_F32; }
 __host__ __device__ constexpr bool is_planar(int w) { return w == WARP_AFFINE_F32 || w == WARP_HOMOGRAPHY_F32; }
+// the camera rotation's row is (wx, wy, wz, fx, fy): the angular velocity, then the focal lengths
 __host__ __device__ constexpr int model_dims(int w)
 {
-    return is_linvel(w) ? 2 : is_rotation(w) ? 3 : w == WARP_AFFINE_F32 ? 6 : w == WARP_HOMOGRAPHY_F32 ? 8 : 4;
+    return is_linvel(w) ? 2 : is_rotation(w) ? 3 : w == WARP_AFFINE_F32 ? 6 : w == WARP_HOMOGRAPHY_F32 ? 8 :
+           w == WARP_CAMERA_ROTATION_F32 ? 5 : 4;
 }
 // length of the Jacobian rows model_taps fills (at least 4: the smaller models keep the rows they always had)
 __host__ __device__ constexpr int jac_dims(int w) { return model_dims(w) > 4 ? model_dims(w) : 4; }
 
 // The parameter block of a model as model_taps reads it: the K parameters, then the fixed centre (cx, cy) of xyztheta
-// and the planar models.  At least 6 doubles (WarpModel, the block of the single-window entries and of every model of
-// up to 4 parameters); the planar models take K + 2, so that the smaller models keep their registers and shared memory.
+// and the planar models (the principal point of the camera rotation).  At least 6 doubles (WarpModel, the block of the
+// single-window entries and of every model of up to 4 parameters); the larger models take K + 2, so that the smaller
+// models keep their registers and shared memory.
 __host__ __device__ constexpr int model_slots(int w) { return model_dims(w) + 2 > 6 ? model_dims(w) + 2 : 6; }
 template <int WARP>
 using ModelOf = ModelParams<model_slots(WARP)>;
@@ -300,12 +303,30 @@ __device__ __forceinline__ void ld_vec16(const double *p, double (&v)[2])
 //     dx'/d(hx .. a22) = affine's row / w,  dx'/d(g1, g2) = (nx dt u, nx dt v) / w^2  (y' likewise with ny)
 //     An event with w <= 0 or a non-finite w has crossed the horizon and is not kept.  With g1 = g2 = 0, w is 1 and
 //     the warp and Jacobian are affine's bit for bit; affine at (hx, hy, hz, -theta, theta, hz) is xyztheta's.
+//   camera rotation (wx, wy, wz, fx, fy) with the principal point (cx, cy), exact in the rotation, the batched passes
+//   only (f32): the camera's angular velocity in its own frame (x right, y down, z along the optical axis)
+//     b = ((x - cx) / fx, (y - cy) / fy, 1),  theta = dt w,  phi = |theta|,  c = theta x b,  e = theta x c
+//     P = exp([theta]x) b = (b + A c) + B e,  A = sin(phi) / phi,  B = (1 - cos(phi)) / phi^2
+//     X = Px iz,  Y = Py iz,  iz = 1 / Pz,  x' = cx + fx X,  y' = cy + fy Y
+//     A = r cos(phi/2) and B = r^2 / 2 with r = sin(phi/2) / (phi/2) (1 at phi = 0): no 0/0 and no 1 - cos.  The sine
+//     and cosine of phi/2 come from sincospif((phi/2) (1/pi)), whose exact argument reduction needs no local memory.
+//     An event with Pz <= 0 or a non-finite Pz has rotated behind the camera and is not kept.
+//     dP/dw = -dt [P]x J_l,  J_l = A I + B [theta]x + C theta theta^T (the SO(3) left
+//     Jacobian, C = (phi - sin(phi)) / phi^3, a series below kCamSeriesPhi), so
+//       dx'/dw = -dt fx J_l^T (X Y, -(1 + X X), Y),     dy'/dw = -dt fy J_l^T (1 + Y Y, -X Y, -X)
+//     and through b and the projection, with R e_x, R e_y the first two columns of exp([theta]x):
+//       dx'/dfx = X - (bx iz) ((R e_x)_x - X (R e_x)_z),   dy'/dfx = -(bx iz) (fy / fx) ((R e_x)_y - Y (R e_x)_z)
+//       dx'/dfy = -(by iz) (fx / fy) ((R e_y)_x - X (R e_y)_z),   dy'/dfy = Y - (by iz) ((R e_y)_y - Y (R e_y)_z)
 // in the order written (no FMA: the library builds with -fmad=false), f64 in parity mode, f32 in fast mode.
 // THE one place that turns an event into its bilinear footprint for these models: warp, bounds mask
 // (event_util.py:26-27), f64 -> f32 cast (image.py:180-183) and splat_taps -- the IWE pass and the gradient
 // pass call it alike, so they see identical taps.  JAC: also the f32 Jacobian rows jx[k] = dx'/dp_k, jy[k].
 __device__ __forceinline__ void sin_cos(double a, double *s, double *c) { sincos(a, s, c); }
 __device__ __forceinline__ void sin_cos(float a, float *s, float *c) { sincosf(a, s, c); }
+// below this rotation angle (rad) the camera rotation's C = (phi - sin phi) / phi^3 is its series: above it the f32
+// difference keeps about 6 eps / phi^2 of relative accuracy (2e-6 here), below it the series' first omitted term,
+// phi^8 / 39916800, is under 1e-10
+constexpr float kCamSeriesPhi = 0.5f;
 
 template <int WARP, bool JAC>
 __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> &e, const ModelOf<WARP> &M, unsigned &oob,
@@ -338,6 +359,46 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
             jx[0] = (float)((R)1 - c); jx[1] = (float)(-s); jx[2] = (float)(d * ry);
             jy[0] = (float)s; jy[1] = (float)((R)1 - c); jy[2] = (float)(-(d * rx));
             jx[3] = jy[3] = 0.0f;
+        }
+    } else if constexpr (WARP == WARP_CAMERA_ROTATION_F32) {
+        const R fx = (R)M.m[3], fy = (R)M.m[4], cx = (R)M.m[5], cy = (R)M.m[6];
+        const R bx = (e.x - cx) / fx, by = (e.y - cy) / fy;
+        const R tx = d * (R)M.m[0], ty = d * (R)M.m[1], tz = d * (R)M.m[2];
+        const R p2 = (tx * tx + ty * ty) + tz * tz;
+        const R phi = sqrtf(p2), half = (R)0.5 * phi;
+        R sh, ch;
+        sincospif(half * (R)0.318309886183790671, &sh, &ch);   // sin, cos of phi / 2, reduced exactly: no local memory
+        const R r = phi > (R)0 ? sh / half : (R)1;
+        const R A = r * ch, B = (R)0.5 * (r * r);
+        const R c0 = ty - tz * by, c1 = tz * bx - tx, c2 = tx * by - ty * bx;
+        const R e0 = ty * c2 - tz * c1, e1 = tz * c0 - tx * c2, e2 = tx * c1 - ty * c0;
+        const R Px = (bx + A * c0) + B * e0, Py = (by + A * c1) + B * e1, Pz = ((R)1 + A * c2) + B * e2;
+        if (!(Pz > (R)0) || isinf(Pz)) return false;   // behind the camera: not kept, like an event off the canvas
+        const R iz = (R)1 / Pz, X = Px * iz, Y = Py * iz;
+        xw = cx + fx * X;
+        yw = cy + fy * Y;
+        if (JAC) {
+            // (phi - sin phi) / phi^3 cancels in f32 for small phi: 1/6 - phi^2/120 + phi^4/5040 - phi^6/362880 there
+            const R C = phi < kCamSeriesPhi
+                            ? (R)(1.0 / 6) - p2 * ((R)(1.0 / 120) - p2 * ((R)(1.0 / 5040) - p2 * (R)(1.0 / 362880)))
+                            : (phi - (R)2 * (sh * ch)) / (p2 * phi);
+            // J_l^T w = A w - B (theta x w) + C theta (theta . w), scaled by s
+            auto jlt = [&](R w0, R w1, R w2, R s, float (&j)[jac_dims(WARP)]) {
+                const R k0 = ty * w2 - tz * w1, k1 = tz * w0 - tx * w2, k2 = tx * w1 - ty * w0;
+                const R q = C * ((tx * w0 + ty * w1) + tz * w2);
+                j[0] = s * ((A * w0 - B * k0) + q * tx);
+                j[1] = s * ((A * w1 - B * k1) + q * ty);
+                j[2] = s * ((A * w2 - B * k2) + q * tz);
+            };
+            jlt(X * Y, -((R)1 + X * X), Y, -(d * fx), jx);
+            jlt((R)1 + Y * Y, -(X * Y), -X, -(d * fy), jy);
+            const R rxx = (R)1 - B * (ty * ty + tz * tz), rxy = A * tz + B * (tx * ty), rxz = B * (tx * tz) - A * ty;
+            const R ryx = B * (tx * ty) - A * tz, ryy = (R)1 - B * (tx * tx + tz * tz), ryz = A * tx + B * (ty * tz);
+            const R ux = bx * iz, uy = by * iz;
+            jx[3] = X - ux * (rxx - X * rxz);
+            jy[3] = -(ux * (fy / fx)) * (rxy - Y * rxz);
+            jx[4] = -(uy * (fx / fy)) * (ryx - X * ryz);
+            jy[4] = Y - uy * (ryy - Y * ryz);
         }
     } else if constexpr (is_planar(WARP)) {
         constexpr int K = model_dims(WARP);
@@ -1680,9 +1741,9 @@ __device__ __forceinline__ void for_each_event_batch(int64_t first, int64_t last
     }
 }
 
-// Model `index` of params [..][K] into M as model_taps reads it (xyztheta and the planar models also take the fixed
-// centre, behind their K parameters), and `count` consecutive models from `first` into shared memory for the whole CTA.
-// M is filled in place: a model returned by value costs the linvel forward pass two registers.
+// Model `index` of params [..][K] into M as model_taps reads it (xyztheta, the planar models and the camera rotation
+// also take the fixed centre, behind their K parameters), and `count` consecutive models from `first` into shared
+// memory for the whole CTA.  M is filled in place: a model returned by value costs the linvel forward pass two registers.
 template <int WARP>
 __device__ __forceinline__ void load_model(const double *params, int64_t index, double cx, double cy, ModelOf<WARP> &M)
 {
@@ -2397,7 +2458,7 @@ static int grid_flow_node_grad(const GridArgs &A, int batch, float *grad_grid, c
 
 // ---- parametric motion objective over a batch of samples (evk_cmax_motion_objective_f32 / _grad_f32) ---------------
 // Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by its own model params[b] -- linvel, rotation,
-// xyztheta, affine or homography through model_taps, with the bounds mask of event_util.py:26-27 at img_size = (H, W) and the splat of
+// xyztheta, affine, homography or camera rotation through model_taps, with the bounds mask of event_util.py:26-27 at img_size = (H, W) and the splat of
 // image.py:179-217 on the (H+1)x(W+1) canvas -- then blurred and scored by the flow objective's image-space tail.  The
 // grid of both event passes is (slices, batch), as for the flow objective:
 //   forward:  one v4 reduction per kept event into the sample's 2x2-block image [B][Hc][Wc][4] (16 B per pixel)
@@ -2409,7 +2470,7 @@ struct ModelArgs {
     CmaxArgs C;              // canvas (Hc, Wc) and bounds mask (Hm, Wm) for model_taps; p_scale 1, t_ref 0
     EventSource E;
     const double *params;    // [B][M][J][K] on the device (M models per sample when segmenting, J candidates per model)
-    double cx, cy;           // the centre of xyztheta and the planar models
+    double cx, cy;           // the centre of xyztheta and the planar models, the camera rotation's principal point
     int M, J;
     float *acc;              // forward: the canvases' blocks
     const float *Wimg;       // contrast backward: W of every canvas [B][M][Hc][Wc]
@@ -2469,6 +2530,7 @@ static int motion_obj_dims(int warp)
     case EVK_WARP_XYZTHETA: return 4;
     case EVK_WARP_AFFINE: return 6;
     case EVK_WARP_HOMOGRAPHY: return 8;
+    case EVK_WARP_CAMERA_ROTATION: return 5;
     default: return 0;
     }
 }
@@ -2518,6 +2580,7 @@ static void with_model_warp(int warp, F f)
     else if (warp == EVK_WARP_ROTATION) f(std::integral_constant<int, WARP_ROTATION_F32>{});
     else if (warp == EVK_WARP_AFFINE) f(std::integral_constant<int, WARP_AFFINE_F32>{});
     else if (warp == EVK_WARP_HOMOGRAPHY) f(std::integral_constant<int, WARP_HOMOGRAPHY_F32>{});
+    else if (warp == EVK_WARP_CAMERA_ROTATION) f(std::integral_constant<int, WARP_CAMERA_ROTATION_F32>{});
     else f(std::integral_constant<int, WARP_XYZTHETA_F32>{});
 }
 
@@ -2863,7 +2926,7 @@ static const float2 *ts_obj_backward_ab(const BatchObjWorkspace &ws, const float
 
 // ---- parametric average-timestamp (Zhu) loss over a batch of samples (evk_motion_timestamp_objective_f32 / _grad_f32) --
 // Sample b = events [offsets[b], offsets[b+1]) (clipped to [0, n)) warped by its own model params[b] through model_taps
-// (linvel, rotation, xyztheta, affine or homography, f32, as the motion contrast loss warps), with weight 1: an event contributes iff its splat
+// (linvel, rotation, xyztheta, affine, homography or camera rotation, f32, as the motion contrast loss warps), with weight 1: an event contributes iff its splat
 // there is not zero (finite, 0 < x' < W, 0 < y' < H).  Then the images and f_b of the dense-flow timestamp loss above, on
 // the same 2B images z = 2b + s and through the same image-space halves (ts_obj_forward_tail, ts_obj_backward_ab):
 //   forward:  two v4 reductions per contributing event into the 32-byte block {S taps, C taps} of its polarity (the

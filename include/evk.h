@@ -555,14 +555,24 @@ int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const floa
  *   EVK_WARP_XYZTHETA  (hx, hy, hz, theta)     K = 4   about the centre (cx, cy) given here
  *   EVK_WARP_AFFINE    (hx, hy, a11, a12, a21, a22)            K = 6   about (cx, cy)
  *   EVK_WARP_HOMOGRAPHY (hx, hy, a11, a12, a21, a22, g1, g2)   K = 8   about (cx, cy)
- * (cx, cy) is the fixed centre of xyztheta, affine and homography and is ignored by the other models.  With
+ *   EVK_WARP_CAMERA_ROTATION (wx, wy, wz, fx, fy)              K = 5   principal point (cx, cy)
+ * (cx, cy) is the fixed centre of xyztheta, affine and homography and the principal point of the camera rotation,
+ * and is ignored by the other models.  With
  * d = t_rel, u = x - cx, v = y - cy, the two planar models are first order in d:
  *   affine:      sx = (hx + a11 u) + a12 v,  sy = (hy + a22 v) + a21 u,  x' = x - d sx,  y' = y - d sy
  *   homography:  sx, sy as affine, nx = u - d sx, ny = v - d sy, q = d ((g1 u) + (g2 v)), w = 1 - q,
  *                x' = (x - d sx) + nx q / w,  y' = (y - d sy) + ny q / w
  * An event whose w is <= 0 or not finite (past the homography's horizon) is not kept.  Affine at
  * (hx, hy, hz, -theta, theta, hz) is xyztheta bit for bit, and homography at g1 = g2 = 0 is affine bit for bit.
- * in f32, in the order written.  An event is kept iff 0 < x' <= W and 0 < y' <= H (events_bounds_mask,
+ * The camera rotation is exact in the rotation: w = (wx, wy, wz) is the camera's angular velocity (rad/s) in its own
+ * frame (x right, y down, z along the optical axis), fx, fy its focal lengths (px, no skew), and x, y undistorted:
+ *   b = ((x - cx) / fx, (y - cy) / fy, 1),  theta = d w,  phi = |theta|,  c = theta x b,  e = theta x c,
+ *   P = exp([theta]x) b = (b + A c) + B e,  A = sin(phi) / phi,  B = (1 - cos(phi)) / phi^2,
+ *   x' = cx + fx (Px iz),  y' = cy + fy (Py iz),  iz = 1 / Pz
+ * with A = r cos(phi/2), B = r^2 / 2, r = sin(phi/2) / (phi/2) (1 at phi = 0).  An event with Pz <= 0 or a non-finite
+ * Pz has rotated behind the camera and is not kept.  With fx = fy, w = (0, 0, wz) is EVK_WARP_ROTATION (cx, cy, -wz).
+ * grad_params carries the exact derivatives of all five values, the focal lengths included.
+ * All in f32, in the order written.  An event is kept iff 0 < x' <= W and 0 < y' <= H (events_bounds_mask,
  * lib/util/event_util.py:26-27; NaN compares false and is kept, then contributes nothing) and splatted
  * bilinearly on the (H+1)x(W+1) canvas (events_to_image_drv, lib/representations/image.py:179-217).  Then
  * G = gaussian_filter(IWE, sigma) and f is one of the four objectives of evk_cmax_flow_objective_f32
@@ -579,6 +589,7 @@ int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const floa
 #define EVK_WARP_LINVEL 3
 #define EVK_WARP_AFFINE 4
 #define EVK_WARP_HOMOGRAPHY 5
+#define EVK_WARP_CAMERA_ROTATION 6
 size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W);
 int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
                                   const int64_t *offsets, int batch, int64_t n_events, int warp,
@@ -705,7 +716,8 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
  * sign of a loss to minimise.  Sample b is the events [offsets[b], offsets[b+1]) (clipped to [0, n_events); end < start
  * is empty), warped by its own parameters params[b] (K doubles in DEVICE memory) with the model `warp` and its f32
  * arithmetic exactly as in evk_cmax_motion_objective_f32 (EVK_WARP_LINVEL / _ROTATION / _XYZTHETA / _AFFINE /
- * _HOMOGRAPHY; the centre (cx, cy) of xyztheta and the planar models).  An event contributes iff its splat in that loss is not zero: x', y' finite, 0 < x' < W and
+ * _HOMOGRAPHY / _CAMERA_ROTATION; the centre (cx, cy) of xyztheta and the planar models, the principal point of the
+ * camera rotation, whose events behind the camera are not kept).  An event contributes iff its splat in that loss is not zero: x', y' finite, 0 < x' < W and
  * 0 < y' < H (the bounds mask 0 < x' <= W, then the clip that gives x' = W zero weight).  A non-finite x' or y'
  * contributes nothing and does not poison the sample.  The reference instead zeroes the masked events and piles them
  * at (0, 0) as events with p = 0 and t = 0 (objectives.py:543-545).  tau and the images are those of

@@ -1,0 +1,372 @@
+"""The camera-rotation model (camera_rotation_warp, EVK_WARP_CAMERA_ROTATION) through every batched entry: the contrast
+and timestamp losses, their candidates passes, motion segmentation and its assignment, against the f64 references of
+tests/camera_rotation_reference.py, the focal-length gradient columns of the C entries, events behind the camera, host
+syncs and launch counts, and the fits' recovery of the angular velocity of a rotating camera from a grid search."""
+import ctypes
+
+import numpy as np
+import pytest
+import torch
+
+import camera_rotation_reference as R
+from conftest import assert_close_to_max
+
+pytestmark = pytest.mark.gpu
+
+H, W = 60, 80
+INTR = (70.3, 64.9, 43.7, 27.2)     # fx != fy, the principal point away from the canvas' centre (40, 30)
+CENTRE = INTR[2:]
+# phi = |w| |d| reaches 0.56 rad at d = -0.1: both sides of the kernel's series threshold for C (0.5)
+PARAMS = [(2.0, -3.0, 4.0), (-5.0, 1.5, -2.0), (3.5, 4.0, 1.0)]
+# Tolerances.  The kernel's f32 warp and the reference's f64 one differ by a few f32 ulps of the coordinates (about
+# 1e-5 px at 80 px) and by the ulp in which f32 and f64 sines may differ, so no tap moves (every event lies 1e-3 px
+# from the integers, below) and each bilinear weight differs by about 1e-5 relative.  The planar models, whose f32 warp
+# the reference restates op by op, meet their reference to 1e-5 on f; this model is held to 1e-4 on f and the images
+# and to 1e-3 of the largest component on the gradients, which sum those weight errors over many events.
+F_REL, IMG_REL, GRAD_REL = 1e-4, 1e-4, 1e-3
+
+
+def _warp(intr=INTR):
+    from event_utils_b200.contrast_max.warps import camera_rotation_warp
+    return camera_rotation_warp(intr)
+
+
+def _rows(params, intr=INTR):
+    """(..., 3) angular velocities -> (..., 5) rows (wx, wy, wz, fx, fy) of the C entries"""
+    p = np.asarray(params, np.float64)
+    return np.concatenate((p, np.broadcast_to(np.array(intr[:2]), p.shape[:-1] + (2,))), axis=-1)
+
+
+def safe_stream(seed, sizes, models, intr=INTR):
+    """Windows of random events in the sensor (d = t - t0 in [-0.1, 0] on a 2^-12 grid), keeping only the events whose
+    f64 warp under every model of their window lies at least 1e-3 px from every integer (or off the canvas by more than
+    that): f32 rounding cannot move their taps or keep decisions.  models[b]: the (M,3) angular velocities of window b."""
+    rng = np.random.default_rng(seed)
+    xs, ys, ds, ps, ends = [], [], [], [], []
+    for b, n in enumerate(sizes):
+        x = (rng.random(n) * (W - 1)).astype(np.float32)
+        y = (rng.random(n) * (H - 1)).astype(np.float32)
+        d = (-np.sort(rng.integers(0, 410, n))[::-1] / 4096.0).astype(np.float32)
+        ok = np.ones(n, bool)
+        for om in np.atleast_2d(models[b]) if n else []:
+            xw, yw = R.warp(x, y, d, om, intr)
+            for c in (xw, yw):
+                with np.errstate(invalid="ignore"):
+                    ok &= np.isfinite(c) & (np.abs(c - np.round(c)) >= 1e-3)
+        xs.append(x[ok]), ys.append(y[ok]), ds.append(d[ok])
+        ps.append((rng.integers(0, 2, int(ok.sum())) * 2 - 1).astype(np.float32))
+        ends.append(sum(a.size for a in xs))
+    off = np.array([0] + ends, np.int64)
+    return [np.concatenate(a) for a in (xs, ys, ds, ps)] + [off]
+
+
+def _cuda(*arrays):
+    return [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in arrays]
+
+
+def _ends(off):
+    return torch.from_numpy(off[1:]).cuda()
+
+
+def entry(stem, events, off, rows, scalars, outs, M=None, centre=CENTRE):
+    """a forward C entry with the 5-value rows: events as device tensors, outs the shapes of its f64 f and f32 images"""
+    from event_utils_b200 import _lib
+    L = _lib.lib()
+    B = len(off) - 1
+    prm = torch.tensor(np.asarray(rows, np.float64), device="cuda")
+    res = [torch.empty(s, dtype=torch.float64 if i == 0 else torch.float32, device="cuda") for i, s in enumerate(outs)]
+    ms = () if M is None else (M,)
+    ws = torch.empty(getattr(L, stem + "_workspace_bytes")(B, *ms, H, W), dtype=torch.uint8, device="cuda")
+    O = torch.from_numpy(off).cuda()
+    lead = [a.data_ptr() for a in events] + list(ms) + [O.data_ptr(), B, events[0].shape[0], _lib.WARP_CAMERA_ROTATION,
+                                                        prm.data_ptr(), prm.shape[-1], centre[0], centre[1], H, W]
+    _lib.check(getattr(L, stem + "_f32")(*lead, *scalars, *[r.data_ptr() for r in res], ws.data_ptr(), ws.numel(), None))
+    torch.cuda.synchronize()
+    # the call's arguments for c_gradient, with the tensors behind its pointers kept alive
+    return [r.cpu() for r in res], (lead, res, ws, (events, prm, O))
+
+
+def contrast_forward(x, y, d, p, off, rows, sigma=1.0, name="variance"):
+    B = len(off) - 1
+    return entry("evk_cmax_motion_objective", _cuda(x, y, d, p), off, rows, (sigma, {"variance": 0, "soe": 2}[name], 0.0),
+                 [(B,), (B, H + 1, W + 1)])
+
+
+def ts_forward(x, y, d, tau, p, off, rows, sigma=1.0):
+    B = len(off) - 1
+    return entry("evk_motion_timestamp_objective", _cuda(x, y, d, tau, p), off, rows, (sigma,),
+                 [(B,), (B, 2, H + 1, W + 1), (B, 2, H + 1, W + 1)])
+
+
+def seg_forward(x, y, d, p, w, off, rows, sigma=1.0):
+    B, M = len(off) - 1, w.shape[1]
+    return entry("evk_cmax_motion_segment", _cuda(x, y, d, p, w), off, rows, (sigma, 0, 0.0), [(B, M), (B, M, H + 1, W + 1)],
+                 M=M)
+
+
+def c_gradient(stem, call, scalars, gf):
+    """grad_params (B,5) of the gradient entry `stem`_grad_f32 after the forward `call` of entry(), at grad_f = gf"""
+    from event_utils_b200 import _lib
+    L = _lib.lib()
+    lead, res, ws, _ = call
+    g = torch.from_numpy(np.asarray(gf, np.float32)).cuda()
+    out = torch.empty((len(gf), 5), dtype=torch.float64, device="cuda")
+    _lib.check(getattr(L, stem + "_grad_f32")(*lead, *scalars, *[r.data_ptr() for r in res[1:]], g.data_ptr(),
+                                               out.data_ptr(), ws.data_ptr(), ws.numel(), None))
+    torch.cuda.synchronize()
+    return out.cpu().numpy()
+
+
+def loss(fn, x, y, d, p, off, params, **kw):
+    """(f with autograd, params leaf) of a torch loss, d reaching the kernel unchanged (t0 = 0)"""
+    prm = torch.tensor(np.asarray(params, np.float64), device="cuda", requires_grad=True)
+    f = fn(*_cuda(x, y, d, p), prm, _warp(), t0=0.0, blur_sigma=1.0, img_size=(H, W), batch_end_indices=_ends(off), **kw)
+    return f, prm
+
+
+def _batch_params(batch):
+    return PARAMS[:1] if batch == 1 else [PARAMS[0], PARAMS[1], PARAMS[1], PARAMS[2]]
+
+
+SIZES = {1: [20000], 3: [15000, 0, 12000, 9000]}
+
+
+@pytest.mark.parametrize("name", ["variance", "soe"])
+@pytest.mark.parametrize("batch", [1, 3])
+def test_contrast_loss_against_the_reference(name, batch):
+    from event_utils_b200.contrast_max import motion_contrast_candidates_torch, motion_contrast_objective_torch
+    params = _batch_params(batch)
+    x, y, d, p, off = safe_stream(7 + batch, SIZES[batch], params)
+    rows = _rows(params)
+    (f, iwe), call = contrast_forward(x, y, d, p, off, rows, 1.0, name)
+    p64 = torch.tensor(rows, dtype=torch.float64, requires_grad=True)
+    fr, iwer = R.contrast(x, y, d, p, off, p64, 1.0, name, CENTRE, img_size=(H, W))
+    for b in range(len(params)):
+        assert_close_to_max(iwe[b].numpy(), iwer[b].detach().numpy(), IMG_REL, "iwe %d" % b)
+        assert abs(f[b].item() - fr[b].item()) <= F_REL * max(abs(fr[b].item()), 1e-30), (b, f[b], fr[b])
+    g = np.random.default_rng(5).standard_normal(len(params))
+    (fr * torch.from_numpy(g)).sum().backward()
+    # the C entry's five columns, the focal lengths included
+    gc = c_gradient("evk_cmax_motion_objective", call, (1.0, {"variance": 0, "soe": 2}[name], 0.0), g)
+    assert_close_to_max(gc[:, :3], p64.grad.numpy()[:, :3], GRAD_REL, "C grad w %s" % name)
+    assert_close_to_max(gc[:, 3:], p64.grad.numpy()[:, 3:], GRAD_REL, "C grad f %s" % name)
+    # the torch loss: K = 3, its gradient the first three columns
+    fg, prm = loss(motion_contrast_objective_torch, x, y, d, p, off, params, objective=name)
+    np.testing.assert_allclose(fg.detach().cpu().numpy(), f.numpy(), rtol=1e-6, atol=0)
+    (fg * torch.from_numpy(g).cuda()).sum().backward()
+    assert prm.grad.shape == (len(params), 3)
+    assert_close_to_max(prm.grad.cpu().numpy(), p64.grad.numpy()[:, :3], GRAD_REL, "grad %s" % name)
+    cand = torch.tensor(params, dtype=torch.float64, device="cuda").unsqueeze(1).repeat(1, 3, 1)
+    fc = motion_contrast_candidates_torch(*_cuda(x, y, d, p), cand, _warp(), t0=0.0, objective=name, blur_sigma=1.0,
+                                          img_size=(H, W), batch_end_indices=_ends(off))
+    # f32 image sums in another order (atomics): equal to f32 rounding
+    np.testing.assert_allclose(fc.cpu().numpy(), f.unsqueeze(1).repeat(1, 3).numpy(), rtol=1e-6, atol=0)
+
+
+@pytest.mark.parametrize("batch", [1, 3])
+def test_timestamp_loss_against_the_reference(batch):
+    from event_utils_b200.contrast_max import motion_timestamp_candidates_torch, motion_timestamp_objective_torch
+    params = _batch_params(batch)
+    x, y, d, p, off = safe_stream(17 + batch, SIZES[batch], params)
+    tau = R.tau_f32(d, off)
+    rows = _rows(params)
+    (f, T, C), call = ts_forward(x, y, d, tau, p, off, rows)
+    p64 = torch.tensor(rows, dtype=torch.float64, requires_grad=True)
+    fr, Tr, Cr = R.timestamp(x, y, d, tau, p, off, p64, 1.0, CENTRE, img_size=(H, W))
+    for b in range(len(params)):
+        assert_close_to_max(T[b].numpy(), Tr[b].detach().numpy(), IMG_REL, "T %d" % b)
+        assert_close_to_max(C[b].numpy(), Cr[b].detach().numpy(), IMG_REL, "C %d" % b)
+        assert abs(f[b].item() - fr[b].item()) <= F_REL * max(abs(fr[b].item()), 1e-30), (b, f[b], fr[b])
+    g = np.random.default_rng(6).standard_normal(len(params))
+    (fr * torch.from_numpy(g)).sum().backward()
+    gc = c_gradient("evk_motion_timestamp_objective", call, (1.0,), g)
+    assert_close_to_max(gc[:, :3], p64.grad.numpy()[:, :3], GRAD_REL, "C ts grad w")
+    assert_close_to_max(gc[:, 3:], p64.grad.numpy()[:, 3:], GRAD_REL, "C ts grad f")
+    fg, prm = loss(motion_timestamp_objective_torch, x, y, d, p, off, params)
+    np.testing.assert_allclose(fg.detach().cpu().numpy(), f.numpy(), rtol=1e-6, atol=0)
+    (fg * torch.from_numpy(g).cuda()).sum().backward()
+    assert_close_to_max(prm.grad.cpu().numpy(), p64.grad.numpy()[:, :3], GRAD_REL, "ts grad")
+    cand = torch.tensor(params, dtype=torch.float64, device="cuda").unsqueeze(1).repeat(1, 2, 1)
+    fc = motion_timestamp_candidates_torch(*_cuda(x, y, d, p), cand, _warp(), t0=0.0, blur_sigma=1.0, img_size=(H, W),
+                                           batch_end_indices=_ends(off))
+    np.testing.assert_allclose(fc.cpu().numpy(), f.unsqueeze(1).repeat(1, 2).numpy(), rtol=1e-6, atol=0)
+
+
+def _memberships(n, M, seed):
+    w = np.random.default_rng(seed).random((n, M)).astype(np.float32)
+    return (w / w.sum(1, keepdims=True)).astype(np.float32)
+
+
+@pytest.mark.parametrize("batch", [1, 3])
+def test_segmentation_against_the_reference(batch):
+    from event_utils_b200.contrast_max import (motion_segmentation_assign_torch, motion_segmentation_candidates_torch,
+                                               motion_segmentation_objective_torch)
+    M = 2
+    B = 1 if batch == 1 else 4
+    params = np.array([[PARAMS[b % 3], PARAMS[(b + 1) % 3]] for b in range(B)])
+    x, y, d, p, off = safe_stream(27 + batch, [6000] if batch == 1 else [5000, 0, 4000, 3000], params)
+    w = _memberships(x.shape[0], M, 3)
+    (f, iwe), _ = seg_forward(x, y, d, p, w, off, _rows(params))
+    p64 = torch.tensor(_rows(params), dtype=torch.float64, requires_grad=True)
+    w64 = torch.tensor(w, dtype=torch.float64, requires_grad=True)
+    fr, iwer = R.segmentation(x, y, d, p, w64, off, p64, 1.0, "variance", CENTRE, img_size=(H, W))
+    for b in range(B):
+        for m in range(M):
+            assert_close_to_max(iwe[b, m].numpy(), iwer[b, m].detach().numpy(), IMG_REL, "iwe %d %d" % (b, m))
+    np.testing.assert_allclose(f.numpy(), fr.detach().numpy(), rtol=F_REL, atol=1e-30)
+    prm = torch.tensor(params, device="cuda", requires_grad=True)
+    wt = torch.from_numpy(w).cuda().requires_grad_(True)
+    ev = _cuda(x, y, d, p)
+    fg = motion_segmentation_objective_torch(*ev, wt, prm, _warp(), t0=0.0, blur_sigma=1.0, img_size=(H, W),
+                                             batch_end_indices=_ends(off))
+    np.testing.assert_allclose(fg.detach().cpu().numpy(), f.numpy(), rtol=1e-6, atol=0)
+    g = torch.from_numpy(np.random.default_rng(8).standard_normal((B, M)))
+    (fg * g.cuda()).sum().backward()
+    (fr * g).sum().backward()
+    assert_close_to_max(prm.grad.cpu().numpy(), p64.grad.numpy()[..., :3], GRAD_REL, "seg grad params")
+    assert_close_to_max(wt.grad.cpu().numpy(), w64.grad.numpy(), GRAD_REL, "seg grad weights")
+    cand = torch.tensor(params, device="cuda").unsqueeze(2).repeat(1, 1, 2, 1)
+    fc = motion_segmentation_candidates_torch(*ev, cand, wt.detach(), _warp(), t0=0.0, blur_sigma=1.0, img_size=(H, W),
+                                              batch_end_indices=_ends(off))
+    np.testing.assert_allclose(fc.cpu().numpy(), f.unsqueeze(2).repeat(1, 1, 2).numpy(), rtol=1e-6, atol=0)
+    wa = motion_segmentation_assign_torch(*ev, torch.tensor(params, device="cuda"), _warp(), torch.from_numpy(w).cuda(),
+                                          t0=0.0, blur_sigma=1.0, img_size=(H, W), batch_end_indices=_ends(off), eps=1e-6)
+    wr = R.assign(x, y, d, off, _rows(params), iwe.numpy(), 1.0, 1e-6, CENTRE, img_size=(H, W))
+    # to 1e-4 of the row sum: the torch function forms its own images, whose f32 sums meet in another order
+    np.testing.assert_allclose(wa.cpu().numpy(), wr, rtol=1e-5, atol=1e-4)
+
+
+def test_events_behind_the_camera_add_nothing():
+    """A wide field of view (fx = fy = 30 px on 80 x 60) and phi up to 1.8 rad: the events that rotate behind the
+    camera add nothing to f, the images or the gradient -- the stream of the kept events alone gives the same values,
+    up to summation order -- and the kept events match the reference"""
+    from event_utils_b200.contrast_max import motion_contrast_objective_torch
+    intr = (30.0, 30.0, 40.0, 30.0)
+    om = np.array([[11.0, -13.0, 6.0]])
+    rng = np.random.default_rng(51)
+    n = 20000
+    x = (rng.random(n) * (W - 1)).astype(np.float32)
+    y = (rng.random(n) * (H - 1)).astype(np.float32)
+    d = (-np.sort(rng.integers(0, 410, n))[::-1] / 4096.0).astype(np.float32)
+    p = (rng.integers(0, 2, n) * 2 - 1).astype(np.float32)
+    xw, yw = R.warp(x, y, d, om[0], intr)
+    behind = np.isnan(xw)
+    assert 0.02 < behind.mean() < 0.5, behind.mean()
+    # away from the integers, so that the kept events also meet the reference
+    with np.errstate(invalid="ignore"):
+        safe = behind | ((np.abs(xw - np.round(xw)) >= 1e-3) & (np.abs(yw - np.round(yw)) >= 1e-3))
+    x, y, d, p, behind = x[safe], y[safe], d[safe], p[safe], behind[safe]
+    off = np.array([0, x.size])
+    keep = ~behind
+    offk = np.array([0, int(keep.sum())])
+    rows = _rows(om, intr)
+    tau = R.tau_f32(d, off)
+
+    def fwd(stem, events, o, outs, scalars):
+        return entry(stem, events, o, rows, scalars, outs, centre=intr[2:])[0]
+    c_all = fwd("evk_cmax_motion_objective", _cuda(x, y, d, p), off, [(1,), (1, H + 1, W + 1)], (1.0, 0, 0.0))
+    c_kept = fwd("evk_cmax_motion_objective", _cuda(x[keep], y[keep], d[keep], p[keep]), offk, [(1,), (1, H + 1, W + 1)],
+                 (1.0, 0, 0.0))
+    np.testing.assert_allclose(c_all[1].numpy(), c_kept[1].numpy(), rtol=0, atol=1e-5 * c_all[1].abs().max().item())
+    np.testing.assert_allclose(c_all[0].numpy(), c_kept[0].numpy(), rtol=1e-6)
+    shapes = [(1,), (1, 2, H + 1, W + 1), (1, 2, H + 1, W + 1)]
+    t_all = fwd("evk_motion_timestamp_objective", _cuda(x, y, d, tau, p), off, shapes, (1.0,))
+    t_kept = fwd("evk_motion_timestamp_objective", _cuda(x[keep], y[keep], d[keep], tau[keep], p[keep]), offk, shapes, (1.0,))
+    np.testing.assert_allclose(t_all[0].numpy(), t_kept[0].numpy(), rtol=1e-6)
+    np.testing.assert_allclose(t_all[1].numpy(), t_kept[1].numpy(), rtol=0, atol=1e-6)
+    grads = []
+    for sel, o in ((np.ones(x.size, bool), off), (keep, offk)):
+        prm = torch.tensor(om, device="cuda", requires_grad=True)
+        f = motion_contrast_objective_torch(*_cuda(x[sel], y[sel], d[sel], p[sel]), prm, _warp(intr), t0=0.0,
+                                            img_size=(H, W), batch_end_indices=_ends(o))
+        f.sum().backward()
+        grads.append(prm.grad.cpu().numpy())
+    assert np.isfinite(grads[0]).all()
+    assert_close_to_max(grads[0], grads[1], 1e-6, "behind-the-camera grad")
+    p64 = torch.tensor(rows, dtype=torch.float64, requires_grad=True)
+    fr, _ = R.contrast(x, y, d, p, off, p64, 1.0, "variance", intr[2:], img_size=(H, W))
+    fr.sum().backward()
+    np.testing.assert_allclose(c_all[0].numpy(), fr.detach().numpy(), rtol=F_REL)
+    assert_close_to_max(grads[0], p64.grad.numpy()[:, :3], GRAD_REL, "behind-the-camera grad vs reference")
+
+
+def test_no_host_round_trips_and_constant_launch_count():
+    from event_utils_b200 import _lib
+    from event_utils_b200.contrast_max import motion_contrast_objective_torch, motion_timestamp_objective_torch
+    L = _lib.lib()
+    counts = []
+    for sizes in ([40000], [2500] * 16):
+        params = np.tile(np.array([PARAMS[0]]), (len(sizes), 1))
+        x, y, d, p, off = safe_stream(2, sizes, [params[:1]] * len(sizes))
+        ev = _cuda(x, y, d, p)
+        ends = _ends(off)
+        for _ in range(2):          # the first round warms up (scratch, library load)
+            prm = torch.tensor(params, device="cuda", requires_grad=True)
+            torch.cuda.synchronize()
+            L.evk_prof_enable(1)
+            torch.cuda.set_sync_debug_mode("error")
+            try:
+                f = motion_contrast_objective_torch(*ev, prm, _warp(), objective="soe", img_size=(H, W), batch_end_indices=ends)
+                g = motion_timestamp_objective_torch(*ev, prm, _warp(), img_size=(H, W), batch_end_indices=ends)
+                (f.sum() + g.sum()).backward()
+            finally:
+                torch.cuda.set_sync_debug_mode(0)
+            ms, timed, launches = ctypes.c_double(), ctypes.c_longlong(), ctypes.c_longlong()
+            _lib.check(L.evk_prof_collect(ctypes.byref(ms), ctypes.byref(timed), ctypes.byref(launches)))
+            L.evk_prof_enable(0)
+        assert torch.isfinite(prm.grad).all() and prm.grad.shape == (len(sizes), 3)
+        counts.append(launches.value)
+    assert counts[0] == counts[1] and counts[0] > 0, counts
+
+
+# ---- recovery from a grid search ------------------------------------------------------------------------------------
+CAMERA = (199.1, 198.7, 132.1, 110.8)        # fx, fy, cx, cy of a 180 x 240 camera
+TRUTHS = np.array([(1.3, -1.1, 1.2), (-2.5, 1.5, 0.8), (0.5, 3.5, -2.0), (4.0, 2.5, 1.0), (-3.0, -3.5, 2.0),
+                   (2.0, -4.5, -3.0), (-5.0, 2.0, 3.5), (6.0, 4.0, -3.0)])     # |w| = 2.1 .. 7.8 rad/s
+DURATION = 0.05
+
+
+def _rotation_windows(seed):
+    rng = np.random.default_rng(seed)
+    parts = [R.rotation_scene(om, CAMERA, rng, t_end=DURATION, duration=DURATION) for om in TRUTHS]
+    ends = np.cumsum([a[0].size for a in parts])
+    return parts, [np.concatenate(a) for a in zip(*parts)], ends
+
+
+def test_the_recovery_scene_needs_the_exact_model():
+    """No GPU arithmetic: in every window with |w| >= 5 rad/s (phi >= 0.25 rad over the window) the homography that
+    holds the rotation to first order misplaces the scene's events at the window's start by more than 3 px"""
+    from event_utils_b200.contrast_max.warps import homography_warp
+    parts, _, ends = _rotation_windows(81)
+    # 45 000 events per window, less those that leave the canvas (more of them the faster the camera turns)
+    assert all(35000 <= a[0].size <= 45000 for a in parts), [a[0].size for a in parts]
+    hom = homography_warp(center=CAMERA[2:])
+    for om, (x, y, t, _) in zip(TRUTHS, parts):
+        start = t < 0.1 * DURATION
+        xc, yc = R.warp(x[start], y[start], t[start] - DURATION, om, CAMERA)
+        xh, yh, _, _ = hom.warp(x[start], y[start], t[start], None, DURATION, R.embedding(om, CAMERA))
+        err = np.hypot(xc - xh, yc - yh).max()
+        if np.linalg.norm(om) >= 5.0:
+            assert err > 3.0, (om, err)
+
+
+# largest |w_fit - w_true| (rad/s) over the windows, from the grid search over [-10, 10]^3 (5 samples per axis, 3 levels)
+# and BFGS at blur 4, 2, 1; observed on an H100 (80 GB HBM3, 700 W), three runs
+RECOVERY = {"contrast": 0.08,      # observed 0.0398-0.0399 rad/s (0.010-0.040 per window)
+            "timestamp": 0.02}     # observed 0.0084 rad/s (0.001-0.008 per window)
+
+
+@pytest.mark.parametrize("loss_name", ["contrast", "timestamp"])
+def test_fits_recover_the_angular_velocity(loss_name):
+    from event_utils_b200.contrast_max import motion_contrast_fit_torch, motion_timestamp_fit_torch
+    fit_fn = motion_contrast_fit_torch if loss_name == "contrast" else motion_timestamp_fit_torch
+    _, (x, y, t, p), ends = _rotation_windows(81)
+    ev = [torch.from_numpy(x).float().cuda(), torch.from_numpy(y).float().cuda(), torch.from_numpy(t).cuda(),
+          torch.from_numpy(p).float().cuda()]
+    fit = fit_fn(*ev, _warp(CAMERA), batch_end_indices=torch.tensor(ends, device="cuda"), t0=DURATION,
+                 blur_sigma=[4.0, 2.0, 1.0], param_ranges=[[-10.0, 10.0]] * 3, num_samples_per_param=5, grid_levels=3)
+    got = fit.params.cpu().numpy()
+    assert got.shape == (len(TRUTHS), 3)
+    err = np.linalg.norm(got - TRUTHS, axis=1)
+    print("%s: |w - w_true| rad/s %s" % (loss_name, np.round(err, 4)))
+    assert err.max() <= RECOVERY[loss_name], (err, got)
