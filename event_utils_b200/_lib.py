@@ -41,6 +41,7 @@ CMAX_NO_CHANNEL_MIX = 0x40
 OBJ_VARIANCE, OBJ_SOS, OBJ_SOE, OBJ_MOA, OBJ_ISOA, OBJ_SOSA = range(6)
 WARP_ROTATION, WARP_XYZTHETA, WARP_LINVEL = 1, 2, 3
 WARP_AFFINE, WARP_HOMOGRAPHY, WARP_CAMERA_ROTATION = 4, 5, 6      # the batched motion entries only (evk.h)
+WARP_CAMERA_MOTION = 7      # the batched motion entries with inverse depth (evk_*_depth_*) only
 
 _lib = None
 _lock = threading.Lock()
@@ -189,6 +190,19 @@ def _declare(L):
     L.evk_cmax_motion_candidates_f32.restype = ci
     L.evk_cmax_motion_candidates_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, ci, f64, f64, ci, ci, f64, ci, f64, vp,
                                                  vp, sz, vp]
+    L.evk_cmax_motion_depth_objective_workspace_bytes.restype = sz
+    L.evk_cmax_motion_depth_objective_workspace_bytes.argtypes = [ci, ci, ci]
+    L.evk_cmax_motion_depth_objective_f32.restype = ci
+    L.evk_cmax_motion_depth_objective_f32.argtypes = [vp, vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci, f64, ci, f64,
+                                                      vp, vp, vp, sz, vp]
+    L.evk_cmax_motion_depth_objective_grad_f32.restype = ci
+    L.evk_cmax_motion_depth_objective_grad_f32.argtypes = [vp, vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci, f64, ci,
+                                                           f64, vp, vp, vp, vp, sz, vp]
+    L.evk_cmax_motion_depth_candidates_workspace_bytes.restype = sz
+    L.evk_cmax_motion_depth_candidates_workspace_bytes.argtypes = [ci, ci, ci, ci]
+    L.evk_cmax_motion_depth_candidates_f32.restype = ci
+    L.evk_cmax_motion_depth_candidates_f32.argtypes = [vp, vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, ci, f64, f64, ci, ci, f64, ci,
+                                                       f64, vp, vp, sz, vp]
     L.evk_cmax_motion_segment_workspace_bytes.restype = sz
     L.evk_cmax_motion_segment_workspace_bytes.argtypes = [ci, ci, ci, ci]
     L.evk_cmax_motion_segment_f32.restype = ci
@@ -225,6 +239,19 @@ def _declare(L):
     L.evk_motion_timestamp_candidates_f32.restype = ci
     L.evk_motion_timestamp_candidates_f32.argtypes = [vp, vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, ci, f64, f64, ci, ci, f64,
                                                       vp, vp, sz, vp]
+    L.evk_motion_timestamp_depth_objective_workspace_bytes.restype = sz
+    L.evk_motion_timestamp_depth_objective_workspace_bytes.argtypes = [ci, ci, ci]
+    L.evk_motion_timestamp_depth_objective_f32.restype = ci
+    L.evk_motion_timestamp_depth_objective_f32.argtypes = [vp, vp, vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci, f64,
+                                                           vp, vp, vp, vp, sz, vp]
+    L.evk_motion_timestamp_depth_objective_grad_f32.restype = ci
+    L.evk_motion_timestamp_depth_objective_grad_f32.argtypes = [vp, vp, vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, f64, f64, ci, ci,
+                                                                f64, vp, vp, vp, vp, vp, sz, vp]
+    L.evk_motion_timestamp_depth_candidates_workspace_bytes.restype = sz
+    L.evk_motion_timestamp_depth_candidates_workspace_bytes.argtypes = [ci, ci, ci, ci]
+    L.evk_motion_timestamp_depth_candidates_f32.restype = ci
+    L.evk_motion_timestamp_depth_candidates_f32.argtypes = [vp, vp, vp, vp, vp, vp, vp, ci, i64, ci, vp, ci, ci, f64, f64, ci, ci,
+                                                            f64, vp, vp, sz, vp]
     L.evk_grid_flow_timestamp_objective_workspace_bytes.restype = sz
     L.evk_grid_flow_timestamp_objective_workspace_bytes.argtypes = [ci, ci, ci, ci, ci]
     L.evk_grid_flow_timestamp_objective_f32.restype = ci

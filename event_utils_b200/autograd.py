@@ -317,19 +317,23 @@ class MotionObjective(torch.autograd.Function):
     the linvel, rotation or 4-DoF model, then an objective of objectives.py): f (B,) f64 from params (B,K) and the
     prepared device events.  Only the parameters get a gradient: the exact derivative of f, one pass over the events
     (evk_cmax_motion_objective_grad_f32).  opts = (warp code, centre, H, W, objective, sigma, obj_param); params are the
-    rows the entries take (contrast_max/_batched._rows), so K = 5 for the camera rotation."""
+    rows the entries take (contrast_max/_batched._rows), so K = 5 for the camera rotation and 8 for the camera motion.
+    rho: None, or camera_motion_warp's inverse depth of every event (f32 on the events' device), which routes the loss to
+    the depth entries (evk_cmax_motion_depth_objective_f32 / _grad_f32); it gets no gradient."""
 
     @staticmethod
-    def forward(ctx, params, x, y, t_rel, p, offsets, opts):
+    def forward(ctx, params, x, y, t_rel, p, offsets, opts, rho=None):
+        from .contrast_max._batched import _depth_entry
         warp, centre, H, W, objective, sigma, param = opts
         cx, cy = centre[:2]
-        return _loss_forward(ctx, "evk_cmax_motion_objective", "motion_objective", params, torch.float64, (warp,),
-                             (params.shape[-1], cx, cy, H, W, sigma, objective, param), (H, W), (x, y, t_rel, p), offsets, (1,))
+        stem, events = _depth_entry("evk_cmax_motion_objective", (x, y, t_rel, p), rho)
+        return _loss_forward(ctx, stem, "motion_objective", params, torch.float64, (warp,),
+                             (params.shape[-1], cx, cy, H, W, sigma, objective, param), (H, W), events, offsets, (1,))
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        return _loss_backward(ctx, g)[:1] + (None,) * 6
+        return _loss_backward(ctx, g)[:1] + (None,) * 7
 
 
 class MotionSegmentationObjective(torch.autograd.Function):
@@ -358,19 +362,22 @@ class MotionTimestampObjective(torch.autograd.Function):
     (zhu_timestamp_objective, objectives.py:524-558, with the linvel, rotation or 4-DoF model): f (B,) f64 from params
     (B,K) and the prepared device events with their normalised stamps tau.  Only the parameters get a gradient: the exact
     derivative of f, one pass over the events (evk_motion_timestamp_objective_grad_f32).  The forward keeps the timestamp
-    and count images.  opts = (warp code, centre, H, W, sigma); params are the entries' rows (_batched._rows)."""
+    and count images.  opts = (warp code, centre, H, W, sigma); params are the entries' rows (_batched._rows).  rho is
+    MotionObjective's: camera_motion_warp's inverse depth, through the depth entries, or None."""
 
     @staticmethod
-    def forward(ctx, params, x, y, t_rel, tau, p, offsets, opts):
+    def forward(ctx, params, x, y, t_rel, tau, p, offsets, opts, rho=None):
+        from .contrast_max._batched import _depth_entry
         warp, centre, H, W, sigma = opts
         cx, cy = centre[:2]
-        return _loss_forward(ctx, "evk_motion_timestamp_objective", "motion_timestamp_objective", params, torch.float64,
-                             (warp,), (params.shape[-1], cx, cy, H, W, sigma), (H, W), (x, y, t_rel, tau, p), offsets, (2, 2))
+        stem, events = _depth_entry("evk_motion_timestamp_objective", (x, y, t_rel, tau, p), rho)
+        return _loss_forward(ctx, stem, "motion_timestamp_objective", params, torch.float64,
+                             (warp,), (params.shape[-1], cx, cy, H, W, sigma), (H, W), events, offsets, (2, 2))
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        return _loss_backward(ctx, g)[:1] + (None,) * 7
+        return _loss_backward(ctx, g)[:1] + (None,) * 8
 
 
 class VoxelGrid(torch.autograd.Function):

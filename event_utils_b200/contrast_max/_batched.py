@@ -8,15 +8,18 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from .warps import affine_warp, camera_rotation_warp, homography_warp, linvel_warp, pure_rotation_warp, xyztheta_warp
+from .warps import (affine_warp, camera_motion_warp, camera_rotation_warp, homography_warp, linvel_warp, pure_rotation_warp,
+                    xyztheta_warp)
 
 OBJECTIVES = {"variance": _lib.OBJ_VARIANCE, "sos": _lib.OBJ_SOS, "soe": _lib.OBJ_SOE, "sosa": _lib.OBJ_SOSA}
 DEFAULT_PARAM = {"sosa": 3.0}   # sosa_objective(p=3)
 _WARPS = ((linvel_warp, _lib.WARP_LINVEL), (pure_rotation_warp, _lib.WARP_ROTATION), (xyztheta_warp, _lib.WARP_XYZTHETA),
           (affine_warp, _lib.WARP_AFFINE), (homography_warp, _lib.WARP_HOMOGRAPHY),
-          (camera_rotation_warp, _lib.WARP_CAMERA_ROTATION))
-# the models about a fixed centre (cx, cy), the camera rotation's principal point
-_CENTRED = (_lib.WARP_XYZTHETA, _lib.WARP_AFFINE, _lib.WARP_HOMOGRAPHY, _lib.WARP_CAMERA_ROTATION)
+          (camera_rotation_warp, _lib.WARP_CAMERA_ROTATION), (camera_motion_warp, _lib.WARP_CAMERA_MOTION))
+# the models about a fixed centre (cx, cy), the camera models' principal point
+_CENTRED = (_lib.WARP_XYZTHETA, _lib.WARP_AFFINE, _lib.WARP_HOMOGRAPHY, _lib.WARP_CAMERA_ROTATION, _lib.WARP_CAMERA_MOTION)
+# the camera models, whose rows carry their focal lengths (_rows)
+_FOCAL = (_lib.WARP_CAMERA_ROTATION, _lib.WARP_CAMERA_MOTION)
 MAX_CANDIDATES = 32   # parameter vectors per window and pass over the events
 MAX_GRID_CANDIDATE_NODES = 12288   # candidates times nodes of a grid-flow candidates pass (the grids a CTA holds)
 
@@ -33,22 +36,60 @@ def _warp_code(warpfunc, who):
     warp = next((code for cls, code in _WARPS if type(warpfunc) is cls), None)
     if warp is None:
         raise ValueError("%s supports the models linvel_warp, pure_rotation_warp and xyztheta_warp, the planar models "
-                         "affine_warp and homography_warp, and camera_rotation_warp, got %s" % (who, type(warpfunc).__name__))
+                         "affine_warp and homography_warp, and camera_rotation_warp and camera_motion_warp, got %s"
+                         % (who, type(warpfunc).__name__))
     return warp
 
 
+def _depth_tensor(inv_depth, warp, n, who):
+    """The checks of inv_depth, before any CUDA call: the camera_motion_warp's inverse depth of every event is required
+    with that model and rejected with any other; an (N,) float array aligned with the concatenated events, data (no
+    grad).  Returns it flat, or None."""
+    if warp != _lib.WARP_CAMERA_MOTION:
+        if inv_depth is not None:
+            raise ValueError("%s: inv_depth is the per-event inverse depth of camera_motion_warp; the other models take "
+                             "none" % who)
+        return None
+    if inv_depth is None:
+        raise ValueError("%s: camera_motion_warp needs inv_depth, the inverse depth of every event (an (N,) array aligned "
+                         "with the events)" % who)
+    rho = _float_tensor(inv_depth, "inv_depth")
+    if rho.requires_grad:
+        raise ValueError("%s: inv_depth is data and must not require grad (detach it)" % who)
+    if rho.dim() != 1 or rho.shape[0] != n:
+        raise ValueError("%s: inv_depth must have shape (%d,), one value per event, got %s" % (who, n, tuple(rho.shape)))
+    return rho
+
+
+def _depth_events(rho, dev):
+    """the checked inverse depth as the depth entries take it, f32 on dev (None stays None)"""
+    if rho is None:
+        return None
+    with torch.cuda.device(dev):
+        return E.to_device(rho, dev).to(torch.float32).contiguous()
+
+
+def _depth_entry(stem, events, rho):
+    """the entry stem and event arrays of a motion loss: the depth twin of `stem` (evk_cmax_motion_objective ->
+    evk_cmax_motion_depth_objective), which takes the inverse depth right after the other event arrays, when rho is given"""
+    if rho is None:
+        return stem, events
+    head, tail = stem.rsplit("_", 1)
+    return "%s_depth_%s" % (head, tail), tuple(events) + (rho,)
+
+
 def _centre(warp, warpfunc):
-    """the model's constants: (cx, cy), which the entries take behind K, followed for camera_rotation_warp by its focal
-    lengths (fx, fy), which _rows appends to every parameter row"""
+    """the model's constants: (cx, cy), which the entries take behind K, followed for camera_rotation_warp and
+    camera_motion_warp by their focal lengths (fx, fy), which _rows appends to every parameter row"""
     centre = tuple(float(c) for c in warpfunc.center) if warp in _CENTRED else (0.0, 0.0)
-    if warp == _lib.WARP_CAMERA_ROTATION:
+    if warp in _FOCAL:
         centre += tuple(float(f) for f in warpfunc.focal)
     return centre
 
 
 def _rows(params, centre):
     """params (..., K) as the rows of the motion entries: for camera_rotation_warp (centre (cx, cy, fx, fy)) each row
-    (wx, wy, wz) becomes (wx, wy, wz, fx, fy), in f64.  Differentiable in params, so the focal-length columns of the
+    (wx, wy, wz) becomes (wx, wy, wz, fx, fy), in f64, and camera_motion_warp's (wx, wy, wz, vx, vy, vz) likewise.  Differentiable in params, so the focal-length columns of the
     entries' gradient drop out through autograd; the two columns are fills on params' device, with no host round trip.
     Any other model's params come back as they are."""
     if len(centre) == 2:
@@ -205,8 +246,9 @@ def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget,
     in passes of at most MAX_CANDIDATES candidate images per window over chunks of windows whose workspace
     (`stem`_workspace_bytes) fits `budget` and whose images number at most `cap`.  `events` are the arrays in front of
     the offsets and `scalars` the arguments behind W; model is _model_layout's.  With M, the entry scores M models per
-    window: the last of `events` is the memberships, c64 is (B,M,J,K) and f (B,M,J).  camera_rotation_warp's candidates
-    reach the entry with their focal lengths (_rows)."""
+    window: the last of `events` is the memberships, c64 is (B,M,J,K) and f (B,M,J).  The camera models' candidates
+    reach the entry with their focal lengths (_rows); camera_motion_warp's `events` end with the inverse depth
+    (_depth_entry)."""
     J, K = c64.shape[-2:]
     pre, mid, grid, query, H, W = _model_layout(model, K)
     B = c64.shape[0]
@@ -243,7 +285,7 @@ def _chunked_objective(stem, key, events, offsets, model, scalars, images, budge
     canvases per window of each image the forward hands to the gradient.  With M, the entries score M models per window:
     the last of `events` is the memberships (they get no gradient), params is (B*M,K), f (B*M,) and g (B*M,K).  Without
     `gradient`, g is None and the gradient entry is not called.  A grid-flow entry takes the parameters (the nodes) and
-    returns their gradient in f32.  camera_rotation_warp's rows reach the entries with their focal lengths (_rows), and
+    returns their gradient in f32.  The camera models' rows reach the entries with their focal lengths (_rows), and
     g leaves out the entries' two focal-length columns."""
     ms, no_weight_gradient = ((), ()) if M is None else ((M,), (None,))
     rows = M or 1

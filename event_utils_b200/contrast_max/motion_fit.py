@@ -16,7 +16,8 @@ import torch
 from .. import _lib
 from ..representations import _events as E
 from ._batched import fit_window_chunk  # noqa: F401  (a public name of this module)
-from ._batched import _batch_events, _check_objective, _chunked_objective, _event_tensors, _model, _warp_code, _window_count
+from ._batched import (_batch_events, _check_objective, _chunked_objective, _depth_entry, _depth_events, _depth_tensor,
+                       _event_tensors, _model, _warp_code, _window_count)
 from .motion_objective import _candidates
 
 MotionFit = collections.namedtuple("MotionFit", "params f status iterations")
@@ -30,7 +31,7 @@ ARMIJO_C1 = 1e-4
 def motion_contrast_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None, t0=None, objective="variance",
                               blur_sigma=1.0, obj_param=None, img_size=(180, 240), x0=None, param_ranges=None,
                               num_samples_per_param=5, grid_levels=1, log_scale=False, param_scale=None, max_iter=50,
-                              line_search_steps=8, ftol=1e-9, gtol=1e-9):
+                              line_search_steps=8, ftol=1e-9, gtol=1e-9, inv_depth=None):
     """
     Minimise the f_b of motion_contrast_objective_torch over the parameters of every window b on its own, all windows at
     once.  The windows, t0, objective, obj_param and img_size are those of motion_contrast_objective_torch, so any result
@@ -57,6 +58,9 @@ def motion_contrast_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None, 
     values bit for bit while the others iterate.
     blur_sigma may be a sequence: stage i refines at blur_sigma[i] from stage i-1's result, and the grid search runs
     at blur_sigma[0] only (grid_cmax's grid at blur 2, then refinement at 1, events_cmax.py:28-76).
+    camera_motion_warp takes inv_depth, the inverse depth of every event (motion_contrast_objective_torch).  A grid over
+    its six parameters costs num_samples_per_param^6 candidates per window, so start it from x0: a camera_rotation_warp
+    fit embedded as (w, 0, 0, 0), or an IMU's rates and velocity.
     Every stage runs exactly max_iter iterations on all windows (max_iter = 0 returns the start), so with the events,
     the window ends and x0 (or param_ranges) on the GPU the fit never synchronises with the host.
     Any number of windows B: each candidates call runs the windows in chunks of
@@ -72,16 +76,19 @@ def motion_contrast_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None, 
     warp = _warp_code(warpfunc, "motion_contrast_fit_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_contrast_fit_torch", "nothing")
+    rho = _depth_tensor(inv_depth, warp, xs.shape[0], "motion_contrast_fit_torch")
     sigmas = _fit_arguments("motion_contrast_fit_torch", blur_sigma, line_search_steps, x0, param_ranges)
     H, W = int(img_size[0]), int(img_size[1])
     _lib.lib()
     dev = E.compute_device(*(a for a in (x0, param_ranges, xs, ys, ts, ps) if isinstance(a, torch.Tensor)))
     B = _window_count(batch_end_indices)
     x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows")
+    rho = _depth_events(rho, dev)
 
     def stage(sigma):
         opts = _model(warp, warpfunc, objective, sigma, obj_param, H, W)
-        return _objective_and_gradient(x, y, t_rel, p, offsets, opts), lambda c: _candidates(x, y, t_rel, p, offsets, c, opts)
+        return (_objective_and_gradient(x, y, t_rel, p, offsets, opts, rho),
+                lambda c: _candidates(x, y, t_rel, p, offsets, c, opts, rho))
     with torch.cuda.device(dev):
         return _fit_stages(stage, sigmas, B, warpfunc.dims, dev, x0, param_ranges, num_samples_per_param, grid_levels,
                            log_scale, param_scale, max_iter, line_search_steps, ftol, gtol)
@@ -166,12 +173,14 @@ FIT_MAX_WINDOWS = 65535
 FIT_WORKSPACE_BYTES = 4 << 30
 
 
-def _objective_and_gradient(x, y, t_rel, p, offsets, opts):
-    """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_cmax_motion_objective_f32 / _grad_f32 (grad_f = 1), in
-    chunks of windows (fit_window_chunk); the windows are independent, so a chunk changes no value's arithmetic"""
+def _objective_and_gradient(x, y, t_rel, p, offsets, opts, rho=None):
+    """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_cmax_motion_objective_f32 / _grad_f32 (grad_f = 1), or
+    their depth twins with camera_motion_warp's device inverse depth rho, in chunks of windows (fit_window_chunk); the
+    windows are independent, so a chunk changes no value's arithmetic"""
     warp, centre, H, W, objective, sigma, param = opts
-    return _chunked_objective("evk_cmax_motion_objective", "motion_objective", (x, y, t_rel, p), offsets, (warp, centre, H, W),
-                              (sigma, objective, param), (1,), FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS)
+    stem, events = _depth_entry("evk_cmax_motion_objective", (x, y, t_rel, p), rho)
+    return _chunked_objective(stem, "motion_objective", events, offsets, (warp, centre, H, W), (sigma, objective, param), (1,),
+                              FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS)
 
 
 def _grid_axes(ranges, num_samples_per_param, log_scale):

@@ -12,12 +12,12 @@ import torch
 from .. import _lib
 from ..representations import _events as E
 from ._batched import MAX_CANDIDATES  # noqa: F401  (a public name of this module)
-from ._batched import (_batch_events, _candidates_tensor, _check_objective, _chunked_candidates, _event_tensors, _model,
-                       _params_tensor, _rows, _warp_code)
+from ._batched import (_batch_events, _candidates_tensor, _check_objective, _chunked_candidates, _depth_entry,
+                       _depth_events, _depth_tensor, _event_tensors, _model, _params_tensor, _rows, _warp_code)
 
 
 def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, objective="variance", blur_sigma=1.0,
-                                    obj_param=None, img_size=(180, 240), batch_end_indices=None):
+                                    obj_param=None, img_size=(180, 240), batch_end_indices=None, inv_depth=None):
     """
     Contrast objective f_b of every sample b of a batch of event windows, each warped by its own motion params[b].
     Sample b holds the events [start_b, end_b) of the concatenated stream, end_b = batch_end_indices[b] and start_b the
@@ -31,6 +31,10 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
                                                                     (w <= 0) is not kept
         camera_rotation_warp (wx, wy, wz)                           exact camera rotation with warpfunc's intrinsics;
                                                                     an event behind the camera (Pz <= 0) is not kept
+        camera_motion_warp  (wx, wy, wz, vx, vy, vz)                exact camera rotation and translation with the
+                                                                    events' inverse depth inv_depth (warps.py); an
+                                                                    event behind the camera or with a negative or
+                                                                    non-finite inverse depth is not kept
     An event is kept iff 0 < x' <= W and 0 < y' <= H with (H, W) = img_size (events_bounds_mask, event_util.py:26-27; a
     NaN position compares false and is kept, then contributes nothing, as in the single-window evaluation) and is splatted
     bilinearly on the (H+1, W+1) canvas (events_to_image_drv, image.py:179-217).  Then G = gaussian_filter(IWE,
@@ -46,11 +50,14 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
     @param xs, ys, ts, ps the concatenated events, (N,) tensors or arrays; they are data, not differentiable
     @param params (B,K) or (K,) for one sample, K = warpfunc.dims, any float dtype; the only differentiable input
            (expanded views work)
-    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp, homography_warp or
-           camera_rotation_warp
+    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp, homography_warp,
+           camera_rotation_warp or camera_motion_warp
     @param t0 None (each sample's last timestamp, get_iwe's ts[-1]), a number, or B values
     @param batch_end_indices the cumulative end indices of BaseVoxelDataset.collate_fn
            (lib/data_loaders/base_dataset.py:513-539), a list or an int64 tensor; None means one sample of all events
+    @param inv_depth camera_motion_warp only (required there, rejected with any other model): the inverse depth 1/Z of
+           every event's scene point at the event's time, an (N,) float tensor or array aligned with the concatenated
+           events; data like them (taken to f32 on their device, no gradient)
     @returns (B,) tensor of f in params' dtype, on params' device.  With every input already on the GPU neither the
            forward nor the backward synchronises with the host.  The backward rounds the incoming gradient g_b to
            f32, as it stores W_b = G(g_b df_b/dG) in f32: the gradient is accurate to f32 rounding whatever
@@ -59,6 +66,7 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
     warp = _warp_code(warpfunc, "motion_contrast_objective_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_contrast_objective_torch", "params")
+    rho = _depth_tensor(inv_depth, warp, xs.shape[0], "motion_contrast_objective_torch")
     params = _params_tensor(params, warpfunc)
     B = params.shape[0]
     H, W = int(img_size[0]), int(img_size[1])
@@ -67,7 +75,7 @@ def motion_contrast_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, o
     x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "parameter vectors")
     from ..autograd import MotionObjective
     opts = _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W)
-    f = MotionObjective.apply(_rows(params, opts[1]), x, y, t_rel, p, offsets, opts)
+    f = MotionObjective.apply(_rows(params, opts[1]), x, y, t_rel, p, offsets, opts, _depth_events(rho, dev))
     return f.to(device=params.device, dtype=params.dtype)
 
 
@@ -77,7 +85,7 @@ CANDIDATES_WORKSPACE_BYTES = 4 << 30
 
 
 def motion_contrast_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=None, objective="variance", blur_sigma=1.0,
-                                     obj_param=None, img_size=(180, 240), batch_end_indices=None):
+                                     obj_param=None, img_size=(180, 240), batch_end_indices=None, inv_depth=None):
     """
     The contrast objective of every window b under each of its J candidate parameter vectors candidates[b, j]: f[b, j] is
     the f_b that motion_contrast_objective_torch returns with params[b] = candidates[b, j] (same windows, t0, objective,
@@ -87,11 +95,13 @@ def motion_contrast_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=No
     motion_contrast_fit_torch.  J is split into passes of at most 32 candidates, and the windows into chunks whose
     workspace stays under CANDIDATES_WORKSPACE_BYTES; neither split changes a value's arithmetic.
     @param candidates (B,J,K) parameter vectors, any float dtype, K = warpfunc.dims, any J >= 1
+    @param inv_depth camera_motion_warp's inverse depth of every event, as in motion_contrast_objective_torch
     @returns (B,J) f64 tensor of values (no autograd graph) on candidates' device
     """
     warp = _warp_code(warpfunc, "motion_contrast_candidates_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_contrast_candidates_torch", "nothing")
+    rho = _depth_tensor(inv_depth, warp, xs.shape[0], "motion_contrast_candidates_torch")
     cand = _candidates_tensor(candidates, warpfunc)
     B = cand.shape[0]
     H, W = int(img_size[0]), int(img_size[1])
@@ -100,13 +110,16 @@ def motion_contrast_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=No
     x, y, t_rel, p, offsets = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "candidate sets")
     with torch.cuda.device(dev):
         c64 = cand.detach().to(device=dev, dtype=torch.float64)
-        f = _candidates(x, y, t_rel, p, offsets, c64, _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W))
+        f = _candidates(x, y, t_rel, p, offsets, c64, _model(warp, warpfunc, objective, blur_sigma, obj_param, H, W),
+                        _depth_events(rho, dev))
     return f.to(cand.device)
 
 
-def _candidates(x, y, t_rel, p, offsets, c64, opts):
+def _candidates(x, y, t_rel, p, offsets, c64, opts, rho=None):
     """f (B,J) f64 of the prepared device events under the device candidates c64 (B,J,K) f64, in passes of at most
-    MAX_CANDIDATES candidates over chunks of windows whose workspace fits CANDIDATES_WORKSPACE_BYTES"""
+    MAX_CANDIDATES candidates over chunks of windows whose workspace fits CANDIDATES_WORKSPACE_BYTES; rho: the device
+    inverse depth of camera_motion_warp, or None"""
     warp, centre, H, W, objective, sigma, param = opts
-    return _chunked_candidates("evk_cmax_motion_candidates", "motion_candidates", (x, y, t_rel, p), offsets, c64,
-                               (warp, centre, H, W), (sigma, objective, param), CANDIDATES_WORKSPACE_BYTES, 65535)
+    stem, events = _depth_entry("evk_cmax_motion_candidates", (x, y, t_rel, p), rho)
+    return _chunked_candidates(stem, "motion_candidates", events, offsets, c64, (warp, centre, H, W), (sigma, objective, param),
+                               CANDIDATES_WORKSPACE_BYTES, 65535)

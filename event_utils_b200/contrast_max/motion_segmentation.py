@@ -32,6 +32,16 @@ MotionSegmentation.__doc__ = """motion_segmentation_fit_torch's result: params (
 status (B,M) int8, iterations (B,M) int32"""
 
 
+def _segment_warp_code(warpfunc, who):
+    """_warp_code of the models segmentation takes: camera_motion_warp needs the inverse depth of every event, which the
+    segmentation entries do not take"""
+    warp = _warp_code(warpfunc, who)
+    if warp == _lib.WARP_CAMERA_MOTION:
+        raise ValueError("%s does not take camera_motion_warp: motion segmentation has no inverse-depth input; segment with "
+                         "camera_rotation_warp or a planar model" % who)
+    return warp
+
+
 def motion_segmentation_objective_torch(xs, ys, ts, ps, weights, params, warpfunc, t0=None, objective="variance",
                                         blur_sigma=1.0, obj_param=None, img_size=(180, 240), batch_end_indices=None):
     """
@@ -49,7 +59,7 @@ def motion_segmentation_objective_torch(xs, ys, ts, ps, weights, params, warpfun
     @returns (B,M) tensor in params' dtype on params' device.  B * M <= 65535.  With every input on the GPU neither the
            forward nor the backward synchronises with the host.
     """
-    warp = _warp_code(warpfunc, "motion_segmentation_objective_torch")
+    warp = _segment_warp_code(warpfunc, "motion_segmentation_objective_torch")
     _check_objective(objective, "parameters and weights")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_segmentation_objective_torch", "params and weights")
     weights = _weights_tensor(weights, xs.shape[0])
@@ -77,7 +87,7 @@ def motion_segmentation_candidates_torch(xs, ys, ts, ps, candidates, weights, wa
     @param candidates (B,M,J,K) parameter vectors, any float dtype, any J >= 1
     @returns (B,M,J) f64 tensor of values (no autograd graph) on candidates' device
     """
-    warp = _warp_code(warpfunc, "motion_segmentation_candidates_torch")
+    warp = _segment_warp_code(warpfunc, "motion_segmentation_candidates_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_segmentation_candidates_torch", "nothing")
     weights = _weights_tensor(weights, xs.shape[0])
@@ -112,7 +122,7 @@ def motion_segmentation_assign_torch(xs, ys, ts, ps, params, warpfunc, weights, 
     motion_segmentation_objective_torch.  No autograd graph; the windows run in chunks as in the fit.
     @returns (N,M) f32 tensor on weights' device
     """
-    warp = _warp_code(warpfunc, "motion_segmentation_assign_torch")
+    warp = _segment_warp_code(warpfunc, "motion_segmentation_assign_torch")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_segmentation_assign_torch", "nothing")
     weights = _weights_tensor(weights, xs.shape[0])
     M = weights.shape[1]
@@ -153,7 +163,7 @@ def motion_segmentation_fit_torch(xs, ys, ts, ps, warpfunc, x0, batch_end_indice
              round (motion_fit's codes), iterations (B,M) int32 accepted steps summed over the rounds) on the events'
              device
     """
-    warp = _warp_code(warpfunc, "motion_segmentation_fit_torch")
+    warp = _segment_warp_code(warpfunc, "motion_segmentation_fit_torch")
     _check_objective(objective, "parameters")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_segmentation_fit_torch", "nothing")
     _check_line_search_steps(line_search_steps)

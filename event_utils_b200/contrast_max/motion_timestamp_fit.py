@@ -10,7 +10,8 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from ._batched import _chunked_objective, _event_tensors, _timestamp_events, _ts_model, _warp_code, _window_count
+from ._batched import (_chunked_objective, _depth_entry, _depth_events, _depth_tensor, _event_tensors, _timestamp_events,
+                       _ts_model, _warp_code, _window_count)
 from .motion_fit import FIT_WORKSPACE_BYTES, _check_per_window, _fit_arguments, _fit_stages
 from .motion_timestamp_objective import _ts_candidates
 
@@ -22,7 +23,7 @@ TIMESTAMP_FIT_MAX_WINDOWS = 32767
 def motion_timestamp_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None, t0=None, blur_sigma=2.0,
                                timestamp_reverse=False, img_size=(180, 240), x0=None, param_ranges=None, bounds=None,
                                num_samples_per_param=5, grid_levels=1, log_scale=False, param_scale=None, max_iter=50,
-                               line_search_steps=8, ftol=1e-9, gtol=1e-9):
+                               line_search_steps=8, ftol=1e-9, gtol=1e-9, inv_depth=None):
     """
     Minimise the f_b of motion_timestamp_objective_torch over the parameters of every window b on its own, all windows at
     once.  The windows, t0, stamps (timestamp_reverse), blur and img_size are those of motion_timestamp_objective_torch,
@@ -42,6 +43,8 @@ def motion_timestamp_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None,
     unit of param_scale long.  This loss's gradient is large against its scale (f is a sum over the canvas, not a
     mean), and a first step of H g with H = diag(param_scale^2) overshoots by far more than the 2^-(line_search_steps-1)
     the line search can shorten it by.
+    camera_motion_warp takes inv_depth, the inverse depth of every event, and starts from x0 as in
+    motion_contrast_fit_torch.
     Bounds: an event warped off the canvas adds nothing to f, so a motion that sends every event off the canvas has
     f = 0, the loss's global minimum, and a long step can reach it.  bounds ((K,2) or (B,K,2), [lo, hi] per parameter)
     confines every line search to a box: a point outside scores +inf and is never taken.  With param_ranges and no
@@ -53,6 +56,7 @@ def motion_timestamp_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None,
     """
     warp = _warp_code(warpfunc, "motion_timestamp_fit_torch")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_timestamp_fit_torch", "nothing")
+    rho = _depth_tensor(inv_depth, warp, xs.shape[0], "motion_timestamp_fit_torch")
     sigmas = _fit_arguments("motion_timestamp_fit_torch", blur_sigma, line_search_steps, x0, param_ranges)
     K = warpfunc.dims
     B = _window_count(batch_end_indices)
@@ -62,21 +66,24 @@ def motion_timestamp_fit_torch(xs, ys, ts, ps, warpfunc, batch_end_indices=None,
     _lib.lib()
     dev = E.compute_device(*(a for a in (x0, param_ranges, bounds, xs, ys, ts, ps) if isinstance(a, torch.Tensor)))
     x, y, t_rel, tau, p, offsets = _timestamp_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows", timestamp_reverse)
+    rho = _depth_events(rho, dev)
     with torch.cuda.device(dev):
 
         def stage(sigma):
             opts = _ts_model(warp, warpfunc, sigma, H, W)
-            return (_objective_and_gradient(x, y, t_rel, tau, p, offsets, opts),
-                    lambda c: _ts_candidates(x, y, t_rel, tau, p, offsets, c, opts))
+            return (_objective_and_gradient(x, y, t_rel, tau, p, offsets, opts, rho),
+                    lambda c: _ts_candidates(x, y, t_rel, tau, p, offsets, c, opts, rho))
         return _fit_stages(stage, sigmas, B, K, dev, x0, param_ranges, num_samples_per_param, grid_levels, log_scale,
                            param_scale, max_iter, line_search_steps, ftol, gtol, bounds, bound_to_ranges=True,
                            unit_first_step=True)
 
 
-def _objective_and_gradient(x, y, t_rel, tau, p, offsets, opts):
+def _objective_and_gradient(x, y, t_rel, tau, p, offsets, opts, rho=None):
     """(B,K) f64 params -> (f (B,) f64, g (B,K) f64) through evk_motion_timestamp_objective_f32 / _grad_f32 (grad_f = 1),
-    in chunks of at most TIMESTAMP_FIT_MAX_WINDOWS windows whose workspace and images fit FIT_WORKSPACE_BYTES; the windows
-    are independent, so a chunk changes no value's arithmetic"""
+    or their depth twins with camera_motion_warp's device inverse depth rho, in chunks of at most
+    TIMESTAMP_FIT_MAX_WINDOWS windows whose workspace and images fit FIT_WORKSPACE_BYTES; the windows are independent, so
+    a chunk changes no value's arithmetic"""
     warp, centre, H, W, sigma = opts
-    return _chunked_objective("evk_motion_timestamp_objective", "motion_timestamp_objective", (x, y, t_rel, tau, p), offsets,
-                              (warp, centre, H, W), (sigma,), (2, 2), FIT_WORKSPACE_BYTES, TIMESTAMP_FIT_MAX_WINDOWS)
+    stem, events = _depth_entry("evk_motion_timestamp_objective", (x, y, t_rel, tau, p), rho)
+    return _chunked_objective(stem, "motion_timestamp_objective", events, offsets, (warp, centre, H, W), (sigma,), (2, 2),
+                              FIT_WORKSPACE_BYTES, TIMESTAMP_FIT_MAX_WINDOWS)

@@ -12,12 +12,12 @@ import torch
 
 from .. import _lib
 from ..representations import _events as E
-from ._batched import (_candidates_tensor, _check_window_count, _chunked_candidates, _event_tensors, _params_tensor,
-                       _rows, _timestamp_events, _ts_model, _warp_code)
+from ._batched import (_candidates_tensor, _check_window_count, _chunked_candidates, _depth_entry, _depth_events,
+                       _depth_tensor, _event_tensors, _params_tensor, _rows, _timestamp_events, _ts_model, _warp_code)
 
 
 def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, blur_sigma=2.0, timestamp_reverse=False,
-                                     img_size=(180, 240), batch_end_indices=None):
+                                     img_size=(180, 240), batch_end_indices=None, inv_depth=None):
     """
     Average-timestamp loss f_b of every sample b of a batch of event windows, each warped by its own motion params[b].
     Sample b holds the events [start_b, end_b) of the concatenated stream, end_b = batch_end_indices[b] and start_b the
@@ -29,6 +29,9 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
              xyztheta_warp       (hx, hy, hz, theta)   about warpfunc.center
              affine_warp, homography_warp           about warpfunc.center (warps.py; past the horizon: not kept)
              camera_rotation_warp (wx, wy, wz)      exact camera rotation (warps.py; behind the camera: not kept)
+             camera_motion_warp (wx, wy, wz, vx, vy, vz)  exact camera rotation and translation with the events'
+                                                  inverse depth inv_depth (warps.py; behind the camera or without a
+                                                  finite, non-negative inverse depth: not kept)
       2. tau = (t - t_first_b) / (t_last_b - t_first_b + 1e-6), or (-t + t_last_b) / (...) with timestamp_reverse
          (image.py:324-327), formed in ts' dtype, then f32, as flow_timestamp_objective_torch forms it.
       3. An event contributes iff its f32 x', y' are finite, 0 < x' < W and 0 < y' < H with (H, W) = img_size: those are
@@ -45,12 +48,14 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
     @param xs, ys, ts, ps the concatenated events, (N,) tensors or arrays; they are data, not differentiable
     @param params (B,K) or (K,) for one sample, K = warpfunc.dims, any float dtype; the only differentiable input
            (expanded views work)
-    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp, homography_warp or
-           camera_rotation_warp
+    @param warpfunc an instance of linvel_warp, pure_rotation_warp, xyztheta_warp, affine_warp, homography_warp,
+           camera_rotation_warp or camera_motion_warp
     @param t0 None (each sample's last timestamp, zhu_timestamp_objective's ts[-1]), a number, or B values
     @param img_size (H, W): the bounds of step 3 and the canvas (H+1, W+1)
     @param batch_end_indices the cumulative end indices of BaseVoxelDataset.collate_fn
            (lib/data_loaders/base_dataset.py:513-539), a list or an int64 tensor; None means one sample of all events
+    @param inv_depth camera_motion_warp only (required there, rejected with any other model): the (N,) inverse depth of
+           every event, as in motion_contrast_objective_torch
     @returns (B,) tensor of f in params' dtype, on params' device, 0 <= B <= 32767.  The backward is the exact derivative
            of f with respect to params, with the floor and keep decisions held.  It rounds the incoming gradient g_b to
            f32 and stores the images in f32, so the gradient is accurate to f32 rounding whatever params' dtype.  With
@@ -58,6 +63,7 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
     """
     warp = _warp_code(warpfunc, "motion_timestamp_objective_torch")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_timestamp_objective_torch", "params")
+    rho = _depth_tensor(inv_depth, warp, xs.shape[0], "motion_timestamp_objective_torch")
     params = _params_tensor(params, warpfunc)
     B = params.shape[0]
     _check_window_count(batch_end_indices, B, "parameter vectors")
@@ -68,7 +74,7 @@ def motion_timestamp_objective_torch(xs, ys, ts, ps, params, warpfunc, t0=None, 
                                                      timestamp_reverse)
     from ..autograd import MotionTimestampObjective
     opts = _ts_model(warp, warpfunc, blur_sigma, H, W)
-    f = MotionTimestampObjective.apply(_rows(params, opts[1]), x, y, t_rel, tau, p, offsets, opts)
+    f = MotionTimestampObjective.apply(_rows(params, opts[1]), x, y, t_rel, tau, p, offsets, opts, _depth_events(rho, dev))
     return f.to(device=params.device, dtype=params.dtype)
 
 
@@ -79,7 +85,7 @@ TIMESTAMP_CANDIDATES_WORKSPACE_BYTES = 16 << 30
 
 
 def motion_timestamp_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=None, blur_sigma=2.0, timestamp_reverse=False,
-                                      img_size=(180, 240), batch_end_indices=None):
+                                      img_size=(180, 240), batch_end_indices=None, inv_depth=None):
     """
     The average-timestamp loss of every window b under each of its J candidate parameter vectors candidates[b, j]:
     f[b, j] is the f_b that motion_timestamp_objective_torch returns with params[b] = candidates[b, j] (same windows, t0,
@@ -88,10 +94,12 @@ def motion_timestamp_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=N
     into passes of at most 32 candidates, and the windows into chunks whose workspace stays under
     TIMESTAMP_CANDIDATES_WORKSPACE_BYTES; neither split changes a value's arithmetic.
     @param candidates (B,J,K) parameter vectors, any float dtype, K = warpfunc.dims, any J >= 1
+    @param inv_depth camera_motion_warp's inverse depth of every event, as in motion_timestamp_objective_torch
     @returns (B,J) f64 tensor of values (no autograd graph) on candidates' device
     """
     warp = _warp_code(warpfunc, "motion_timestamp_candidates_torch")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, "motion_timestamp_candidates_torch", "nothing")
+    rho = _depth_tensor(inv_depth, warp, xs.shape[0], "motion_timestamp_candidates_torch")
     cand = _candidates_tensor(candidates, warpfunc)
     B = cand.shape[0]
     H, W = int(img_size[0]), int(img_size[1])
@@ -101,13 +109,16 @@ def motion_timestamp_candidates_torch(xs, ys, ts, ps, candidates, warpfunc, t0=N
                                                      timestamp_reverse)
     with torch.cuda.device(dev):
         c64 = cand.detach().to(device=dev, dtype=torch.float64)
-        f = _ts_candidates(x, y, t_rel, tau, p, offsets, c64, _ts_model(warp, warpfunc, blur_sigma, H, W))
+        f = _ts_candidates(x, y, t_rel, tau, p, offsets, c64, _ts_model(warp, warpfunc, blur_sigma, H, W),
+                           _depth_events(rho, dev))
     return f.to(cand.device)
 
 
-def _ts_candidates(x, y, t_rel, tau, p, offsets, c64, opts):
+def _ts_candidates(x, y, t_rel, tau, p, offsets, c64, opts, rho=None):
     """f (B,J) f64 of the prepared device events under the device candidates c64 (B,J,K) f64, in passes of at most
-    MAX_CANDIDATES candidates over chunks of windows whose workspace fits TIMESTAMP_CANDIDATES_WORKSPACE_BYTES"""
+    MAX_CANDIDATES candidates over chunks of windows whose workspace fits TIMESTAMP_CANDIDATES_WORKSPACE_BYTES; rho: the
+    device inverse depth of camera_motion_warp, or None"""
     warp, centre, H, W, sigma = opts
-    return _chunked_candidates("evk_motion_timestamp_candidates", "motion_timestamp_candidates", (x, y, t_rel, tau, p),
-                               offsets, c64, (warp, centre, H, W), (sigma,), TIMESTAMP_CANDIDATES_WORKSPACE_BYTES, 32767)
+    stem, events = _depth_entry("evk_motion_timestamp_candidates", (x, y, t_rel, tau, p), rho)
+    return _chunked_candidates(stem, "motion_timestamp_candidates", events, offsets, c64, (warp, centre, H, W), (sigma,),
+                               TIMESTAMP_CANDIDATES_WORKSPACE_BYTES, 32767)

@@ -291,3 +291,79 @@ class camera_rotation_warp(warp_function):
             jx = jlt(X * Y, -(1.0 + X * X), Y, -(dt * fx))
             jy = jlt(1.0 + Y * Y, -(X * Y), -X, -(dt * fy))
         return xw, yw, jx, jy
+
+
+class camera_motion_warp(warp_function):
+    """A camera that rotates and translates through a scene with known depth: params = (wx, wy, wz, vx, vy, vz), the
+    camera's angular velocity w (rad/s) in its own frame, with camera_rotation_warp's axes (x to the right, y down, z
+    along the optical axis), and its linear velocity v in the camera frame at t0, in depth units per second (m/s when
+    the inverse depth is in 1/m).  camera_matrix is the 3x3 K (no skew) or (fx, fy, cx, cy); the events are undistorted
+    pixel coordinates, and every event carries rho, the inverse depth 1/Z of its scene point at the event's time (Z
+    along the optical axis; callers sample their depth or disparity map at the events).  With dt = t - t0 and b, theta,
+    A, B exactly as in camera_rotation_warp:
+        P = exp([theta]x) b + (rho dt) v,   iz = 1 / Pz,   X = Px iz,   Y = Py iz,   x' = cx + fx X,   y' = cy + fy Y
+    This is exact for a camera whose pose at t, in the camera frame at t0, is (exp(dt [w]x), dt v): a constant rotation
+    rate and a constant velocity.  rho = 0 (a point at infinity) or v = 0 is camera_rotation_warp.  With Q = exp([theta]x)
+    b iz and the left Jacobian J_l of camera_rotation_warp:
+        d x'/dw = -dt fx J_l^T (X Qy, -(Qz + X Qx), Qy),     d y'/dw = -dt fy J_l^T (Qz + Y Qy, -Y Qx, -Qx)
+        d x'/dv = (rho dt) fx iz (1, 0, -X),                 d y'/dv = (rho dt) fy iz (0, 1, -Y)
+    f64 numpy.  The batched losses drop an event with Pz <= 0 (behind the camera) or with a negative or non-finite rho,
+    like an event off the canvas; this warp() returns its formula unchanged.
+
+    The batched losses, their candidates passes and the fits evaluate the model natively on the GPU with K = 6
+    parameters and an inv_depth array aligned with the events: they append (fx, fy) to every row they hand the C entries
+    (the evk_*_depth_* entries with EVK_WARP_CAMERA_MOTION, whose rows are (wx, wy, wz, vx, vy, vz, fx, fy) about the
+    principal point center = (cx, cy)).  warp() needs inv_depth, so the reference-API objectives, which call warp()
+    without it (fused_kind None), reject the model; motion segmentation does not take it."""
+
+    def __init__(self, camera_matrix):
+        super().__init__('camera_motion_warp', 6)
+        fx, fy, cx, cy = _intrinsics(camera_matrix)
+        self.focal = (fx, fy)
+        self.center = (cx, cy)
+
+    def model(self, params):
+        """the parameter block of the batched GPU evaluation: the angular and linear velocities, the focal lengths (the
+        row the C entries take), then the principal point"""
+        return [float(v) for v in params[:6]] + list(self.focal) + list(self.center)
+
+    def warp(self, xs, ys, ts, ps, t0, params, compute_grad=False, inv_depth=None):
+        if inv_depth is None:
+            raise ValueError("camera_motion_warp.warp needs the inverse depth of every event (inv_depth=...); the "
+                             "reference-API objectives do not pass it, use the batched motion losses and fits")
+        wx, wy, wz, vx, vy, vz = (float(v) for v in params[:6])
+        fx, fy = self.focal
+        cx, cy = self.center
+        dt = ts - t0
+        s = np.asarray(inv_depth, np.float64) * dt
+        bx, by = (xs - cx) / fx, (ys - cy) / fy
+        tx, ty, tz = dt * wx, dt * wy, dt * wz
+        p2 = (tx * tx + ty * ty) + tz * tz
+        phi = np.sqrt(p2)
+        half = 0.5 * phi
+        sh, ch = np.sin(half), np.cos(half)
+        r = np.where(phi > 0, sh / np.where(phi > 0, half, 1.0), 1.0)
+        A, B = r * ch, 0.5 * (r * r)
+        c0, c1, c2 = ty - tz * by, tz * bx - tx, tx * by - ty * bx
+        e0, e1, e2 = ty * c2 - tz * c1, tz * c0 - tx * c2, tx * c1 - ty * c0
+        Ux, Uy, Uz = (bx + A * c0) + B * e0, (by + A * c1) + B * e1, (1.0 + A * c2) + B * e2
+        Px, Py, Pz = Ux + s * vx, Uy + s * vy, Uz + s * vz
+        with np.errstate(divide="ignore", invalid="ignore"):
+            xw, yw = cx + fx * Px / Pz, cy + fy * Py / Pz       # camera_rotation_warp's expressions at s v = 0
+            if not compute_grad:
+                return xw, yw, None, None
+            iz = 1.0 / Pz
+            X, Y = Px / Pz, Py / Pz
+            Qx, Qy, Qz = Ux * iz, Uy * iz, Uz * iz
+            series = 1.0 / 6 - p2 * (1.0 / 120 - p2 * (1.0 / 5040))
+            C = np.where(phi < 1e-2, series, (phi - 2.0 * (sh * ch)) / np.where(phi < 1e-2, 1.0, p2 * phi))
+
+            def jlt(w0, w1, w2, k):
+                k0, k1, k2 = ty * w2 - tz * w1, tz * w0 - tx * w2, tx * w1 - ty * w0
+                q = C * ((tx * w0 + ty * w1) + tz * w2)
+                return [k * ((A * w0 - B * k0) + q * tx), k * ((A * w1 - B * k1) + q * ty), k * ((A * w2 - B * k2) + q * tz)]
+            nothing = np.zeros_like(X)
+            sx, sy = s * fx * iz, s * fy * iz
+            jx = np.stack(jlt(X * Qy, -(Qz + X * Qx), Qy, -(dt * fx)) + [sx, nothing, -(sx * X)])
+            jy = np.stack(jlt(Qz + Y * Qy, -(Y * Qx), -Qx, -(dt * fy)) + [nothing, sy, -(sy * Y)])
+        return xw, yw, jx, jy

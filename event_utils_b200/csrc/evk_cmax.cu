@@ -89,17 +89,21 @@ struct CmaxArgs {
 
 enum { WARP_LINVEL_F64 = 0, WARP_LINVEL_F32 = 1, WARP_FLOW_F32 = 2,
        WARP_ROTATION_F64 = 3, WARP_ROTATION_F32 = 4, WARP_XYZTHETA_F64 = 5, WARP_XYZTHETA_F32 = 6,
-       WARP_AFFINE_F32 = 7, WARP_HOMOGRAPHY_F32 = 8, WARP_CAMERA_ROTATION_F32 = 9 };
+       WARP_AFFINE_F32 = 7, WARP_HOMOGRAPHY_F32 = 8, WARP_CAMERA_ROTATION_F32 = 9, WARP_CAMERA_MOTION_F32 = 10 };
 
 __host__ __device__ constexpr bool is_model_warp(int w) { return w >= WARP_ROTATION_F64; }
 __host__ __device__ constexpr bool is_rotation(int w) { return w == WARP_ROTATION_F64 || w == WARP_ROTATION_F32; }
 __host__ __device__ constexpr bool is_linvel(int w) { return w == WARP_LINVEL_F64 || w == WARP_LINVEL_F32; }
 __host__ __device__ constexpr bool is_planar(int w) { return w == WARP_AFFINE_F32 || w == WARP_HOMOGRAPHY_F32; }
-// the camera rotation's row is (wx, wy, wz, fx, fy): the angular velocity, then the focal lengths
+// the camera motion's events carry their inverse depth (Event<WARP>, EventSource::rho)
+__host__ __device__ constexpr bool has_depth(int w) { return w == WARP_CAMERA_MOTION_F32; }
+__host__ __device__ constexpr bool is_camera(int w) { return w == WARP_CAMERA_ROTATION_F32 || has_depth(w); }
+// the camera rotation's row is (wx, wy, wz, fx, fy): the angular velocity, then the focal lengths; the camera motion's
+// is (wx, wy, wz, vx, vy, vz, fx, fy), the linear velocity between them
 __host__ __device__ constexpr int model_dims(int w)
 {
     return is_linvel(w) ? 2 : is_rotation(w) ? 3 : w == WARP_AFFINE_F32 ? 6 : w == WARP_HOMOGRAPHY_F32 ? 8 :
-           w == WARP_CAMERA_ROTATION_F32 ? 5 : 4;
+           w == WARP_CAMERA_ROTATION_F32 ? 5 : w == WARP_CAMERA_MOTION_F32 ? 8 : 4;
 }
 // length of the Jacobian rows model_taps fills (at least 4: the smaller models keep the rows they always had)
 __host__ __device__ constexpr int jac_dims(int w) { return model_dims(w) > 4 ? model_dims(w) : 4; }
@@ -257,6 +261,11 @@ template <int WARP>
 struct Event {
     typename EvT<WARP>::type x, y, t, p;
 };
+// the camera motion's events also carry rho, the inverse depth of their scene point
+template <>
+struct Event<WARP_CAMERA_MOTION_F32> {
+    float x, y, t, p, rho;
+};
 
 template <int WARP>
 __device__ __forceinline__ Event<WARP> load_event(const CmaxArgs &A, int64_t i)
@@ -317,6 +326,14 @@ __device__ __forceinline__ void ld_vec16(const double *p, double (&v)[2])
 //     and through b and the projection, with R e_x, R e_y the first two columns of exp([theta]x):
 //       dx'/dfx = X - (bx iz) ((R e_x)_x - X (R e_x)_z),   dy'/dfx = -(bx iz) (fy / fx) ((R e_x)_y - Y (R e_x)_z)
 //       dx'/dfy = -(by iz) (fx / fy) ((R e_y)_x - X (R e_y)_z),   dy'/dfy = Y - (by iz) ((R e_y)_y - Y (R e_y)_z)
+//   camera motion (wx, wy, wz, vx, vy, vz, fx, fy) with the principal point (cx, cy) and the event's inverse depth rho,
+//   the batched passes with depth only (f32): the camera rotation's branch with the translation added to P,
+//     U = exp([theta]x) b (the rotation's P),  s = rho dt,  P = U + s v,  iz, X, Y, x', y' as above
+//     exact for the camera pose (exp(dt [w]x), dt v) at t in the camera frame at t0.  An event with a negative or
+//     non-finite rho is not kept, nor one with Pz <= 0 or a non-finite Pz.  At s v = 0 (rho = 0 or v = 0) the
+//     translation adds an exact zero, so x', y' are the camera rotation's bit for bit.  With Q = U iz:
+//       dx'/dw = -dt fx J_l^T (X Qy, -(Qz + X Qx), Qy),   dy'/dw = -dt fy J_l^T (Qz + Y Qy, -Y Qx, -Qx)
+//       dx'/dv = s fx iz (1, 0, -X),   dy'/dv = s fy iz (0, 1, -Y),   d/dfx, d/dfy: the camera rotation's with this P
 // in the order written (no FMA: the library builds with -fmad=false), f64 in parity mode, f32 in fast mode.
 // THE one place that turns an event into its bilinear footprint for these models: warp, bounds mask
 // (event_util.py:26-27), f64 -> f32 cast (image.py:180-183) and splat_taps -- the IWE pass and the gradient
@@ -360,8 +377,12 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
             jy[0] = (float)s; jy[1] = (float)((R)1 - c); jy[2] = (float)(-(d * rx));
             jx[3] = jy[3] = 0.0f;
         }
-    } else if constexpr (WARP == WARP_CAMERA_ROTATION_F32) {
-        const R fx = (R)M.m[3], fy = (R)M.m[4], cx = (R)M.m[5], cy = (R)M.m[6];
+    } else if constexpr (is_camera(WARP)) {
+        constexpr int F = model_dims(WARP) - 2;   // the focal lengths' slots, behind the motion
+        if constexpr (has_depth(WARP)) {
+            if (!(e.rho >= (R)0) || isinf(e.rho)) return false;   // no depth: not kept, like an event off the canvas
+        }
+        const R fx = (R)M.m[F], fy = (R)M.m[F + 1], cx = (R)M.m[F + 2], cy = (R)M.m[F + 3];
         const R bx = (e.x - cx) / fx, by = (e.y - cy) / fy;
         const R tx = d * (R)M.m[0], ty = d * (R)M.m[1], tz = d * (R)M.m[2];
         const R p2 = (tx * tx + ty * ty) + tz * tz;
@@ -372,7 +393,14 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
         const R A = r * ch, B = (R)0.5 * (r * r);
         const R c0 = ty - tz * by, c1 = tz * bx - tx, c2 = tx * by - ty * bx;
         const R e0 = ty * c2 - tz * c1, e1 = tz * c0 - tx * c2, e2 = tx * c1 - ty * c0;
-        const R Px = (bx + A * c0) + B * e0, Py = (by + A * c1) + B * e1, Pz = ((R)1 + A * c2) + B * e2;
+        const R Ux = (bx + A * c0) + B * e0, Uy = (by + A * c1) + B * e1, Uz = ((R)1 + A * c2) + B * e2;
+        R Px = Ux, Py = Uy, Pz = Uz, s = (R)0;
+        if constexpr (has_depth(WARP)) {
+            s = e.rho * d;   // the translation s v: an exact zero added at rho = 0 or v = 0
+            Px = Ux + s * (R)M.m[3];
+            Py = Uy + s * (R)M.m[4];
+            Pz = Uz + s * (R)M.m[5];
+        }
         if (!(Pz > (R)0) || isinf(Pz)) return false;   // behind the camera: not kept, like an event off the canvas
         const R iz = (R)1 / Pz, X = Px * iz, Y = Py * iz;
         xw = cx + fx * X;
@@ -390,15 +418,24 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
                 j[1] = s * ((A * w1 - B * k1) + q * ty);
                 j[2] = s * ((A * w2 - B * k2) + q * tz);
             };
-            jlt(X * Y, -((R)1 + X * X), Y, -(d * fx), jx);
-            jlt((R)1 + Y * Y, -(X * Y), -X, -(d * fy), jy);
+            if constexpr (has_depth(WARP)) {
+                const R Qx = Ux * iz, Qy = Uy * iz, Qz = Uz * iz;
+                jlt(X * Qy, -(Qz + X * Qx), Qy, -(d * fx), jx);
+                jlt(Qz + Y * Qy, -(Y * Qx), -Qx, -(d * fy), jy);
+                const R sx = (s * fx) * iz, sy = (s * fy) * iz;
+                jx[3] = sx; jx[4] = 0.0f; jx[5] = -(sx * X);
+                jy[3] = 0.0f; jy[4] = sy; jy[5] = -(sy * Y);
+            } else {
+                jlt(X * Y, -((R)1 + X * X), Y, -(d * fx), jx);
+                jlt((R)1 + Y * Y, -(X * Y), -X, -(d * fy), jy);
+            }
             const R rxx = (R)1 - B * (ty * ty + tz * tz), rxy = A * tz + B * (tx * ty), rxz = B * (tx * tz) - A * ty;
             const R ryx = B * (tx * ty) - A * tz, ryy = (R)1 - B * (tx * tx + tz * tz), ryz = A * tx + B * (ty * tz);
             const R ux = bx * iz, uy = by * iz;
-            jx[3] = X - ux * (rxx - X * rxz);
-            jy[3] = -(ux * (fy / fx)) * (rxy - Y * rxz);
-            jx[4] = -(uy * (fx / fy)) * (ryx - X * ryz);
-            jy[4] = Y - uy * (ryy - Y * ryz);
+            jx[F] = X - ux * (rxx - X * rxz);
+            jy[F] = -(ux * (fy / fx)) * (rxy - Y * rxz);
+            jx[F + 1] = -(uy * (fx / fy)) * (ryx - X * ryz);
+            jy[F + 1] = Y - uy * (ryy - Y * ryz);
         }
     } else if constexpr (is_planar(WARP)) {
         constexpr int K = model_dims(WARP);
@@ -1672,6 +1709,7 @@ struct EventSource {
     const float *tau;            // the timestamp losses: the normalised stamp of every event
     const int64_t *offsets;
     int64_t n;
+    const float *rho;            // the camera motion: the inverse depth of every event (null for the other models)
 };
 
 __device__ __forceinline__ void sample_range(const EventSource &E, int b, int64_t &first, int64_t &last)
@@ -1700,6 +1738,28 @@ __device__ __forceinline__ EvXYTUP load_xytup(const EventSource &E, int64_t i)
 {
     return {ld_stream(E.x + i), ld_stream(E.y + i), ld_stream(E.t + i), ld_stream(E.tau + i), ld_stream(E.p + i)};
 }
+
+// A record of the loaders above with, for a model whose events carry it (has_depth), the event's inverse depth: the
+// other models' records stay what they were.  depth_of reads it back (0 without).
+template <class Rec, bool DEPTH>
+struct Depthed : Rec {};
+template <class Rec>
+struct Depthed<Rec, true> : Rec {
+    float rho;
+};
+
+template <int WARP, class Rec>
+__device__ __forceinline__ Depthed<Rec, has_depth(WARP)> with_depth(const EventSource &E, int64_t i, const Rec &r)
+{
+    Depthed<Rec, has_depth(WARP)> q;
+    static_cast<Rec &>(q) = r;
+    if constexpr (has_depth(WARP)) q.rho = ld_stream(E.rho + i);
+    return q;
+}
+template <class Rec>
+__device__ __forceinline__ float depth_of(const Depthed<Rec, false> &) { return 0.0f; }
+template <class Rec>
+__device__ __forceinline__ float depth_of(const Depthed<Rec, true> &r) { return r.rho; }
 
 constexpr int kFlowObjThreads = 256;
 
@@ -1766,12 +1826,14 @@ __device__ __forceinline__ void load_models(const double *params, int64_t first,
     __syncthreads();
 }
 
-// an event of the (f32) model passes, splatted with weight p
+// an event of the (f32) model passes, splatted with weight p; rho is its inverse depth, which only the camera motion's
+// events carry
 template <int WARP>
-__device__ __forceinline__ Event<WARP> model_event(float x, float y, float t, float p)
+__device__ __forceinline__ Event<WARP> model_event(float x, float y, float t, float p, float rho = 0.0f)
 {
     Event<WARP> e;
     e.x = x; e.y = y; e.t = t; e.p = p;
+    if constexpr (has_depth(WARP)) e.rho = rho;
     return e;
 }
 
@@ -2503,10 +2565,11 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_obj_event_kernel(const
 #pragma unroll
     for (int k = 0; k < K; ++k) u[k] = 0.0;
     unsigned oob = 0;   // a kept finite event lies inside the canvas; a non-finite one contributes nothing
-    for_each_event(first, last, [&](int64_t i) { return load_xytp(A.E, i); }, [&](int64_t, const EvXYTP &e) {
+    auto load = [&](int64_t i) { return with_depth<WARP>(A.E, i, load_xytp(A.E, i)); };
+    for_each_event(first, last, load, [&](int64_t, const Depthed<EvXYTP, has_depth(WARP)> &e) {
         Taps T;
         float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
-        if (!model_taps<WARP, GRAD>(A.C, model_event<WARP>(e.x, e.y, e.t, e.p), M, oob, T, jx, jy)) return;
+        if (!model_taps<WARP, GRAD>(A.C, model_event<WARP>(e.x, e.y, e.t, e.p, depth_of(e)), M, oob, T, jx, jy)) return;
         if (!GRAD) {
             red_add4(acc + ((int64_t)T.y0 * A.C.Wc + T.x0) * 4, T.ti);
             return;
@@ -2538,20 +2601,26 @@ static int motion_obj_dims(int warp)
 // Shared argument checks and set-up of the model entries.  `images` per sample: 1 for the contrast losses, 2 for the
 // timestamp losses (one per polarity; they also need tau), so that the tail's 65535 images allow 65535 or 32767 samples.
 // n_cand 0: the differentiable entries, one set of images per sample; else a forward-only set per sample and candidate.
-// acc_blocks: 16-byte accumulator blocks per image (batch_obj_carve).
+// acc_blocks: 16-byte accumulator blocks per image (batch_obj_carve).  depth: the entries with the inverse depth rho of
+// every event, which take EVK_WARP_CAMERA_MOTION (K = 8) and nothing else; the other entries pass a null rho.
 static int model_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
-                       const int64_t *offsets, int batch, int64_t n, int warp, const double *params, int K, double cx, double cy,
-                       int H, int W, double sigma, int objective, int images, size_t acc_blocks, int n_cand, void *workspace,
-                       size_t workspace_bytes, ModelArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
+                       const float *rho, bool depth, const int64_t *offsets, int batch, int64_t n, int warp,
+                       const double *params, int K, double cx, double cy, int H, int W, double sigma, int objective,
+                       int images, size_t acc_blocks, int n_cand, void *workspace, size_t workspace_bytes, ModelArgs &A,
+                       BatchObjWorkspace &ws, BlurTaps &taps)
 {
     if (int rc = check_sigma(who, sigma)) return rc;
     const int max_batch = 65535 / images;
     if (batch < 0 || batch > max_batch || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
-        (n > 0 && (!x || !y || !t || (images == 2 && !tau) || !p))) {
+        (n > 0 && (!x || !y || !t || (images == 2 && !tau) || !p || (depth && !rho)))) {
         set_error("%s: bad arguments (0 <= batch <= %d, H, W >= 2)", who, max_batch);
         return EVK_E_ARG;
     }
-    const int dims = motion_obj_dims(warp);
+    const int dims = depth ? (warp == EVK_WARP_CAMERA_MOTION ? 8 : 0) : motion_obj_dims(warp);
+    if (!dims && depth) {
+        set_error("%s: warp %d takes no inverse depth (only EVK_WARP_CAMERA_MOTION, %d)", who, warp, EVK_WARP_CAMERA_MOTION);
+        return EVK_E_ARG;
+    }
     if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
     if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
     if (n_cand && (n_cand < 1 || n_cand > kMaxCandidates || (int64_t)batch * n_cand > max_batch)) {
@@ -2564,7 +2633,7 @@ static int model_setup(const char *who, const float *x, const float *y, const fl
     A = ModelArgs{};
     A.C.Hm = H; A.C.Wm = W; A.C.Hc = H + 1; A.C.Wc = W + 1;
     A.C.p_scale = 1.0;
-    A.E = EventSource{x, y, t, p, tau, offsets, n};
+    A.E = EventSource{x, y, t, p, tau, offsets, n, rho};
     A.params = params; A.cx = cx; A.cy = cy;
     A.M = 1;
     A.J = n_cand ? n_cand : 1;
@@ -2582,6 +2651,14 @@ static void with_model_warp(int warp, F f)
     else if (warp == EVK_WARP_HOMOGRAPHY) f(std::integral_constant<int, WARP_HOMOGRAPHY_F32>{});
     else if (warp == EVK_WARP_CAMERA_ROTATION) f(std::integral_constant<int, WARP_CAMERA_ROTATION_F32>{});
     else f(std::integral_constant<int, WARP_XYZTHETA_F32>{});
+}
+
+// with_model_warp, and the camera motion for the entries with depth (the segmentation entries do not take it)
+template <class F>
+static void with_motion_warp(int warp, F f)
+{
+    if (warp == EVK_WARP_CAMERA_MOTION) f(std::integral_constant<int, WARP_CAMERA_MOTION_F32>{});
+    else with_model_warp(warp, f);
 }
 
 // ---- motion segmentation by motion compensation (evk_cmax_motion_segment_*) ----------------------------------------
@@ -2618,9 +2695,11 @@ __device__ __forceinline__ void load_seg_weights(const ModelArgs &A, int64_t i, 
     }
 }
 
-// what motion_seg_cand_kernel reads of an event: x, y, t, p and, weighted, its row of M weights
+// what motion_seg_cand_kernel reads of an event: x, y, t, p, with DEPTH its inverse depth and, weighted, its row of M
+// weights
+template <bool DEPTH>
 struct SegEvent {
-    EvXYTP e;
+    Depthed<EvXYTP, DEPTH> e;
     float w[kMaxSegModels];
 };
 
@@ -2638,12 +2717,12 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const 
     float *acc = A.acc + (int64_t)b * M * J * npix * 4;
     unsigned oob = 0;   // as in motion_obj_event_kernel: a kept finite event lies inside the canvas
     auto load = [&](int64_t q) {
-        SegEvent r;
-        r.e = load_xytp(A.E, q);
+        SegEvent<has_depth(WARP)> r;
+        r.e = with_depth<WARP>(A.E, q, load_xytp(A.E, q));
         if (WEIGHTED) load_seg_weights(A, q, r.w);
         return r;
     };
-    for_each_event_batch(first, last, load, [&](const SegEvent (&e)[kBatch], int ne) {
+    for_each_event_batch(first, last, load, [&](const SegEvent<has_depth(WARP)> (&e)[kBatch], int ne) {
 #pragma unroll
         for (int m = 0; m < kMaxSegModels; ++m) {
             if (m >= M) break;
@@ -2653,11 +2732,11 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_cand_kernel(const 
 #pragma unroll
                 for (int k = 0; k < kBatch; ++k) {
                     if (k >= ne) continue;
-                    const EvXYTP &ek = e[k].e;
+                    const auto &ek = e[k].e;
                     const float p = WEIGHTED ? __fmul_rn(ek.p, e[k].w[m]) : ek.p;   // the splat weight p w, formed in f32
                     Taps T;
                     float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
-                    if (model_taps<WARP, false>(A.C, model_event<WARP>(ek.x, ek.y, ek.t, p), Mo, oob, T, jx, jy))
+                    if (model_taps<WARP, false>(A.C, model_event<WARP>(ek.x, ek.y, ek.t, p, depth_of(ek)), Mo, oob, T, jx, jy))
                         red_add4(accq + ((int64_t)T.y0 * Wc + T.x0) * 4, T.ti);
                 }
             }
@@ -2773,7 +2852,7 @@ static int motion_seg_setup(const char *who, const float *x, const float *y, con
         return EVK_E_ARG;
     }
     if (n > 0 && !weights) { set_error("%s: null weights", who); return EVK_E_ARG; }
-    const int rc = model_setup(who, x, y, t, nullptr, p, offsets, n_cand || batch < 0 ? batch : batch * n_models, n, warp, params, K,
+    const int rc = model_setup(who, x, y, t, nullptr, p, nullptr, false, offsets, n_cand || batch < 0 ? batch : batch * n_models, n, warp, params, K,
                                cx, cy, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), n_models * n_cand, workspace,
                                workspace_bytes, A, ws, taps);
     if (rc) return rc;
@@ -2952,12 +3031,13 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_ts_event_kernel(const 
 #pragma unroll
     for (int k = 0; k < K; ++k) u[k] = 0.0;
     unsigned oob = 0;   // a contributing event lies inside the canvas; a non-finite one contributes nothing
-    for_each_event(first, last, [&](int64_t i) { return load_xytup(A.E, i); }, [&](int64_t, const EvXYTUP &e) {
+    auto load = [&](int64_t i) { return with_depth<WARP>(A.E, i, load_xytup(A.E, i)); };
+    for_each_event(first, last, load, [&](int64_t, const Depthed<EvXYTUP, has_depth(WARP)> &e) {
         const int pol = ts_polarity(e.p);
         if (pol < 0) return;
         Taps T;
         float jx[jac_dims(WARP)], jy[jac_dims(WARP)];
-        if (!model_taps<WARP, GRAD>(A.C, model_event<WARP>(e.x, e.y, e.t, 1.0f), M, oob, T, jx, jy)) return;
+        if (!model_taps<WARP, GRAD>(A.C, model_event<WARP>(e.x, e.y, e.t, 1.0f, depth_of(e)), M, oob, T, jx, jy)) return;
         if (!GRAD) {
             ts_block_add(acc, npix, Wc, pol, T, e.tau);
             return;
@@ -3016,9 +3096,9 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_ts_cand_kernel(const M
     float *acc = A.acc + (int64_t)b * J * 2 * npix * 8;
     unsigned oob = 0;   // as in motion_ts_event_kernel: a contributing event lies inside the canvas
     auto load = [&](int64_t q) {
-        const EvXYTUP r = load_xytup(A.E, q);
+        const auto r = with_depth<WARP>(A.E, q, load_xytup(A.E, q));
         TsCandEvent<WARP> c;
-        c.e = model_event<WARP>(r.x, r.y, r.t, 1.0f);
+        c.e = model_event<WARP>(r.x, r.y, r.t, 1.0f, depth_of(r));
         c.tau = r.tau;
         c.pol = ts_polarity(r.p);
         return c;
@@ -3536,19 +3616,22 @@ size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W)
     return evk::batch_obj_carve(nullptr, batch, H, W, (size_t)(H + 1) * (W + 1), nullptr);
 }
 
-int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
-                                  int batch, int64_t n_events, int warp, const double *params, int K, double cx, double cy,
-                                  int H, int W, double sigma, int objective, double obj_param, double *f_out, float *iwe_out,
-                                  void *workspace, size_t workspace_bytes, void *stream)
+// The contrast entries and their depth twins share these bodies: rho is the inverse depth of every event, which the
+// twins (depth) take for EVK_WARP_CAMERA_MOTION and the others pass as null.
+static int cmax_motion_objective(const char *who, bool depth, const float *x, const float *y, const float *t_rel,
+                                 const float *p, const float *rho, const int64_t *offsets, int batch, int64_t n_events,
+                                 int warp, const double *params, int K, double cx, double cy, int H, int W, double sigma,
+                                 int objective, double obj_param, double *f_out, float *iwe_out, void *workspace,
+                                 size_t workspace_bytes, void *stream)
 {
     using namespace evk;
     ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = model_setup("evk_cmax_motion_objective_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, warp, params, K, cx,
-                         cy, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), 0, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup(who, x, y, t_rel, nullptr, p, rho, depth, offsets, batch, n_events, warp, params, K, cx, cy, H, W,
+                         sigma, objective, 1, (size_t)(H + 1) * (W + 1), 0, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
-    if (batch > 0 && (!f_out || !iwe_out)) { set_error("evk_cmax_motion_objective_f32: null output"); return EVK_E_ARG; }
+    if (batch > 0 && (!f_out || !iwe_out)) { set_error("%s: null output", who); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc;
@@ -3557,7 +3640,7 @@ int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        with_model_warp(warp, [&](auto wt) {
+        with_motion_warp(warp, [&](auto wt) {
             motion_obj_event_kernel<wt.value, false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
         });
     }
@@ -3566,20 +3649,21 @@ int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t
     return EVK_OK;
 }
 
-int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
-                                       int batch, int64_t n_events, int warp, const double *params, int K, double cx, double cy,
-                                       int H, int W, double sigma, int objective, double obj_param, const float *iwe,
-                                       const float *grad_f, double *grad_params, void *workspace, size_t workspace_bytes,
-                                       void *stream)
+static int cmax_motion_objective_grad(const char *who, bool depth, const float *x, const float *y, const float *t_rel,
+                                      const float *p, const float *rho, const int64_t *offsets, int batch,
+                                      int64_t n_events, int warp, const double *params, int K, double cx, double cy,
+                                      int H, int W, double sigma, int objective, double obj_param, const float *iwe,
+                                      const float *grad_f, double *grad_params, void *workspace, size_t workspace_bytes,
+                                      void *stream)
 {
     using namespace evk;
     ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = model_setup("evk_cmax_motion_objective_grad_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, warp, params, K,
-                         cx, cy, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), 0, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup(who, x, y, t_rel, nullptr, p, rho, depth, offsets, batch, n_events, warp, params, K, cx, cy, H, W,
+                         sigma, objective, 1, (size_t)(H + 1) * (W + 1), 0, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
-    if (batch > 0 && (!iwe || !grad_f || !grad_params)) { set_error("evk_cmax_motion_objective_grad_f32: null array"); return EVK_E_ARG; }
+    if (batch > 0 && (!iwe || !grad_f || !grad_params)) { set_error("%s: null array", who); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     EVK_CUDA(cudaMemsetAsync(grad_params, 0, (size_t)batch * K * sizeof(double), st));
@@ -3589,12 +3673,66 @@ int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const flo
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        with_model_warp(warp, [&](auto wt) {
+        with_motion_warp(warp, [&](auto wt) {
             motion_obj_event_kernel<wt.value, true><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
         });
     }
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
+}
+
+static int cmax_motion_candidates(const char *who, bool depth, const float *x, const float *y, const float *t_rel,
+                                  const float *p, const float *rho, const int64_t *offsets, int batch, int64_t n_events,
+                                  int warp, const double *cand, int n_cand, int K, double cx, double cy, int H, int W,
+                                  double blur_sigma, int objective, double obj_param, double *f_out, void *workspace,
+                                  size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    ModelArgs A;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = model_setup(who, x, y, t_rel, nullptr, p, rho, depth, offsets, batch, n_events, warp, cand, K, cx, cy, H, W,
+                         blur_sigma, objective, 1, (size_t)(H + 1) * (W + 1), n_cand < 1 ? -1 : n_cand, workspace,
+                         workspace_bytes, A, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && !f_out) { set_error("%s: null output", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_cand;
+    // nonfinite stays zero, as in evk_cmax_motion_objective_f32
+    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
+    if (n_events > 0) {
+        ProfScope prof(st);
+        prof_count(1);
+        with_motion_warp(warp, [&](auto wt) {
+            motion_seg_cand_kernel<wt.value, false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
+        });
+    }
+    // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
+    batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, ws.Wimg, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_cmax_motion_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                  int batch, int64_t n_events, int warp, const double *params, int K, double cx, double cy,
+                                  int H, int W, double sigma, int objective, double obj_param, double *f_out, float *iwe_out,
+                                  void *workspace, size_t workspace_bytes, void *stream)
+{
+    return cmax_motion_objective("evk_cmax_motion_objective_f32", false, x, y, t_rel, p, nullptr, offsets, batch, n_events,
+                                 warp, params, K, cx, cy, H, W, sigma, objective, obj_param, f_out, iwe_out, workspace,
+                                 workspace_bytes, stream);
+}
+
+int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p, const int64_t *offsets,
+                                       int batch, int64_t n_events, int warp, const double *params, int K, double cx, double cy,
+                                       int H, int W, double sigma, int objective, double obj_param, const float *iwe,
+                                       const float *grad_f, double *grad_params, void *workspace, size_t workspace_bytes,
+                                       void *stream)
+{
+    return cmax_motion_objective_grad("evk_cmax_motion_objective_grad_f32", false, x, y, t_rel, p, nullptr, offsets, batch,
+                                      n_events, warp, params, K, cx, cy, H, W, sigma, objective, obj_param, iwe, grad_f,
+                                      grad_params, workspace, workspace_bytes, stream);
 }
 
 size_t evk_cmax_motion_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
@@ -3608,31 +3746,53 @@ int evk_cmax_motion_candidates_f32(const float *x, const float *y, const float *
                                    double cy, int H, int W, double blur_sigma, int objective, double obj_param, double *f_out,
                                    void *workspace, size_t workspace_bytes, void *stream)
 {
-    using namespace evk;
-    ModelArgs A;
-    BatchObjWorkspace ws;
-    BlurTaps taps;
-    int rc = model_setup("evk_cmax_motion_candidates_f32", x, y, t_rel, nullptr, p, offsets, batch, n_events, warp, cand, K, cx, cy,
-                         H, W, blur_sigma, objective, 1, (size_t)(H + 1) * (W + 1), n_cand < 1 ? -1 : n_cand, workspace,
-                         workspace_bytes, A, ws, taps);
-    if (rc) return rc;
-    if (batch > 0 && !f_out) { set_error("evk_cmax_motion_candidates_f32: null output"); return EVK_E_ARG; }
-    if (batch == 0) return EVK_OK;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, canvases = batch * n_cand;
-    // nonfinite stays zero, as in evk_cmax_motion_objective_f32
-    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
-    if (n_events > 0) {
-        ProfScope prof(st);
-        prof_count(1);
-        with_model_warp(warp, [&](auto wt) {
-            motion_seg_cand_kernel<wt.value, false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
-        });
-    }
-    // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
-    batch_obj_forward_tail(ws, Hc, Wc, taps, canvases, objective, obj_param, ws.Wimg, f_out, st);
-    EVK_CUDA(cudaGetLastError());
-    return EVK_OK;
+    return cmax_motion_candidates("evk_cmax_motion_candidates_f32", false, x, y, t_rel, p, nullptr, offsets, batch, n_events,
+                                  warp, cand, n_cand, K, cx, cy, H, W, blur_sigma, objective, obj_param, f_out, workspace,
+                                  workspace_bytes, stream);
+}
+
+size_t evk_cmax_motion_depth_objective_workspace_bytes(int batch, int H, int W)
+{
+    return evk_cmax_motion_objective_workspace_bytes(batch, H, W);
+}
+
+int evk_cmax_motion_depth_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                        const float *inv_depth, const int64_t *offsets, int batch, int64_t n_events,
+                                        int warp, const double *params, int K, double cx, double cy, int H, int W,
+                                        double sigma, int objective, double obj_param, double *f_out, float *iwe_out,
+                                        void *workspace, size_t workspace_bytes, void *stream)
+{
+    return cmax_motion_objective("evk_cmax_motion_depth_objective_f32", true, x, y, t_rel, p, inv_depth, offsets, batch,
+                                 n_events, warp, params, K, cx, cy, H, W, sigma, objective, obj_param, f_out, iwe_out,
+                                 workspace, workspace_bytes, stream);
+}
+
+int evk_cmax_motion_depth_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                             const float *inv_depth, const int64_t *offsets, int batch,
+                                             int64_t n_events, int warp, const double *params, int K, double cx,
+                                             double cy, int H, int W, double sigma, int objective, double obj_param,
+                                             const float *iwe, const float *grad_f, double *grad_params,
+                                             void *workspace, size_t workspace_bytes, void *stream)
+{
+    return cmax_motion_objective_grad("evk_cmax_motion_depth_objective_grad_f32", true, x, y, t_rel, p, inv_depth, offsets,
+                                      batch, n_events, warp, params, K, cx, cy, H, W, sigma, objective, obj_param, iwe,
+                                      grad_f, grad_params, workspace, workspace_bytes, stream);
+}
+
+size_t evk_cmax_motion_depth_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
+{
+    return evk_cmax_motion_candidates_workspace_bytes(batch, n_cand, H, W);
+}
+
+int evk_cmax_motion_depth_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                         const float *inv_depth, const int64_t *offsets, int batch, int64_t n_events,
+                                         int warp, const double *cand, int n_cand, int K, double cx, double cy, int H,
+                                         int W, double blur_sigma, int objective, double obj_param, double *f_out,
+                                         void *workspace, size_t workspace_bytes, void *stream)
+{
+    return cmax_motion_candidates("evk_cmax_motion_depth_candidates_f32", true, x, y, t_rel, p, inv_depth, offsets, batch,
+                                  n_events, warp, cand, n_cand, K, cx, cy, H, W, blur_sigma, objective, obj_param, f_out,
+                                  workspace, workspace_bytes, stream);
 }
 
 size_t evk_cmax_motion_segment_workspace_bytes(int batch, int n_models, int H, int W)
@@ -3857,19 +4017,21 @@ size_t evk_motion_timestamp_objective_workspace_bytes(int batch, int H, int W)
     return evk::batch_obj_carve(nullptr, 2 * batch, H, W, evk::flow_ts_acc_blocks(H, W), nullptr);
 }
 
-int evk_motion_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
-                                       const int64_t *offsets, int batch, int64_t n_events, int warp, const double *params,
-                                       int K, double cx, double cy, int H, int W, double sigma, double *f_out, float *ts_out,
-                                       float *cnt_out, void *workspace, size_t workspace_bytes, void *stream)
+// The timestamp entries and their depth twins share these bodies, as the contrast entries do.
+static int motion_timestamp_objective(const char *who, bool depth, const float *x, const float *y, const float *t_rel,
+                                      const float *tau, const float *p, const float *rho, const int64_t *offsets, int batch,
+                                      int64_t n_events, int warp, const double *params, int K, double cx, double cy, int H,
+                                      int W, double sigma, double *f_out, float *ts_out, float *cnt_out, void *workspace,
+                                      size_t workspace_bytes, void *stream)
 {
     using namespace evk;
     ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = model_setup("evk_motion_timestamp_objective_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp, params, K, cx,
-                         cy, H, W, sigma, OBJ_SOS, 2, flow_ts_acc_blocks(H, W), 0, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup(who, x, y, t_rel, tau, p, rho, depth, offsets, batch, n_events, warp, params, K, cx, cy, H, W, sigma,
+                         OBJ_SOS, 2, flow_ts_acc_blocks(H, W), 0, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
-    if (batch > 0 && (!f_out || !ts_out || !cnt_out)) { set_error("evk_motion_timestamp_objective_f32: null output"); return EVK_E_ARG; }
+    if (batch > 0 && (!f_out || !ts_out || !cnt_out)) { set_error("%s: null output", who); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int Hc = H + 1, Wc = W + 1, npix = Hc * Wc, images = 2 * batch;
@@ -3878,7 +4040,7 @@ int evk_motion_timestamp_objective_f32(const float *x, const float *y, const flo
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        with_model_warp(warp, [&](auto wt) {
+        with_motion_warp(warp, [&](auto wt) {
             motion_ts_event_kernel<wt.value, false><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
         });
     }
@@ -3887,21 +4049,22 @@ int evk_motion_timestamp_objective_f32(const float *x, const float *y, const flo
     return EVK_OK;
 }
 
-int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
-                                            const int64_t *offsets, int batch, int64_t n_events, int warp, const double *params,
-                                            int K, double cx, double cy, int H, int W, double sigma, const float *ts_img,
-                                            const float *cnt_img, const float *grad_f, double *grad_params, void *workspace,
-                                            size_t workspace_bytes, void *stream)
+static int motion_timestamp_objective_grad(const char *who, bool depth, const float *x, const float *y, const float *t_rel,
+                                           const float *tau, const float *p, const float *rho, const int64_t *offsets,
+                                           int batch, int64_t n_events, int warp, const double *params, int K, double cx,
+                                           double cy, int H, int W, double sigma, const float *ts_img, const float *cnt_img,
+                                           const float *grad_f, double *grad_params, void *workspace,
+                                           size_t workspace_bytes, void *stream)
 {
     using namespace evk;
     ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = model_setup("evk_motion_timestamp_objective_grad_f32", x, y, t_rel, tau, p, offsets, batch, n_events, warp, params, K,
-                         cx, cy, H, W, sigma, OBJ_SOS, 2, flow_ts_acc_blocks(H, W), 0, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup(who, x, y, t_rel, tau, p, rho, depth, offsets, batch, n_events, warp, params, K, cx, cy, H, W, sigma,
+                         OBJ_SOS, 2, flow_ts_acc_blocks(H, W), 0, workspace, workspace_bytes, A, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!ts_img || !cnt_img || !grad_f || !grad_params)) {
-        set_error("evk_motion_timestamp_objective_grad_f32: null array");
+        set_error("%s: null array", who);
         return EVK_E_ARG;
     }
     if (batch == 0) return EVK_OK;
@@ -3912,7 +4075,7 @@ int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, cons
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        with_model_warp(warp, [&](auto wt) {
+        with_motion_warp(warp, [&](auto wt) {
             motion_ts_event_kernel<wt.value, true><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
         });
     }
@@ -3920,24 +4083,19 @@ int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, cons
     return EVK_OK;
 }
 
-size_t evk_motion_timestamp_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
-{
-    if (batch < 0 || n_cand < 1 || n_cand > evk::kMaxCandidates || H < 2 || W < 2) return 0;
-    return evk::motion_ts_cand_bytes(2 * batch * n_cand, H, W);
-}
-
-int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
-                                        const int64_t *offsets, int batch, int64_t n_events, int warp, const double *cand,
-                                        int n_cand, int K, double cx, double cy, int H, int W, double blur_sigma, double *f_out,
-                                        void *workspace, size_t workspace_bytes, void *stream)
+static int motion_timestamp_candidates(const char *who, bool depth, const float *x, const float *y, const float *t_rel,
+                                       const float *tau, const float *p, const float *rho, const int64_t *offsets,
+                                       int batch, int64_t n_events, int warp, const double *cand, int n_cand, int K,
+                                       double cx, double cy, int H, int W, double blur_sigma, double *f_out,
+                                       void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
-    const char *who = "evk_motion_timestamp_candidates_f32";
     ModelArgs A;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = model_setup(who, x, y, t_rel, tau, p, offsets, batch, n_events, warp, cand, K, cx, cy, H, W, blur_sigma, OBJ_SOS, 2,
-                         flow_ts_acc_blocks(H, W), n_cand < 1 ? -1 : n_cand, workspace, workspace_bytes, A, ws, taps);
+    int rc = model_setup(who, x, y, t_rel, tau, p, rho, depth, offsets, batch, n_events, warp, cand, K, cx, cy, H, W,
+                         blur_sigma, OBJ_SOS, 2, flow_ts_acc_blocks(H, W), n_cand < 1 ? -1 : n_cand, workspace,
+                         workspace_bytes, A, ws, taps);
     if (rc) return rc;
     const int images = 2 * batch * n_cand;
     if (workspace_bytes < motion_ts_cand_bytes(images, H, W)) {
@@ -3953,7 +4111,7 @@ int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const fl
     if (n_events > 0) {
         ProfScope prof(st);
         prof_count(1);
-        with_model_warp(warp, [&](auto wt) {
+        with_motion_warp(warp, [&](auto wt) {
             motion_ts_cand_kernel<wt.value><<<batch_grid(n_events, batch), kFlowObjThreads, 0, st>>>(A);
         });
     }
@@ -3961,6 +4119,88 @@ int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const fl
     ts_obj_forward_tail(ws, Hc, Wc, taps, batch * n_cand, ws.Wimg, cnt, f_out, st);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
+}
+
+int evk_motion_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                       const int64_t *offsets, int batch, int64_t n_events, int warp, const double *params,
+                                       int K, double cx, double cy, int H, int W, double sigma, double *f_out, float *ts_out,
+                                       float *cnt_out, void *workspace, size_t workspace_bytes, void *stream)
+{
+    return motion_timestamp_objective("evk_motion_timestamp_objective_f32", false, x, y, t_rel, tau, p, nullptr, offsets,
+                                      batch, n_events, warp, params, K, cx, cy, H, W, sigma, f_out, ts_out, cnt_out,
+                                      workspace, workspace_bytes, stream);
+}
+
+int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                            const int64_t *offsets, int batch, int64_t n_events, int warp, const double *params,
+                                            int K, double cx, double cy, int H, int W, double sigma, const float *ts_img,
+                                            const float *cnt_img, const float *grad_f, double *grad_params, void *workspace,
+                                            size_t workspace_bytes, void *stream)
+{
+    return motion_timestamp_objective_grad("evk_motion_timestamp_objective_grad_f32", false, x, y, t_rel, tau, p, nullptr,
+                                           offsets, batch, n_events, warp, params, K, cx, cy, H, W, sigma, ts_img, cnt_img,
+                                           grad_f, grad_params, workspace, workspace_bytes, stream);
+}
+
+size_t evk_motion_timestamp_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
+{
+    if (batch < 0 || n_cand < 1 || n_cand > evk::kMaxCandidates || H < 2 || W < 2) return 0;
+    return evk::motion_ts_cand_bytes(2 * batch * n_cand, H, W);
+}
+
+int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                        const int64_t *offsets, int batch, int64_t n_events, int warp, const double *cand,
+                                        int n_cand, int K, double cx, double cy, int H, int W, double blur_sigma, double *f_out,
+                                        void *workspace, size_t workspace_bytes, void *stream)
+{
+    return motion_timestamp_candidates("evk_motion_timestamp_candidates_f32", false, x, y, t_rel, tau, p, nullptr, offsets,
+                                       batch, n_events, warp, cand, n_cand, K, cx, cy, H, W, blur_sigma, f_out, workspace,
+                                       workspace_bytes, stream);
+}
+
+size_t evk_motion_timestamp_depth_objective_workspace_bytes(int batch, int H, int W)
+{
+    return evk_motion_timestamp_objective_workspace_bytes(batch, H, W);
+}
+
+int evk_motion_timestamp_depth_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                             const float *p, const float *inv_depth, const int64_t *offsets, int batch,
+                                             int64_t n_events, int warp, const double *params, int K, double cx,
+                                             double cy, int H, int W, double blur_sigma, double *f_out, float *ts_out,
+                                             float *cnt_out, void *workspace, size_t workspace_bytes, void *stream)
+{
+    return motion_timestamp_objective("evk_motion_timestamp_depth_objective_f32", true, x, y, t_rel, tau, p, inv_depth,
+                                      offsets, batch, n_events, warp, params, K, cx, cy, H, W, blur_sigma, f_out, ts_out,
+                                      cnt_out, workspace, workspace_bytes, stream);
+}
+
+int evk_motion_timestamp_depth_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                                  const float *p, const float *inv_depth, const int64_t *offsets,
+                                                  int batch, int64_t n_events, int warp, const double *params, int K,
+                                                  double cx, double cy, int H, int W, double blur_sigma,
+                                                  const float *ts_img, const float *cnt_img, const float *grad_f,
+                                                  double *grad_params, void *workspace, size_t workspace_bytes,
+                                                  void *stream)
+{
+    return motion_timestamp_objective_grad("evk_motion_timestamp_depth_objective_grad_f32", true, x, y, t_rel, tau, p,
+                                           inv_depth, offsets, batch, n_events, warp, params, K, cx, cy, H, W, blur_sigma,
+                                           ts_img, cnt_img, grad_f, grad_params, workspace, workspace_bytes, stream);
+}
+
+size_t evk_motion_timestamp_depth_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
+{
+    return evk_motion_timestamp_candidates_workspace_bytes(batch, n_cand, H, W);
+}
+
+int evk_motion_timestamp_depth_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                              const float *p, const float *inv_depth, const int64_t *offsets,
+                                              int batch, int64_t n_events, int warp, const double *cand, int n_cand,
+                                              int K, double cx, double cy, int H, int W, double blur_sigma,
+                                              double *f_out, void *workspace, size_t workspace_bytes, void *stream)
+{
+    return motion_timestamp_candidates("evk_motion_timestamp_depth_candidates_f32", true, x, y, t_rel, tau, p, inv_depth,
+                                       offsets, batch, n_events, warp, cand, n_cand, K, cx, cy, H, W, blur_sigma, f_out,
+                                       workspace, workspace_bytes, stream);
 }
 
 size_t evk_grid_flow_timestamp_objective_workspace_bytes(int batch, int gh, int gw, int H, int W)

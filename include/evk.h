@@ -623,6 +623,50 @@ int evk_cmax_motion_candidates_f32(const float *x, const float *y, const float *
                                    double blur_sigma, int objective, double obj_param, double *f_out,
                                    void *workspace, size_t workspace_bytes, void *stream);
 
+/* Camera motion with known depth: the three entries above for the model EVK_WARP_CAMERA_MOTION, whose warp needs the
+ * inverse depth of every event.  Each has the signature of its depth-free twin with inv_depth inserted right after p:
+ *   inv_depth: n_events floats on the device, rho = 1 / Z of the event's scene point at the event's time (Z along the
+ *              optical axis, in the depth unit of v)
+ * and accepts warp = EVK_WARP_CAMERA_MOTION only (any other code: EVK_E_ARG), with K = 8 and rows
+ *   EVK_WARP_CAMERA_MOTION (wx, wy, wz, vx, vy, vz, fx, fy)    K = 8   principal point (cx, cy)
+ * w is the camera's angular velocity (rad/s) in its own frame (x right, y down, z along the optical axis), v its linear
+ * velocity in the camera frame at t0 (depth units per second), fx, fy its focal lengths (px, no skew), and x, y are
+ * undistorted.  With d = t_rel and b, theta, phi, A, B exactly as in the camera rotation above:
+ *   P = exp([theta]x) b + (rho d) v,  iz = 1 / Pz,  X = Px iz,  Y = Py iz,  x' = cx + fx X,  y' = cy + fy Y
+ * exact for a camera whose pose at time t, in the camera frame at t0, is (exp(d [w]x), d v): it rotates at a constant
+ * rate and moves at a constant velocity.  Keep rules: an event with Pz <= 0 or a non-finite Pz (behind the camera), or
+ * with a negative or non-finite rho, is not kept (no contribution, no gradient); rho = 0 is a point at infinity.
+ * Derivatives, with Q = exp([theta]x) b iz and the left Jacobian J_l = A I + B [theta]x + C theta theta^T of the camera
+ * rotation:
+ *   dx'/dw = -d fx J_l^T (X Qy, -(Qz + X Qx), Qy),     dy'/dw = -d fy J_l^T (Qz + Y Qy, -Y Qx, -Qx)
+ *   dx'/dv = (rho d) fx iz (1, 0, -X),                 dy'/dv = (rho d) fy iz (0, 1, -Y)
+ * and dx'/dfx, dy'/dfx, dx'/dfy, dy'/dfy those of the camera rotation with this P's iz, X and Y.  grad_params carries
+ * all eight derivatives, the focal lengths included.  Identities: at v = 0 or rho = 0 the translation is an added exact
+ * zero, so x', y', the images and f equal EVK_WARP_CAMERA_ROTATION's at (wx, wy, wz, fx, fy) bit for bit (the w
+ * columns of the gradient to f32 rounding); at w = 0 the warp is the exact projective translation.  All in f32, in the
+ * order written.  Everything else -- keep rule on the canvas, splat, blur, objectives, argument checks, images,
+ * workspaces (the _workspace_bytes queries return what the twins' return), no synchronisation and a launch count
+ * independent of the batch -- is the twin's. */
+#define EVK_WARP_CAMERA_MOTION 7
+size_t evk_cmax_motion_depth_objective_workspace_bytes(int batch, int H, int W);
+int evk_cmax_motion_depth_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                        const float *inv_depth, const int64_t *offsets, int batch, int64_t n_events,
+                                        int warp, const double *params, int K, double cx, double cy, int H, int W,
+                                        double blur_sigma, int objective, double obj_param, double *f_out,
+                                        float *iwe_out, void *workspace, size_t workspace_bytes, void *stream);
+int evk_cmax_motion_depth_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                             const float *inv_depth, const int64_t *offsets, int batch,
+                                             int64_t n_events, int warp, const double *params, int K, double cx,
+                                             double cy, int H, int W, double blur_sigma, int objective, double obj_param,
+                                             const float *iwe, const float *grad_f, double *grad_params,
+                                             void *workspace, size_t workspace_bytes, void *stream);
+size_t evk_cmax_motion_depth_candidates_workspace_bytes(int batch, int n_cand, int H, int W);
+int evk_cmax_motion_depth_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                         const float *inv_depth, const int64_t *offsets, int batch, int64_t n_events,
+                                         int warp, const double *cand, int n_cand, int K, double cx, double cy, int H,
+                                         int W, double blur_sigma, int objective, double obj_param, double *f_out,
+                                         void *workspace, size_t workspace_bytes, void *stream);
+
 /* Motion segmentation by motion compensation (Stoffregen, Gallego, Drummond, Kleeman, Scaramuzza, ICCV 2019):
  * n_models = M motion models per sample (1 <= M <= 8) and a soft membership weights[e][m] (n_events x M floats,
  * row-major, in DEVICE memory) of every event in every model.  Samples, t_rel, warp models, keep rule, canvas,
@@ -766,6 +810,29 @@ int evk_motion_timestamp_candidates_f32(const float *x, const float *y, const fl
                                         const double *cand, int n_cand, int K, double cx, double cy, int H, int W,
                                         double blur_sigma, double *f_out, void *workspace, size_t workspace_bytes,
                                         void *stream);
+
+/* Camera motion with known depth for the average-timestamp loss: the three entries above with inv_depth (n_events
+ * floats on the device) inserted right after p, for EVK_WARP_CAMERA_MOTION only, with K = 8 and the warp, keep rules,
+ * derivatives and identities of evk_cmax_motion_depth_objective_f32.  Everything else is the twin's. */
+size_t evk_motion_timestamp_depth_objective_workspace_bytes(int batch, int H, int W);
+int evk_motion_timestamp_depth_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                             const float *p, const float *inv_depth, const int64_t *offsets, int batch,
+                                             int64_t n_events, int warp, const double *params, int K, double cx,
+                                             double cy, int H, int W, double blur_sigma, double *f_out, float *ts_out,
+                                             float *cnt_out, void *workspace, size_t workspace_bytes, void *stream);
+int evk_motion_timestamp_depth_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                                  const float *p, const float *inv_depth, const int64_t *offsets,
+                                                  int batch, int64_t n_events, int warp, const double *params, int K,
+                                                  double cx, double cy, int H, int W, double blur_sigma,
+                                                  const float *ts_img, const float *cnt_img, const float *grad_f,
+                                                  double *grad_params, void *workspace, size_t workspace_bytes,
+                                                  void *stream);
+size_t evk_motion_timestamp_depth_candidates_workspace_bytes(int batch, int n_cand, int H, int W);
+int evk_motion_timestamp_depth_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                              const float *p, const float *inv_depth, const int64_t *offsets,
+                                              int batch, int64_t n_events, int warp, const double *cand, int n_cand,
+                                              int K, double cx, double cy, int H, int W, double blur_sigma,
+                                              double *f_out, void *workspace, size_t workspace_bytes, void *stream);
 
 /* The dense-flow average-timestamp loss with the flow of every sample given on a coarse grid of nodes: the node grid,
  * its interpolation and limits of evk_cmax_grid_flow_objective_f32 (grid_flow: [batch][2][gh][gw] f32 on the device,
