@@ -17,6 +17,7 @@ Which inputs get a gradient (as in the reference; the others get None):
     flow_timestamp_objective_torch   flow only (contrast_max/flow_timestamp_objective.py; the events are data)
     grid_flow_contrast_objective_torch  the node grid only (contrast_max/grid_flow.py; the events are data)
     grid_flow_timestamp_objective_torch  the node grid only (contrast_max/grid_flow_timestamp.py; the events are data)
+    depth_grid_contrast_objective_torch  the inverse-depth grid only (contrast_max/depth_grid.py; events and motion are data)
     motion_contrast_objective_torch  params only (contrast_max/motion_objective.py; the events are data)
     motion_segmentation_objective_torch  params and weights (contrast_max/motion_segmentation.py; the events are data)
     motion_timestamp_objective_torch params only (contrast_max/motion_timestamp_objective.py; the events are data)
@@ -266,6 +267,28 @@ class GridFlowObjective(torch.autograd.Function):
         return _loss_forward(ctx, "evk_cmax_grid_flow_objective", "grid_flow_objective", grid_flow, torch.float32, (),
                              (gh, gw, H, W, sigma, objective, param), (H, W), (x, y, t_rel, p), offsets, (1,),
                              query=(gh, gw))
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return _loss_backward(ctx, g)[:1] + (None,) * 6
+
+
+class DepthGridObjective(torch.autograd.Function):
+    """The batched depth-grid contrast objective of contrast_max/depth_grid.py (the camera-motion contrast loss with each
+    event's inverse depth bilinearly interpolated from a gh x gw grid of nodes): f (B,) f64 from inv_depth_grid
+    (B,gh,gw) and the prepared device events.  Only the nodes get a gradient: the exact derivative of f, one pass over
+    the events (evk_cmax_depth_grid_objective_grad_f32).  opts = (rows, cx, cy, H, W, sigma, objective, obj_param) with
+    rows the device motion rows (B,8) f64 (_batched._rows)."""
+
+    @staticmethod
+    def forward(ctx, inv_depth_grid, x, y, t_rel, p, offsets, opts):
+        rows, cx, cy, H, W, sigma, objective, param = opts
+        gh, gw = inv_depth_grid.shape[1:]
+        ctx.rows = rows   # the entries read the rows through a pointer, in the backward too
+        return _loss_forward(ctx, "evk_cmax_depth_grid_objective", "depth_grid_objective", inv_depth_grid, torch.float32,
+                             (_lib.ptr(rows), cx, cy), (gh, gw, H, W, sigma, objective, param), (H, W), (x, y, t_rel, p),
+                             offsets, (1,), query=(gh, gw))
 
     @staticmethod
     @once_differentiable

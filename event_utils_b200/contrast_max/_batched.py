@@ -234,11 +234,19 @@ def _model_layout(model, K):
     """the arguments of a motion entry in front of its parameter pointer, between the parameter count and (H, W), and
     those its workspace query takes in front of (H, W): model = (warp, _centre, H, W); K is the parameters per row
     before _rows.  A grid-flow entry takes model = ("grid", (gh, gw), H, W): its grids of K = 2 gh gw floats are
-    followed by gh, gw, which its query takes too."""
-    kind, extra, H, W = model
+    followed by gh, gw, which its query takes too.  A depth-grid entry takes model = ("grid", (gh, gw), H, W,
+    (rows, cx, cy)): the device motion rows (B,8) f64 of the windows and the principal point go in front of its grids
+    of K = gh gw floats (_lead passes the rows of a chunk's windows)."""
+    kind, extra, H, W = model[:4]
     if kind == "grid":
-        return (), (), extra, extra, H, W
+        return tuple(model[4]) if len(model) > 4 else (), (), extra, extra, H, W
     return (kind,), (K + len(extra) - 2, extra[0], extra[1]), (), (), H, W
+
+
+def _lead(pre, b0):
+    """_model_layout's arguments in front of the parameter pointer for the chunk from window b0: a tensor of per-window
+    rows goes as the pointer to row b0"""
+    return tuple(_lib.ptr(a[b0:]) if isinstance(a, torch.Tensor) else a for a in pre)
 
 
 def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget, cap, M=None):
@@ -271,8 +279,8 @@ def _chunked_candidates(stem, key, events, offsets, c64, model, scalars, budget,
             j1 = min(J, j0 + jc)
             c = _rows(c64[b0:b1, ..., j0:j1, :], model[1]).contiguous()
             out = torch.empty(c.shape[:-1], dtype=torch.float64, device=dev)
-            _lib.check(entry(*front, _lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], *pre, _lib.ptr(c), j1 - j0,
-                             *mid, *grid, H, W, *scalars, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream()))
+            _lib.check(entry(*front, _lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], *_lead(pre, b0), _lib.ptr(c),
+                             j1 - j0, *mid, *grid, H, W, *scalars, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream()))
             f[b0:b1, ..., j0:j1] = out
     return f
 
@@ -310,8 +318,8 @@ def _chunked_objective(stem, key, events, offsets, model, scalars, images, budge
         for b0 in range(0, B, wb):
             b1 = min(B, b0 + wb)
             r0, r1 = b0 * rows, b1 * rows
-            ev = front + (_lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], *pre, _lib.ptr(prm[r0:r1]), *mid, *grid, H, W,
-                          *scalars)
+            ev = front + (_lib.ptr(offsets[b0:]), b1 - b0, events[0].shape[0], *_lead(pre, b0), _lib.ptr(prm[r0:r1]), *mid,
+                          *grid, H, W, *scalars)
             _lib.check(forward(*ev, _lib.ptr(f[r0:r1]), *imgs, _lib.ptr(ws), ws.numel(), _lib.stream()))
             if gradient:
                 _lib.check(grad(*ev, *imgs, _lib.ptr(ones), _lib.ptr(g[r0:r1]), *no_weight_gradient, _lib.ptr(ws),

@@ -123,7 +123,8 @@ def charbonnier_smoothness(grid_flow, eps):
     """
     R of every window and its gradient: with rho(d) = sqrt(d^2 + eps^2) - eps (the Charbonnier penalty, 0 at d = 0),
         R = sum_c [ sum_{i, j < gw-1} rho(g[c,i,j+1] - g[c,i,j]) + sum_{i < gh-1, j} rho(g[c,i+1,j] - g[c,i,j]) ]
-    over both flow components c, every horizontally and every vertically neighbouring pair of nodes.
+    over both flow components c (every channel c of any (..., C, gh, gw) grid), every horizontally and every vertically
+    neighbouring pair of nodes.
     @param grid_flow (..., 2, gh, gw) float tensor
     @returns (R (...), dR/dgrid_flow (..., 2, gh, gw)) in grid_flow's dtype
     """
@@ -252,44 +253,53 @@ def _grid_fit(who, tensors, size, grid_shapes, smoothness, charbonnier_eps, batc
     ev = events(B, dev)
     with torch.cuda.device(dev):
         scale = torch.as_tensor(1.0 if param_scale is None else param_scale, dtype=torch.float64, device=dev)
-        iters = torch.zeros(B, dtype=torch.int32, device=dev)
-        status = f = None
-        for gh, gw in shapes:
-            if tuple(flow.shape[2:]) != (gh, gw):
-                flow = torch.nn.functional.interpolate(flow, (gh, gw), mode="bilinear", align_corners=True)
-            K = 2 * gh * gw
-            sc = scale.reshape(-1, 1).expand(B, K)
-            lim = None
-            if box is not None:
-                # every node of component c in [lo_c, hi_c]: the clamp moves a start outside the box onto it, and undoes
-                # the rounding of the upsampling
-                lim = box.unsqueeze(2).expand(B, 2, gh * gw, 2).reshape(B, K, 2)
-                flow = torch.minimum(torch.maximum(flow, box[..., 0, None, None]), box[..., 1, None, None])
-            xk = flow.reshape(B, K)
-            for sigma in sigmas:
-                fg, candidates = _stage(*loss(ev, (gh, gw), sigma), (gh, gw), lam, eps)
-                xk, f, status, it = _batched_bfgs(fg, candidates, xk, sc, max_iter, line_search_steps, ftol, gtol, lim,
-                                                  unit_first_step=True)
-                iters += it
-            flow = xk.reshape(B, 2, gh, gw)
-        rest = f - lam * charbonnier_smoothness(flow, eps)[0]
-    return flow, f, rest, status, iters
+        return _stages(flow, shapes, sigmas, box, scale, ev, loss, lam, eps, max_iter, line_search_steps, ftol, gtol)
+
+
+def _stages(grid, shapes, sigmas, box, scale, ev, loss, lam, eps, max_iter, line_search_steps, ftol, gtol):
+    """The BFGS stages of the coarse-to-fine node-grid fits (grid flow, depth grid): grid (B,C,gh0,gw0) f64 is the start
+    on the first of the (gh, gw) shapes, with C channels per node; box None or (B,C,2) [lo, hi] of every node of
+    channel c; scale a number or (B,) tensor, the BFGS param_scale of every node; loss(ev, (gh, gw), sigma) -> (fg of f,
+    candidates of f on f32 node grids).  Returns (grid, F, f, status, iterations) on the last shape."""
+    B, C = grid.shape[:2]
+    iters = torch.zeros(B, dtype=torch.int32, device=grid.device)
+    status = f = None
+    for gh, gw in shapes:
+        if tuple(grid.shape[2:]) != (gh, gw):
+            grid = torch.nn.functional.interpolate(grid, (gh, gw), mode="bilinear", align_corners=True)
+        K = C * gh * gw
+        sc = scale.reshape(-1, 1).expand(B, K)
+        lim = None
+        if box is not None:
+            # every node of channel c in [lo_c, hi_c]: the clamp moves a start outside the box onto it, and undoes the
+            # rounding of the upsampling
+            lim = box.unsqueeze(2).expand(B, C, gh * gw, 2).reshape(B, K, 2)
+            grid = torch.minimum(torch.maximum(grid, box[..., 0, None, None]), box[..., 1, None, None])
+        xk = grid.reshape(B, K)
+        for sigma in sigmas:
+            fg, candidates = _stage(*loss(ev, (gh, gw), sigma), (C, gh, gw), lam, eps)
+            xk, f, status, it = _batched_bfgs(fg, candidates, xk, sc, max_iter, line_search_steps, ftol, gtol, lim,
+                                              unit_first_step=True)
+            iters += it
+        grid = xk.reshape(B, C, gh, gw)
+    rest = f - lam * charbonnier_smoothness(grid, eps)[0]
+    return grid, f, rest, status, iters
 
 
 def _stage(obj, cand, grid, lam, eps):
-    """fg and candidates of F = f + lam R on the (gh, gw) grid, for _batched_bfgs: obj (B,K) nodes -> (f, g) of the loss,
-    cand (B,J,K) f32 node grids -> (B,J) f"""
-    gh, gw = grid
+    """fg and candidates of F = f + lam R on the grid (C, gh, gw) of C channels, for _batched_bfgs: obj (B,K) nodes ->
+    (f, g) of the loss, cand (B,J,K) f32 node grids -> (B,J) f"""
+    C, gh, gw = grid
 
     def fg(xk):
         f, g = obj(xk)
-        R, gR = charbonnier_smoothness(xk.view(-1, 2, gh, gw), eps)
+        R, gR = charbonnier_smoothness(xk.view(-1, C, gh, gw), eps)
         return f + lam * R, g + lam * gR.reshape(g.shape)
 
     def candidates(pts):
         B, J, K = pts.shape
         f = cand(pts.to(torch.float32))
-        R = charbonnier_smoothness(pts.reshape(B, J, 2, gh, gw), eps)[0]
+        R = charbonnier_smoothness(pts.reshape(B, J, C, gh, gw), eps)[0]
         return f + lam * R
 
     return fg, candidates

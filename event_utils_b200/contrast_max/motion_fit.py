@@ -219,14 +219,17 @@ def _new_ranges(axes, best):
     return torch.stack((best - below, best + above), dim=-1)
 
 
-def _grid_search(evaluate, ranges, num_samples_per_param=5, levels=1, log_scale=False):
+def _grid_search(evaluate, ranges, num_samples_per_param=5, levels=1, log_scale=False, bounds=None):
     """Coarse-to-fine grid search of every window: `levels` levels of grid_search_initial's grid, each re-centred with
     find_new_range.  evaluate((B,P,K) points) -> (B,P) f.  Returns the (B,K) best point of the last level (the first of
-    equal values; a NaN counts as +inf)."""
+    equal values; a NaN counts as +inf).  bounds: None, or (B,K,2) [lo, hi] that every re-centred range is clamped to
+    (find_new_range can step beyond the first level's ranges)."""
     best = None
     for level in range(levels):
         if level:
             ranges = _new_ranges(axes, best)
+            if bounds is not None:
+                ranges = torch.minimum(torch.maximum(ranges, bounds[..., :1]), bounds[..., 1:])
         axes = _grid_axes(ranges, num_samples_per_param, log_scale)
         pts = _grid_points(axes)
         f = evaluate(pts)

@@ -345,6 +345,62 @@ __device__ __forceinline__ void sin_cos(float a, float *s, float *c) { sincosf(a
 // phi^8 / 39916800, is under 1e-10
 constexpr float kCamSeriesPhi = 0.5f;
 
+// The camera models' warp in two halves, which the camera branch of model_taps and the depth-grid passes share (f32, in
+// the order written): cam_rotate is the rotation U = exp([theta]x) b of the event's bearing, which depends on neither
+// rho nor v, and cam_project adds the translation s v (TRANSLATE) and projects.
+struct CamRot {
+    float fx, fy, cx, cy, bx, by, tx, ty, tz, p2, phi, sh, ch, A, B, Ux, Uy, Uz;
+};
+struct CamProj {
+    float iz, X, Y, xw, yw;
+};
+
+__device__ __forceinline__ CamRot cam_rotate(float x, float y, float d, float wx, float wy, float wz, float fx, float fy,
+                                             float cx, float cy)
+{
+    CamRot c;
+    c.fx = fx; c.fy = fy; c.cx = cx; c.cy = cy;
+    c.bx = (x - cx) / fx; c.by = (y - cy) / fy;
+    c.tx = d * wx; c.ty = d * wy; c.tz = d * wz;
+    const float tx = c.tx, ty = c.ty, tz = c.tz, bx = c.bx, by = c.by;
+    c.p2 = (tx * tx + ty * ty) + tz * tz;
+    c.phi = sqrtf(c.p2);
+    const float half = 0.5f * c.phi;
+    sincospif(half * (float)0.318309886183790671, &c.sh, &c.ch);   // sin, cos of phi / 2, reduced exactly: no local memory
+    const float r = c.phi > 0.0f ? c.sh / half : 1.0f;
+    c.A = r * c.ch; c.B = 0.5f * (r * r);
+    const float c0 = ty - tz * by, c1 = tz * bx - tx, c2 = tx * by - ty * bx;
+    const float e0 = ty * c2 - tz * c1, e1 = tz * c0 - tx * c2, e2 = tx * c1 - ty * c0;
+    c.Ux = (bx + c.A * c0) + c.B * e0; c.Uy = (by + c.A * c1) + c.B * e1; c.Uz = (1.0f + c.A * c2) + c.B * e2;
+    return c;
+}
+
+// false for Pz <= 0 or a non-finite Pz: behind the camera, not kept.  Without TRANSLATE, P = U (s, v unused).
+template <bool TRANSLATE>
+__device__ __forceinline__ bool cam_project(const CamRot &c, float s, float vx, float vy, float vz, CamProj &q)
+{
+    float Px = c.Ux, Py = c.Uy, Pz = c.Uz;
+    if constexpr (TRANSLATE) {
+        Px = c.Ux + s * vx;   // the translation s v: an exact zero added at s = 0 or v = 0
+        Py = c.Uy + s * vy;
+        Pz = c.Uz + s * vz;
+    }
+    if (!(Pz > 0.0f) || isinf(Pz)) return false;
+    q.iz = 1.0f / Pz; q.X = Px * q.iz; q.Y = Py * q.iz;
+    q.xw = c.cx + c.fx * q.X;
+    q.yw = c.cy + c.fy * q.Y;
+    return true;
+}
+
+// event_util.py:26-27: keep iff 0 < x' <= Wm and 0 < y' <= Hm (NaN compares false -> kept), then the f32 splat taps
+template <class R>
+__device__ __forceinline__ bool model_keep_taps(const CmaxArgs &A, R xw, R yw, R p, unsigned &oob, Taps &T)
+{
+    const bool keep = !(xw <= (R)0 || xw > (R)A.Wm) && !(yw <= (R)0 || yw > (R)A.Hm);
+    if (!keep) return false;
+    return splat_taps<false>(A, (float)xw, (float)yw, (float)p, 0.0f, true, oob, T);
+}
+
 template <int WARP, bool JAC>
 __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> &e, const ModelOf<WARP> &M, unsigned &oob,
                                            Taps &T, float (&jx)[jac_dims(WARP)], float (&jy)[jac_dims(WARP)])
@@ -382,30 +438,19 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
         if constexpr (has_depth(WARP)) {
             if (!(e.rho >= (R)0) || isinf(e.rho)) return false;   // no depth: not kept, like an event off the canvas
         }
-        const R fx = (R)M.m[F], fy = (R)M.m[F + 1], cx = (R)M.m[F + 2], cy = (R)M.m[F + 3];
-        const R bx = (e.x - cx) / fx, by = (e.y - cy) / fy;
-        const R tx = d * (R)M.m[0], ty = d * (R)M.m[1], tz = d * (R)M.m[2];
-        const R p2 = (tx * tx + ty * ty) + tz * tz;
-        const R phi = sqrtf(p2), half = (R)0.5 * phi;
-        R sh, ch;
-        sincospif(half * (R)0.318309886183790671, &sh, &ch);   // sin, cos of phi / 2, reduced exactly: no local memory
-        const R r = phi > (R)0 ? sh / half : (R)1;
-        const R A = r * ch, B = (R)0.5 * (r * r);
-        const R c0 = ty - tz * by, c1 = tz * bx - tx, c2 = tx * by - ty * bx;
-        const R e0 = ty * c2 - tz * c1, e1 = tz * c0 - tx * c2, e2 = tx * c1 - ty * c0;
-        const R Ux = (bx + A * c0) + B * e0, Uy = (by + A * c1) + B * e1, Uz = ((R)1 + A * c2) + B * e2;
-        R Px = Ux, Py = Uy, Pz = Uz, s = (R)0;
-        if constexpr (has_depth(WARP)) {
-            s = e.rho * d;   // the translation s v: an exact zero added at rho = 0 or v = 0
-            Px = Ux + s * (R)M.m[3];
-            Py = Uy + s * (R)M.m[4];
-            Pz = Uz + s * (R)M.m[5];
-        }
-        if (!(Pz > (R)0) || isinf(Pz)) return false;   // behind the camera: not kept, like an event off the canvas
-        const R iz = (R)1 / Pz, X = Px * iz, Y = Py * iz;
-        xw = cx + fx * X;
-        yw = cy + fy * Y;
+        const CamRot cr = cam_rotate(e.x, e.y, d, (R)M.m[0], (R)M.m[1], (R)M.m[2], (R)M.m[F], (R)M.m[F + 1], (R)M.m[F + 2],
+                                     (R)M.m[F + 3]);
+        R s = (R)0;
+        if constexpr (has_depth(WARP)) s = e.rho * d;
+        CamProj cp;
+        // behind the camera: not kept, like an event off the canvas
+        if (!cam_project<has_depth(WARP)>(cr, s, (R)M.m[3], (R)M.m[4], (R)M.m[5], cp)) return false;
+        xw = cp.xw;
+        yw = cp.yw;
         if (JAC) {
+            const R fx = cr.fx, fy = cr.fy, bx = cr.bx, by = cr.by, tx = cr.tx, ty = cr.ty, tz = cr.tz, p2 = cr.p2;
+            const R phi = cr.phi, sh = cr.sh, ch = cr.ch, A = cr.A, B = cr.B;
+            const R iz = cp.iz, X = cp.X, Y = cp.Y;
             // (phi - sin phi) / phi^3 cancels in f32 for small phi: 1/6 - phi^2/120 + phi^4/5040 - phi^6/362880 there
             const R C = phi < kCamSeriesPhi
                             ? (R)(1.0 / 6) - p2 * ((R)(1.0 / 120) - p2 * ((R)(1.0 / 5040) - p2 * (R)(1.0 / 362880)))
@@ -419,7 +464,7 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
                 j[2] = s * ((A * w2 - B * k2) + q * tz);
             };
             if constexpr (has_depth(WARP)) {
-                const R Qx = Ux * iz, Qy = Uy * iz, Qz = Uz * iz;
+                const R Qx = cr.Ux * iz, Qy = cr.Uy * iz, Qz = cr.Uz * iz;
                 jlt(X * Qy, -(Qz + X * Qx), Qy, -(d * fx), jx);
                 jlt(Qz + Y * Qy, -(Y * Qx), -Qx, -(d * fy), jy);
                 const R sx = (s * fx) * iz, sy = (s * fy) * iz;
@@ -476,10 +521,7 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
             jy[0] = 0.0f; jy[1] = (float)(-d); jy[2] = (float)(-(d * v)); jy[3] = (float)(-(d * u));
         }
     }
-    // event_util.py:26-27: keep iff 0 < x' <= Wm and 0 < y' <= Hm (NaN compares false -> kept)
-    const bool keep = !(xw <= (R)0 || xw > (R)A.Wm) && !(yw <= (R)0 || yw > (R)A.Hm);
-    if (!keep) return false;
-    return splat_taps<false>(A, (float)xw, (float)yw, (float)p, 0.0f, true, oob, T);
+    return model_keep_taps(A, xw, yw, p, oob, T);
 }
 
 // pass 1 of the motion models: the IWE only, through the same two accumulator back ends as linvel
@@ -2294,9 +2336,11 @@ __global__ void __launch_bounds__(kFlowObjThreads) grid_flow_cand_kernel(const G
         if (nonfinite >> j & 1u) A.F.nonfinite[(int64_t)b * J + j] = 1u;
 }
 
-// v[0..7] summed over the lanes of the warp that share `key` (all 32 lanes call this); the lowest lane of each key holds
-// the sum and gets true.  A shuffle tree over each key's peers (the lanes of rank 2^r k add the next peer's partial sum).
-__device__ __forceinline__ bool warp_key_sum(int key, float (&v)[8])
+// v[0..N-1] summed over the lanes of the warp that share `key` (all 32 lanes call this); the lowest lane of each key
+// holds the sum and gets true.  A shuffle tree over each key's peers (the lanes of rank 2^r k add the next peer's partial
+// sum).
+template <int N>
+__device__ __forceinline__ bool warp_key_sum(int key, float (&v)[N])
 {
     const unsigned full = 0xffffffffu;
     const int lane = threadIdx.x & 31;
@@ -2305,12 +2349,12 @@ __device__ __forceinline__ bool warp_key_sum(int key, float (&v)[8])
     unsigned rest = peers & (0xfffffffeu << lane);   // the peers above this lane
     while (__any_sync(full, rest != 0u)) {
         const int next = __ffs(rest);
-        float t[8];
+        float t[N];
 #pragma unroll
-        for (int k = 0; k < 8; ++k) t[k] = __shfl_sync(full, v[k], (next - 1) & 31);
+        for (int k = 0; k < N; ++k) t[k] = __shfl_sync(full, v[k], (next - 1) & 31);
         if (next) {
 #pragma unroll
-            for (int k = 0; k < 8; ++k) v[k] += t[k];
+            for (int k = 0; k < N; ++k) v[k] += t[k];
         }
         rest &= __ballot_sync(full, !(rank & 1u));
         rank >>= 1;
@@ -2331,17 +2375,32 @@ __device__ __forceinline__ void node_terms(const NodeSample &s, float gu, float 
     }
 }
 
+// The depth grid's one-channel node_terms: g = df/drho times the four node weights of s into val, keyed by the node cell
+__device__ __forceinline__ void node_terms(const NodeSample &s, float g, float (&val)[4], int &key)
+{
+    if (g != 0.0f) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (s.inside >> q & 1u) val[q] = g * s.w[q];
+        }
+        key = s.cell;
+    }
+}
+
 // The terms of the lanes of the warp with the same key summed (warp_key_sum) and added by one lane per node cell to the
-// CTA's f64 accumulator acc [2][G] in shared memory.  All 32 lanes call this; a lane without a term has its own key.
-__device__ __forceinline__ void node_grad_flush(double *acc, int G, const NodeSample &s, int key, float (&val)[8])
+// CTA's f64 accumulator acc [NC][G] in shared memory (NC channels: 2 for the flow, 1 for the inverse depth; val holds
+// the four taps of each channel in turn).  All 32 lanes call this; a lane without a term has its own key.
+template <int NC>
+__device__ __forceinline__ void node_grad_flush(double *acc, int G, const NodeSample &s, int key, float (&val)[4 * NC])
 {
     if (warp_key_sum(key, val) && key >= 0) {
         // the peers share the leader's cell and so its taps inside the grid
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             if (!(s.inside >> q & 1u)) continue;
-            if (val[q] != 0.0f) atomicAdd(acc + s.o[q], (double)val[q]);
-            if (val[4 + q] != 0.0f) atomicAdd(acc + G + s.o[q], (double)val[4 + q]);
+#pragma unroll
+            for (int c = 0; c < NC; ++c)
+                if (val[4 * c + q] != 0.0f) atomicAdd(acc + c * G + s.o[q], (double)val[4 * c + q]);
         }
     }
 }
@@ -2413,7 +2472,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) grid_flow_grad_kernel(const G
                 tap_slopes(ox, oy, T.dx, T.dy, w00, w01, w10, w11, sx, sy);
                 node_terms(s, T.wm * sx * e.t, T.wm * sy * e.t, val, key);
             }
-            node_grad_flush(grid_acc, G, s, key, val);
+            node_grad_flush<2>(grid_acc, G, s, key, val);
         }
     }
     __syncthreads();
@@ -2446,7 +2505,7 @@ static int grid_flow_limits(int batch, int n_cand, int gh, int gw, int H, int W,
 static int grid_flow_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
                            const int64_t *offsets, int batch, int64_t n, const float *grid, int n_cand, int gh, int gw, int H, int W,
                            double sigma, int objective, int images, size_t acc_blocks, void *workspace, size_t workspace_bytes,
-                           GridArgs &A, BatchObjWorkspace &ws, BlurTaps &taps)
+                           GridArgs &A, BatchObjWorkspace &ws, BlurTaps &taps, const char *wrt = "flow")
 {
     if (int rc = check_sigma(who, sigma)) return rc;
     if (!grid_flow_limits(batch, n_cand, gh, gw, H, W, images) || n < 0 || (batch > 0 && (!offsets || !grid)) ||
@@ -2457,7 +2516,7 @@ static int grid_flow_setup(const char *who, const float *x, const float *y, cons
         return EVK_E_ARG;
     }
     const int J = n_cand ? n_cand : 1;
-    int rc = batch_obj_check(who, "flow", images * batch * J, H, W, sigma, objective, acc_blocks, workspace, workspace_bytes, ws,
+    int rc = batch_obj_check(who, wrt, images * batch * J, H, W, sigma, objective, acc_blocks, workspace, workspace_bytes, ws,
                              taps, !n_cand);
     if (rc) return rc;
     A = GridArgs{};
@@ -2514,6 +2573,188 @@ static int grid_flow_node_grad(const GridArgs &A, int batch, float *grad_grid, c
     }
     prof_count(1);
     grid_flow_grad_cast_kernel<<<grid_simple(nodes, 256), 256, 0, st>>>(A.grad, grad_grid, nodes);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+// ---- depth from a known camera motion: an inverse-depth node grid per sample (evk_cmax_depth_grid_*) ---------------
+// The camera-motion contrast objective (model_taps<WARP_CAMERA_MOTION_F32>) with each event's rho interpolated from a
+// gh x gw grid of inverse-depth nodes of its sample instead of read from memory: node_sample and node_flow's arithmetic
+// with one channel (a tap outside the grid reads 0), then the camera motion's keep rules, warp, bounds mask and splat,
+// and the contrast loss's image tail.  The motion rows (wx, wy, wz, vx, vy, vz, fx, fy) are data; only the nodes get a
+// gradient.  The grid of both event passes is (slices, batch), and every CTA holds its sample's nodes in dynamic shared
+// memory as f32:
+//   forward / candidates: depth_grid_cand_kernel.  Per event one 16-byte record, the node cell and its weights once and
+//             the rotation U = exp([theta]x) b once (cam_rotate: it depends on neither rho nor the candidate), then per
+//             candidate j the interpolated rho, P = U + (rho d) v, the projection, the keep rules and one v4 reduction into
+//             canvas z = b J + j, scored by batch_obj_forward_tail.
+//   backward: batch_obj_backward_W, then depth_grid_grad_kernel: per event the four gathers of W_b give df/dx', df/dy',
+//             times dx'/drho = d fx iz (vx - X vz) and dy'/drho = d fy iz (vy - Y vz) and the four node weights; the
+//             lanes of a warp with the same node cell sum their four values (warp_key_sum), one lane per cell adds them to
+//             a per-CTA f64 accumulator [gh][gw] in shared memory, and one f64 atomic per node and CTA goes to
+//             [B][gh][gw] in the workspace, cast to the f32 output by grid_flow_grad_cast_kernel.
+// The limits are the grid flow's (grid_flow_limits): gh gw <= kMaxGridNodes for the loss and n_cand gh gw <=
+// kMaxGridCandNodes for the candidates -- half the grid flow's shared memory, since a node is one float.
+struct DepthGridArgs {
+    GridArgs G;             // canvas and bounds mask (F.C), events, nodes [B][J][gh][gw], accumulators, node sums
+    const double *motion;   // [B][8] rows (wx, wy, wz, vx, vy, vz, fx, fy)
+    double cx, cy;          // the principal point
+};
+
+// sample b's camera motion as model_taps reads it: every value rounded to f32
+struct CamMotion {
+    float wx, wy, wz, vx, vy, vz, fx, fy, cx, cy;
+};
+__device__ __forceinline__ CamMotion cam_motion(const DepthGridArgs &D, int b)
+{
+    const double *m = D.motion + (int64_t)b * 8;
+    return {(float)m[0], (float)m[1], (float)m[2], (float)m[3], (float)m[4], (float)m[5], (float)m[6], (float)m[7],
+            (float)D.cx, (float)D.cy};
+}
+
+// the J inverse-depth grids of sample b, [J][gh gw] floats, into shared memory
+__device__ __forceinline__ void load_depth_nodes(const GridArgs &A, int b, float *nodes)
+{
+    const int n = A.J * A.gh * A.gw;
+    const float *src = A.grid + (int64_t)b * n;
+    for (int q = threadIdx.x; q < n; q += kFlowObjThreads) nodes[q] = __ldg(src + q);
+    __syncthreads();
+}
+
+// one candidate's inverse depth at an event: node_flow with one channel
+__device__ __forceinline__ float node_depth(const float *nodes, const NodeSample &s)
+{
+    float r = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) r = __fadd_rn(r, __fmul_rn(s.inside >> k & 1u ? nodes[s.o[k]] : 0.0f, s.w[k]));
+    return r;
+}
+
+// The camera motion's warp of one event at inverse depth rho, from its rotation r: the keep rules of model_taps (a
+// negative or non-finite rho, Pz <= 0 or a non-finite Pz, the bounds mask) and the taps.  q: the projection.
+__device__ __forceinline__ bool depth_taps(const CmaxArgs &C, const CamMotion &m, const CamRot &r, float rho, float d, float p,
+                                           CamProj &q, Taps &T)
+{
+    if (!(rho >= 0.0f) || isinf(rho)) return false;
+    if (!cam_project<true>(r, rho * d, m.vx, m.vy, m.vz, q)) return false;
+    unsigned oob = 0;   // a kept finite event lies inside the canvas; a non-finite one contributes nothing
+    return model_keep_taps(C, q.xw, q.yw, p, oob, T);
+}
+
+__global__ void __launch_bounds__(kFlowObjThreads) depth_grid_cand_kernel(const DepthGridArgs D)
+{
+    extern __shared__ float depth_nodes[];   // [J][gh gw]
+    const GridArgs &A = D.G;
+    const int b = blockIdx.y, J = A.J, G = A.gh * A.gw;
+    load_depth_nodes(A, b, depth_nodes);
+    int64_t first, last;
+    sample_range(A.F.E, b, first, last);
+    const CmaxArgs &C = A.F.C;
+    const int64_t npix = (int64_t)C.Hc * C.Wc;
+    float *acc = A.F.acc + (int64_t)b * J * npix * 4;
+    const CamMotion m = cam_motion(D, b);
+    for_each_event(first, last, [&](int64_t i) { return load_xytp(A.F.E, i); }, [&](int64_t, const EvXYTP &e) {
+        const NodeSample s = node_sample(A, e.x, e.y);
+        const CamRot r = cam_rotate(e.x, e.y, e.t, m.wx, m.wy, m.wz, m.fx, m.fy, m.cx, m.cy);
+        for (int j = 0; j < J; ++j) {
+            CamProj q;
+            Taps T;
+            if (depth_taps(C, m, r, node_depth(depth_nodes + j * G, s), e.t, e.p, q, T))
+                red_add4(acc + ((int64_t)j * npix + (int64_t)T.y0 * C.Wc + T.x0) * 4, T.ti);
+        }
+    });
+}
+
+// The node-gradient pass, written out like grid_flow_grad_kernel (warp_key_sum needs every lane)
+__global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const DepthGridArgs D)
+{
+    extern __shared__ double depth_acc[];   // [gh gw] f64, then the nodes [gh gw] f32
+    const GridArgs &A = D.G;
+    const int b = blockIdx.y, G = A.gh * A.gw;
+    float *nodes = reinterpret_cast<float *>(depth_acc + G);
+    for (int q = threadIdx.x; q < G; q += kFlowObjThreads) depth_acc[q] = 0.0;
+    load_depth_nodes(A, b, nodes);   // and the barrier
+    int64_t first, last;
+    sample_range(A.F.E, b, first, last);
+    const CmaxArgs &C = A.F.C;
+    const int Wc = C.Wc;
+    const int64_t npix = (int64_t)C.Hc * Wc;
+    const float *Wb = A.F.Wimg + b * npix;
+    const CamMotion m = cam_motion(D, b);
+    const int lane = threadIdx.x & 31;
+    const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
+    for (int64_t i0 = first + (int64_t)blockIdx.x * kFlowObjThreads + (threadIdx.x - lane); i0 < last; i0 += kBatch * stride) {
+        EvXYTP ev[kBatch];
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const int64_t q = i0 + k * stride + lane;
+            ev[k] = q < last ? load_xytp(A.F.E, q) : EvXYTP{};
+            if (!(q < last)) ev[k].x = __int_as_float(0x7fc00000);   // a NaN position: no cell, no term
+        }
+#pragma unroll
+        for (int k = 0; k < kBatch; ++k) {
+            const EvXYTP &e = ev[k];
+            const NodeSample s = node_sample(A, e.x, e.y);
+            float val[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+            int key = -1 - lane;   // a lane without a term is alone with its key
+            if (s.cell >= 0) {
+                const CamRot r = cam_rotate(e.x, e.y, e.t, m.wx, m.wy, m.wz, m.fx, m.fy, m.cx, m.cy);
+                CamProj q;
+                Taps T;
+                if (depth_taps(C, m, r, node_depth(nodes, s), e.t, e.p, q, T)) {
+                    const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
+                    const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0),
+                                w11 = __ldg(Wb + r1 + T.x1);
+                    const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
+                    float sx, sy;
+                    tap_slopes(ox, oy, T.dx, T.dy, w00, w01, w10, w11, sx, sy);
+                    const float di = e.t * q.iz;   // dx'/drho = d fx iz (vx - X vz), dy'/drho = d fy iz (vy - Y vz)
+                    const float jx = (di * m.fx) * (m.vx - q.X * m.vz), jy = (di * m.fy) * (m.vy - q.Y * m.vz);
+                    node_terms(s, T.wm * (sx * jx + sy * jy), val, key);
+                }
+            }
+            node_grad_flush<1>(depth_acc, G, s, key, val);
+        }
+    }
+    __syncthreads();
+    double *dst = A.grad + (int64_t)b * G;
+    for (int q = threadIdx.x; q < G; q += kFlowObjThreads)
+        if (depth_acc[q] != 0.0) atomicAdd(dst + q, depth_acc[q]);
+}
+
+// The checks and set-up of the depth-grid entries: grid_flow_setup's (one image per canvas), then the motion rows
+static int depth_grid_setup(const char *who, const float *x, const float *y, const float *t, const float *p,
+                            const int64_t *offsets, int batch, int64_t n, const double *motion, double cx, double cy,
+                            const float *grid, int n_cand, int gh, int gw, int H, int W, double sigma, int objective,
+                            void *workspace, size_t workspace_bytes, DepthGridArgs &D, BatchObjWorkspace &ws, BlurTaps &taps)
+{
+    int rc = grid_flow_setup(who, x, y, t, nullptr, p, offsets, batch, n, grid, n_cand, gh, gw, H, W, sigma, objective, 1,
+                             (size_t)(H + 1) * (W + 1), workspace, workspace_bytes, D.G, ws, taps, "inverse depth");
+    if (rc) return rc;
+    if (batch > 0 && !motion) { set_error("%s: null motion", who); return EVK_E_ARG; }
+    D.G.F.C.Hm = H; D.G.F.C.Wm = W;
+    D.G.F.C.p_scale = 1.0;
+    D.motion = motion;
+    D.cx = cx; D.cy = cy;
+    return EVK_OK;
+}
+
+// forward and candidates: zero the counters and the accumulators of the batch J canvases, the event pass, the tail into
+// iwe_out (the candidates: ws.Wimg).  nonfinite stays zero: a non-finite event contributes nothing (model_taps).
+static int depth_grid_forward(const DepthGridArgs &D, const BatchObjWorkspace &ws, const BlurTaps &taps, int batch,
+                              int objective, double obj_param, float *iwe_out, double *f_out, cudaStream_t st)
+{
+    const GridArgs &A = D.G;
+    const int npix = A.F.C.Hc * A.F.C.Wc, canvases = batch * A.J;
+    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
+    if (A.F.E.n > 0) {
+        const size_t smem = (size_t)A.J * A.gh * A.gw * sizeof(float);
+        EVK_CUDA(cudaFuncSetAttribute(depth_grid_cand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ProfScope prof(st);
+        prof_count(1);
+        depth_grid_cand_kernel<<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(D);
+    }
+    batch_obj_forward_tail(ws, A.F.C.Hc, A.F.C.Wc, taps, canvases, objective, obj_param, iwe_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }
@@ -3608,6 +3849,92 @@ int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const floa
     if (batch == 0) return EVK_OK;
     // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
     return grid_flow_forward(A, ws, taps, batch, objective, obj_param, ws.Wimg, f_out, static_cast<cudaStream_t>(stream));
+}
+
+size_t evk_cmax_depth_grid_objective_workspace_bytes(int batch, int gh, int gw, int H, int W)
+{
+    return evk_cmax_grid_flow_objective_workspace_bytes(batch, gh, gw, H, W);
+}
+
+int evk_cmax_depth_grid_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                      const int64_t *offsets, int batch, int64_t n_events, const double *motion, double cx,
+                                      double cy, const float *inv_depth_grid, int gh, int gw, int H, int W, double sigma,
+                                      int objective, double obj_param, double *f_out, float *iwe_out, void *workspace,
+                                      size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_cmax_depth_grid_objective_f32";
+    DepthGridArgs D;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = depth_grid_setup(who, x, y, t_rel, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H, W,
+                              sigma, objective, workspace, workspace_bytes, D, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !iwe_out)) { set_error("%s: null output", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    return depth_grid_forward(D, ws, taps, batch, objective, obj_param, iwe_out, f_out, static_cast<cudaStream_t>(stream));
+}
+
+int evk_cmax_depth_grid_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                           const int64_t *offsets, int batch, int64_t n_events, const double *motion,
+                                           double cx, double cy, const float *inv_depth_grid, int gh, int gw, int H, int W,
+                                           double sigma, int objective, double obj_param, const float *iwe,
+                                           const float *grad_f, float *grad_grid, void *workspace, size_t workspace_bytes,
+                                           void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_cmax_depth_grid_objective_grad_f32";
+    DepthGridArgs D;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = depth_grid_setup(who, x, y, t_rel, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H, W,
+                              sigma, objective, workspace, workspace_bytes, D, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!iwe || !grad_f || !grad_grid)) { set_error("%s: null array", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int64_t G = (int64_t)gh * gw, nodes = batch * G;
+    // the f64 node sums live in the accumulator, which the backward has no other use for ((H+1)(W+1) 16 B >= gh gw 8 B)
+    D.G.grad = reinterpret_cast<double *>(ws.acc);
+    EVK_CUDA(cudaMemsetAsync(D.G.grad, 0, (size_t)nodes * sizeof(double), st));
+    batch_obj_backward_W(ws, iwe, H + 1, W + 1, taps, batch, objective, obj_param, grad_f, st);
+    D.G.F.Wimg = ws.Wimg;
+    if (n_events > 0) {
+        const size_t smem = (size_t)G * (sizeof(double) + sizeof(float));
+        EVK_CUDA(cudaFuncSetAttribute(depth_grid_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ProfScope prof(st);
+        prof_count(1);
+        depth_grid_grad_kernel<<<batch_grid(n_events, batch), kFlowObjThreads, smem, st>>>(D);
+    }
+    prof_count(1);
+    grid_flow_grad_cast_kernel<<<grid_simple(nodes, 256), 256, 0, st>>>(D.G.grad, grad_grid, nodes);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_cmax_depth_grid_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
+{
+    return evk_cmax_grid_flow_candidates_workspace_bytes(batch, n_cand, gh, gw, H, W);
+}
+
+int evk_cmax_depth_grid_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                       const int64_t *offsets, int batch, int64_t n_events, const double *motion, double cx,
+                                       double cy, const float *cand, int n_cand, int gh, int gw, int H, int W,
+                                       double blur_sigma, int objective, double obj_param, double *f_out, void *workspace,
+                                       size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_cmax_depth_grid_candidates_f32";
+    DepthGridArgs D;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = depth_grid_setup(who, x, y, t_rel, p, offsets, batch, n_events, motion, cx, cy, cand, n_cand < 1 ? -1 : n_cand, gh,
+                              gw, H, W, blur_sigma, objective, workspace, workspace_bytes, D, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && !f_out) { set_error("%s: null output", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
+    return depth_grid_forward(D, ws, taps, batch, objective, obj_param, ws.Wimg, f_out, static_cast<cudaStream_t>(stream));
 }
 
 size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W)

@@ -545,6 +545,59 @@ int evk_cmax_grid_flow_candidates_f32(const float *x, const float *y, const floa
                                       double obj_param, double *f_out, void *workspace, size_t workspace_bytes,
                                       void *stream);
 
+/* Depth from a known camera motion: the contrast objective of evk_cmax_motion_depth_objective_f32 with
+ * EVK_WARP_CAMERA_MOTION, where the inverse depth of every event is interpolated from a gh x gw grid of nodes of its
+ * sample instead of read from an array.
+ *   motion        : [batch][8] doubles on the device, the rows (wx, wy, wz, vx, vy, vz, fx, fy) of the camera motion
+ *                   (data: they get no gradient), principal point (cx, cy)
+ *   inv_depth_grid: [batch][gh][gw] f32 on the device, 2 <= gh <= H, 2 <= gw <= W, gh * gw <= 4096
+ * Node (i, j) sits at pixel (j (W-1)/(gw-1), i (H-1)/(gh-1)) (align_corners), and an event at (x, y) takes
+ * rho = bilinear interpolation of inv_depth_grid[b] at (x rx, y ry), with the node cell, weights, f32 products and
+ * zero outside taps of evk_cmax_grid_flow_objective_f32.  Everything after that is the camera motion's: the keep rules
+ * (a negative or non-finite rho, Pz <= 0 or a non-finite Pz: not kept), the warp, the bounds mask, the splat on the
+ * (H+1)x(W+1) canvas, the blur and the four objectives (EVK_OBJ_MOA / EVK_OBJ_ISOA: EVK_E_UNSUPPORTED).  The rotation
+ * exp([theta]x) b of an event is computed once per pass, then the translation and projection per candidate, in
+ * the camera motion's order of operations, so every event's taps are the camera motion's bit for bit: at gh = H,
+ * gw = W with events at integer pixels rho is the node and f is evk_cmax_motion_depth_objective_f32's with that rho, and
+ * at v = 0 f is EVK_WARP_CAMERA_ROTATION's, up to the order in which the f32 image sums add the taps.
+ *   f_out: batch doubles;  iwe_out: [batch][H+1][W+1] floats, which the backward takes as `iwe`
+ * evk_cmax_depth_grid_objective_grad_f32 writes grad_grid [batch][gh][gw] floats = grad_f[b] df_b/dinv_depth_grid[b]:
+ * per kept event df/dx' and df/dy' of evk_cmax_motion_objective_grad_f32 times
+ *   dx'/drho = d fx iz (vx - X vz),  dy'/drho = d fy iz (vy - Y vz)   (d = t_rel)
+ * spread over the event's four node taps with their bilinear weights, summed per CTA in shared memory and across CTAs
+ * in f64, then rounded to f32.  At v = 0 the gradient is exactly zero.
+ * workspace: evk_cmax_depth_grid_objective_workspace_bytes(batch, gh, gw, H, W) bytes (what the grid flow's query
+ * returns), 256-byte aligned, for either call; 0 for arguments the entries reject.  batch <= 65535.  Neither call
+ * synchronises, and both launch the same kernels whatever the batch. */
+size_t evk_cmax_depth_grid_objective_workspace_bytes(int batch, int gh, int gw, int H, int W);
+int evk_cmax_depth_grid_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                      const int64_t *offsets, int batch, int64_t n_events, const double *motion,
+                                      double cx, double cy, const float *inv_depth_grid, int gh, int gw, int H, int W,
+                                      double blur_sigma, int objective, double obj_param, double *f_out,
+                                      float *iwe_out, void *workspace, size_t workspace_bytes, void *stream);
+int evk_cmax_depth_grid_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                           const int64_t *offsets, int batch, int64_t n_events, const double *motion,
+                                           double cx, double cy, const float *inv_depth_grid, int gh, int gw, int H,
+                                           int W, double blur_sigma, int objective, double obj_param,
+                                           const float *iwe, const float *grad_f, float *grad_grid, void *workspace,
+                                           size_t workspace_bytes, void *stream);
+
+/* Many inverse-depth grids per sample in one pass over the events: f_out[b][j] is exactly the f_b of
+ * evk_cmax_depth_grid_objective_f32 with inv_depth_grid[b] = cand[b][j].
+ *   cand : [batch][n_cand][gh][gw] floats on the device, 1 <= n_cand <= 32, n_cand * gh * gw <= 12288 (the limit of
+ *          the grid flow, 48 KB of f32 nodes here), batch * n_cand <= 65535
+ *   f_out: [batch][n_cand] doubles
+ * Every event is read once; its node cell, weights and rotation are computed once and used for every candidate.  All
+ * limits are checked before any CUDA call.  Forward only.  workspace: evk_cmax_depth_grid_candidates_workspace_bytes(
+ * batch, n_cand, gh, gw, H, W) bytes, 256-byte aligned; 0 for arguments the entry rejects.  The call does not
+ * synchronise and launches the same kernels whatever batch and n_cand. */
+size_t evk_cmax_depth_grid_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W);
+int evk_cmax_depth_grid_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                       const int64_t *offsets, int batch, int64_t n_events, const double *motion,
+                                       double cx, double cy, const float *cand, int n_cand, int gh, int gw, int H,
+                                       int W, double blur_sigma, int objective, double obj_param, double *f_out,
+                                       void *workspace, size_t workspace_bytes, void *stream);
+
 /* Parametric contrast maximisation over a batch of samples, as a differentiable loss: per sample the f32
  * fast-mode evaluation of evk_cmax_warp_objective_f32 / evk_cmax_linvel_objective_f32 with Hm = Hs = H,
  * Wm = Ws = W, p_scale 1 and no flags (get_iwe, lib/contrast_max/objectives.py:184-192).  Sample b is the
