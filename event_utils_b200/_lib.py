@@ -278,6 +278,19 @@ def _declare(L):
     L.evk_grid_flow_timestamp_candidates_f32.restype = ci
     L.evk_grid_flow_timestamp_candidates_f32.argtypes = [vp, vp, vp, vp, vp, vp, ci, i64, vp, ci, ci, ci, ci, ci, f64, vp, vp, sz,
                                                          vp]
+    L.evk_depth_grid_timestamp_objective_workspace_bytes.restype = sz
+    L.evk_depth_grid_timestamp_objective_workspace_bytes.argtypes = [ci, ci, ci, ci, ci]
+    L.evk_depth_grid_timestamp_objective_f32.restype = ci
+    L.evk_depth_grid_timestamp_objective_f32.argtypes = [vp, vp, vp, vp, vp, vp, ci, i64, vp, f64, f64, vp, ci, ci, ci, ci, f64,
+                                                         vp, vp, vp, vp, sz, vp]
+    L.evk_depth_grid_timestamp_objective_grad_f32.restype = ci
+    L.evk_depth_grid_timestamp_objective_grad_f32.argtypes = [vp, vp, vp, vp, vp, vp, ci, i64, vp, f64, f64, vp, ci, ci, ci, ci,
+                                                              f64, vp, vp, vp, vp, vp, sz, vp]
+    L.evk_depth_grid_timestamp_candidates_workspace_bytes.restype = sz
+    L.evk_depth_grid_timestamp_candidates_workspace_bytes.argtypes = [ci, ci, ci, ci, ci, ci]
+    L.evk_depth_grid_timestamp_candidates_f32.restype = ci
+    L.evk_depth_grid_timestamp_candidates_f32.argtypes = [vp, vp, vp, vp, vp, vp, ci, i64, vp, f64, f64, vp, ci, ci, ci, ci, ci,
+                                                          f64, vp, vp, sz, vp]
     L.evk_robust_norm_workspace_bytes.restype = sz
     L.evk_robust_norm_workspace_bytes.argtypes = []
     L.evk_robust_norm_f32.restype = ci

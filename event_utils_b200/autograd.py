@@ -335,6 +335,29 @@ class GridFlowTimestampObjective(torch.autograd.Function):
         return _loss_backward(ctx, g)[:1] + (None,) * 7
 
 
+class DepthGridTimestampObjective(torch.autograd.Function):
+    """The batched depth-grid average-timestamp loss of contrast_max/depth_grid_timestamp.py (the camera-motion timestamp
+    loss with each event's inverse depth bilinearly interpolated from a gh x gw grid of nodes): f (B,) f64 from
+    inv_depth_grid (B,gh,gw) and the prepared device events with their normalised stamps tau.  Only the nodes get a
+    gradient: the exact derivative of f, one pass over the events (evk_depth_grid_timestamp_objective_grad_f32).  The
+    forward keeps the timestamp and count images.  opts = (rows, cx, cy, H, W, sigma) with rows the device motion rows
+    (B,8) f64 (_batched._rows)."""
+
+    @staticmethod
+    def forward(ctx, inv_depth_grid, x, y, t_rel, tau, p, offsets, opts):
+        rows, cx, cy, H, W, sigma = opts
+        gh, gw = inv_depth_grid.shape[1:]
+        ctx.rows = rows   # the entries read the rows through a pointer, in the backward too
+        return _loss_forward(ctx, "evk_depth_grid_timestamp_objective", "depth_grid_timestamp_objective", inv_depth_grid,
+                             torch.float32, (_lib.ptr(rows), cx, cy), (gh, gw, H, W, sigma), (H, W), (x, y, t_rel, tau, p),
+                             offsets, (2, 2), query=(gh, gw))
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return _loss_backward(ctx, g)[:1] + (None,) * 7
+
+
 class MotionObjective(torch.autograd.Function):
     """The batched parametric contrast objective of contrast_max/motion_objective.py (get_iwe, objectives.py:184-192, with
     the linvel, rotation or 4-DoF model, then an objective of objectives.py): f (B,) f64 from params (B,K) and the

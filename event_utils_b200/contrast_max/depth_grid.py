@@ -161,6 +161,30 @@ def depth_grid_fit_torch(xs, ys, ts, ps, motion, warpfunc, img_size, inv_depth_r
     _check_warp(warpfunc, who)
     _check_objective(objective, "inverse depth")
     xs, ys, ts, ps = _event_tensors(xs, ys, ts, ps, t0, who, "nothing")
+
+    def events(B, dev):
+        return _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows")
+
+    def loss(ev, model, sigma):
+        return _chunked_objective("evk_cmax_depth_grid_objective", "depth_grid_objective", ev[:4], ev[4], model,
+                                  _scalars(objective, sigma, obj_param), (1,), FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS)
+
+    def candidates(ev, c, model, sigma):
+        return _candidates(ev, c, model, _scalars(objective, sigma, obj_param))
+    return DepthGridFit(*_depth_grid_fit(who, (xs, ys, ts, ps), motion, warpfunc, img_size, inv_depth_range, grid_shapes,
+                                         smoothness, charbonnier_eps, batch_end_indices, blur_sigma, x0, num_samples,
+                                         grid_levels, max_iter, line_search_steps, ftol, gtol, events, loss, candidates))
+
+
+def _depth_grid_fit(who, tensors, motion, warpfunc, img_size, inv_depth_range, grid_shapes, smoothness, charbonnier_eps,
+                    batch_end_indices, blur_sigma, x0, num_samples, grid_levels, max_iter, line_search_steps, ftol, gtol,
+                    events, loss, candidates):
+    """The coarse-to-fine, boxed fit of F = f + smoothness R that depth_grid_fit_torch and depth_grid_timestamp_fit_torch
+    share: the argument checks (before any CUDA call), the constant start and the BFGS stages per grid shape and blur.
+    tensors: the events, which with x0, inv_depth_range and motion choose the device;  events(B, dev) -> the prepared
+    device events;  loss(events, model, sigma) -> fg of f on the nodes (_chunked_objective);  candidates(events, c,
+    model, sigma) -> f (B,J) f64 of the f32 node grids c (B,J,gh gw), with model = _model's layout for the grid (gh, gw).
+    Returns (inv_depth (B,gh,gw), F, f, status, iterations)."""
     H, W = int(img_size[0]), int(img_size[1])
     shapes = [(int(a), int(b)) for a, b in grid_shapes]
     if not shapes:
@@ -192,36 +216,34 @@ def depth_grid_fit_torch(xs, ys, ts, ps, motion, warpfunc, img_size, inv_depth_r
         raise ValueError("num_samples must be odd and grid_levels >= 1, got %r and %r" % (num_samples, grid_levels))
     lam, eps = float(smoothness), float(charbonnier_eps)
     _lib.lib()
-    dev = E.compute_device(*(a for a in (x0, inv_depth_range, motion, xs, ys, ts, ps) if isinstance(a, torch.Tensor)))
-    ev = _batch_events(xs, ys, ts, ps, t0, batch_end_indices, B, dev, "windows")
+    dev = E.compute_device(*(a for a in (x0, inv_depth_range, motion) + tuple(tensors) if isinstance(a, torch.Tensor)))
+    ev = events(B, dev)
     with torch.cuda.device(dev):
         box = _per_window(inv_depth_range, B, (2,), "inv_depth_range", dev).unsqueeze(1)     # (B,1,2)
         scale = (box[:, 0, 1] - box[:, 0, 0]) / (max(int(num_samples), 2) - 1)
         motion_model = _model(motion, warpfunc, B, dev, None, H, W)[4]
 
-        def loss(ev, grid, sigma):
+        def stage_loss(ev, grid, sigma):
             model = ("grid", grid, H, W, motion_model)
-            scalars = _scalars(objective, sigma, obj_param)
-            return (_chunked_objective("evk_cmax_depth_grid_objective", "depth_grid_objective", ev[:4], ev[4], model,
-                                       scalars, (1,), FIT_WORKSPACE_BYTES, FIT_MAX_WINDOWS),
-                    lambda c: _candidates(ev, c, model, scalars))
+            return loss(ev, model, sigma), lambda c: candidates(ev, c, model, sigma)
         if x0 is None:
-            start = _constant_start(ev, box, (gh0, gw0), H, W, motion_model, _scalars(objective, sigmas[0], obj_param),
-                                    int(num_samples), int(grid_levels))
+            start = _constant_start(ev, box, (gh0, gw0), H, W, motion_model, sigmas[0], int(num_samples), int(grid_levels),
+                                    candidates)
             grid = start.view(B, 1, 1, 1).expand(B, 1, gh0, gw0).contiguous()
         else:
             grid = _per_window(x0, B, (gh0, gw0), "x0", dev).unsqueeze(1)
-        D, f, rest, status, iters = _stages(grid, shapes, sigmas, box, scale, ev, loss, lam, eps, max_iter,
+        D, f, rest, status, iters = _stages(grid, shapes, sigmas, box, scale, ev, stage_loss, lam, eps, max_iter,
                                             line_search_steps, ftol, gtol)
-    return DepthGridFit(D[:, 0], f, rest, status, iters)
+    return D[:, 0], f, rest, status, iters
 
 
-def _constant_start(ev, box, grid, H, W, motion_model, scalars, num_samples, levels):
-    """(B,) f64: the best constant inverse depth of every window, grid-searched inside the box (B,1,2)"""
+def _constant_start(ev, box, grid, H, W, motion_model, sigma, num_samples, levels, candidates):
+    """(B,) f64: the best constant inverse depth of every window, grid-searched inside the box (B,1,2) with the
+    candidates function of _depth_grid_fit"""
     gh, gw = grid
     model = ("grid", grid, H, W, motion_model)
 
     def evaluate(pts):
         B, P, _ = pts.shape
-        return _candidates(ev, pts.to(torch.float32).expand(B, P, gh * gw).contiguous(), model, scalars)
+        return candidates(ev, pts.to(torch.float32).expand(B, P, gh * gw).contiguous(), model, sigma)
     return _grid_search(evaluate, box, num_samples, levels, bounds=box)[:, 0]

@@ -1895,6 +1895,10 @@ __device__ __forceinline__ void ts_block_add(float *acc, int64_t npix, int Wc, i
     red_add4(blk + 4, make_float4(__fmul_rn(ox, oy), __fmul_rn(dx, oy), __fmul_rn(ox, dy), __fmul_rn(dx, dy)));
 }
 
+// 16-byte accumulator blocks per image of the timestamp losses: one 32-byte block per canvas pixel and polarity; the
+// dense-flow backward's flow-gradient blocks ([2][H][W] per sample) are fewer
+static size_t flow_ts_acc_blocks(int H, int W) { return (size_t)2 * (H + 1) * (W + 1); }
+
 // ---- the dense-flow passes ----
 struct FlowArgs {
     CmaxArgs C;            // canvas (Hc, Wc) for splat_taps
@@ -2595,6 +2599,11 @@ static int grid_flow_node_grad(const GridArgs &A, int batch, float *grad_grid, c
 //             [B][gh][gw] in the workspace, cast to the f32 output by grid_flow_grad_cast_kernel.
 // The limits are the grid flow's (grid_flow_limits): gh gw <= kMaxGridNodes for the loss and n_cand gh gw <=
 // kMaxGridCandNodes for the candidates -- half the grid flow's shared memory, since a node is one float.
+// The depth-grid average-timestamp loss (evk_depth_grid_timestamp_*) runs the same passes with TS = true: a 20-byte
+// record per event, weight 1, the two v4 reductions of ts_block_add into image pair z = 2 (b J + j) + s and
+// ts_obj_forward_tail; a non-finite warp contributes nothing and flags no sample (motion_ts_event_kernel's rule).  Its
+// backward gathers the (A, B) pairs of ts_obj_backward_ab instead of W_b, as grid_flow_grad_kernel<true> does, and
+// contracts df/dx', df/dy' with the same dx'/drho, dy'/drho, without the splat weight.
 struct DepthGridArgs {
     GridArgs G;             // canvas and bounds mask (F.C), events, nodes [B][J][gh][gw], accumulators, node sums
     const double *motion;   // [B][8] rows (wx, wy, wz, vx, vy, vz, fx, fy)
@@ -2641,6 +2650,7 @@ __device__ __forceinline__ bool depth_taps(const CmaxArgs &C, const CamMotion &m
     return model_keep_taps(C, q.xw, q.yw, p, oob, T);
 }
 
+template <bool TS>
 __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_cand_kernel(const DepthGridArgs D)
 {
     extern __shared__ float depth_nodes[];   // [J][gh gw]
@@ -2651,23 +2661,32 @@ __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_cand_kernel(const 
     sample_range(A.F.E, b, first, last);
     const CmaxArgs &C = A.F.C;
     const int64_t npix = (int64_t)C.Hc * C.Wc;
-    float *acc = A.F.acc + (int64_t)b * J * npix * 4;
+    float *acc = A.F.acc + (int64_t)b * J * npix * (TS ? 2 * 8 : 4);   // per canvas: one IWE block or two {S, C} blocks
     const CamMotion m = cam_motion(D, b);
-    for_each_event(first, last, [&](int64_t i) { return load_xytp(A.F.E, i); }, [&](int64_t, const EvXYTP &e) {
+    for_each_event(first, last, [&](int64_t i) { return load_grid_event<TS>(A.F.E, i); }, [&](int64_t, const auto &e) {
+        const int pol = TS ? ts_polarity(e.p) : 0;
+        if (pol < 0) return;   // a NaN p is in neither timestamp image
         const NodeSample s = node_sample(A, e.x, e.y);
         const CamRot r = cam_rotate(e.x, e.y, e.t, m.wx, m.wy, m.wz, m.fx, m.fy, m.cx, m.cy);
         for (int j = 0; j < J; ++j) {
             CamProj q;
             Taps T;
-            if (depth_taps(C, m, r, node_depth(depth_nodes + j * G, s), e.t, e.p, q, T))
+            if constexpr (TS) {
+                if (depth_taps(C, m, r, node_depth(depth_nodes + j * G, s), e.t, 1.0f, q, T))
+                    ts_block_add(acc + (int64_t)j * 2 * npix * 8, npix, C.Wc, pol, T, e.tau);
+            } else if (depth_taps(C, m, r, node_depth(depth_nodes + j * G, s), e.t, e.p, q, T)) {
                 red_add4(acc + ((int64_t)j * npix + (int64_t)T.y0 * C.Wc + T.x0) * 4, T.ti);
+            }
         }
     });
 }
 
-// The node-gradient pass, written out like grid_flow_grad_kernel (warp_key_sum needs every lane)
+// The node-gradient pass of both depth-grid losses, written out like grid_flow_grad_kernel (warp_key_sum needs every
+// lane)
+template <bool TS>
 __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const DepthGridArgs D)
 {
+    using Ev = decltype(load_grid_event<TS>(D.G.F.E, 0));
     extern __shared__ double depth_acc[];   // [gh gw] f64, then the nodes [gh gw] f32
     const GridArgs &A = D.G;
     const int b = blockIdx.y, G = A.gh * A.gw;
@@ -2679,38 +2698,55 @@ __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const 
     const CmaxArgs &C = A.F.C;
     const int Wc = C.Wc;
     const int64_t npix = (int64_t)C.Hc * Wc;
-    const float *Wb = A.F.Wimg + b * npix;
+    const float *Wb = TS ? nullptr : A.F.Wimg + b * npix;        // contrast: W_b
+    const float2 *ab = TS ? A.F.ab + b * 2 * npix : nullptr;     // timestamp: the (A, B) pairs of both polarities
     const CamMotion m = cam_motion(D, b);
     const int lane = threadIdx.x & 31;
     const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
     for (int64_t i0 = first + (int64_t)blockIdx.x * kFlowObjThreads + (threadIdx.x - lane); i0 < last; i0 += kBatch * stride) {
-        EvXYTP ev[kBatch];
+        Ev ev[kBatch];
 #pragma unroll
         for (int k = 0; k < kBatch; ++k) {
             const int64_t q = i0 + k * stride + lane;
-            ev[k] = q < last ? load_xytp(A.F.E, q) : EvXYTP{};
+            ev[k] = q < last ? load_grid_event<TS>(A.F.E, q) : Ev{};
             if (!(q < last)) ev[k].x = __int_as_float(0x7fc00000);   // a NaN position: no cell, no term
         }
 #pragma unroll
         for (int k = 0; k < kBatch; ++k) {
-            const EvXYTP &e = ev[k];
+            const Ev &e = ev[k];
             const NodeSample s = node_sample(A, e.x, e.y);
             float val[4] = {0.0f, 0.0f, 0.0f, 0.0f};
             int key = -1 - lane;   // a lane without a term is alone with its key
-            if (s.cell >= 0) {
+            const int pol = TS ? ts_polarity(e.p) : 0;   // a NaN p: no term
+            if (s.cell >= 0 && pol >= 0) {
                 const CamRot r = cam_rotate(e.x, e.y, e.t, m.wx, m.wy, m.wz, m.fx, m.fy, m.cx, m.cy);
                 CamProj q;
                 Taps T;
-                if (depth_taps(C, m, r, node_depth(nodes, s), e.t, e.p, q, T)) {
-                    const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
-                    const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0),
-                                w11 = __ldg(Wb + r1 + T.x1);
-                    const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
+                if (depth_taps(C, m, r, node_depth(nodes, s), e.t, TS ? 1.0f : e.p, q, T)) {
                     float sx, sy;
-                    tap_slopes(ox, oy, T.dx, T.dy, w00, w01, w10, w11, sx, sy);
+                    if constexpr (TS) {
+                        // dF/dk = tau A + B per tap of the event's polarity, as in grid_flow_grad_kernel<true>
+                        const float2 *abs_ = pol ? ab + npix : ab;
+                        const float dx = T.dx, dy = T.dy;
+                        const float ox = __fsub_rn(1.0f, dx), oy = __fsub_rn(1.0f, dy);
+                        const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
+                        const float2 a00 = __ldg(abs_ + r0 + T.x0), a01 = __ldg(abs_ + r0 + T.x1),
+                                     a10 = __ldg(abs_ + r1 + T.x0), a11 = __ldg(abs_ + r1 + T.x1);
+                        const float tau = e.tau;
+                        const float q00 = tau * a00.x + a00.y, q01 = tau * a01.x + a01.y, q10 = tau * a10.x + a10.y,
+                                    q11 = tau * a11.x + a11.y;
+                        tap_slopes(ox, oy, dx, dy, q00, q01, q10, q11, sx, sy);
+                    } else {
+                        const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
+                        const float w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0),
+                                    w11 = __ldg(Wb + r1 + T.x1);
+                        const float ox = 1.0f - T.dx, oy = 1.0f - T.dy;
+                        tap_slopes(ox, oy, T.dx, T.dy, w00, w01, w10, w11, sx, sy);
+                    }
                     const float di = e.t * q.iz;   // dx'/drho = d fx iz (vx - X vz), dy'/drho = d fy iz (vy - Y vz)
                     const float jx = (di * m.fx) * (m.vx - q.X * m.vz), jy = (di * m.fy) * (m.vy - q.Y * m.vz);
-                    node_terms(s, T.wm * (sx * jx + sy * jy), val, key);
+                    if constexpr (TS) node_terms(s, sx * jx + sy * jy, val, key);
+                    else node_terms(s, T.wm * (sx * jx + sy * jy), val, key);
                 }
             }
             node_grad_flush<1>(depth_acc, G, s, key, val);
@@ -2722,14 +2758,17 @@ __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const 
         if (depth_acc[q] != 0.0) atomicAdd(dst + q, depth_acc[q]);
 }
 
-// The checks and set-up of the depth-grid entries: grid_flow_setup's (one image per canvas), then the motion rows
-static int depth_grid_setup(const char *who, const float *x, const float *y, const float *t, const float *p,
+// The checks and set-up of the depth-grid entries: grid_flow_setup's, then the motion rows.  `images` per canvas: 1 for
+// the contrast loss, 2 for the timestamp loss (with its stamps tau, objective OBJ_SOS and acc_blocks flow_ts_acc_blocks).
+static int depth_grid_setup(const char *who, const float *x, const float *y, const float *t, const float *tau, const float *p,
                             const int64_t *offsets, int batch, int64_t n, const double *motion, double cx, double cy,
                             const float *grid, int n_cand, int gh, int gw, int H, int W, double sigma, int objective,
-                            void *workspace, size_t workspace_bytes, DepthGridArgs &D, BatchObjWorkspace &ws, BlurTaps &taps)
+                            int images, void *workspace, size_t workspace_bytes, DepthGridArgs &D, BatchObjWorkspace &ws,
+                            BlurTaps &taps)
 {
-    int rc = grid_flow_setup(who, x, y, t, nullptr, p, offsets, batch, n, grid, n_cand, gh, gw, H, W, sigma, objective, 1,
-                             (size_t)(H + 1) * (W + 1), workspace, workspace_bytes, D.G, ws, taps, "inverse depth");
+    const size_t acc_blocks = images == 2 ? flow_ts_acc_blocks(H, W) : (size_t)(H + 1) * (W + 1);
+    int rc = grid_flow_setup(who, x, y, t, tau, p, offsets, batch, n, grid, n_cand, gh, gw, H, W, sigma, objective, images,
+                             acc_blocks, workspace, workspace_bytes, D.G, ws, taps, "inverse depth");
     if (rc) return rc;
     if (batch > 0 && !motion) { set_error("%s: null motion", who); return EVK_E_ARG; }
     D.G.F.C.Hm = H; D.G.F.C.Wm = W;
@@ -2739,22 +2778,50 @@ static int depth_grid_setup(const char *who, const float *x, const float *y, con
     return EVK_OK;
 }
 
-// forward and candidates: zero the counters and the accumulators of the batch J canvases, the event pass, the tail into
-// iwe_out (the candidates: ws.Wimg).  nonfinite stays zero: a non-finite event contributes nothing (model_taps).
-static int depth_grid_forward(const DepthGridArgs &D, const BatchObjWorkspace &ws, const BlurTaps &taps, int batch,
-                              int objective, double obj_param, float *iwe_out, double *f_out, cudaStream_t st)
+// forward and candidates, before the tail: zero the counters and the accumulators of the batch J canvases, the event
+// pass.  nonfinite stays zero: a non-finite event contributes nothing (model_taps).
+template <bool TS>
+static int depth_grid_event_pass(const DepthGridArgs &D, const BatchObjWorkspace &ws, int batch, cudaStream_t st)
 {
     const GridArgs &A = D.G;
     const int npix = A.F.C.Hc * A.F.C.Wc, canvases = batch * A.J;
-    EVK_CUDA(batch_obj_zero(ws, canvases, npix, 4, st));
+    EVK_CUDA(batch_obj_zero(ws, (TS ? 2 : 1) * (int64_t)canvases, npix, TS ? 8 : 4, st));
     if (A.F.E.n > 0) {
         const size_t smem = (size_t)A.J * A.gh * A.gw * sizeof(float);
-        EVK_CUDA(cudaFuncSetAttribute(depth_grid_cand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        EVK_CUDA(cudaFuncSetAttribute(depth_grid_cand_kernel<TS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         ProfScope prof(st);
         prof_count(1);
-        depth_grid_cand_kernel<<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(D);
+        depth_grid_cand_kernel<TS><<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(D);
     }
-    batch_obj_forward_tail(ws, A.F.C.Hc, A.F.C.Wc, taps, canvases, objective, obj_param, iwe_out, f_out, st);
+    return EVK_OK;
+}
+
+// forward and candidates of the contrast loss: the event pass, the tail into iwe_out (the candidates: ws.Wimg)
+static int depth_grid_forward(const DepthGridArgs &D, const BatchObjWorkspace &ws, const BlurTaps &taps, int batch,
+                              int objective, double obj_param, float *iwe_out, double *f_out, cudaStream_t st)
+{
+    if (int rc = depth_grid_event_pass<false>(D, ws, batch, st)) return rc;
+    batch_obj_forward_tail(ws, D.G.F.C.Hc, D.G.F.C.Wc, taps, batch * D.G.J, objective, obj_param, iwe_out, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+// backward, after the image-space half (which set D.G.F.Wimg or D.G.F.ab): the node pass into the f64 sums D.G.grad
+// (zeroed by the caller), then their cast to grad_grid
+template <bool TS>
+static int depth_grid_node_grad(const DepthGridArgs &D, int batch, float *grad_grid, cudaStream_t st)
+{
+    const GridArgs &A = D.G;
+    const int64_t G = (int64_t)A.gh * A.gw, nodes = batch * G;
+    if (A.F.E.n > 0) {
+        const size_t smem = (size_t)G * (sizeof(double) + sizeof(float));
+        EVK_CUDA(cudaFuncSetAttribute(depth_grid_grad_kernel<TS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ProfScope prof(st);
+        prof_count(1);
+        depth_grid_grad_kernel<TS><<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(D);
+    }
+    prof_count(1);
+    grid_flow_grad_cast_kernel<<<grid_simple(nodes, 256), 256, 0, st>>>(A.grad, grad_grid, nodes);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }
@@ -3115,8 +3182,7 @@ static int motion_seg_setup(const char *who, const float *x, const float *y, con
 //   backward: U_s = G(2 g_b G_s) (f64 adjoint blur); (A_s, B_s) = (U_s / C_s, -U_s T_s / C_s) as f32 pairs
 //             [B][2][Hc][Wc][2]; per kept event the four pairs of its polarity give dF/dk = tau A + B per tap, then
 //             df/dx', df/dy' through the tap weights as in flow_obj_event, spread by flow_obj_spread.
-// one 32-byte block per canvas pixel and polarity; the backward's flow-gradient blocks ([2][H][W] per sample) are fewer
-static size_t flow_ts_acc_blocks(int H, int W) { return (size_t)2 * (H + 1) * (W + 1); }
+// The accumulator is flow_ts_acc_blocks' (defined with ts_block_add).
 
 template <bool GRAD>
 __device__ __forceinline__ void flow_ts_event(const FlowArgs &A, const float *flow, float *acc, const float2 *ab, const EvXYTUP &e,
@@ -3867,8 +3933,8 @@ int evk_cmax_depth_grid_objective_f32(const float *x, const float *y, const floa
     DepthGridArgs D;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = depth_grid_setup(who, x, y, t_rel, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H, W,
-                              sigma, objective, workspace, workspace_bytes, D, ws, taps);
+    int rc = depth_grid_setup(who, x, y, t_rel, nullptr, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H,
+                              W, sigma, objective, 1, workspace, workspace_bytes, D, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!f_out || !iwe_out)) { set_error("%s: null output", who); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
@@ -3887,29 +3953,18 @@ int evk_cmax_depth_grid_objective_grad_f32(const float *x, const float *y, const
     DepthGridArgs D;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = depth_grid_setup(who, x, y, t_rel, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H, W,
-                              sigma, objective, workspace, workspace_bytes, D, ws, taps);
+    int rc = depth_grid_setup(who, x, y, t_rel, nullptr, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H,
+                              W, sigma, objective, 1, workspace, workspace_bytes, D, ws, taps);
     if (rc) return rc;
     if (batch > 0 && (!iwe || !grad_f || !grad_grid)) { set_error("%s: null array", who); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int64_t G = (int64_t)gh * gw, nodes = batch * G;
     // the f64 node sums live in the accumulator, which the backward has no other use for ((H+1)(W+1) 16 B >= gh gw 8 B)
     D.G.grad = reinterpret_cast<double *>(ws.acc);
-    EVK_CUDA(cudaMemsetAsync(D.G.grad, 0, (size_t)nodes * sizeof(double), st));
+    EVK_CUDA(cudaMemsetAsync(D.G.grad, 0, (size_t)batch * gh * gw * sizeof(double), st));
     batch_obj_backward_W(ws, iwe, H + 1, W + 1, taps, batch, objective, obj_param, grad_f, st);
     D.G.F.Wimg = ws.Wimg;
-    if (n_events > 0) {
-        const size_t smem = (size_t)G * (sizeof(double) + sizeof(float));
-        EVK_CUDA(cudaFuncSetAttribute(depth_grid_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ProfScope prof(st);
-        prof_count(1);
-        depth_grid_grad_kernel<<<batch_grid(n_events, batch), kFlowObjThreads, smem, st>>>(D);
-    }
-    prof_count(1);
-    grid_flow_grad_cast_kernel<<<grid_simple(nodes, 256), 256, 0, st>>>(D.G.grad, grad_grid, nodes);
-    EVK_CUDA(cudaGetLastError());
-    return EVK_OK;
+    return depth_grid_node_grad<false>(D, batch, grad_grid, st);
 }
 
 size_t evk_cmax_depth_grid_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
@@ -3928,8 +3983,8 @@ int evk_cmax_depth_grid_candidates_f32(const float *x, const float *y, const flo
     DepthGridArgs D;
     BatchObjWorkspace ws;
     BlurTaps taps;
-    int rc = depth_grid_setup(who, x, y, t_rel, p, offsets, batch, n_events, motion, cx, cy, cand, n_cand < 1 ? -1 : n_cand, gh,
-                              gw, H, W, blur_sigma, objective, workspace, workspace_bytes, D, ws, taps);
+    int rc = depth_grid_setup(who, x, y, t_rel, nullptr, p, offsets, batch, n_events, motion, cx, cy, cand, n_cand < 1 ? -1 : n_cand,
+                              gh, gw, H, W, blur_sigma, objective, 1, workspace, workspace_bytes, D, ws, taps);
     if (rc) return rc;
     if (batch > 0 && !f_out) { set_error("%s: null output", who); return EVK_E_ARG; }
     if (batch == 0) return EVK_OK;
@@ -4612,6 +4667,95 @@ int evk_grid_flow_timestamp_candidates_f32(const float *x, const float *y, const
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if ((rc = grid_flow_event_pass<true>(A, ws, batch, st))) return rc;
     // T goes to ws.Wimg and C behind the forward-only carve, as in evk_motion_timestamp_candidates_f32
+    float *cnt = reinterpret_cast<float *>(static_cast<char *>(workspace) + motion_ts_cand_head(images, H, W));
+    ts_obj_forward_tail(ws, H + 1, W + 1, taps, batch * n_cand, ws.Wimg, cnt, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+size_t evk_depth_grid_timestamp_objective_workspace_bytes(int batch, int gh, int gw, int H, int W)
+{
+    return evk_grid_flow_timestamp_objective_workspace_bytes(batch, gh, gw, H, W);
+}
+
+int evk_depth_grid_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                           const int64_t *offsets, int batch, int64_t n_events, const double *motion, double cx,
+                                           double cy, const float *inv_depth_grid, int gh, int gw, int H, int W, double sigma,
+                                           double *f_out, float *ts_out, float *cnt_out, void *workspace,
+                                           size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_depth_grid_timestamp_objective_f32";
+    DepthGridArgs D;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = depth_grid_setup(who, x, y, t_rel, tau, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H,
+                              W, sigma, OBJ_SOS, 2, workspace, workspace_bytes, D, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!f_out || !ts_out || !cnt_out)) { set_error("%s: null output", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if ((rc = depth_grid_event_pass<true>(D, ws, batch, st))) return rc;
+    ts_obj_forward_tail(ws, H + 1, W + 1, taps, batch, ts_out, cnt_out, f_out, st);
+    EVK_CUDA(cudaGetLastError());
+    return EVK_OK;
+}
+
+int evk_depth_grid_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                                const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                                const double *motion, double cx, double cy, const float *inv_depth_grid, int gh,
+                                                int gw, int H, int W, double sigma, const float *ts_img, const float *cnt_img,
+                                                const float *grad_f, float *grad_grid, void *workspace, size_t workspace_bytes,
+                                                void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_depth_grid_timestamp_objective_grad_f32";
+    DepthGridArgs D;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = depth_grid_setup(who, x, y, t_rel, tau, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H,
+                              W, sigma, OBJ_SOS, 2, workspace, workspace_bytes, D, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!ts_img || !cnt_img || !grad_f || !grad_grid)) { set_error("%s: null array", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // the f64 node sums live in the accumulator, which the backward has no other use for (ts_obj_backward_ab writes
+    // ws.Wimg and ws.wt): 2 batch 2 (H+1)(W+1) 16 B >= batch gh gw 8 B
+    D.G.grad = reinterpret_cast<double *>(ws.acc);
+    EVK_CUDA(cudaMemsetAsync(D.G.grad, 0, (size_t)batch * gh * gw * sizeof(double), st));
+    D.G.F.ab = ts_obj_backward_ab(ws, ts_img, cnt_img, H + 1, W + 1, taps, batch, grad_f, st);
+    return depth_grid_node_grad<true>(D, batch, grad_grid, st);
+}
+
+size_t evk_depth_grid_timestamp_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
+{
+    return evk_grid_flow_timestamp_candidates_workspace_bytes(batch, n_cand, gh, gw, H, W);
+}
+
+int evk_depth_grid_timestamp_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau, const float *p,
+                                            const int64_t *offsets, int batch, int64_t n_events, const double *motion,
+                                            double cx, double cy, const float *cand, int n_cand, int gh, int gw, int H, int W,
+                                            double blur_sigma, double *f_out, void *workspace, size_t workspace_bytes,
+                                            void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_depth_grid_timestamp_candidates_f32";
+    DepthGridArgs D;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = depth_grid_setup(who, x, y, t_rel, tau, p, offsets, batch, n_events, motion, cx, cy, cand, n_cand < 1 ? -1 : n_cand,
+                              gh, gw, H, W, blur_sigma, OBJ_SOS, 2, workspace, workspace_bytes, D, ws, taps);
+    if (rc) return rc;
+    const int images = 2 * batch * n_cand;
+    if (workspace_bytes < motion_ts_cand_bytes(images, H, W)) {
+        set_error("%s: 256-byte aligned workspace of %zu bytes required", who, motion_ts_cand_bytes(images, H, W));
+        return EVK_E_WORKSPACE;
+    }
+    if (batch > 0 && !f_out) { set_error("%s: null output", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if ((rc = depth_grid_event_pass<true>(D, ws, batch, st))) return rc;
+    // T goes to ws.Wimg and C behind the forward-only carve, as in evk_grid_flow_timestamp_candidates_f32
     float *cnt = reinterpret_cast<float *>(static_cast<char *>(workspace) + motion_ts_cand_head(images, H, W));
     ts_obj_forward_tail(ws, H + 1, W + 1, taps, batch * n_cand, ws.Wimg, cnt, f_out, st);
     EVK_CUDA(cudaGetLastError());

@@ -932,6 +932,66 @@ int evk_grid_flow_timestamp_candidates_f32(const float *x, const float *y, const
                                            double blur_sigma, double *f_out, void *workspace, size_t workspace_bytes,
                                            void *stream);
 
+/* Depth from a known camera motion with the average-timestamp loss: the inverse depth of every event interpolated from
+ * a gh x gw grid of nodes of its sample, exactly as in evk_cmax_depth_grid_objective_f32 (motion rows, principal point,
+ * node layout, f32 weights, zero outside taps, rotation once per pass), then the loss of
+ * evk_motion_timestamp_depth_objective_f32 at that rho.
+ *   motion        : [batch][8] doubles on the device, rows (wx, wy, wz, vx, vy, vz, fx, fy) (data: no gradient)
+ *   inv_depth_grid: [batch][gh][gw] f32 on the device, 2 <= gh <= H, 2 <= gw <= W, gh * gw <= 4096
+ *   tau           : the normalised stamps of evk_motion_timestamp_objective_f32
+ * Keep rules: an event with a negative or non-finite rho, with Pz <= 0 or a non-finite Pz, or outside the bounds mask
+ * (0 < x' <= W, 0 < y' <= H) contributes nothing, with weight 1, and so does an event with a NaN p; a non-finite warp
+ * flags no sample, so f is never NaN from the events.  The T and C images per polarity, the blur and
+ * f_b = sum G(T_+)^2 + sum G(T_-)^2 are evk_motion_timestamp_objective_f32's.  Blur sigma: <= 0 blurs nothing, a
+ * NaN is rejected (EVK_E_ARG) and a sigma whose radius round(4 sigma) exceeds 64 is EVK_E_UNSUPPORTED.
+ *   f_out: batch doubles;  ts_out, cnt_out: [batch][2][H+1][W+1] floats, which the backward takes as ts_img, cnt_img.
+ *   0 <= batch <= 32767.
+ * evk_depth_grid_timestamp_objective_grad_f32 writes grad_grid [batch][gh][gw] floats = grad_f[b] df_b/dinv_depth_grid[b]:
+ * per contributing event df/dx' and df/dy' of evk_motion_timestamp_objective_grad_f32 times
+ *   dx'/drho = d fx iz (vx - X vz),  dy'/drho = d fy iz (vy - Y vz)   (d = t_rel)
+ * spread over the event's four node taps with their bilinear weights, summed per CTA in shared memory and across CTAs
+ * in f64, then rounded to f32.
+ * Identities: at gh = H, gw = W with events at integer pixels rho is the node and f is
+ * evk_motion_timestamp_depth_objective_f32's with that rho; for a constant grid c, f is that loss at rho = c to f32
+ * rounding (the four f32 node weights need not sum to exactly 1); at v = 0 f is EVK_WARP_CAMERA_ROTATION's timestamp
+ * loss, up to the order in which the f32 image sums add the taps, and the gradient is exactly zero (dx'/drho and
+ * dy'/drho are exact zeros, so no node term is formed).
+ * workspace: evk_depth_grid_timestamp_objective_workspace_bytes(batch, gh, gw, H, W) bytes (what the grid flow's
+ * timestamp query returns), 256-byte aligned, for either call; 0 for arguments the entries reject.  All limits and the
+ * blur-sigma rule are checked before any CUDA call.  Neither call synchronises, and both launch the same kernels
+ * whatever the batch. */
+size_t evk_depth_grid_timestamp_objective_workspace_bytes(int batch, int gh, int gw, int H, int W);
+int evk_depth_grid_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                           const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                           const double *motion, double cx, double cy, const float *inv_depth_grid,
+                                           int gh, int gw, int H, int W, double blur_sigma, double *f_out,
+                                           float *ts_out, float *cnt_out, void *workspace, size_t workspace_bytes,
+                                           void *stream);
+int evk_depth_grid_timestamp_objective_grad_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                                const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                                const double *motion, double cx, double cy,
+                                                const float *inv_depth_grid, int gh, int gw, int H, int W,
+                                                double blur_sigma, const float *ts_img, const float *cnt_img,
+                                                const float *grad_f, float *grad_grid, void *workspace,
+                                                size_t workspace_bytes, void *stream);
+
+/* Many inverse-depth grids per sample in one pass over the events, for the depth-grid average-timestamp loss:
+ * f_out[b][j] is exactly the f_b of evk_depth_grid_timestamp_objective_f32 with inv_depth_grid[b] = cand[b][j].
+ *   cand : [batch][n_cand][gh][gw] floats on the device, 1 <= n_cand <= 32, n_cand * gh * gw <= 12288,
+ *          batch * n_cand <= 32767
+ *   f_out: [batch][n_cand] doubles
+ * Every event is read once (20 bytes); its node cell, weights and rotation are computed once and used for every
+ * candidate.  All limits are checked before any CUDA call.  Forward only.  workspace:
+ * evk_depth_grid_timestamp_candidates_workspace_bytes(batch, n_cand, gh, gw, H, W) bytes, 256-byte aligned; 0 for
+ * arguments the entry rejects.  The call does not synchronise and launches the same kernels whatever batch and
+ * n_cand. */
+size_t evk_depth_grid_timestamp_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W);
+int evk_depth_grid_timestamp_candidates_f32(const float *x, const float *y, const float *t_rel, const float *tau,
+                                            const float *p, const int64_t *offsets, int batch, int64_t n_events,
+                                            const double *motion, double cx, double cy, const float *cand,
+                                            int n_cand, int gh, int gw, int H, int W, double blur_sigma,
+                                            double *f_out, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---------------------------------------------------------------------------------------------
  * RobustNorm (row f4): clamp a tensor between two of its order statistics and rescale it.  Replaces
  * RobustNorm.__call__ / .percentile, lib/data_loaders/data_augmentation.py:82-130 (two kthvalue sorts),
