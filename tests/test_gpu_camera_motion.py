@@ -4,6 +4,7 @@ images, the parameter gradient and the C-level focal-length gradient, the identi
 and rho = 0, events that are not kept, chunked windows, host syncs and launch counts, and the fits' recovery of the
 angular and linear velocity of a camera moving through a scene with depth, from an embedded camera_rotation_warp fit."""
 import ctypes
+import functools
 
 import numpy as np
 import pytest
@@ -11,6 +12,7 @@ import torch
 
 import camera_motion_reference as R
 import camera_rotation_reference as CR
+import candidate_checks as C
 from conftest import assert_close_to_max
 
 pytestmark = pytest.mark.gpu
@@ -380,6 +382,141 @@ def test_no_host_round_trips_and_constant_launch_count():
         assert torch.isfinite(prm.grad).all() and prm.grad.shape == (len(sizes), 6)
         counts.append(launches.value)
     assert counts[0] == counts[1] and counts[0] > 0, counts
+
+
+# ---- the candidates passes with distinct candidates (tests/candidate_checks.py) -------------------------------------
+SPREAD = (0.3, 0.3, 0.3, 0.1, 0.1, 0.1)
+# GONE turns every bearing by phi = |w| |d| in [1.25, 2.5] rad about the y axis, past the 59 degree field of view or
+# behind the camera, at |d| >= 0.05.  PARTIAL moves the camera forward: Pz = 1 - 12 rho |d| takes the events of large
+# rho |d| behind the camera and zooms the others out of the canvas, so what it keeps depends on every event's rho.
+GONE_M, PARTIAL_M = (0.0, 25.0, 0.0, 0.0, 0.0, 0.0), (0.0, 0.0, 0.0, 0.0, 0.0, 12.0)
+CAND_SIZES = {1: [12000], 5: [9000, 0, 6000, 12000, 1], 6: [5000, 0, 4000, 7000, 1, 3000]}
+
+
+def cand_warp(intr=INTR):
+    """the reference warp of candidate_stream, NaN for the events that are not kept"""
+    return lambda x, y, d, rho, prm: R.warp(x, y, d, rho, prm[:3], prm[3:6], intr)
+
+
+@functools.lru_cache(maxsize=None)
+def candidate_case(batch):
+    """(B,70,6) distinct candidates with GONE and PARTIAL, and the windows CAND_SIZES[batch] safe under every one; the
+    events' rho spread over [1/8, 1] in every window"""
+    base = np.array([PARAMS[b % 3] for b in range(batch)])
+    cand = C.distinct_sets(base, 70, np.random.default_rng(700 + batch), SPREAD, GONE_M, PARTIAL_M)
+    return cand, C.candidate_stream(batch, CAND_SIZES[batch], cand, cand_warp(), H, W)
+
+
+# three candidates of the sparse stream, on the 180 x 240 camera CAMERA: their v differ, and rho varies per event
+SPARSE = [(1.0, -0.8, 0.6, 1.5, 0.0, 0.5), (0.8, -1.0, 0.7, -1.0, 1.0, 1.5), (1.2, -0.6, 0.5, 2.0, -0.5, -1.0)]
+
+
+@functools.lru_cache(maxsize=None)
+def sparse_case():
+    """window 0: events whose footprints lie 3 px apart under each of SPARSE; window 1: 30000 dense events.  x, y, d, p,
+    rho, offsets."""
+    rng = np.random.default_rng(37)
+    x, y, d, p, rho = C.draw(rng, 40000, 180, 240, (-0.1, 0.0))
+    pick = C.sparse_pick([cand_warp(CAMERA)(x, y, d, rho, q) for q in SPARSE], 180, 240)
+    dense = C.draw(rng, 30000, 180, 240, (-0.1, 0.0))
+    off = np.array([0, pick.size, pick.size + 30000], np.int64)
+    return [np.concatenate((a[pick], b)) for a, b in zip((x, y, d, p, rho), dense)] + [off]
+
+
+def contrast_candidates(ev, rho, off, cand, sigma, name, img_size=(H, W), intr=INTR):
+    from event_utils_b200.contrast_max import motion_contrast_candidates_torch
+    return motion_contrast_candidates_torch(*ev, torch.tensor(cand, device="cuda"), _warp(intr), t0=0.0, objective=name,
+                                            blur_sigma=sigma, obj_param=0.3, img_size=img_size, batch_end_indices=_ends(off),
+                                            inv_depth=rho).cpu().numpy()
+
+
+def contrast_per_candidate(ev, rho, off, cand, sigma, name, img_size=(H, W), intr=INTR):
+    """motion_contrast_objective_torch once per candidate index j: (B,J)"""
+    from event_utils_b200.contrast_max import motion_contrast_objective_torch
+    return np.stack([motion_contrast_objective_torch(*ev, torch.tensor(cand[:, j], device="cuda"), _warp(intr), t0=0.0,
+                                                     objective=name, blur_sigma=sigma, obj_param=0.3, img_size=img_size,
+                                                     batch_end_indices=_ends(off), inv_depth=rho).cpu().numpy()
+                     for j in range(cand.shape[1])], 1)
+
+
+def ts_candidates(ev, rho, off, cand, sigma, reverse):
+    from event_utils_b200.contrast_max import motion_timestamp_candidates_torch
+    return motion_timestamp_candidates_torch(*ev, torch.tensor(cand, device="cuda"), _warp(), t0=0.0, blur_sigma=sigma,
+                                             timestamp_reverse=reverse, img_size=(H, W), batch_end_indices=_ends(off),
+                                             inv_depth=rho).cpu().numpy()
+
+
+def ts_per_candidate(ev, rho, off, cand, sigma, reverse):
+    from event_utils_b200.contrast_max import motion_timestamp_objective_torch
+    return np.stack([motion_timestamp_objective_torch(*ev, torch.tensor(cand[:, j], device="cuda"), _warp(), t0=0.0,
+                                                      blur_sigma=sigma, timestamp_reverse=reverse, img_size=(H, W),
+                                                      batch_end_indices=_ends(off), inv_depth=rho).cpu().numpy()
+                     for j in range(cand.shape[1])], 1)
+
+
+@pytest.mark.parametrize("name", ["variance", "sos", "soe", "sosa"])
+@pytest.mark.parametrize("sigma", [0.0, 1.0, 3.0])
+@pytest.mark.parametrize("batch", [1, 5])
+def test_contrast_candidates_distinct_against_the_forward_and_the_reference(name, sigma, batch):
+    master, (x, y, d, p, rho, off) = candidate_case(batch)
+    ev, r = _cuda(x, y, d, p), torch.from_numpy(rho).cuda()
+
+    def reference(cand):
+        return np.stack([R.contrast(x, y, d, p, rho, off, torch.from_numpy(_rows(cand[:, j])), sigma, name, CENTRE, 0.3, (H, W))[0]
+                         .numpy() for j in range(cand.shape[1])], 1), F_REL
+    C.check_sets(master, lambda c: contrast_candidates(ev, r, off, c, sigma, name),
+                 lambda c: contrast_per_candidate(ev, r, off, c, sigma, name), reference, C.no_event_value(name, H, W),
+                 [1] if batch == 5 else [], "%s %g" % (name, sigma))
+
+
+@pytest.mark.parametrize("sigma", [0.0, 1.0, 2.0, 3.0])
+@pytest.mark.parametrize("reverse", [False, True])
+@pytest.mark.parametrize("batch", [1, 5])
+def test_timestamp_candidates_distinct_against_the_forward_and_the_reference(sigma, reverse, batch):
+    """the stamps are d (t0 = 0 lies 0.05 or more after every window's last stamp); a lone event has tau = 0"""
+    master, (x, y, d, p, rho, off) = candidate_case(batch)
+    ev, r = _cuda(x, y, d, p), torch.from_numpy(rho).cuda()
+    tau = R.tau_f32(d, off, reverse)
+
+    def reference(cand):
+        return np.stack([R.timestamp(x, y, d, tau, p, rho, off, torch.from_numpy(_rows(cand[:, j])), sigma, CENTRE, (H, W))[0]
+                         .numpy() for j in range(cand.shape[1])], 1), F_REL
+    C.check_sets(master, lambda c: ts_candidates(ev, r, off, c, sigma, reverse),
+                 lambda c: ts_per_candidate(ev, r, off, c, sigma, reverse), reference, C.no_event_value(None, H, W),
+                 [1, 4] if batch == 5 else [], "%g %s" % (sigma, reverse))
+
+
+def test_candidates_of_sparse_footprints_bit_for_bit():
+    """at most one tap per pixel under each candidate: the images equal the forward's bit for bit, so f agrees to the
+    f64 rounding of the statistics' reduction order (a dense second window to f32 summation order)"""
+    x, y, d, p, rho, off = sparse_case()
+    assert off[1] > 500, off
+    ev, r = _cuda(x, y, d, p), torch.from_numpy(rho).cuda()
+    cand = np.array([SPARSE] * 2, np.float64)
+    for name, sigma in (("variance", 0.0), ("soe", 1.0)):
+        kw = dict(img_size=(180, 240), intr=CAMERA)
+        f = contrast_candidates(ev, r, off, cand, sigma, name, **kw)
+        ref = contrast_per_candidate(ev, r, off, cand, sigma, name, **kw)
+        np.testing.assert_allclose(f[0], ref[0], rtol=1e-12, atol=0, err_msg=name)
+        np.testing.assert_allclose(f[1], ref[1], rtol=1e-6, atol=0, err_msg=name)
+
+
+def test_window_chunks_with_distinct_candidates(monkeypatch):
+    """six skewed windows x 70 distinct candidates in chunks of two windows (three J passes each), rho read through
+    each chunk's offsets: every entry equals the one-chunk run and the per-candidate forward"""
+    from event_utils_b200 import _lib
+    from event_utils_b200.contrast_max import motion_objective as MO
+    from event_utils_b200.contrast_max import motion_timestamp_objective as MT
+    L = _lib.lib()
+    cand, (x, y, d, p, rho, off) = candidate_case(6)
+    ev, r = _cuda(x, y, d, p), torch.from_numpy(rho).cuda()
+    budgets = [(MO, "CANDIDATES_WORKSPACE_BYTES", 2 * L.evk_cmax_motion_depth_candidates_workspace_bytes(1, 32, H, W) + 1),
+               (MT, "TIMESTAMP_CANDIDATES_WORKSPACE_BYTES",
+                2 * L.evk_motion_timestamp_depth_candidates_workspace_bytes(1, 32, H, W) + 1)]
+    C.check_chunks(monkeypatch, budgets, lambda c: contrast_candidates(ev, r, off, c, 1.0, "variance"),
+                   lambda c: contrast_per_candidate(ev, r, off, c, 1.0, "variance"), cand, "contrast")
+    C.check_chunks(monkeypatch, budgets, lambda c: ts_candidates(ev, r, off, c, 1.0, False),
+                   lambda c: ts_per_candidate(ev, r, off, c, 1.0, False), cand, "timestamp")
 
 
 # ---- recovery on a scene with depth -----------------------------------------------------------------------------

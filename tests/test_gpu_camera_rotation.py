@@ -3,12 +3,14 @@ and timestamp losses, their candidates passes, motion segmentation and its assig
 tests/camera_rotation_reference.py, the focal-length gradient columns of the C entries, events behind the camera, host
 syncs and launch counts, and the fits' recovery of the angular velocity of a rotating camera from a grid search."""
 import ctypes
+import functools
 
 import numpy as np
 import pytest
 import torch
 
 import camera_rotation_reference as R
+import candidate_checks as C
 from conftest import assert_close_to_max
 
 pytestmark = pytest.mark.gpu
@@ -317,6 +319,170 @@ def test_no_host_round_trips_and_constant_launch_count():
         assert torch.isfinite(prm.grad).all() and prm.grad.shape == (len(sizes), 3)
         counts.append(launches.value)
     assert counts[0] == counts[1] and counts[0] > 0, counts
+
+
+# ---- the candidates passes with distinct candidates (tests/candidate_checks.py) -------------------------------------
+SPREAD = (0.3, 0.3, 0.3)
+# GONE turns every bearing by phi = |w| |d| in [1.25, 2.5] rad about the y axis, past the 59 degree field of view or
+# behind the camera, at |d| >= 0.05; PARTIAL by 0.3-0.6 rad, which takes part of the events off the canvas
+GONE_W, PARTIAL_W = (0.0, 25.0, 0.0), (0.0, 6.0, 0.0)
+CAND_SIZES = {1: [12000], 5: [9000, 0, 6000, 12000, 1], 6: [5000, 0, 4000, 7000, 1, 3000]}
+
+
+def cand_warp(intr=INTR):
+    """the reference warp of candidate_stream, NaN behind the camera"""
+    return lambda x, y, d, rho, prm: R.warp(x, y, d, prm[:3], intr)
+
+
+def _base(n, scale=0.0):
+    return np.array([np.array(PARAMS[b % 3]) * (1 + scale * b) for b in range(n)])
+
+
+@functools.lru_cache(maxsize=None)
+def candidate_case(batch):
+    """(B,70,3) distinct candidates with GONE and PARTIAL, and the windows CAND_SIZES[batch] safe under every one"""
+    cand = C.distinct_sets(_base(batch), 70, np.random.default_rng(500 + batch), SPREAD, GONE_W, PARTIAL_W)
+    return cand, C.candidate_stream(batch, CAND_SIZES[batch], cand, cand_warp(), H, W)
+
+
+@functools.lru_cache(maxsize=None)
+def segmentation_case(M):
+    """(6,M,37,3) candidates distinct across the models and the candidates of a window, and windows safe under all"""
+    base = np.stack([_base(6, 0.1) * (1 + 0.1 * m) for m in range(M)], 1)
+    cand = C.distinct_sets(base.reshape(6 * M, 3), 37, np.random.default_rng(600 + M), SPREAD).reshape(6, M, 37, 3)
+    return cand, C.candidate_stream(M, CAND_SIZES[6], cand, cand_warp(), H, W)
+
+
+# three candidates of the sparse stream, on the 180 x 240 camera CAMERA
+SPARSE = [(1.3, -1.1, 1.2), (1.0, -1.4, 0.9), (1.6, -0.8, 1.5)]
+
+
+@functools.lru_cache(maxsize=None)
+def sparse_case():
+    """window 0: events whose footprints lie 3 px apart under each of SPARSE; window 1: 30000 dense events"""
+    rng = np.random.default_rng(37)
+    x, y, d, p, rho = C.draw(rng, 40000, 180, 240, (-0.1, 0.0))
+    pick = C.sparse_pick([cand_warp(CAMERA)(x, y, d, rho, q) for q in SPARSE], 180, 240)
+    dense = C.draw(rng, 30000, 180, 240, (-0.1, 0.0))
+    off = np.array([0, pick.size, pick.size + 30000], np.int64)
+    return [np.concatenate((a[pick], b)) for a, b in zip((x, y, d, p), dense)] + [off]
+
+
+def contrast_candidates(ev, off, cand, sigma, name, img_size=(H, W), intr=INTR):
+    from event_utils_b200.contrast_max import motion_contrast_candidates_torch
+    return motion_contrast_candidates_torch(*ev, torch.tensor(cand, device="cuda"), _warp(intr), t0=0.0, objective=name,
+                                            blur_sigma=sigma, obj_param=0.3, img_size=img_size,
+                                            batch_end_indices=_ends(off)).cpu().numpy()
+
+
+def contrast_per_candidate(ev, off, cand, sigma, name, img_size=(H, W), intr=INTR):
+    """motion_contrast_objective_torch once per candidate index j: (B,J)"""
+    from event_utils_b200.contrast_max import motion_contrast_objective_torch
+    return np.stack([motion_contrast_objective_torch(*ev, torch.tensor(cand[:, j], device="cuda"), _warp(intr), t0=0.0,
+                                                     objective=name, blur_sigma=sigma, obj_param=0.3, img_size=img_size,
+                                                     batch_end_indices=_ends(off)).cpu().numpy()
+                     for j in range(cand.shape[1])], 1)
+
+
+def ts_candidates(ev, off, cand, sigma, reverse):
+    from event_utils_b200.contrast_max import motion_timestamp_candidates_torch
+    return motion_timestamp_candidates_torch(*ev, torch.tensor(cand, device="cuda"), _warp(), t0=0.0, blur_sigma=sigma,
+                                             timestamp_reverse=reverse, img_size=(H, W),
+                                             batch_end_indices=_ends(off)).cpu().numpy()
+
+
+def ts_per_candidate(ev, off, cand, sigma, reverse):
+    from event_utils_b200.contrast_max import motion_timestamp_objective_torch
+    return np.stack([motion_timestamp_objective_torch(*ev, torch.tensor(cand[:, j], device="cuda"), _warp(), t0=0.0,
+                                                      blur_sigma=sigma, timestamp_reverse=reverse, img_size=(H, W),
+                                                      batch_end_indices=_ends(off)).cpu().numpy()
+                     for j in range(cand.shape[1])], 1)
+
+
+@pytest.mark.parametrize("name", ["variance", "sos", "soe", "sosa"])
+@pytest.mark.parametrize("sigma", [0.0, 1.0, 3.0])
+@pytest.mark.parametrize("batch", [1, 5])
+def test_contrast_candidates_distinct_against_the_forward_and_the_reference(name, sigma, batch):
+    master, (x, y, d, p, _, off) = candidate_case(batch)
+    ev = _cuda(x, y, d, p)
+
+    def reference(cand):
+        return np.stack([R.contrast(x, y, d, p, off, torch.from_numpy(_rows(cand[:, j])), sigma, name, CENTRE, 0.3, (H, W))[0]
+                         .numpy() for j in range(cand.shape[1])], 1), F_REL
+    C.check_sets(master, lambda c: contrast_candidates(ev, off, c, sigma, name),
+                 lambda c: contrast_per_candidate(ev, off, c, sigma, name), reference, C.no_event_value(name, H, W),
+                 [1] if batch == 5 else [], "%s %g" % (name, sigma))
+
+
+@pytest.mark.parametrize("sigma", [0.0, 1.0, 2.0, 3.0])
+@pytest.mark.parametrize("reverse", [False, True])
+@pytest.mark.parametrize("batch", [1, 5])
+def test_timestamp_candidates_distinct_against_the_forward_and_the_reference(sigma, reverse, batch):
+    """the stamps are d (t0 = 0 lies 0.05 or more after every window's last stamp); a lone event has tau = 0"""
+    master, (x, y, d, p, _, off) = candidate_case(batch)
+    ev = _cuda(x, y, d, p)
+    tau = R.tau_f32(d, off, reverse)
+
+    def reference(cand):
+        return np.stack([R.timestamp(x, y, d, tau, p, off, torch.from_numpy(_rows(cand[:, j])), sigma, CENTRE, (H, W))[0].numpy()
+                         for j in range(cand.shape[1])], 1), F_REL
+    C.check_sets(master, lambda c: ts_candidates(ev, off, c, sigma, reverse),
+                 lambda c: ts_per_candidate(ev, off, c, sigma, reverse), reference, C.no_event_value(None, H, W),
+                 [1, 4] if batch == 5 else [], "%g %s" % (sigma, reverse))
+
+
+@pytest.mark.parametrize("M", [2, 3, 4])
+def test_segmentation_candidates_distinct_per_model_and_candidate(M, monkeypatch):
+    from event_utils_b200 import _lib
+    from event_utils_b200.contrast_max import motion_segmentation as MS
+    from event_utils_b200.contrast_max import motion_segmentation_candidates_torch
+    cand, (x, y, d, p, _, off) = segmentation_case(M)
+    w = _memberships(x.shape[0], M, 40 + M)
+    ev, wt = _cuda(x, y, d, p), torch.from_numpy(w).cuda()
+
+    def run():
+        return motion_segmentation_candidates_torch(*ev, torch.tensor(cand, device="cuda"), wt, _warp(), t0=0.0, blur_sigma=1.0,
+                                                    img_size=(H, W), batch_end_indices=_ends(off)).cpu().numpy()
+
+    def reference(c):
+        fr, _ = R.segmentation(x, y, d, p, torch.from_numpy(w.astype(np.float64)), off, torch.from_numpy(_rows(c)), 1.0,
+                               "variance", CENTRE, img_size=(H, W))
+        return fr.numpy(), F_REL
+    per = _lib.lib().evk_cmax_motion_segment_candidates_workspace_bytes(1, M, 32 // M, H, W)
+    C.check_segmentation(run(), lambda c: seg_forward(x, y, d, p, w, off, _rows(c))[0][0].numpy(), cand, reference, monkeypatch,
+                         MS, 2 * per + 1, run)
+
+
+def test_candidates_of_sparse_footprints_bit_for_bit():
+    """at most one tap per pixel under each candidate: the images equal the forward's bit for bit, so f agrees to the
+    f64 rounding of the statistics' reduction order (a dense second window to f32 summation order)"""
+    x, y, d, p, off = sparse_case()
+    assert off[1] > 500, off
+    ev = _cuda(x, y, d, p)
+    cand = np.array([SPARSE] * 2, np.float64)
+    for name, sigma in (("variance", 0.0), ("soe", 1.0)):
+        kw = dict(img_size=(180, 240), intr=CAMERA)
+        f = contrast_candidates(ev, off, cand, sigma, name, **kw)
+        ref = contrast_per_candidate(ev, off, cand, sigma, name, **kw)
+        np.testing.assert_allclose(f[0], ref[0], rtol=1e-12, atol=0, err_msg=name)
+        np.testing.assert_allclose(f[1], ref[1], rtol=1e-6, atol=0, err_msg=name)
+
+
+def test_window_chunks_with_distinct_candidates(monkeypatch):
+    """six skewed windows x 70 distinct candidates in chunks of two windows (three J passes each): every entry equals
+    the one-chunk run and the per-candidate forward"""
+    from event_utils_b200 import _lib
+    from event_utils_b200.contrast_max import motion_objective as MO
+    from event_utils_b200.contrast_max import motion_timestamp_objective as MT
+    L = _lib.lib()
+    cand, (x, y, d, p, _, off) = candidate_case(6)
+    ev = _cuda(x, y, d, p)
+    budgets = [(MO, "CANDIDATES_WORKSPACE_BYTES", 2 * L.evk_cmax_motion_candidates_workspace_bytes(1, 32, H, W) + 1),
+               (MT, "TIMESTAMP_CANDIDATES_WORKSPACE_BYTES", 2 * L.evk_motion_timestamp_candidates_workspace_bytes(1, 32, H, W) + 1)]
+    C.check_chunks(monkeypatch, budgets, lambda c: contrast_candidates(ev, off, c, 1.0, "variance"),
+                   lambda c: contrast_per_candidate(ev, off, c, 1.0, "variance"), cand, "contrast")
+    C.check_chunks(monkeypatch, budgets, lambda c: ts_candidates(ev, off, c, 1.0, False),
+                   lambda c: ts_per_candidate(ev, off, c, 1.0, False), cand, "timestamp")
 
 
 # ---- recovery from a grid search ------------------------------------------------------------------------------------

@@ -3,11 +3,13 @@ their candidates passes, motion segmentation and its assignment, against the f64
 tests/planar_motion_reference.py; the embeddings xyztheta -> affine -> homography bit for bit on the GPU; the horizon;
 and the fits' recovery of planar motions from the documented start."""
 import ctypes
+import functools
 
 import numpy as np
 import pytest
 import torch
 
+import candidate_checks as C
 import planar_motion_reference as P
 from conftest import assert_close_to_max
 
@@ -391,6 +393,185 @@ def test_no_host_round_trips_and_constant_launch_count():
             assert torch.isfinite(prm.grad).all()
             counts.append(launches.value)
         assert counts[0] == counts[1] and counts[0] > 0, counts
+
+
+# ---- the candidates passes with distinct candidates (tests/candidate_checks.py) -------------------------------------
+F_REL = 1e-5        # f against the f64 reference, as above
+SPREAD = {"affine": (1.0, 1.0, 0.1, 0.1, 0.1, 0.1), "homography": (1.0, 1.0, 0.1, 0.1, 0.1, 0.1, 0.002, 0.002)}
+# GONE moves every event 5000 px or more at |d| >= 0.05.  PARTIAL moves the affine's events 20-40 px to the right, and
+# puts the homography's events left of u = -1 / (g1 |d|) (33 px left of the centre at |d| = 0.1) past its horizon and
+# those near it off the canvas.  A larger g1 heaps the events right of the centre onto the few pixels about the
+# vanishing point, where soe at blur 0 turns the f32 rounding of their positions into more than F_REL of f.
+GONE_PRM = {"affine": (1e5, -1e5, 0.0, 0.0, 0.0, 0.0), "homography": (1e5, -1e5, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0)}
+PARTIAL_PRM = {"affine": (400.0, 0.0, 0.0, 0.0, 0.0, 0.0), "homography": (5.0, -3.0, 0.5, 0.2, -0.1, 0.3, 0.3, 0.0)}
+CAND_SIZES = {1: [12000], 5: [9000, 0, 6000, 12000, 1], 6: [5000, 0, 4000, 7000, 1, 3000]}
+
+
+def cand_warp(kind, centre=CENTRE):
+    """the reference warp of candidate_stream: the kernel's f32 warp, NaN past the horizon"""
+    return lambda x, y, d, rho, prm: P.warp_f32(kind, x, y, d, prm, centre)
+
+
+def _base(kind, n, scale=0.0):
+    return np.array([np.array(PARAMS[kind][b % 3]) * (1 + scale * b) for b in range(n)])
+
+
+@functools.lru_cache(maxsize=None)
+def candidate_case(kind, batch):
+    """(B,70,K) distinct candidates with GONE and PARTIAL, and the windows CAND_SIZES[batch] safe under every one"""
+    rng = np.random.default_rng({"affine": 100, "homography": 200}[kind] + batch)
+    cand = C.distinct_sets(_base(kind, batch), 70, rng, SPREAD[kind], GONE_PRM[kind], PARTIAL_PRM[kind])
+    return cand, C.candidate_stream(batch, CAND_SIZES[batch], cand, cand_warp(kind), H, W)
+
+
+@functools.lru_cache(maxsize=None)
+def segmentation_case(kind, M):
+    """(6,M,37,K) candidates distinct across the models and the candidates of a window, and windows safe under all"""
+    rng = np.random.default_rng({"affine": 300, "homography": 400}[kind] + M)
+    base = np.stack([_base(kind, 6, 0.1) * (1 + 0.1 * m) for m in range(M)], 1)
+    cand = C.distinct_sets(base.reshape(6 * M, -1), 37, rng, SPREAD[kind]).reshape(6, M, 37, -1)
+    return cand, C.candidate_stream(M, CAND_SIZES[6], cand, cand_warp(kind), H, W)
+
+
+# three candidates of the sparse streams (180 x 240 about (120, 90)): every component differs, the homography's
+# perspective terms too
+SPARSE = {"affine": [(30.0, -20.0, 3.0, -2.0, 1.5, -4.0), (25.0, -18.0, 2.5, -1.5, 2.0, -3.0), (33.0, -24.0, 3.5, -2.5, 1.0, -5.0)],
+          "homography": [(30.0, -20.0, 3.0, -2.0, 1.5, -4.0, 0.004, -0.003), (25.0, -18.0, 2.5, -1.5, 2.0, -3.0, -0.003, 0.005),
+                         (33.0, -24.0, 3.5, -2.5, 1.0, -5.0, 0.006, 0.002)]}
+
+
+@functools.lru_cache(maxsize=None)
+def sparse_case(kind):
+    """window 0: events whose footprints lie 3 px apart under each of SPARSE[kind] (180 x 240); window 1: 30000 dense
+    events.  x, y, d, p, offsets."""
+    rng = np.random.default_rng({"affine": 37, "homography": 38}[kind])
+    x, y, d, p, rho = C.draw(rng, 40000, 180, 240, (-0.1, 0.0))
+    pick = C.sparse_pick([cand_warp(kind, (120.0, 90.0))(x, y, d, rho, q) for q in SPARSE[kind]], 180, 240)
+    dense = C.draw(rng, 30000, 180, 240, (-0.1, 0.0))
+    off = np.array([0, pick.size, pick.size + 30000], np.int64)
+    return [np.concatenate((a[pick], b)) for a, b in zip((x, y, d, p), dense)] + [off]
+
+
+def contrast_candidates(kind, ev, off, cand, sigma, name, img_size=(H, W), centre=CENTRE):
+    from event_utils_b200.contrast_max import motion_contrast_candidates_torch
+    return motion_contrast_candidates_torch(*ev, torch.tensor(cand, device="cuda"), _warp(kind, centre), t0=0.0, objective=name,
+                                            blur_sigma=sigma, obj_param=0.3, img_size=img_size,
+                                            batch_end_indices=_ends(off)).cpu().numpy()
+
+
+def contrast_per_candidate(kind, ev, off, cand, sigma, name, img_size=(H, W), centre=CENTRE):
+    """motion_contrast_objective_torch once per candidate index j: (B,J)"""
+    from event_utils_b200.contrast_max import motion_contrast_objective_torch
+    return np.stack([motion_contrast_objective_torch(*ev, torch.tensor(cand[:, j], device="cuda"), _warp(kind, centre), t0=0.0,
+                                                     objective=name, blur_sigma=sigma, obj_param=0.3, img_size=img_size,
+                                                     batch_end_indices=_ends(off)).cpu().numpy()
+                     for j in range(cand.shape[1])], 1)
+
+
+def ts_candidates(kind, ev, off, cand, sigma, reverse):
+    from event_utils_b200.contrast_max import motion_timestamp_candidates_torch
+    return motion_timestamp_candidates_torch(*ev, torch.tensor(cand, device="cuda"), _warp(kind), t0=0.0, blur_sigma=sigma,
+                                             timestamp_reverse=reverse, img_size=(H, W),
+                                             batch_end_indices=_ends(off)).cpu().numpy()
+
+
+def ts_per_candidate(kind, ev, off, cand, sigma, reverse):
+    from event_utils_b200.contrast_max import motion_timestamp_objective_torch
+    return np.stack([motion_timestamp_objective_torch(*ev, torch.tensor(cand[:, j], device="cuda"), _warp(kind), t0=0.0,
+                                                      blur_sigma=sigma, timestamp_reverse=reverse, img_size=(H, W),
+                                                      batch_end_indices=_ends(off)).cpu().numpy()
+                     for j in range(cand.shape[1])], 1)
+
+
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+@pytest.mark.parametrize("name", ["variance", "sos", "soe", "sosa"])
+@pytest.mark.parametrize("sigma", [0.0, 1.0, 3.0])
+@pytest.mark.parametrize("batch", [1, 5])
+def test_contrast_candidates_distinct_against_the_forward_and_the_reference(kind, name, sigma, batch):
+    master, (x, y, d, p, _, off) = candidate_case(kind, batch)
+    ev = _cuda(x, y, d, p)
+
+    def reference(cand):
+        return np.stack([P.contrast(kind, x, y, d, p, off, torch.tensor(cand[:, j]), sigma, name, 0.3, (H, W), CENTRE)[0].numpy()
+                         for j in range(cand.shape[1])], 1), F_REL
+    C.check_sets(master, lambda c: contrast_candidates(kind, ev, off, c, sigma, name),
+                 lambda c: contrast_per_candidate(kind, ev, off, c, sigma, name), reference, C.no_event_value(name, H, W),
+                 [1] if batch == 5 else [], "%s %s %g" % (kind, name, sigma))
+
+
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+@pytest.mark.parametrize("sigma", [0.0, 1.0, 2.0, 3.0])
+@pytest.mark.parametrize("reverse", [False, True])
+@pytest.mark.parametrize("batch", [1, 5])
+def test_timestamp_candidates_distinct_against_the_forward_and_the_reference(kind, sigma, reverse, batch):
+    """the stamps are d (t0 = 0 lies 0.05 or more after every window's last stamp); a lone event has tau = 0"""
+    master, (x, y, d, p, _, off) = candidate_case(kind, batch)
+    ev = _cuda(x, y, d, p)
+    tau = P.tau_f32(d, off, reverse)
+
+    def reference(cand):
+        return np.stack([P.timestamp(kind, x, y, d, tau, p, off, torch.tensor(cand[:, j]), sigma, (H, W), CENTRE)[0].numpy()
+                         for j in range(cand.shape[1])], 1), F_REL
+    C.check_sets(master, lambda c: ts_candidates(kind, ev, off, c, sigma, reverse),
+                 lambda c: ts_per_candidate(kind, ev, off, c, sigma, reverse), reference, C.no_event_value(None, H, W),
+                 [1, 4] if batch == 5 else [], "%s %g %s" % (kind, sigma, reverse))
+
+
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+@pytest.mark.parametrize("M", [2, 3, 4])
+def test_segmentation_candidates_distinct_per_model_and_candidate(kind, M, monkeypatch):
+    from event_utils_b200 import _lib
+    from event_utils_b200.contrast_max import motion_segmentation as MS
+    from event_utils_b200.contrast_max import motion_segmentation_candidates_torch
+    cand, (x, y, d, p, _, off) = segmentation_case(kind, M)
+    w = _memberships(x.shape[0], M, 40 + M)
+    ev, wt = _cuda(x, y, d, p), torch.from_numpy(w).cuda()
+
+    def run():
+        return motion_segmentation_candidates_torch(*ev, torch.tensor(cand, device="cuda"), wt, _warp(kind), t0=0.0, blur_sigma=1.0,
+                                                    img_size=(H, W), batch_end_indices=_ends(off)).cpu().numpy()
+
+    def reference(c):
+        fr, _ = P.segmentation(kind, x, y, d, p, torch.from_numpy(w.astype(np.float64)), off, torch.tensor(c), 1.0, "variance",
+                               img_size=(H, W), centre=CENTRE)
+        return fr.numpy(), F_REL
+    per = _lib.lib().evk_cmax_motion_segment_candidates_workspace_bytes(1, M, 32 // M, H, W)
+    C.check_segmentation(run(), lambda c: seg_forward(kind, x, y, d, p, w, off, c)[0].numpy(), cand, reference, monkeypatch,
+                         MS, 2 * per + 1, run)
+
+
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+def test_candidates_of_sparse_footprints_bit_for_bit(kind):
+    """at most one tap per pixel under each candidate: the images equal the forward's bit for bit, so f agrees to the
+    f64 rounding of the statistics' reduction order (a dense second window to f32 summation order)"""
+    x, y, d, p, off = sparse_case(kind)
+    assert off[1] > 500, off
+    ev = _cuda(x, y, d, p)
+    cand = np.array([SPARSE[kind]] * 2, np.float64)
+    for name, sigma in (("variance", 0.0), ("soe", 1.0)):
+        kw = dict(img_size=(180, 240), centre=(120.0, 90.0))
+        f = contrast_candidates(kind, ev, off, cand, sigma, name, **kw)
+        ref = contrast_per_candidate(kind, ev, off, cand, sigma, name, **kw)
+        np.testing.assert_allclose(f[0], ref[0], rtol=1e-12, atol=0, err_msg="%s %s" % (kind, name))
+        np.testing.assert_allclose(f[1], ref[1], rtol=1e-6, atol=0, err_msg="%s %s" % (kind, name))
+
+
+@pytest.mark.parametrize("kind", ["affine", "homography"])
+def test_window_chunks_with_distinct_candidates(kind, monkeypatch):
+    """six skewed windows x 70 distinct candidates in chunks of two windows (three J passes each): every entry equals
+    the one-chunk run and the per-candidate forward"""
+    from event_utils_b200 import _lib
+    from event_utils_b200.contrast_max import motion_objective as MO
+    from event_utils_b200.contrast_max import motion_timestamp_objective as MT
+    L = _lib.lib()
+    cand, (x, y, d, p, _, off) = candidate_case(kind, 6)
+    ev = _cuda(x, y, d, p)
+    budgets = [(MO, "CANDIDATES_WORKSPACE_BYTES", 2 * L.evk_cmax_motion_candidates_workspace_bytes(1, 32, H, W) + 1),
+               (MT, "TIMESTAMP_CANDIDATES_WORKSPACE_BYTES", 2 * L.evk_motion_timestamp_candidates_workspace_bytes(1, 32, H, W) + 1)]
+    C.check_chunks(monkeypatch, budgets, lambda c: contrast_candidates(kind, ev, off, c, 1.0, "variance"),
+                   lambda c: contrast_per_candidate(kind, ev, off, c, 1.0, "variance"), cand, kind + " contrast")
+    C.check_chunks(monkeypatch, budgets, lambda c: ts_candidates(kind, ev, off, c, 1.0, False),
+                   lambda c: ts_per_candidate(kind, ev, off, c, 1.0, False), cand, kind + " timestamp")
 
 
 # ---- recovery from the documented start -----------------------------------------------------------------------------
