@@ -82,7 +82,7 @@ def random_stream(B, giant_at=None, seed=0):
                 p=(rng.integers(0, 2, n) * 2 - 1).astype(f), off=_offsets(sizes), sizes=sizes)
 
 
-EVENT_KEYS = ("x", "y", "d", "tau", "p", "t", "k")
+EVENT_KEYS = ("x", "y", "d", "tau", "p", "t", "k", "r", "w")
 
 
 def reversed_stream(s):
@@ -99,15 +99,18 @@ def window_ids(off):
     return np.repeat(np.arange(len(off) - 1), np.diff(off))
 
 
-def linvel_taps(s, v):
+def linvel_taps(s, v, flow=False):
     """the bilinear taps of every contributing event under linvel velocity v ((2,) or per window (B,2)), in f64: (window,
-    pixel index y*WC+x of the top-left tap, dx, dy, keep).  Exact for exact_stream under a velocity of EXACT_VELOCITIES"""
+    pixel index y*WC+x of the top-left tap, dx, dy, keep).  Exact for exact_stream under a velocity of EXACT_VELOCITIES.
+    The motion entries keep 0 < x' < W, 0 < y' < H (x' = W has zero weight); with `flow`, the keep rule of the flow and
+    grid-flow entries, 0 <= x' < W, 0 <= y' < H"""
     b = window_ids(s["off"])
     v = np.asarray(v, np.float64)
     vx, vy = (v[b, 0], v[b, 1]) if v.ndim == 2 else (v[0], v[1])
     xw = s["x"].astype(np.float64) - s["d"].astype(np.float64) * vx
     yw = s["y"].astype(np.float64) - s["d"].astype(np.float64) * vy
-    keep = np.isfinite(xw) & np.isfinite(yw) & (xw > 0) & (xw < W) & (yw > 0) & (yw < H)
+    lo = (xw >= 0) & (yw >= 0) if flow else (xw > 0) & (yw > 0)
+    keep = np.isfinite(xw) & np.isfinite(yw) & lo & (xw < W) & (yw < H)
     px, py = np.floor(np.where(keep, xw, 0)), np.floor(np.where(keep, yw, 0))
     return b, (py * WC + px).astype(np.int64), xw - px, yw - py, keep
 
@@ -120,17 +123,19 @@ def _splat(B, b, pix, dx, dy, keep, w):
     return img.reshape(B, HC, WC)
 
 
-def linvel_iwe(s, v):
-    """(B, HC, WC) f64 images of p of the contrast loss under linvel velocity v"""
+def linvel_iwe(s, v, flow=False, weight=None):
+    """(B, HC, WC) f64 images of p of the contrast loss under linvel velocity v (each event's p times `weight`, a
+    segmentation's membership, when given)"""
     B = len(s["sizes"])
-    b, pix, dx, dy, keep = linvel_taps(s, v)
-    return _splat(B, b, pix, dx, dy, keep, s["p"].astype(np.float64))
+    b, pix, dx, dy, keep = linvel_taps(s, v, flow)
+    w = s["p"].astype(np.float64) * (1.0 if weight is None else np.asarray(weight, np.float64))
+    return _splat(B, b, pix, dx, dy, keep, w)
 
 
-def linvel_ts_images(s, v):
+def linvel_ts_images(s, v, flow=False):
     """(S, C) of the timestamp loss, each (B, 2, HC, WC) f64, polarity 0 positive"""
     B = len(s["sizes"])
-    b, pix, dx, dy, keep = linvel_taps(s, v)
+    b, pix, dx, dy, keep = linvel_taps(s, v, flow)
     S, C = np.zeros((B, 2, HC, WC)), np.ones((B, 2, HC, WC))
     for i, sel in enumerate((s["p"] > 0, s["p"] <= 0)):
         S[:, i] = _splat(B, b, pix, dx, dy, keep & sel, s["tau"].astype(np.float64))
@@ -151,23 +156,24 @@ def timestamp_f(S, C):
     return (T * T).sum(axis=(1, 2, 3)), T
 
 
-def tap_magnitudes(s, v):
+def tap_magnitudes(s, v, flow=False):
     """per window and pixel: the sum of |tap| of the contrast image and the sum of |tau tap| of the timestamp images"""
     B = len(s["sizes"])
-    b, pix, dx, dy, keep = linvel_taps(s, v)
+    b, pix, dx, dy, keep = linvel_taps(s, v, flow)
     ones = np.ones(b.shape[0])
     return _splat(B, b, pix, dx, dy, keep, ones), _splat(B, b, pix, dx, dy, keep, np.abs(s["tau"].astype(np.float64)))
 
 
-def assert_exactly_summable(s, velocities):
+def assert_exactly_summable(s, velocities, flow=False):
     """Every warped coordinate on the quarter grid, so every tap weight on the 1/16 grid (tau taps on the 1/256 grid),
     and per pixel sum |tap| <= 2^20 and sum |tau tap| <= 2^16: every partial sum of every image, in any order, is then
-    an f32 value, and so is C = 1 + sum |tap|"""
+    an f32 value, and so is C = 1 + sum |tap|.  A segmentation's memberships on the 1/4 grid keep every tap on the
+    1/64 grid and every sum below 2^20."""
     for v in velocities:
-        _, _, dx, dy, keep = linvel_taps(s, v)
+        _, _, dx, dy, keep = linvel_taps(s, v, flow)
         for a in (dx[keep], dy[keep]):
             assert (a * 4 == np.round(a * 4)).all(), v
-        mag, tmag = tap_magnitudes(s, v)
+        mag, tmag = tap_magnitudes(s, v, flow)
         assert mag.max() <= 2.0 ** 20 and tmag.max() <= 2.0 ** 16, (v, mag.max(), tmag.max())
         assert ((s["tau"].astype(np.float64) * 16) == np.round(s["tau"].astype(np.float64) * 16)).all()
 
@@ -180,6 +186,184 @@ def window_chunk(B, J, cap, per_window_bytes, budget):
 
 def chunk_sizes(B, wb):
     return [min(wb, B - b0) for b0 in range(0, B, wb)]
+
+
+def sampled_windows(sizes, giant, tail_images_per_window, seed=0, count=40):
+    """0, 1, B-2, B-1, the giant and its neighbours, the nearest empty and one-event windows on either side of it, the
+    windows whose tail index z crosses 2^15 and the last one, then seeded random windows up to `count`"""
+    B = len(sizes)
+    pick = {0, 1, B - 2, B - 1, giant, giant - 1, giant + 1}
+    for want in (0, 1):
+        below = np.flatnonzero(sizes[:giant] == want)
+        above = np.flatnonzero(sizes[giant + 1:] == want)
+        if below.size:
+            pick.add(int(below[-1]))
+        if above.size:
+            pick.add(int(giant + 1 + above[0]))
+    for z in ((1 << 15) - 1, 1 << 15, 65534):
+        pick.add(z // tail_images_per_window)
+    pick = {b for b in pick if 0 <= b < B}
+    rng = np.random.default_rng(seed)
+    while len(pick) < count:
+        pick.add(int(rng.integers(0, B)))
+    return np.array(sorted(pick))
+
+
+# ---- the newer families: affine, homography, camera rotation, camera motion, grid flow, depth grid, segmentation ----
+FAMILIES = ("affine", "homography", "camera_rotation", "camera_motion", "grid_flow", "depth_grid", "segmentation")
+# every family but the camera rotation, which has no translation, reproduces the linvel warp exactly (exact_rows)
+EXACT_FAMILIES = ("affine", "homography", "camera_motion", "grid_flow", "depth_grid", "segmentation")
+FOCAL = 8.0                          # a power of two: (x - cx) / fx and fx X are exact
+INTR = (FOCAL, FOCAL, 4.5, 2.5)      # fx, fy and a dyadic principal point
+EXACT_RHOS = np.array([0.5, 1.0, 2.0])
+# the depth grid's candidate nodes under motion rows built for rho 1 (exact_rows("camera_motion", vel, 1)): node rho r
+# moves the events at r vel, a multiple of 16 for r in {1, 2}
+DEPTH_CANDIDATE_RHOS = np.array([1.0, 2.0])
+RANDOM_GRID = (3, 4)                 # the random variant's node grid: rx = 9/3 and ry = 5/2 are not dyadic
+K = {"affine": 6, "homography": 8, "camera_rotation": 5, "camera_motion": 8, "segmentation": 6}
+
+
+def _sensor_events(rng, n):
+    x = rng.integers(0, 4 * (W - 1) + 1, n) / 4.0
+    y = rng.integers(0, 4 * (H - 1) + 1, n) / 4.0
+    d = -rng.integers(0, 5, n) / 64.0
+    return x, y, d, rng.choice(np.array([-1.0, 1.0]), n), rng.integers(0, 17, n) / 16.0
+
+
+def sensor_stream(B, giant_at=None, seed=0, M=None):
+    """exact_stream for the newer families: every event on the quarter grid inside [0, W-1] x [0, H-1], where the grid
+    families interpolate their nodes (a node tap outside the grid is zero), d on the 2^-6 grid in [-1/16, 0], so that
+    under EXACT_VELOCITIES x' = x - d vx moves by at most 4 px and stays on the quarter grid; tau on the 1/16 grid and
+    p = +-1.  The giant window's events come from their own seed, so the giant is the same window wherever it sits.
+    Also `r`, each event's inverse depth: its window's rho of window_rhos(B, seed), and with M, `w`, memberships (n, M)
+    on the 1/4 grid in [1/4, 1]."""
+    sizes = window_sizes(B, giant_at, seed)
+    off = _offsets(sizes)
+    n = int(off[-1])
+    x, y, d, p, tau = _sensor_events(np.random.default_rng(seed + 1), n)
+    if giant_at is not None:
+        sl = slice(off[giant_at], off[giant_at + 1])
+        for a, v in zip((x, y, d, p, tau), _sensor_events(np.random.default_rng(seed + 2), GIANT)):
+            a[sl] = v
+    f = np.float32
+    s = dict(x=x.astype(f), y=y.astype(f), d=d.astype(f), tau=tau.astype(f), p=p.astype(f), off=off, sizes=sizes)
+    s["r"] = window_rhos(B, seed)[window_ids(off)].astype(f)
+    if M is not None:
+        s["w"] = (np.random.default_rng(seed + 3).integers(1, 5, (n, M)) / 4.0).astype(f)
+    return s
+
+
+def window_rhos(B, seed):
+    """a constant inverse depth per window, of EXACT_RHOS"""
+    return EXACT_RHOS[np.random.default_rng(seed + 4).integers(0, len(EXACT_RHOS), B)]
+
+
+def exact_rows(family, vel, rho=None):
+    """The family's parameters that reproduce the linvel warp at velocity vel ((B,2); the segmentation's (B,M,2)) bit
+    for bit (tests/test_batch_limits_models_cpu.py proves it with the kernels' f32 restatements):
+      affine, homography, segmentation (affine models): (hx, hy) = (vx, vy), every other term 0;
+      camera_motion: w = 0, vz = 0, (vx, vy) = -vel / (FOCAL rho) for the window's rho, rows with (fx, fy);
+      grid_flow: a uniform full-resolution grid (B,2,H,W) f32 of u = -vx, v = -vy;
+      depth_grid: (motion rows (B,8) of camera_motion, a uniform full-resolution grid (B,H,W) f32 of rho)."""
+    vel = np.asarray(vel, np.float64)
+    if family in ("affine", "homography", "segmentation"):
+        rows = np.zeros(vel.shape[:-1] + (K[family],))
+        rows[..., :2] = vel
+        return rows
+    if family == "grid_flow":
+        return np.broadcast_to(-vel[:, :, None, None], (vel.shape[0], 2, H, W)).astype(np.float32)
+    rows = np.zeros((vel.shape[0], 8))
+    rows[:, 3:5] = -vel / (FOCAL * np.asarray(rho, np.float64)[:, None])
+    rows[:, 6:] = FOCAL
+    if family == "camera_motion":
+        return rows
+    return rows, np.broadcast_to(np.asarray(rho, np.float64)[:, None, None], (vel.shape[0], H, W)).astype(np.float32)
+
+
+def exact_velocity_set(shape, seed):
+    """a velocity of EXACT_VELOCITIES per entry of `shape` (windows, models, candidates)"""
+    vel = exact_velocities()
+    return vel[np.random.default_rng(seed).integers(0, len(vel), shape)]
+
+
+def random_stream_models(B, giant_at=None, seed=0, M=None):
+    """random_stream with every event's inverse depth `r` in [1/8, 1] and, with M, random memberships `w` (n, M)"""
+    s = random_stream(B, giant_at, seed)
+    rng = np.random.default_rng(seed + 5)
+    n = int(s["off"][-1])
+    s["r"] = rng.uniform(0.125, 1.0, n).astype(np.float32)
+    if M is not None:
+        s["w"] = rng.random((n, M)).astype(np.float32)
+    return s
+
+
+def random_rows(family, B, seed, M=None):
+    """The random variant's parameters, every term in play: a non-zero perspective, a non-zero w and vz, non-uniform
+    node grids (RANDOM_GRID).  About a pixel of motion at |d| <= 0.1 on the 6x10 sensor.  grid_flow: (B,2,3,4) f32;
+    depth_grid: (motion rows (B,8), nodes (B,3,4) f32 in [1/8, 1]); segmentation: (B,M,6) affine rows."""
+    rng = np.random.default_rng(seed)
+    gh, gw = RANDOM_GRID
+    if family == "grid_flow":
+        return rng.uniform(-20, 20, (B, 2, gh, gw)).astype(np.float32)
+    shape = (B,) if M is None else (B, M)
+    if family in ("affine", "homography", "segmentation"):
+        a = [rng.uniform(-20, 20, shape + (2,)), rng.uniform(-3, 3, shape + (4,))]
+        if family == "homography":
+            a.append(rng.uniform(-0.3, 0.3, shape + (2,)))
+        return np.concatenate(a, axis=-1)
+    w = rng.uniform(-3, 3, (B, 3))
+    if family == "camera_rotation":
+        return np.column_stack((w, np.full((B, 2), FOCAL)))
+    rows = np.column_stack((w, rng.uniform(-2, 2, (B, 3)), np.full((B, 2), FOCAL)))
+    if family == "camera_motion":
+        return rows
+    return rows, rng.uniform(0.125, 1.0, (B, gh, gw)).astype(np.float32)
+
+
+def family_warp(family, x, y, d, r, prm):
+    """(x', y') of the events of one window under the family's parameters prm (the node grid for grid_flow, (motion
+    row, nodes) for depth_grid) in the kernel's f32 order of operations: the warp whose distance from the integers
+    decides whether f32 and f64 may take different taps"""
+    import camera_motion_reference as CM
+    import camera_rotation_reference as CR
+    import depth_grid_reference as DR
+    import grid_flow_reference as GR
+    import planar_motion_reference as P
+    with np.errstate(all="ignore"):
+        if family in ("affine", "homography", "segmentation"):
+            return P.warp_f32("affine" if family == "segmentation" else family, x, y, d, prm, CENTRE)
+        if family == "camera_rotation":
+            return CR.warp(x, y, d, prm[:3], tuple(prm[3:5]) + INTR[2:])
+        if family == "camera_motion":
+            return CM.warp(x, y, d, r, prm[:3], prm[3:6], tuple(prm[6:8]) + INTR[2:])
+        if family == "grid_flow":
+            u, v = GR.event_flow_f32(x, y, prm, H, W)
+            return (x + u * d).astype(np.float32), (y + v * d).astype(np.float32)
+        rows, nodes = prm
+        r32 = DR.event_rho_f32(x, y, nodes, H, W)
+        return CM.warp(x, y, d, r32, rows[:3], rows[3:6], tuple(rows[6:8]) + INTR[2:])
+
+
+def drop_unsafe(s, family, windows, params, drop):
+    """Give the events of `windows` that lie within 1e-3 px of an integer under any of `params` (a function of the
+    window returning a list of the family's parameter sets) the polarity `drop`, which adds no term (0 for the
+    contrast losses, NaN for the timestamp losses), so that f32 and the f64 references take the same taps and keep
+    decisions there.  In place; returns the fraction of events dropped."""
+    off, dropped, total = s["off"], 0, 0
+    for b in windows:
+        lo, hi = int(off[b]), int(off[b + 1])
+        if hi == lo:
+            continue
+        ev = [s[k][lo:hi] for k in ("x", "y", "d")] + [s["r"][lo:hi]]
+        bad = np.zeros(hi - lo, bool)
+        for prm in params(b):
+            xw, yw = family_warp(family, *ev, prm)
+            with np.errstate(invalid="ignore"):
+                bad |= np.isfinite(xw) & np.isfinite(yw) & ((np.abs(xw - np.round(xw)) < 1e-3) |
+                                                            (np.abs(yw - np.round(yw)) < 1e-3))
+        s["p"][lo:hi][bad] = drop
+        dropped, total = dropped + int(bad.sum()), total + hi - lo
+    return dropped / max(total, 1)
 
 
 VOXEL_BINS = 5

@@ -14,6 +14,7 @@ import pytest
 import torch
 
 import batch_limit_streams as S
+from batch_limit_streams import sampled_windows
 import flow_objective_reference as FR
 import flow_timestamp_reference as FTR
 import motion_objective_reference as MR
@@ -178,27 +179,6 @@ def random_params(kind, B, seed):
 
 def incoming(B, seed):
     return np.random.default_rng(seed).standard_normal(B).astype(np.float32)
-
-
-def sampled_windows(sizes, giant, tail_images_per_window, seed=0, count=40):
-    """0, 1, B-2, B-1, the giant and its neighbours, the nearest empty and one-event windows on either side of it, the
-    windows whose tail index z crosses 2^15 and the last one, then seeded random windows up to `count`"""
-    B = len(sizes)
-    pick = {0, 1, B - 2, B - 1, giant, giant - 1, giant + 1}
-    for want in (0, 1):
-        below = np.flatnonzero(sizes[:giant] == want)
-        above = np.flatnonzero(sizes[giant + 1:] == want)
-        if below.size:
-            pick.add(int(below[-1]))
-        if above.size:
-            pick.add(int(giant + 1 + above[0]))
-    for z in ((1 << 15) - 1, 1 << 15, 65534):
-        pick.add(z // tail_images_per_window)
-    pick = {b for b in pick if 0 <= b < B}
-    rng = np.random.default_rng(seed)
-    while len(pick) < count:
-        pick.add(int(rng.integers(0, B)))
-    return np.array(sorted(pick))
 
 
 def _rtol(b, giant):
