@@ -190,6 +190,16 @@ def _declare(L):
     L.evk_cmax_depth_grid_candidates_f32.restype = ci
     L.evk_cmax_depth_grid_candidates_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, vp, f64, f64, vp, ci, ci, ci, ci, ci, f64, ci,
                                                      f64, vp, vp, sz, vp]
+    L.evk_cmax_depth_grid_joint_grad_workspace_bytes.restype = sz
+    L.evk_cmax_depth_grid_joint_grad_workspace_bytes.argtypes = [ci, ci, ci, ci, ci]
+    L.evk_cmax_depth_grid_joint_grad_f32.restype = ci
+    L.evk_cmax_depth_grid_joint_grad_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, vp, f64, f64, vp, ci, ci, ci, ci, f64, ci,
+                                                     f64, vp, vp, vp, vp, vp, sz, vp]
+    L.evk_cmax_depth_grid_joint_candidates_workspace_bytes.restype = sz
+    L.evk_cmax_depth_grid_joint_candidates_workspace_bytes.argtypes = [ci, ci, ci, ci, ci, ci]
+    L.evk_cmax_depth_grid_joint_candidates_f32.restype = ci
+    L.evk_cmax_depth_grid_joint_candidates_f32.argtypes = [vp, vp, vp, vp, vp, ci, i64, vp, f64, f64, vp, ci, ci, ci, ci, ci,
+                                                           f64, ci, f64, vp, vp, sz, vp]
     L.evk_cmax_motion_objective_workspace_bytes.restype = sz
     L.evk_cmax_motion_objective_workspace_bytes.argtypes = [ci, ci, ci]
     L.evk_cmax_motion_objective_f32.restype = ci

@@ -296,6 +296,44 @@ class DepthGridObjective(torch.autograd.Function):
         return _loss_backward(ctx, g)[:1] + (None,) * 6
 
 
+class MotionAndDepthObjective(torch.autograd.Function):
+    """The depth-grid contrast objective of DepthGridObjective, differentiable in the camera motion as well as in the
+    nodes (contrast_max/motion_and_depth.py): f (B,) f64 from inv_depth_grid (B,gh,gw), motion (B,6) and the prepared
+    device events.  The forward is evk_cmax_depth_grid_objective_f32's; the backward is one pass over the events
+    (evk_cmax_depth_grid_joint_grad_f32) that returns both gradients.  opts = (centre (cx, cy, fx, fy), H, W, sigma,
+    objective, obj_param)."""
+
+    @staticmethod
+    def forward(ctx, inv_depth_grid, motion, x, y, t_rel, p, offsets, opts):
+        from .contrast_max._batched import _rows
+        centre, H, W, sigma, objective, param = opts
+        gh, gw = inv_depth_grid.shape[1:]
+        with torch.cuda.device(x.device):
+            rows = _rows(motion.detach().to(device=x.device, dtype=torch.float64), centre).contiguous()
+        ctx.rows = rows   # the entries read the rows through a pointer, in the backward too
+        ctx.motion_meta = _meta(motion)
+        return _loss_forward(ctx, "evk_cmax_depth_grid_objective", "depth_grid_objective", inv_depth_grid, torch.float32,
+                             (_lib.ptr(rows), centre[0], centre[1]), (gh, gw, H, W, sigma, objective, param), (H, W),
+                             (x, y, t_rel, p), offsets, (1,), query=(gh, gw))
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        saved = ctx.saved_tensors
+        events, offsets, d, iwe = saved[:4], saved[4], saved[5], saved[6]
+        dev = d.device
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            g = _grad_in(g, dev)
+            gd = torch.empty_like(d)
+            gm = torch.empty((d.shape[0], 6), dtype=torch.float64, device=dev)
+            entry = ("evk_cmax_depth_grid_joint_grad",) + ctx.entry[1:]
+            lead, ws = _loss_entry(L, entry, events, offsets, d)
+            _lib.check(L.evk_cmax_depth_grid_joint_grad_f32(*lead, _lib.ptr(iwe), _lib.ptr(g), _lib.ptr(gd), _lib.ptr(gm),
+                                                            _lib.ptr(ws), ws.numel(), _lib.stream()))
+        return (_as_input(gd, ctx.metas[0]), _as_input(gm, ctx.motion_meta)) + (None,) * 6
+
+
 class FlowTimestampObjective(torch.autograd.Function):
     """The batched dense-flow average-timestamp loss of contrast_max/flow_timestamp_objective.py (optic_flow.py:5-46,
     image.py:286-353, then the sum of squares of objectives.py:524-551): f (B,) f64 from flow (B,2,H,W) and the prepared

@@ -7,10 +7,11 @@ loss of `motion_timestamp_objective`), the batched fits of one motion per window
 window into several motions (`motion_segmentation`), and the loss, candidates pass and coarse-to-fine fit of a dense
 flow given on a grid of nodes, to the contrast loss (`grid_flow`) and to the average-timestamp loss
 (`grid_flow_timestamp`), and of an inverse-depth field on a grid of nodes under a known camera motion, to the
-contrast loss (`depth_grid`) and to the average-timestamp loss (`depth_grid_timestamp`).  The batched losses share their
+contrast loss (`depth_grid`) and to the average-timestamp loss (`depth_grid_timestamp`), and of the camera motion and
+such a field together (`motion_and_depth`).  The batched losses share their
 event preparation, argument checks and loops over chunks of windows (`_batched`).
 
-Everything public in the fourteen modules is re-exported here, so `from event_utils_b200.contrast_max
+Everything public in the fifteen modules is re-exported here, so `from event_utils_b200.contrast_max
 import linvel_warp, variance_objective, optimize_contrast` works the way the same import from the
 reference's `lib.contrast_max` package does.
 """
@@ -21,6 +22,7 @@ from . import flow_objective as _flow_objective
 from . import flow_timestamp_objective as _flow_timestamp_objective
 from . import grid_flow as _grid_flow
 from . import grid_flow_timestamp as _grid_flow_timestamp
+from . import motion_and_depth as _motion_and_depth
 from . import motion_fit as _motion_fit
 from . import motion_objective as _motion_objective
 from . import motion_segmentation as _motion_segmentation
@@ -31,6 +33,6 @@ from . import warps as _warps
 
 for _module in (_drivers, _warps, _objectives, _flow_objective, _flow_timestamp_objective, _motion_objective,
                 _motion_timestamp_objective, _motion_fit, _motion_timestamp_fit, _motion_segmentation, _grid_flow,
-                _grid_flow_timestamp, _depth_grid, _depth_grid_timestamp):
+                _grid_flow_timestamp, _depth_grid, _depth_grid_timestamp, _motion_and_depth):
     globals().update({_name: getattr(_module, _name) for _name in dir(_module) if not _name.startswith("_")})
 del _module

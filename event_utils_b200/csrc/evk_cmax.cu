@@ -392,6 +392,51 @@ __device__ __forceinline__ bool cam_project(const CamRot &c, float s, float vx, 
     return true;
 }
 
+// The f32 Jacobian rows of a camera model's warp at its rotation cr and projection cp: jx[k] = dx'/dp_k, jy[k] for the
+// motion (wx, wy, wz, and with DEPTH vx, vy, vz at the translation scale s = rho d) and, in the two slots behind it
+// (N - 2, N - 1), the focal lengths (fx, fy).  Shared by model_taps and the depth-grid joint backward, so both see the
+// same rows bit for bit.
+template <bool DEPTH, int N>
+__device__ __forceinline__ void cam_jacobian(const CamRot &cr, const CamProj &cp, float s, float d, float (&jx)[N],
+                                             float (&jy)[N])
+{
+    using R = float;
+    constexpr int F = N - 2;
+    const R fx = cr.fx, fy = cr.fy, bx = cr.bx, by = cr.by, tx = cr.tx, ty = cr.ty, tz = cr.tz, p2 = cr.p2;
+    const R phi = cr.phi, sh = cr.sh, ch = cr.ch, A = cr.A, B = cr.B;
+    const R iz = cp.iz, X = cp.X, Y = cp.Y;
+    // (phi - sin phi) / phi^3 cancels in f32 for small phi: 1/6 - phi^2/120 + phi^4/5040 - phi^6/362880 there
+    const R C = phi < kCamSeriesPhi
+                    ? (R)(1.0 / 6) - p2 * ((R)(1.0 / 120) - p2 * ((R)(1.0 / 5040) - p2 * (R)(1.0 / 362880)))
+                    : (phi - (R)2 * (sh * ch)) / (p2 * phi);
+    // J_l^T w = A w - B (theta x w) + C theta (theta . w), scaled by s
+    auto jlt = [&](R w0, R w1, R w2, R s, float (&j)[N]) {
+        const R k0 = ty * w2 - tz * w1, k1 = tz * w0 - tx * w2, k2 = tx * w1 - ty * w0;
+        const R q = C * ((tx * w0 + ty * w1) + tz * w2);
+        j[0] = s * ((A * w0 - B * k0) + q * tx);
+        j[1] = s * ((A * w1 - B * k1) + q * ty);
+        j[2] = s * ((A * w2 - B * k2) + q * tz);
+    };
+    if constexpr (DEPTH) {
+        const R Qx = cr.Ux * iz, Qy = cr.Uy * iz, Qz = cr.Uz * iz;
+        jlt(X * Qy, -(Qz + X * Qx), Qy, -(d * fx), jx);
+        jlt(Qz + Y * Qy, -(Y * Qx), -Qx, -(d * fy), jy);
+        const R sx = (s * fx) * iz, sy = (s * fy) * iz;
+        jx[3] = sx; jx[4] = 0.0f; jx[5] = -(sx * X);
+        jy[3] = 0.0f; jy[4] = sy; jy[5] = -(sy * Y);
+    } else {
+        jlt(X * Y, -((R)1 + X * X), Y, -(d * fx), jx);
+        jlt((R)1 + Y * Y, -(X * Y), -X, -(d * fy), jy);
+    }
+    const R rxx = (R)1 - B * (ty * ty + tz * tz), rxy = A * tz + B * (tx * ty), rxz = B * (tx * tz) - A * ty;
+    const R ryx = B * (tx * ty) - A * tz, ryy = (R)1 - B * (tx * tx + tz * tz), ryz = A * tx + B * (ty * tz);
+    const R ux = bx * iz, uy = by * iz;
+    jx[F] = X - ux * (rxx - X * rxz);
+    jy[F] = -(ux * (fy / fx)) * (rxy - Y * rxz);
+    jx[F + 1] = -(uy * (fx / fy)) * (ryx - X * ryz);
+    jy[F + 1] = Y - uy * (ryy - Y * ryz);
+}
+
 // event_util.py:26-27: keep iff 0 < x' <= Wm and 0 < y' <= Hm (NaN compares false -> kept), then the f32 splat taps
 template <class R>
 __device__ __forceinline__ bool model_keep_taps(const CmaxArgs &A, R xw, R yw, R p, unsigned &oob, Taps &T)
@@ -447,41 +492,7 @@ __device__ __forceinline__ bool model_taps(const CmaxArgs &A, const Event<WARP> 
         if (!cam_project<has_depth(WARP)>(cr, s, (R)M.m[3], (R)M.m[4], (R)M.m[5], cp)) return false;
         xw = cp.xw;
         yw = cp.yw;
-        if (JAC) {
-            const R fx = cr.fx, fy = cr.fy, bx = cr.bx, by = cr.by, tx = cr.tx, ty = cr.ty, tz = cr.tz, p2 = cr.p2;
-            const R phi = cr.phi, sh = cr.sh, ch = cr.ch, A = cr.A, B = cr.B;
-            const R iz = cp.iz, X = cp.X, Y = cp.Y;
-            // (phi - sin phi) / phi^3 cancels in f32 for small phi: 1/6 - phi^2/120 + phi^4/5040 - phi^6/362880 there
-            const R C = phi < kCamSeriesPhi
-                            ? (R)(1.0 / 6) - p2 * ((R)(1.0 / 120) - p2 * ((R)(1.0 / 5040) - p2 * (R)(1.0 / 362880)))
-                            : (phi - (R)2 * (sh * ch)) / (p2 * phi);
-            // J_l^T w = A w - B (theta x w) + C theta (theta . w), scaled by s
-            auto jlt = [&](R w0, R w1, R w2, R s, float (&j)[jac_dims(WARP)]) {
-                const R k0 = ty * w2 - tz * w1, k1 = tz * w0 - tx * w2, k2 = tx * w1 - ty * w0;
-                const R q = C * ((tx * w0 + ty * w1) + tz * w2);
-                j[0] = s * ((A * w0 - B * k0) + q * tx);
-                j[1] = s * ((A * w1 - B * k1) + q * ty);
-                j[2] = s * ((A * w2 - B * k2) + q * tz);
-            };
-            if constexpr (has_depth(WARP)) {
-                const R Qx = cr.Ux * iz, Qy = cr.Uy * iz, Qz = cr.Uz * iz;
-                jlt(X * Qy, -(Qz + X * Qx), Qy, -(d * fx), jx);
-                jlt(Qz + Y * Qy, -(Y * Qx), -Qx, -(d * fy), jy);
-                const R sx = (s * fx) * iz, sy = (s * fy) * iz;
-                jx[3] = sx; jx[4] = 0.0f; jx[5] = -(sx * X);
-                jy[3] = 0.0f; jy[4] = sy; jy[5] = -(sy * Y);
-            } else {
-                jlt(X * Y, -((R)1 + X * X), Y, -(d * fx), jx);
-                jlt((R)1 + Y * Y, -(X * Y), -X, -(d * fy), jy);
-            }
-            const R rxx = (R)1 - B * (ty * ty + tz * tz), rxy = A * tz + B * (tx * ty), rxz = B * (tx * tz) - A * ty;
-            const R ryx = B * (tx * ty) - A * tz, ryy = (R)1 - B * (tx * tx + tz * tz), ryz = A * tx + B * (ty * tz);
-            const R ux = bx * iz, uy = by * iz;
-            jx[F] = X - ux * (rxx - X * rxz);
-            jy[F] = -(ux * (fy / fx)) * (rxy - Y * rxz);
-            jx[F + 1] = -(uy * (fx / fy)) * (ryx - X * ryz);
-            jy[F + 1] = Y - uy * (ryy - Y * ryz);
-        }
+        if (JAC) cam_jacobian<has_depth(WARP)>(cr, cp, s, d, jx, jy);
     } else if constexpr (is_planar(WARP)) {
         constexpr int K = model_dims(WARP);
         const R hx = (R)M.m[0], hy = (R)M.m[1], a11 = (R)M.m[2], a12 = (R)M.m[3], a21 = (R)M.m[4], a22 = (R)M.m[5];
@@ -2606,19 +2617,24 @@ static int grid_flow_node_grad(const GridArgs &A, int batch, float *grad_grid, c
 // contracts df/dx', df/dy' with the same dx'/drho, dy'/drho, without the splat weight.
 struct DepthGridArgs {
     GridArgs G;             // canvas and bounds mask (F.C), events, nodes [B][J][gh][gw], accumulators, node sums
-    const double *motion;   // [B][8] rows (wx, wy, wz, vx, vy, vz, fx, fy)
+    const double *motion;   // [B][8] rows (wx, wy, wz, vx, vy, vz, fx, fy); the joint candidates: [B][J][8]
     double cx, cy;          // the principal point
+    double *grad_motion;    // the joint backward: [B][6]
 };
 
-// sample b's camera motion as model_taps reads it: every value rounded to f32
+// a camera motion as model_taps reads it: every value rounded to f32
 struct CamMotion {
     float wx, wy, wz, vx, vy, vz, fx, fy, cx, cy;
 };
+__device__ __forceinline__ CamMotion cam_motion_row(const double *m, double cx, double cy)
+{
+    return {(float)m[0], (float)m[1], (float)m[2], (float)m[3], (float)m[4], (float)m[5], (float)m[6], (float)m[7],
+            (float)cx, (float)cy};
+}
+// sample b's camera motion
 __device__ __forceinline__ CamMotion cam_motion(const DepthGridArgs &D, int b)
 {
-    const double *m = D.motion + (int64_t)b * 8;
-    return {(float)m[0], (float)m[1], (float)m[2], (float)m[3], (float)m[4], (float)m[5], (float)m[6], (float)m[7],
-            (float)D.cx, (float)D.cy};
+    return cam_motion_row(D.motion + (int64_t)b * 8, D.cx, D.cy);
 }
 
 // the J inverse-depth grids of sample b, [J][gh gw] floats, into shared memory
@@ -2650,31 +2666,41 @@ __device__ __forceinline__ bool depth_taps(const CmaxArgs &C, const CamMotion &m
     return model_keep_taps(C, q.xw, q.yw, p, oob, T);
 }
 
-template <bool TS>
+// JOINT: the joint candidates pass (evk_cmax_depth_grid_joint_candidates_f32), whose candidate j is the pair (motion
+// row [b][j], grid [b][j]): the J motions sit behind the J grids in shared memory, and the rotation is per candidate.
+template <bool TS, bool JOINT = false>
 __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_cand_kernel(const DepthGridArgs D)
 {
-    extern __shared__ float depth_nodes[];   // [J][gh gw]
+    extern __shared__ float depth_nodes[];   // [J][gh gw], then JOINT: CamMotion [J]
     const GridArgs &A = D.G;
     const int b = blockIdx.y, J = A.J, G = A.gh * A.gw;
-    load_depth_nodes(A, b, depth_nodes);
+    CamMotion *motions = reinterpret_cast<CamMotion *>(depth_nodes + J * G);
+    if constexpr (JOINT) {
+        for (int j = threadIdx.x; j < J; j += kFlowObjThreads)
+            motions[j] = cam_motion_row(D.motion + ((int64_t)b * J + j) * 8, D.cx, D.cy);
+    }
+    load_depth_nodes(A, b, depth_nodes);   // and the barrier
     int64_t first, last;
     sample_range(A.F.E, b, first, last);
     const CmaxArgs &C = A.F.C;
     const int64_t npix = (int64_t)C.Hc * C.Wc;
     float *acc = A.F.acc + (int64_t)b * J * npix * (TS ? 2 * 8 : 4);   // per canvas: one IWE block or two {S, C} blocks
-    const CamMotion m = cam_motion(D, b);
+    const CamMotion m = JOINT ? CamMotion{} : cam_motion(D, b);
     for_each_event(first, last, [&](int64_t i) { return load_grid_event<TS>(A.F.E, i); }, [&](int64_t, const auto &e) {
         const int pol = TS ? ts_polarity(e.p) : 0;
         if (pol < 0) return;   // a NaN p is in neither timestamp image
         const NodeSample s = node_sample(A, e.x, e.y);
-        const CamRot r = cam_rotate(e.x, e.y, e.t, m.wx, m.wy, m.wz, m.fx, m.fy, m.cx, m.cy);
+        CamRot r;
+        if constexpr (!JOINT) r = cam_rotate(e.x, e.y, e.t, m.wx, m.wy, m.wz, m.fx, m.fy, m.cx, m.cy);
         for (int j = 0; j < J; ++j) {
             CamProj q;
             Taps T;
+            const CamMotion &mj = JOINT ? motions[j] : m;
+            if constexpr (JOINT) r = cam_rotate(e.x, e.y, e.t, mj.wx, mj.wy, mj.wz, mj.fx, mj.fy, mj.cx, mj.cy);
             if constexpr (TS) {
-                if (depth_taps(C, m, r, node_depth(depth_nodes + j * G, s), e.t, 1.0f, q, T))
+                if (depth_taps(C, mj, r, node_depth(depth_nodes + j * G, s), e.t, 1.0f, q, T))
                     ts_block_add(acc + (int64_t)j * 2 * npix * 8, npix, C.Wc, pol, T, e.tau);
-            } else if (depth_taps(C, m, r, node_depth(depth_nodes + j * G, s), e.t, e.p, q, T)) {
+            } else if (depth_taps(C, mj, r, node_depth(depth_nodes + j * G, s), e.t, e.p, q, T)) {
                 red_add4(acc + ((int64_t)j * npix + (int64_t)T.y0 * C.Wc + T.x0) * 4, T.ti);
             }
         }
@@ -2682,10 +2708,13 @@ __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_cand_kernel(const 
 }
 
 // The node-gradient pass of both depth-grid losses, written out like grid_flow_grad_kernel (warp_key_sum needs every
-// lane)
-template <bool TS>
+// lane).  MOTION: the joint backward (evk_cmax_depth_grid_joint_grad_f32), which also contracts df/dx', df/dy' with the
+// camera motion's Jacobian rows at the event's rho (cam_jacobian), in f64 as motion_obj_event_kernel does, into six
+// per-thread sums that one CTA reduction and one f64 atomic per component and CTA add to grad_motion [B][6].
+template <bool TS, bool MOTION = false>
 __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const DepthGridArgs D)
 {
+    static_assert(!(TS && MOTION), "the average-timestamp loss has no joint backward");
     using Ev = decltype(load_grid_event<TS>(D.G.F.E, 0));
     extern __shared__ double depth_acc[];   // [gh gw] f64, then the nodes [gh gw] f32
     const GridArgs &A = D.G;
@@ -2701,6 +2730,9 @@ __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const 
     const float *Wb = TS ? nullptr : A.F.Wimg + b * npix;        // contrast: W_b
     const float2 *ab = TS ? A.F.ab + b * 2 * npix : nullptr;     // timestamp: the (A, B) pairs of both polarities
     const CamMotion m = cam_motion(D, b);
+    double u[6];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) u[k] = 0.0;
     const int lane = threadIdx.x & 31;
     const int64_t stride = (int64_t)gridDim.x * kFlowObjThreads;
     for (int64_t i0 = first + (int64_t)blockIdx.x * kFlowObjThreads + (threadIdx.x - lane); i0 < last; i0 += kBatch * stride) {
@@ -2718,11 +2750,15 @@ __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const 
             float val[4] = {0.0f, 0.0f, 0.0f, 0.0f};
             int key = -1 - lane;   // a lane without a term is alone with its key
             const int pol = TS ? ts_polarity(e.p) : 0;   // a NaN p: no term
-            if (s.cell >= 0 && pol >= 0) {
+            // an event with no node cell (beyond the grid's outer nodes, or the NaN padding) has rho = 0 and no node
+            // term, but where its taps are kept it counts in f and depends on the motion, as in the forward
+            if ((MOTION || s.cell >= 0) && pol >= 0) {
                 const CamRot r = cam_rotate(e.x, e.y, e.t, m.wx, m.wy, m.wz, m.fx, m.fy, m.cx, m.cy);
                 CamProj q;
                 Taps T;
-                if (depth_taps(C, m, r, node_depth(nodes, s), e.t, TS ? 1.0f : e.p, q, T)) {
+                const float rho = node_depth(nodes, s);
+                const bool kept = depth_taps(C, m, r, rho, e.t, TS ? 1.0f : e.p, q, T);
+                if (kept && (!MOTION || s.cell >= 0)) {
                     float sx, sy;
                     if constexpr (TS) {
                         // dF/dk = tau A + B per tap of the event's polarity, as in grid_flow_grad_kernel<true>
@@ -2748,6 +2784,20 @@ __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const 
                     if constexpr (TS) node_terms(s, sx * jx + sy * jy, val, key);
                     else node_terms(s, T.wm * (sx * jx + sy * jy), val, key);
                 }
+                if constexpr (MOTION && !TS) {
+                    if (kept) {
+                        float mx[8], my[8];
+                        cam_jacobian<true>(r, q, rho * e.t, e.t, mx, my);
+                        const int r0 = T.y0 * Wc, r1 = T.y1 * Wc;
+                        const double w00 = __ldg(Wb + r0 + T.x0), w01 = __ldg(Wb + r0 + T.x1), w10 = __ldg(Wb + r1 + T.x0),
+                                     w11 = __ldg(Wb + r1 + T.x1);
+                        const double dx = T.dx, dy = T.dy, ox = 1.0 - dx, oy = 1.0 - dy, wm = T.wm;
+                        double dsx, dsy;
+                        tap_slopes(ox, oy, dx, dy, w00, w01, w10, w11, dsx, dsy);
+#pragma unroll
+                        for (int k = 0; k < 6; ++k) u[k] += wm * ((double)mx[k] * dsx + (double)my[k] * dsy);
+                    }
+                }
             }
             node_grad_flush<1>(depth_acc, G, s, key, val);
         }
@@ -2756,6 +2806,7 @@ __global__ void __launch_bounds__(kFlowObjThreads) depth_grid_grad_kernel(const 
     double *dst = A.grad + (int64_t)b * G;
     for (int q = threadIdx.x; q < G; q += kFlowObjThreads)
         if (depth_acc[q] != 0.0) atomicAdd(dst + q, depth_acc[q]);
+    if constexpr (MOTION) cta_add<6, kFlowObjThreads>(u, D.grad_motion + (int64_t)b * 6);
 }
 
 // The checks and set-up of the depth-grid entries: grid_flow_setup's, then the motion rows.  `images` per canvas: 1 for
@@ -2775,50 +2826,55 @@ static int depth_grid_setup(const char *who, const float *x, const float *y, con
     D.G.F.C.p_scale = 1.0;
     D.motion = motion;
     D.cx = cx; D.cy = cy;
+    D.grad_motion = nullptr;
     return EVK_OK;
 }
 
 // forward and candidates, before the tail: zero the counters and the accumulators of the batch J canvases, the event
-// pass.  nonfinite stays zero: a non-finite event contributes nothing (model_taps).
-template <bool TS>
+// pass.  nonfinite stays zero: a non-finite event contributes nothing (model_taps).  JOINT: one motion per candidate.
+template <bool TS, bool JOINT = false>
 static int depth_grid_event_pass(const DepthGridArgs &D, const BatchObjWorkspace &ws, int batch, cudaStream_t st)
 {
     const GridArgs &A = D.G;
     const int npix = A.F.C.Hc * A.F.C.Wc, canvases = batch * A.J;
     EVK_CUDA(batch_obj_zero(ws, (TS ? 2 : 1) * (int64_t)canvases, npix, TS ? 8 : 4, st));
     if (A.F.E.n > 0) {
-        const size_t smem = (size_t)A.J * A.gh * A.gw * sizeof(float);
-        EVK_CUDA(cudaFuncSetAttribute(depth_grid_cand_kernel<TS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const size_t smem = (size_t)A.J * A.gh * A.gw * sizeof(float) + (JOINT ? A.J * sizeof(CamMotion) : 0);
+        EVK_CUDA(cudaFuncSetAttribute(depth_grid_cand_kernel<TS, JOINT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
         ProfScope prof(st);
         prof_count(1);
-        depth_grid_cand_kernel<TS><<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(D);
+        depth_grid_cand_kernel<TS, JOINT><<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(D);
     }
     return EVK_OK;
 }
 
 // forward and candidates of the contrast loss: the event pass, the tail into iwe_out (the candidates: ws.Wimg)
+template <bool JOINT = false>
 static int depth_grid_forward(const DepthGridArgs &D, const BatchObjWorkspace &ws, const BlurTaps &taps, int batch,
                               int objective, double obj_param, float *iwe_out, double *f_out, cudaStream_t st)
 {
-    if (int rc = depth_grid_event_pass<false>(D, ws, batch, st)) return rc;
+    if (int rc = depth_grid_event_pass<false, JOINT>(D, ws, batch, st)) return rc;
     batch_obj_forward_tail(ws, D.G.F.C.Hc, D.G.F.C.Wc, taps, batch * D.G.J, objective, obj_param, iwe_out, f_out, st);
     EVK_CUDA(cudaGetLastError());
     return EVK_OK;
 }
 
 // backward, after the image-space half (which set D.G.F.Wimg or D.G.F.ab): the node pass into the f64 sums D.G.grad
-// (zeroed by the caller), then their cast to grad_grid
-template <bool TS>
+// (zeroed by the caller), then their cast to grad_grid.  MOTION: also the motion gradient into D.grad_motion (zeroed
+// by the caller).
+template <bool TS, bool MOTION = false>
 static int depth_grid_node_grad(const DepthGridArgs &D, int batch, float *grad_grid, cudaStream_t st)
 {
     const GridArgs &A = D.G;
     const int64_t G = (int64_t)A.gh * A.gw, nodes = batch * G;
     if (A.F.E.n > 0) {
         const size_t smem = (size_t)G * (sizeof(double) + sizeof(float));
-        EVK_CUDA(cudaFuncSetAttribute(depth_grid_grad_kernel<TS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        EVK_CUDA(cudaFuncSetAttribute(depth_grid_grad_kernel<TS, MOTION>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
         ProfScope prof(st);
         prof_count(1);
-        depth_grid_grad_kernel<TS><<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(D);
+        depth_grid_grad_kernel<TS, MOTION><<<batch_grid(A.F.E.n, batch), kFlowObjThreads, smem, st>>>(D);
     }
     prof_count(1);
     grid_flow_grad_cast_kernel<<<grid_simple(nodes, 256), 256, 0, st>>>(A.grad, grad_grid, nodes);
@@ -3990,6 +4046,64 @@ int evk_cmax_depth_grid_candidates_f32(const float *x, const float *y, const flo
     if (batch == 0) return EVK_OK;
     // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
     return depth_grid_forward(D, ws, taps, batch, objective, obj_param, ws.Wimg, f_out, static_cast<cudaStream_t>(stream));
+}
+
+size_t evk_cmax_depth_grid_joint_grad_workspace_bytes(int batch, int gh, int gw, int H, int W)
+{
+    return evk_cmax_depth_grid_objective_workspace_bytes(batch, gh, gw, H, W);
+}
+
+int evk_cmax_depth_grid_joint_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                       const int64_t *offsets, int batch, int64_t n_events, const double *motion, double cx,
+                                       double cy, const float *inv_depth_grid, int gh, int gw, int H, int W, double sigma,
+                                       int objective, double obj_param, const float *iwe, const float *grad_f,
+                                       float *grad_grid, double *grad_motion, void *workspace, size_t workspace_bytes,
+                                       void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_cmax_depth_grid_joint_grad_f32";
+    DepthGridArgs D;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = depth_grid_setup(who, x, y, t_rel, nullptr, p, offsets, batch, n_events, motion, cx, cy, inv_depth_grid, 0, gh, gw, H,
+                              W, sigma, objective, 1, workspace, workspace_bytes, D, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && (!iwe || !grad_f || !grad_grid || !grad_motion)) { set_error("%s: null array", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // the node sums in the accumulator, as in evk_cmax_depth_grid_objective_grad_f32
+    D.G.grad = reinterpret_cast<double *>(ws.acc);
+    D.grad_motion = grad_motion;
+    EVK_CUDA(cudaMemsetAsync(D.G.grad, 0, (size_t)batch * gh * gw * sizeof(double), st));
+    EVK_CUDA(cudaMemsetAsync(grad_motion, 0, (size_t)batch * 6 * sizeof(double), st));
+    batch_obj_backward_W(ws, iwe, H + 1, W + 1, taps, batch, objective, obj_param, grad_f, st);
+    D.G.F.Wimg = ws.Wimg;
+    return depth_grid_node_grad<false, true>(D, batch, grad_grid, st);
+}
+
+size_t evk_cmax_depth_grid_joint_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
+{
+    return evk_cmax_depth_grid_candidates_workspace_bytes(batch, n_cand, gh, gw, H, W);
+}
+
+int evk_cmax_depth_grid_joint_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                             const int64_t *offsets, int batch, int64_t n_events, const double *motion,
+                                             double cx, double cy, const float *cand, int n_cand, int gh, int gw, int H, int W,
+                                             double blur_sigma, int objective, double obj_param, double *f_out, void *workspace,
+                                             size_t workspace_bytes, void *stream)
+{
+    using namespace evk;
+    const char *who = "evk_cmax_depth_grid_joint_candidates_f32";
+    DepthGridArgs D;
+    BatchObjWorkspace ws;
+    BlurTaps taps;
+    int rc = depth_grid_setup(who, x, y, t_rel, nullptr, p, offsets, batch, n_events, motion, cx, cy, cand, n_cand < 1 ? -1 : n_cand,
+                              gh, gw, H, W, blur_sigma, objective, 1, workspace, workspace_bytes, D, ws, taps);
+    if (rc) return rc;
+    if (batch > 0 && !f_out) { set_error("%s: null output", who); return EVK_E_ARG; }
+    if (batch == 0) return EVK_OK;
+    // the folded images go to ws.Wimg, which a forward-only workspace has no other use for
+    return depth_grid_forward<true>(D, ws, taps, batch, objective, obj_param, ws.Wimg, f_out, static_cast<cudaStream_t>(stream));
 }
 
 size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W)

@@ -598,6 +598,39 @@ int evk_cmax_depth_grid_candidates_f32(const float *x, const float *y, const flo
                                        int W, double blur_sigma, int objective, double obj_param, double *f_out,
                                        void *workspace, size_t workspace_bytes, void *stream);
 
+/* Camera motion and depth together: the joint backward of evk_cmax_depth_grid_objective_f32, whose f it leaves as it is.
+ * The arguments are those of evk_cmax_depth_grid_objective_grad_f32, and it writes, besides the same grad_grid,
+ *   grad_motion: [batch][6] doubles = grad_f[b] df_b/d(wx, wy, wz, vx, vy, vz) (the focal lengths and the principal
+ *                point are constants)
+ * per kept event df/dx' and df/dy' of evk_cmax_motion_objective_grad_f32 contracted with the f32 Jacobian rows of
+ * EVK_WARP_CAMERA_MOTION at the event's interpolated rho, in f64, summed per CTA and across CTAs in f64: the first six
+ * components of evk_cmax_motion_depth_objective_grad_f32's gradient at that rho, up to the order of the sums.
+ * workspace: evk_cmax_depth_grid_joint_grad_workspace_bytes(batch, gh, gw, H, W) bytes (the depth grid's), 256-byte
+ * aligned; 0 for arguments the entry rejects.  The call does not synchronise. */
+size_t evk_cmax_depth_grid_joint_grad_workspace_bytes(int batch, int gh, int gw, int H, int W);
+int evk_cmax_depth_grid_joint_grad_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                       const int64_t *offsets, int batch, int64_t n_events, const double *motion,
+                                       double cx, double cy, const float *inv_depth_grid, int gh, int gw, int H, int W,
+                                       double blur_sigma, int objective, double obj_param, const float *iwe,
+                                       const float *grad_f, float *grad_grid, double *grad_motion, void *workspace,
+                                       size_t workspace_bytes, void *stream);
+
+/* Many (motion, inverse-depth grid) pairs per sample in one pass over the events: f_out[b][j] is exactly the f_b of
+ * evk_cmax_depth_grid_objective_f32 with motion row [b] = motion[b][j] and inv_depth_grid[b] = cand[b][j].
+ *   motion: [batch][n_cand][8] doubles on the device, rows (wx, wy, wz, vx, vy, vz, fx, fy)
+ *   cand  : [batch][n_cand][gh][gw] floats; the limits of evk_cmax_depth_grid_candidates_f32 (1 <= n_cand <= 32,
+ *           n_cand * gh * gw <= 12288, batch * n_cand <= 65535), checked before any CUDA call
+ *   f_out : [batch][n_cand] doubles
+ * Every event is read once and its node cell computed once; the rotation is computed per candidate.  Forward only.
+ * workspace: evk_cmax_depth_grid_joint_candidates_workspace_bytes(batch, n_cand, gh, gw, H, W) bytes (the depth grid
+ * candidates'), 256-byte aligned; 0 for arguments the entry rejects.  The call does not synchronise. */
+size_t evk_cmax_depth_grid_joint_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W);
+int evk_cmax_depth_grid_joint_candidates_f32(const float *x, const float *y, const float *t_rel, const float *p,
+                                             const int64_t *offsets, int batch, int64_t n_events, const double *motion,
+                                             double cx, double cy, const float *cand, int n_cand, int gh, int gw, int H,
+                                             int W, double blur_sigma, int objective, double obj_param, double *f_out,
+                                             void *workspace, size_t workspace_bytes, void *stream);
+
 /* Parametric contrast maximisation over a batch of samples, as a differentiable loss: per sample the f32
  * fast-mode evaluation of evk_cmax_warp_objective_f32 / evk_cmax_linvel_objective_f32 with Hm = Hs = H,
  * Wm = Ws = W, p_scale 1 and no flags (get_iwe, lib/contrast_max/objectives.py:184-192).  Sample b is the
