@@ -2100,6 +2100,24 @@ static size_t batch_obj_carve(void *base, int batch, int H, int W, size_t acc_bl
     return off;
 }
 
+// The canvas every batched objective needs: H, W >= 2 and at most 2^30 canvas pixels (H+1)(W+1), so that pixel counts and
+// indices fit an int.
+static bool batch_canvas_ok(int H, int W)
+{
+    return H >= 2 && W >= 2 && (int64_t)(H + 1) * (W + 1) <= (int64_t)1 << 30;
+}
+
+// The limits of the dense-flow and model entries, which their workspace queries share.  `images` tail images per canvas
+// (1 for the contrast losses, 2 for the timestamp losses), and at most 65535 images: 0 <= batch <= 65535 / images.
+// n_cand 0: one canvas per sample; else n_cand forward-only canvases per sample, 1 <= n_cand <= kMaxCandidates and
+// batch n_cand <= 65535 / images.
+static bool batch_limits(int batch, int n_cand, int H, int W, int images)
+{
+    const int64_t max_batch = 65535 / images;
+    if (batch < 0 || batch > max_batch || !batch_canvas_ok(H, W)) return false;
+    return !n_cand || (n_cand >= 1 && n_cand <= kMaxCandidates && (int64_t)batch * n_cand <= max_batch);
+}
+
 // the flow objective's accumulator: the IWE blocks (forward) or the flow-gradient blocks (backward), whichever is larger
 static size_t flow_obj_acc_blocks(int H, int W)
 {
@@ -2119,7 +2137,6 @@ static int batch_obj_check(const char *who, const char *wrt, int batch, int H, i
         set_error("%s: unknown objective %d", who, objective);
         return EVK_E_ARG;
     }
-    if ((size_t)(H + 1) * (W + 1) > (size_t)1 << 30) { set_error("%s: canvas too large", who); return EVK_E_ARG; }
     const size_t need = batch_obj_carve(nullptr, batch, H, W, acc_blocks, nullptr, backward);
     if (!workspace || workspace_bytes < need || ((uintptr_t)workspace & 255)) {
         set_error("%s: 256-byte aligned workspace of %zu bytes required", who, need);
@@ -2144,9 +2161,9 @@ static int flow_setup(const char *who, const float *x, const float *y, const flo
 {
     if (int rc = check_sigma(who, sigma)) return rc;
     const int max_batch = 65535 / images;
-    if (batch < 0 || batch > max_batch || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !flow)) ||
+    if (!batch_limits(batch, 0, H, W, images) || n < 0 || (batch > 0 && (!offsets || !flow)) ||
         (n > 0 && (!x || !y || !t || (images == 2 && !tau) || !p))) {
-        set_error("%s: bad arguments (0 <= batch <= %d, H, W >= 2)", who, max_batch);
+        set_error("%s: bad arguments (0 <= batch <= %d, H, W >= 2, (H+1)(W+1) <= 2^30)", who, max_batch);
         return EVK_E_ARG;
     }
     int rc = batch_obj_check(who, "flow", images * batch, H, W, sigma, objective, acc_blocks, workspace, workspace_bytes, ws, taps);
@@ -2509,7 +2526,7 @@ __global__ void __launch_bounds__(256) grid_flow_grad_cast_kernel(const double *
 // one per polarity), and at most 65535 images: batch (n_cand) <= 65535 / images.
 static int grid_flow_limits(int batch, int n_cand, int gh, int gw, int H, int W, int images = 1)
 {
-    if (batch < 0 || H < 2 || W < 2 || gh < 2 || gw < 2 || gh > H || gw > W) return 0;
+    if (batch < 0 || !batch_canvas_ok(H, W) || gh < 2 || gw < 2 || gh > H || gw > W) return 0;
     const int64_t G = (int64_t)gh * gw, canvases = 65535 / images;
     if (!n_cand) return batch <= canvases && G <= kMaxGridNodes;
     return n_cand >= 1 && n_cand <= kMaxCandidates && (int64_t)n_cand * G <= kMaxGridCandNodes && (int64_t)batch * n_cand <= canvases;
@@ -2975,9 +2992,9 @@ static int model_setup(const char *who, const float *x, const float *y, const fl
 {
     if (int rc = check_sigma(who, sigma)) return rc;
     const int max_batch = 65535 / images;
-    if (batch < 0 || batch > max_batch || n < 0 || H < 2 || W < 2 || (batch > 0 && (!offsets || !params)) ||
+    if (!batch_limits(batch, 0, H, W, images) || n < 0 || (batch > 0 && (!offsets || !params)) ||
         (n > 0 && (!x || !y || !t || (images == 2 && !tau) || !p || (depth && !rho)))) {
-        set_error("%s: bad arguments (0 <= batch <= %d, H, W >= 2)", who, max_batch);
+        set_error("%s: bad arguments (0 <= batch <= %d, H, W >= 2, (H+1)(W+1) <= 2^30)", who, max_batch);
         return EVK_E_ARG;
     }
     const int dims = depth ? (warp == EVK_WARP_CAMERA_MOTION ? 8 : 0) : motion_obj_dims(warp);
@@ -2987,7 +3004,7 @@ static int model_setup(const char *who, const float *x, const float *y, const fl
     }
     if (!dims) { set_error("%s: unknown warp %d", who, warp); return EVK_E_ARG; }
     if (K != dims) { set_error("%s: warp %d has %d parameters, K = %d", who, warp, dims, K); return EVK_E_ARG; }
-    if (n_cand && (n_cand < 1 || n_cand > kMaxCandidates || (int64_t)batch * n_cand > max_batch)) {
+    if (n_cand && !batch_limits(batch, n_cand, H, W, images)) {
         set_error("%s: bad arguments (1 <= n_cand <= %d, batch * n_cand <= %d)", who, kMaxCandidates, max_batch);
         return EVK_E_ARG;
     }
@@ -3197,26 +3214,28 @@ __global__ void __launch_bounds__(kFlowObjThreads) motion_seg_assign_kernel(cons
 
 // shared argument checks and set-up of the segmentation entries: M models per sample, J candidates per model (0: the
 // differentiable entries, batch M canvases with the backward's images; else batch M J forward-only canvases)
+// The limits of the segmentation entries, which their workspace queries share: 1 <= n_models <= kMaxSegModels and the
+// batch_limits of batch M canvases (n_cand 0), or of batch samples with M n_cand candidates each.
+static bool seg_limits(int batch, int n_models, int n_cand, int H, int W)
+{
+    if (n_models < 1 || n_models > kMaxSegModels || batch < 0) return false;
+    if (!n_cand) return (int64_t)batch * n_models <= 65535 && batch_limits(batch * n_models, 0, H, W, 1);
+    return n_cand >= 1 && (int64_t)n_models * n_cand <= kMaxCandidates && batch_limits(batch, n_models * n_cand, H, W, 1);
+}
+
 static int motion_seg_setup(const char *who, const float *x, const float *y, const float *t, const float *p, const float *weights,
                             int n_models, const int64_t *offsets, int batch, int64_t n, int warp, const double *params, int K,
                             double cx, double cy, int H, int W, double sigma, int objective, void *workspace,
                             size_t workspace_bytes, ModelArgs &A, BatchObjWorkspace &ws, BlurTaps &taps, int n_cand = 0)
 {
-    if (n_models < 1 || n_models > kMaxSegModels) {
-        set_error("%s: bad n_models %d (1 <= n_models <= %d)", who, n_models, kMaxSegModels);
-        return EVK_E_ARG;
-    }
-    if (!n_cand && (int64_t)batch * n_models > 65535) {
-        set_error("%s: bad arguments (batch * n_models <= 65535 canvases)", who);
-        return EVK_E_ARG;
-    }
-    if (n_cand && (n_cand < 1 || n_models * n_cand > kMaxCandidates || (int64_t)batch * n_models * n_cand > 65535)) {
-        set_error("%s: bad arguments (1 <= n_cand, n_models * n_cand <= %d, batch * n_models * n_cand <= 65535)", who,
+    if (!seg_limits(batch, n_models, n_cand, H, W)) {
+        set_error("%s: bad arguments (1 <= n_models <= %d, H, W >= 2, (H+1)(W+1) <= 2^30; batch * n_models <= 65535 canvases; "
+                  "candidates: 1 <= n_cand, n_models * n_cand <= %d, batch * n_models * n_cand <= 65535)", who, kMaxSegModels,
                   kMaxCandidates);
         return EVK_E_ARG;
     }
     if (n > 0 && !weights) { set_error("%s: null weights", who); return EVK_E_ARG; }
-    const int rc = model_setup(who, x, y, t, nullptr, p, nullptr, false, offsets, n_cand || batch < 0 ? batch : batch * n_models, n, warp, params, K,
+    const int rc = model_setup(who, x, y, t, nullptr, p, nullptr, false, offsets, n_cand ? batch : batch * n_models, n, warp, params, K,
                                cx, cy, H, W, sigma, objective, 1, (size_t)(H + 1) * (W + 1), n_models * n_cand, workspace,
                                workspace_bytes, A, ws, taps);
     if (rc) return rc;
@@ -3491,7 +3510,7 @@ size_t evk_cmax_workspace_bytes(int Hs, int Ws)
     return evk::carve(nullptr, Hs, Ws, nullptr);
 }
 
-int evk_cmax_linvel_objective_f64(const double *x, const double *y, const double *t, const double *p, int64_t n,
+static int linvel_objective_f64(const double *x, const double *y, const double *t, const double *p, int64_t n,
                                   double p_scale, double vx, double vy, double t_ref, int Hm, int Wm, int Hs, int Ws,
                                   double sigma, unsigned flags, int objective, double obj_param, double *result,
                                   float *iwe_out, float *diwe_out, void *workspace, size_t workspace_bytes, void *stream)
@@ -3507,7 +3526,7 @@ int evk_cmax_linvel_objective_f64(const double *x, const double *y, const double
                                      workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
-int evk_cmax_linvel_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, int64_t n,
+static int linvel_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, int64_t n,
                                   float p_scale, float vx, float vy, int Hm, int Wm, int Hs, int Ws, double sigma,
                                   unsigned flags, int objective, double obj_param, double *result, float *iwe_out,
                                   float *diwe_out, void *workspace, size_t workspace_bytes, void *stream)
@@ -3523,12 +3542,43 @@ int evk_cmax_linvel_objective_f32(const float *x, const float *y, const float *t
                                      workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
+// The objective entries' result has 12 slots, the variance entries' 8; the variance tails fill the first 8, so the objective
+// entries zero [8..11] for EVK_OBJ_VARIANCE (n results of `stride` doubles)
+static int zero_variance_stats(int rc, int objective, double *result, int n, int stride, void *stream)
+{
+    using namespace evk;
+    if (rc || objective != OBJ_VARIANCE || !result) return rc;
+    EVK_CUDA(cudaMemset2DAsync(result + 8, (size_t)stride * sizeof(double), 0, 4 * sizeof(double), n,
+                               static_cast<cudaStream_t>(stream)));
+    return EVK_OK;
+}
+
+int evk_cmax_linvel_objective_f64(const double *x, const double *y, const double *t, const double *p, int64_t n,
+                                  double p_scale, double vx, double vy, double t_ref, int Hm, int Wm, int Hs, int Ws,
+                                  double sigma, unsigned flags, int objective, double obj_param, double *result,
+                                  float *iwe_out, float *diwe_out, void *workspace, size_t workspace_bytes, void *stream)
+{
+    const int rc = linvel_objective_f64(x, y, t, p, n, p_scale, vx, vy, t_ref, Hm, Wm, Hs, Ws, sigma, flags, objective, obj_param,
+                                        result, iwe_out, diwe_out, workspace, workspace_bytes, stream);
+    return zero_variance_stats(rc, objective, result, 1, 12, stream);
+}
+
+int evk_cmax_linvel_objective_f32(const float *x, const float *y, const float *t_rel, const float *p, int64_t n,
+                                  float p_scale, float vx, float vy, int Hm, int Wm, int Hs, int Ws, double sigma,
+                                  unsigned flags, int objective, double obj_param, double *result, float *iwe_out,
+                                  float *diwe_out, void *workspace, size_t workspace_bytes, void *stream)
+{
+    const int rc = linvel_objective_f32(x, y, t_rel, p, n, p_scale, vx, vy, Hm, Wm, Hs, Ws, sigma, flags, objective, obj_param,
+                                        result, iwe_out, diwe_out, workspace, workspace_bytes, stream);
+    return zero_variance_stats(rc, objective, result, 1, 12, stream);
+}
+
 int evk_cmax_linvel_variance_f64(const double *x, const double *y, const double *t, const double *p, int64_t n,
                                  double p_scale, double vx, double vy, double t_ref, int Hm, int Wm, int Hs, int Ws,
                                  double sigma, unsigned flags, double *result, float *iwe_out, float *diwe_out,
                                  void *workspace, size_t workspace_bytes, void *stream)
 {
-    return evk_cmax_linvel_objective_f64(x, y, t, p, n, p_scale, vx, vy, t_ref, Hm, Wm, Hs, Ws, sigma, flags, 0, 0.0, result,
+    return linvel_objective_f64(x, y, t, p, n, p_scale, vx, vy, t_ref, Hm, Wm, Hs, Ws, sigma, flags, 0, 0.0, result,
                                          iwe_out, diwe_out, workspace, workspace_bytes, stream);
 }
 
@@ -3537,7 +3587,7 @@ int evk_cmax_linvel_variance_f32(const float *x, const float *y, const float *t_
                                  unsigned flags, double *result, float *iwe_out, float *diwe_out, void *workspace,
                                  size_t workspace_bytes, void *stream)
 {
-    return evk_cmax_linvel_objective_f32(x, y, t_rel, p, n, p_scale, vx, vy, Hm, Wm, Hs, Ws, sigma, flags, 0, 0.0, result,
+    return linvel_objective_f32(x, y, t_rel, p, n, p_scale, vx, vy, Hm, Wm, Hs, Ws, sigma, flags, 0, 0.0, result,
                                          iwe_out, diwe_out, workspace, workspace_bytes, stream);
 }
 
@@ -3624,8 +3674,8 @@ int evk_cmax_flow_variance_f32(const float *x, const float *y, const float *t, c
                                    static_cast<cudaStream_t>(stream));
 }
 
-int evk_iwe_objective_f32(const float *iwe, const float *diwe, int Hc, int Wc, double sigma, unsigned flags, int objective,
-                          double obj_param, double *result, void *workspace, size_t workspace_bytes, void *stream)
+static int iwe_objective(const float *iwe, const float *diwe, int Hc, int Wc, double sigma, unsigned flags, int objective,
+                         double obj_param, double *result, void *workspace, size_t workspace_bytes, void *stream)
 {
     using namespace evk;
     if (int rc = check_sigma("evk_iwe_objective_f32", sigma)) return rc;
@@ -3643,10 +3693,17 @@ int evk_iwe_objective_f32(const float *iwe, const float *diwe, int Hc, int Wc, d
     return launch_tail(ws, Hc, Wc, sigma, flags, objective, obj_param, grad, result, st);
 }
 
+int evk_iwe_objective_f32(const float *iwe, const float *diwe, int Hc, int Wc, double sigma, unsigned flags, int objective,
+                          double obj_param, double *result, void *workspace, size_t workspace_bytes, void *stream)
+{
+    const int rc = iwe_objective(iwe, diwe, Hc, Wc, sigma, flags, objective, obj_param, result, workspace, workspace_bytes, stream);
+    return zero_variance_stats(rc, objective, result, 1, 12, stream);
+}
+
 int evk_variance_objective_f32(const float *iwe, const float *diwe, int Hc, int Wc, double sigma, unsigned flags,
                                double *result, void *workspace, size_t workspace_bytes, void *stream)
 {
-    return evk_iwe_objective_f32(iwe, diwe, Hc, Wc, sigma, flags, 0, 0.0, result, workspace, workspace_bytes, stream);
+    return iwe_objective(iwe, diwe, Hc, Wc, sigma, flags, 0, 0.0, result, workspace, workspace_bytes, stream);
 }
 
 int evk_gaussian_blur_f32(const float *img, int H, int W, double sigma, float *out, float *tmp, void *stream)
@@ -3720,7 +3777,7 @@ int evk_cmax_linvel_objective_batch_f64(const double *x, const double *y, const 
         cmax_fused_var_tail_kernel_t<false><<<tgrid, tblock, 0, st>>>(CmaxPeers{}, ws.acc, nullptr, 1, A.Hc, A.Wc, taps, do_blur, grad ? 1 : 0, mix_a, mix_b, nullptr,
                                                                nullptr, ws.bsums, ws.btickets, ws.oob, results);
         EVK_CUDA(cudaGetLastError());
-        return EVK_OK;
+        return zero_variance_stats(EVK_OK, objective, results, n_params, 12, stream);
     }
     for (int k = 0; k < n_params; ++k) {
         // per-candidate image-space tail on the shared scratch images (stream-ordered)
@@ -3731,7 +3788,7 @@ int evk_cmax_linvel_objective_batch_f64(const double *x, const double *y, const 
         int rc = launch_tail(ws, A.Hc, A.Wc, sigma, flags, objective, obj_param, grad, results + 12 * k, st);
         if (rc) return rc;
     }
-    return EVK_OK;
+    return zero_variance_stats(EVK_OK, objective, results, n_params, 12, stream);
 }
 
 int evk_cmax_warp_objective_f64(const double *x, const double *y, const double *t, const double *p, int64_t n, double p_scale,
@@ -3833,7 +3890,7 @@ int evk_cmax_warp_objective_batch_f64(const double *x, const double *y, const do
 
 size_t evk_cmax_flow_objective_workspace_bytes(int batch, int H, int W)
 {
-    if (batch < 0 || H < 2 || W < 2) return 0;
+    if (!evk::batch_limits(batch, 0, H, W, 1)) return 0;
     return evk::batch_obj_carve(nullptr, batch, H, W, evk::flow_obj_acc_blocks(H, W), nullptr);
 }
 
@@ -3950,7 +4007,7 @@ int evk_cmax_grid_flow_objective_grad_f32(const float *x, const float *y, const 
 
 size_t evk_cmax_grid_flow_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
 {
-    if (!evk::grid_flow_limits(batch, n_cand, gh, gw, H, W)) return 0;
+    if (!evk::grid_flow_limits(batch, n_cand < 1 ? -1 : n_cand, gh, gw, H, W)) return 0;
     return evk::batch_obj_carve(nullptr, batch * n_cand, H, W, (size_t)(H + 1) * (W + 1), nullptr, false);
 }
 
@@ -4108,7 +4165,7 @@ int evk_cmax_depth_grid_joint_candidates_f32(const float *x, const float *y, con
 
 size_t evk_cmax_motion_objective_workspace_bytes(int batch, int H, int W)
 {
-    if (batch < 0 || H < 2 || W < 2) return 0;
+    if (!evk::batch_limits(batch, 0, H, W, 1)) return 0;
     return evk::batch_obj_carve(nullptr, batch, H, W, (size_t)(H + 1) * (W + 1), nullptr);
 }
 
@@ -4233,7 +4290,7 @@ int evk_cmax_motion_objective_grad_f32(const float *x, const float *y, const flo
 
 size_t evk_cmax_motion_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
 {
-    if (batch < 0 || n_cand < 1 || n_cand > evk::kMaxCandidates || H < 2 || W < 2) return 0;
+    if (!evk::batch_limits(batch, n_cand < 1 ? -1 : n_cand, H, W, 1)) return 0;
     return evk::batch_obj_carve(nullptr, batch * n_cand, H, W, (size_t)(H + 1) * (W + 1), nullptr, false);
 }
 
@@ -4293,7 +4350,7 @@ int evk_cmax_motion_depth_candidates_f32(const float *x, const float *y, const f
 
 size_t evk_cmax_motion_segment_workspace_bytes(int batch, int n_models, int H, int W)
 {
-    if (batch < 0 || n_models < 1 || n_models > evk::kMaxSegModels || H < 2 || W < 2) return 0;
+    if (!evk::seg_limits(batch, n_models, 0, H, W)) return 0;
     return evk::batch_obj_carve(nullptr, batch * n_models, H, W, (size_t)(H + 1) * (W + 1), nullptr);
 }
 
@@ -4372,9 +4429,7 @@ int evk_cmax_motion_segment_grad_f32(const float *x, const float *y, const float
 
 size_t evk_cmax_motion_segment_candidates_workspace_bytes(int batch, int n_models, int n_cand, int H, int W)
 {
-    if (batch < 0 || n_models < 1 || n_models > evk::kMaxSegModels || n_cand < 1 || n_models * n_cand > evk::kMaxCandidates ||
-        H < 2 || W < 2)
-        return 0;
+    if (!evk::seg_limits(batch, n_models, n_cand < 1 ? -1 : n_cand, H, W)) return 0;
     return evk::batch_obj_carve(nullptr, batch * n_models * n_cand, H, W, (size_t)(H + 1) * (W + 1), nullptr, false);
 }
 
@@ -4444,7 +4499,7 @@ int evk_cmax_motion_segment_assign_f32(const float *x, const float *y, const flo
 
 size_t evk_flow_timestamp_objective_workspace_bytes(int batch, int H, int W)
 {
-    if (batch < 0 || H < 2 || W < 2) return 0;
+    if (!evk::batch_limits(batch, 0, H, W, 2)) return 0;
     return evk::batch_obj_carve(nullptr, 2 * batch, H, W, evk::flow_ts_acc_blocks(H, W), nullptr);
 }
 
@@ -4509,7 +4564,7 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
 
 size_t evk_motion_timestamp_objective_workspace_bytes(int batch, int H, int W)
 {
-    if (batch < 0 || H < 2 || W < 2) return 0;
+    if (!evk::batch_limits(batch, 0, H, W, 2)) return 0;
     return evk::batch_obj_carve(nullptr, 2 * batch, H, W, evk::flow_ts_acc_blocks(H, W), nullptr);
 }
 
@@ -4640,7 +4695,7 @@ int evk_motion_timestamp_objective_grad_f32(const float *x, const float *y, cons
 
 size_t evk_motion_timestamp_candidates_workspace_bytes(int batch, int n_cand, int H, int W)
 {
-    if (batch < 0 || n_cand < 1 || n_cand > evk::kMaxCandidates || H < 2 || W < 2) return 0;
+    if (!evk::batch_limits(batch, n_cand < 1 ? -1 : n_cand, H, W, 2)) return 0;
     return evk::motion_ts_cand_bytes(2 * batch * n_cand, H, W);
 }
 
@@ -4754,7 +4809,7 @@ int evk_grid_flow_timestamp_objective_grad_f32(const float *x, const float *y, c
 
 size_t evk_grid_flow_timestamp_candidates_workspace_bytes(int batch, int n_cand, int gh, int gw, int H, int W)
 {
-    if (!evk::grid_flow_limits(batch, n_cand, gh, gw, H, W, 2)) return 0;
+    if (!evk::grid_flow_limits(batch, n_cand < 1 ? -1 : n_cand, gh, gw, H, W, 2)) return 0;
     return evk::motion_ts_cand_bytes(2 * batch * n_cand, H, W);
 }
 

@@ -297,13 +297,19 @@ void launch_image_fold(const float *ws, float *out, int H, int W, cudaStream_t s
     image_fold_kernel<false><<<grid_simple((int64_t)H * W, 256), 256, 0, st>>>(ws, out, H, W, 0.0f);
 }
 
+// the canvas evk_image_f32 and evk_image_workspace_bytes accept: at least 1x1, and 2x2 for the bilinear splat
+static bool image_canvas_ok(int H, int W, unsigned flags)
+{
+    return (flags & EVK_BILINEAR) ? H >= 2 && W >= 2 : H >= 1 && W >= 1;
+}
+
 }  // namespace evk
 
 extern "C" {
 
 size_t evk_image_workspace_bytes(int Himg, int Wimg, unsigned flags)
 {
-    if (Himg < 1 || Wimg < 1 || !(flags & EVK_BILINEAR)) return 0;
+    if (!(flags & EVK_BILINEAR) || !evk::image_canvas_ok(Himg, Wimg, flags)) return 0;
     return (size_t)Himg * Wimg * 4 * sizeof(float);
 }
 
@@ -318,7 +324,7 @@ int evk_image_f32(const float *x, const float *y, const float *p, int64_t n, int
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool bil = (flags & EVK_BILINEAR) != 0, accum = (flags & EVK_ACCUMULATE) != 0;
-    if (bil && (Himg < 2 || Wimg < 2)) { set_error("evk_image_f32: bilinear needs a canvas of at least 2x2"); return EVK_E_ARG; }
+    if (!image_canvas_ok(Himg, Wimg, flags)) { set_error("evk_image_f32: bilinear needs a canvas of at least 2x2"); return EVK_E_ARG; }
     ImageArgs A{};
     A.x = x; A.y = y; A.p = p; A.n = n; A.H = Himg; A.W = Wimg;
     A.clip = (flags & EVK_CLIP) ? 1 : 0; A.clipx = clipx; A.clipy = clipy;

@@ -63,6 +63,10 @@ __global__ void __launch_bounds__(256) select_hist_kernel(const float *__restric
     }
 }
 
+// the selection state of a call, from the launch's parameters: a kernel argument is copied when the launch is enqueued
+// (or captured), where a copy from a host variable would be read again at every replay of a captured graph
+__global__ void select_init_kernel(SelectState *st, SelectState init) { *st = init; }
+
 // one CTA: for each target find the bin holding its rank, narrow the prefix, clear the histogram
 __global__ void __launch_bounds__(64) select_scan_kernel(unsigned *hist, int shift, int nbits, int last, SelectState *st)
 {
@@ -127,7 +131,8 @@ int evk_robust_norm_f32(const float *x, int64_t n, int64_t k_low, int64_t k_top,
     SelectState init{};
     init.rank[0] = (unsigned long long)k_low; init.rank[1] = (unsigned long long)k_top;
     EVK_CUDA(cudaMemsetAsync(hist, 0, 2 * kBins * sizeof(unsigned), st));
-    EVK_CUDA(cudaMemcpyAsync(state, &init, sizeof(init), cudaMemcpyHostToDevice, st));
+    prof_count(1);
+    select_init_kernel<<<1, 1, 0, st>>>(state, init);
     const int shifts[3] = {21, 10, 0}, bits[3] = {11, 11, 10};
     const int grid = grid_for(select_hist_kernel, 256, n, 256 * 8);
     for (int p = 0; p < 3; ++p) {

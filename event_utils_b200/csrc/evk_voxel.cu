@@ -747,13 +747,19 @@ static int launch_voxel(const VoxelArgs &A0, unsigned flags, int layout, cudaStr
     return EVK_OK;
 }
 
+// the grid every voxel entry and evk_voxel_workspace_bytes accept: B, H, W >= 1 and fewer than 2^40 cells
+static bool voxel_grid_ok(int B, int H, int W)
+{
+    return B >= 1 && H >= 1 && W >= 1 && (int64_t)B * H * W < ((int64_t)1 << 40);
+}
+
 static int check_common(int64_t n, int B, int H, int W, const void *out)
 {
     if (n < 0 || B < 1 || H < 1 || W < 1 || out == nullptr) {
         set_error("evk_voxel: bad arguments (n=%lld B=%d H=%d W=%d out=%p)", (long long)n, B, H, W, out);
         return EVK_E_ARG;
     }
-    if ((int64_t)B * H * W >= ((int64_t)1 << 40)) { set_error("evk_voxel: grid too large"); return EVK_E_ARG; }
+    if (!voxel_grid_ok(B, H, W)) { set_error("evk_voxel: grid too large"); return EVK_E_ARG; }
     return EVK_OK;
 }
 
@@ -763,7 +769,7 @@ extern "C" {
 
 size_t evk_voxel_workspace_bytes(int B, int H, int W, unsigned flags)
 {
-    if (B < 1 || H < 1 || W < 1) return 0;
+    if (!evk::voxel_grid_ok(B, H, W)) return 0;
     if (flags & EVK_BILINEAR) return (size_t)B * H * W * 4 * sizeof(float);   // 2x2 blocks per bin
     size_t need = (size_t)H * W * evk::quads_for_bins(B) * 4 * sizeof(float);      // temporal quads per pixel
     need = ((need + 255) & ~(size_t)255) + 256;                                    // + the launch-level contention verdict

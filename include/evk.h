@@ -79,7 +79,7 @@ extern "C" {
 
 int evk_version(void);
 const char *evk_last_error(void);
-/* 0 if the current device is compute capability 10.x, EVK_E_DEVICE otherwise */
+/* 0 if the current device is compute capability 9.0 (the library is built for sm_90a only), EVK_E_DEVICE otherwise */
 int evk_device_check(void);
 
 /* ---------------------------------------------------------------------------------------------
@@ -348,7 +348,7 @@ int evk_cmax_linvel_variance_f32(const float *x, const float *y, const float *t_
 /* The reference's other objective functions on the same fused event pass (row f3).  `objective` is
  * one of EVK_OBJ_*; `obj_param` is the ISOA threshold / the SOSA exponent p.  result: 12 doubles --
  * [0] f, [1..2] g, [3] sum(IWE), [4] events outside the canvas, [5] mean(G), [6..7] un-mixed gradient,
- * [8] mean(G^2), [9] sum(exp(-p G)), [10] max(G), [11] #(G > thresh)   (G = blurred IWE).
+ * [8] mean(G^2), [9] sum(exp(-p G)), [10] max(G), [11] #(G > thresh)   (G = blurred IWE; 0 for EVK_OBJ_VARIANCE).
  *   EVK_OBJ_VARIANCE  variance_objective  objectives.py:202-264   (result as documented above)
  *   EVK_OBJ_SOS       sos_ / rms_objective objectives.py:266-357   f = -mean(G^2), g = -mean(2 IWE * G3(dIWE))
  *   EVK_OBJ_SOE       soe_objective       objectives.py:358-400   f = -mean(exp G), g = -mean(exp(G) G3(dIWE))
@@ -486,7 +486,8 @@ int evk_cmax_flow_variance_f32(const float *x, const float *y, const float *t, c
  * derivative of the f above (grad_f: batch floats on the device): with W_b = G(grad_f[b] df_b/dG), per kept event
  *   df/dx' = p[(1-dy)(W01-W00) + dy(W11-W10)],  df/dy' = p[(1-dx)(W10-W00) + dx(W11-W01)]
  * times t_rel, spread over the four grid_sample taps of the event's (x, y); taps outside the field get nothing.
- * workspace: evk_cmax_flow_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
+ * workspace: evk_cmax_flow_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call; 0 for
+ * arguments the entries reject (the canvas of every batched entry is at most 2^30 pixels (H+1)(W+1)).
  * Neither call synchronises, and both launch the same kernels whatever the batch. */
 size_t evk_cmax_flow_objective_workspace_bytes(int batch, int H, int W);
 int evk_cmax_flow_objective_f32(const float *x, const float *y, const float *t_rel, const float *p,
@@ -670,7 +671,8 @@ int evk_cmax_depth_grid_joint_candidates_f32(const float *x, const float *y, con
  *   df/dparams_k += p[(1-dy)(W01-W00) + dy(W11-W10)] dx'/dparams_k + p[(1-dx)(W10-W00) + dx(W11-W01)] dy'/dparams_k
  * For linvel this is not the reference's evaluate_gradient (objectives.py:251-264), which mixes the two
  * channels in its 3-D blur and multiplies by the un-blurred IWE.  No limit on the canvas size.
- * workspace: evk_cmax_motion_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
+ * workspace: evk_cmax_motion_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call; 0 for
+ * arguments the entries reject (the canvas of every batched entry is at most 2^30 pixels (H+1)(W+1)).
  * Neither call synchronises, and both launch the same kernels whatever the batch. */
 #define EVK_WARP_LINVEL 3
 #define EVK_WARP_AFFINE 4
@@ -828,7 +830,8 @@ int evk_cmax_motion_segment_assign_f32(const float *x, const float *y, const flo
  * four taps q = tau A_s + B_s, and
  *   df/dx' = (1-dy)(q01-q00) + dy(q11-q10),  df/dy' = (1-dx)(q10-q00) + dx(q11-q01)
  * times t_rel, spread over the four grid_sample taps of the event's (x, y); taps outside the field get nothing.
- * workspace: evk_flow_timestamp_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
+ * workspace: evk_flow_timestamp_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call; 0 for
+ * arguments the entries reject (the canvas of every batched entry is at most 2^30 pixels (H+1)(W+1)).
  * Neither call synchronises, and both launch the same kernels whatever the batch. */
 size_t evk_flow_timestamp_objective_workspace_bytes(int batch, int H, int W);
 int evk_flow_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau,
@@ -864,7 +867,8 @@ int evk_flow_timestamp_objective_grad_f32(const float *x, const float *y, const 
  * its four taps q = tau A_s + B_s,
  *   df/dx' = (1-dy)(q01-q00) + dy(q11-q10),  df/dy' = (1-dx)(q10-q00) + dx(q11-q01),
  *   df/dparams_k += df/dx' dx'/dparams_k + df/dy' dy'/dparams_k.
- * workspace: evk_motion_timestamp_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call.
+ * workspace: evk_motion_timestamp_objective_workspace_bytes(batch, H, W) bytes, 256-byte aligned, for either call; 0 for
+ * arguments the entries reject (the canvas of every batched entry is at most 2^30 pixels (H+1)(W+1)).
  * Neither call synchronises, and both launch the same kernels whatever the batch. */
 size_t evk_motion_timestamp_objective_workspace_bytes(int batch, int H, int W);
 int evk_motion_timestamp_objective_f32(const float *x, const float *y, const float *t_rel, const float *tau,
