@@ -30,9 +30,8 @@ VARIANT_GLOBAL_RED = 1 << 8
 VARIANT_VECTOR_RED = 2 << 8
 VARIANT_SMEM_TILE = 3 << 8
 VARIANT_WARP_AGG = 4 << 8
-VARIANT_ROUTED = 5 << 8
+VARIANT_ROUTED = 5 << 8           # evk.h: retired, the voxel entries treat it as VARIANT_AUTO
 VARIANT_MASK = 0xF << 8
-ROUTED_ABORT_MARK = 1 << 62       # evk.h: added to the oob counter when the routed kernel's watchdog fired
 TS_REVERSE = 0x80
 TS_RAW = 0x1000
 CMAX_WANT_GRAD = 0x10

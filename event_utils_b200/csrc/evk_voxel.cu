@@ -41,20 +41,10 @@ struct VoxelArgs {
     float *ws;   // [H*W][nq][4]
     unsigned long long *oob;
     const unsigned *skip_unless;  // launch-level choice between the plain and the hot-pixel instantiation: return unless *skip_unless != 0
-    const unsigned *skip_if;  // AUTO with the routed kernel in play: this kernel returns at once when *skip_if != 0 (the
-                              // probe chose the routed kernel, which has already built the grid)
+    const unsigned *skip_if;      // the same choice seen from the plain instantiation: return at once when *skip_if != 0
 };
 
 enum { SINK_SCALAR = 0, SINK_QUAD = 1, SINK_QUAD_HOT = 2 };
-
-// evk_voxel_routed.cu: output tiles in shared memory, events routed to the owning SM through L2-resident rings
-size_t voxel_routed_workspace_bytes(int B, int H, int W);
-bool voxel_routed_supported(int B, int H, int W);
-int launch_voxel_routed(const float *x, const float *y, const float *t, const float *p, int64_t n, int64_t head, float t0, float dt,
-                        int B, int H, int W, int auto_span, float *out, void *workspace, size_t workspace_bytes,
-                        unsigned long long *oob, cudaStream_t st, int probe);
-const unsigned *voxel_routed_mode_flag(void *workspace, int B, int H, int W);   // device word the probe writes: 1 = routed ran
-int64_t voxel_routed_min_events();
 
 // Per-CTA write-combining cache in front of the vector reductions (SINK_QUAD_HOT): a direct-mapped
 // {quad index -> float4 partial sum} table in shared memory, same idea as evk_hot.cu.  Real sensors
@@ -418,9 +408,8 @@ __global__ void __launch_bounds__(kThreads, EVK_VOXEL_MIN_CTAS) voxel_scatter_ke
 // also in quad b/3-1 (slot 3).
 template <bool ACCUM>
 __global__ void __launch_bounds__(256) voxel_fold_kernel(const float *__restrict__ ws, float *__restrict__ out,
-                                                         int64_t npix, int B, int nq, const unsigned *skip_if = nullptr)
+                                                         int64_t npix, int B, int nq)
 {
-    if (skip_if && *skip_if) return;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t pix = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pix < npix; pix += stride) {
         const float4 *src = reinterpret_cast<const float4 *>(ws) + pix * nq;
@@ -614,38 +603,19 @@ static int launch_voxel(const VoxelArgs &A0, unsigned flags, int layout, cudaStr
     const bool accum = (flags & EVK_ACCUMULATE) != 0;
     const int64_t npix = (int64_t)A.H * A.W;
     unsigned variant = variant_of(flags);
+    if (variant == EVK_VARIANT_ROUTED) variant = EVK_VARIANT_AUTO;   // retired variant (evk.h)
     // AUTO: big streams take the vector-red path with the adaptive hot-pixel cache; small ones the
     // scalar path (no workspace, no fold).  SMEM_TILE forces the cache on, VECTOR_RED leaves it out.
     bool hot = false;
-    bool routed_probe = false;
     if (variant == EVK_VARIANT_AUTO) {
         variant = (A.n >= (int64_t)1 << 20 && workspace != nullptr) ? EVK_VARIANT_VECTOR_RED : EVK_VARIANT_GLOBAL_RED;
         hot = variant == EVK_VARIANT_VECTOR_RED && !bil;
-        // large plain streams: a probe looks at a sample of the events on the device and picks the routed kernel (unit
-        // polarities, no hot pixels) or the vector-reduction kernel below; the one not chosen returns at once
-        routed_probe = A.n >= voxel_routed_min_events() && !bil && !A.negpos && !(flags & EVK_NO_FOLD) && !accum && layout == LAYOUT_SOA4 &&
-                       voxel_routed_supported(A.B, A.H, A.W) && workspace != nullptr &&
-                       workspace_bytes >= voxel_routed_workspace_bytes(A.B, A.H, A.W) + (size_t)npix * quads_for_bins(A.B) * 16;
     } else if (variant == EVK_VARIANT_SMEM_TILE && !bil) {
         variant = EVK_VARIANT_VECTOR_RED;
         hot = true;
         A.hot_force = 1;
     }
     const bool no_fold = (flags & EVK_NO_FOLD) != 0;
-    if (variant == EVK_VARIANT_ROUTED &&
-        (bil || A.negpos || no_fold || layout != LAYOUT_SOA4 || !voxel_routed_supported(A.B, A.H, A.W) ||
-         workspace == nullptr || workspace_bytes < voxel_routed_workspace_bytes(A.B, A.H, A.W))) {
-        // the routed kernel covers the plain (nearest, combined) grid on f32 SoA arrays with a common alignment whose
-        // B*H*W/SMs cells fit in shared memory; everything else takes the automatic choice
-        variant = (A.n >= (int64_t)1 << 20 && workspace != nullptr) ? EVK_VARIANT_VECTOR_RED : EVK_VARIANT_GLOBAL_RED;
-        hot = variant == EVK_VARIANT_VECTOR_RED && !bil;
-    }
-    if (variant == EVK_VARIANT_ROUTED) {
-        if (!accum) EVK_CUDA(cudaMemsetAsync(A.out, 0, (size_t)npix * A.B * sizeof(float), st));
-        if (A.n == 0) return EVK_OK;
-        return launch_voxel_routed(A.x, A.y, A.t, A.p, A.n, A.head, A.t0, A.dt, A.B, A.H, A.W, A.auto_span, A.out, workspace,
-                                   workspace_bytes, A.oob, st, 0);
-    }
     if (no_fold) {
         // the caller folds (and reduces across GPUs) itself: the sums stay in the quad workspace
         if (bil || A.negpos || workspace == nullptr) { set_error("evk_voxel: EVK_NO_FOLD needs a workspace and the plain (nearest, combined) grid"); return EVK_E_UNSUPPORTED; }
@@ -655,20 +625,6 @@ static int launch_voxel(const VoxelArgs &A0, unsigned flags, int layout, cudaStr
     if (variant != EVK_VARIANT_VECTOR_RED && variant != EVK_VARIANT_GLOBAL_RED) {
         set_error("evk_voxel: variant 0x%x not available for this entry point", variant);
         return EVK_E_UNSUPPORTED;
-    }
-    // probe mode: ONE timed scope for "probe + the kernel it selects" (the inner scopes of the two alternatives nest in it)
-    struct OptScope { ProfScope *p = nullptr; ~OptScope() { delete p; } } outer;
-    if (routed_probe) {
-        outer.p = new ProfScope(st);
-        // the routed kernel's rings come first in the workspace, the quad workspace of the fallback after them
-        EVK_CUDA(cudaMemsetAsync(A.out, 0, (size_t)npix * A.B * sizeof(float), st));
-        int rc = launch_voxel_routed(A.x, A.y, A.t, A.p, A.n, A.head, A.t0, A.dt, A.B, A.H, A.W, A.auto_span, A.out, workspace,
-                                     workspace_bytes, A.oob, st, 1);
-        if (rc) return rc;
-        A.skip_if = voxel_routed_mode_flag(workspace, A.B, A.H, A.W);
-        const size_t roff = (voxel_routed_workspace_bytes(A.B, A.H, A.W) + 255) & ~(size_t)255;
-        workspace = static_cast<char *>(workspace) + roff;
-        workspace_bytes -= roff;
     }
     const int sink = (variant == EVK_VARIANT_VECTOR_RED) ? SINK_QUAD : SINK_SCALAR;
     A.nq = quads_for_bins(A.B);
@@ -683,7 +639,7 @@ static int launch_voxel(const VoxelArgs &A0, unsigned flags, int layout, cudaStr
         A.ws = static_cast<float *>(workspace);
         EVK_CUDA(cudaMemsetAsync(A.ws, 0, need, st));
         const size_t flag_off = (need + 255) & ~(size_t)255;
-        if (workspace_bytes >= flag_off + 256 && !A.skip_if) hot_flag = reinterpret_cast<unsigned *>(static_cast<char *>(workspace) + flag_off);
+        if (workspace_bytes >= flag_off + 256) hot_flag = reinterpret_cast<unsigned *>(static_cast<char *>(workspace) + flag_off);
     } else if (!accum) {
         EVK_CUDA(cudaMemsetAsync(A.out, 0, (size_t)npix * A.B * sizeof(float) * grids, st));
     }
@@ -708,10 +664,9 @@ static int launch_voxel(const VoxelArgs &A0, unsigned flags, int layout, cudaStr
                 if (layout == LAYOUT_SOA4 || layout == LAYOUT_SOA1) voxel_hot_probe_kernel<LAYOUT_SOA1><<<1, 1024, 0, st>>>(A, hot_flag);
                 else if (layout == LAYOUT_PACKED) voxel_hot_probe_kernel<LAYOUT_PACKED><<<1, 1024, 0, st>>>(A, hot_flag);
                 else voxel_hot_probe_kernel<LAYOUT_AOS><<<1, 1024, 0, st>>>(A, hot_flag);
-                const unsigned *outer_skip = A.skip_if;
                 A.skip_if = hot_flag;                          // plain kernel: unless the probe found contention
                 EVK_DISPATCH_L(SINK_QUAD, false);
-                A.skip_if = outer_skip;
+                A.skip_if = nullptr;
                 A.skip_unless = hot_flag;                      // table kernel: only if it did
                 A.hot_force = 1;
                 EVK_DISPATCH_L(SINK_QUAD_HOT, false);
@@ -725,8 +680,6 @@ static int launch_voxel(const VoxelArgs &A0, unsigned flags, int layout, cudaStr
 #undef EVK_LAUNCH
         EVK_CUDA(cudaGetLastError());
     }
-    delete outer.p;
-    outer.p = nullptr;
     if (sink == SINK_QUAD && !no_fold) {
         const int grid = grid_simple(npix, 256);
         prof_count(1);
@@ -738,8 +691,8 @@ static int launch_voxel(const VoxelArgs &A0, unsigned flags, int layout, cudaStr
                 const float *wsg = A.ws + (size_t)g * npix * A.nq * 4;
                 float *og = A.out + (size_t)g * npix * A.B;
                 if (g) prof_count(1);
-                if (accum) voxel_fold_kernel<true><<<grid, 256, 0, st>>>(wsg, og, npix, A.B, A.nq, A.skip_if);
-                else voxel_fold_kernel<false><<<grid, 256, 0, st>>>(wsg, og, npix, A.B, A.nq, A.skip_if);
+                if (accum) voxel_fold_kernel<true><<<grid, 256, 0, st>>>(wsg, og, npix, A.B, A.nq);
+                else voxel_fold_kernel<false><<<grid, 256, 0, st>>>(wsg, og, npix, A.B, A.nq);
             }
         }
         EVK_CUDA(cudaGetLastError());
@@ -772,14 +725,7 @@ size_t evk_voxel_workspace_bytes(int B, int H, int W, unsigned flags)
     if (!evk::voxel_grid_ok(B, H, W)) return 0;
     if (flags & EVK_BILINEAR) return (size_t)B * H * W * 4 * sizeof(float);   // 2x2 blocks per bin
     size_t need = (size_t)H * W * evk::quads_for_bins(B) * 4 * sizeof(float);      // temporal quads per pixel
-    need = ((need + 255) & ~(size_t)255) + 256;                                    // + the launch-level contention verdict
-    const unsigned v = evk::variant_of(flags);
-    if ((v == EVK_VARIANT_AUTO || v == EVK_VARIANT_ROUTED) && evk::voxel_routed_supported(B, H, W)) {
-        // the routed kernel's rings, followed (AUTO) by the quad workspace of the kernel the probe may choose instead
-        const size_t r = (evk::voxel_routed_workspace_bytes(B, H, W) + 255) & ~(size_t)255;
-        need = (v == EVK_VARIANT_AUTO) ? r + need : (r > need ? r : need);
-    }
-    return need;
+    return ((need + 255) & ~(size_t)255) + 256;                                    // + the launch-level contention verdict
 }
 
 int evk_voxel_f32(const float *x, const float *y, const float *t, const float *p, int64_t n, float t0,

@@ -84,15 +84,10 @@ def aos_base(xs, ys, ts, ps):
     return torch.as_strided(xs, (n, 4), (4, 1))
 
 
-def raise_if_oob(counter, what, shape, always=False):
-    """Reproduce the reference's IndexError (image.py:96-99) from the device counter.  `always`: read the counter even
-    with config.check_index_errors off (the routed voxel kernel reports its watchdog through it)."""
-    if not (config.check_index_errors or always):
+def raise_if_oob(counter, what, shape):
+    """Reproduce the reference's IndexError (image.py:96-99) from the device counter."""
+    if not config.check_index_errors:
         return
     bad = int(counter.item())
-    if bad >= _lib.ROUTED_ABORT_MARK:
-        counter.zero_()
-        raise RuntimeError("the routed voxel kernel's watchdog gave up (no progress for 0.5 s): the %s is incomplete; "
-                           "use another config.variant" % what)
-    if bad and config.check_index_errors:
+    if bad:
         raise IndexError("%d events index outside the %s of shape %s" % (bad, what, tuple(shape)))

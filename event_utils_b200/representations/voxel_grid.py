@@ -4,7 +4,6 @@ Same signatures and return types; the work is one CUDA pass over the events
 (csrc/evk_voxel.cu) instead of B passes of ~15 temporaries each.
 """
 import ctypes
-import os
 
 import numpy as np
 import torch
@@ -12,8 +11,6 @@ import torch
 from .. import _lib, config
 from . import _events as E
 from .image import events_to_image, events_to_image_torch  # noqa: F401  (re-exported like the reference)
-
-_ROUTED_AUTO = os.environ.get("EVK_VOXEL_ROUTED_MIN", "") not in ("", "0")
 
 
 def _voxel_device(x, y, t, p, t0, dt, B, H, W, flags=0, aos=None, out=None):
@@ -34,8 +31,7 @@ def _voxel_device(x, y, t, p, t0, dt, B, H, W, flags=0, aos=None, out=None):
             _lib.check(L.evk_voxel_f32(_lib.ptr(x), _lib.ptr(y), _lib.ptr(t), _lib.ptr(p), x.shape[0], t0, dt,
                                        B, H, W, flags, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.ptr(oob),
                                        _lib.stream()))
-        # the routed kernel (explicit variant, or AUTO with EVK_VOXEL_ROUTED_MIN set) reports its watchdog through the counter
-        E.raise_if_oob(oob, "voxel grid", (B, H, W), always=(flags & _lib.VARIANT_MASK) == _lib.VARIANT_ROUTED or _ROUTED_AUTO)
+        E.raise_if_oob(oob, "voxel grid", (B, H, W))
     return out
 
 

@@ -63,11 +63,7 @@ extern "C" {
                                                           * fixed-point write-combining table (forced on; AUTO probes for contention); cmax = the whole image of
                                                           * warped events in the CTA's shared memory, flushed by TMA bulk reductions (cmax_onchip_kernel) */
 #define EVK_VARIANT_WARP_AGG (4u << EVK_VARIANT_SHIFT)   /* warp-aggregated (match.any) global reds, for hot-spot streams */
-#define EVK_VARIANT_ROUTED (5u << EVK_VARIANT_SHIFT)     /* voxel: output tiles in shared memory, events routed to the owning SM through L2-resident rings; tiles leave by TMA bulk reduction (correct, 2x SLOWER than AUTO: opt-in, DESIGN.md section 4) */
-/* The routed kernel is a cooperative web of spin waits; a watchdog inside it gives up after 0.5 s without progress
- * (the kernel takes about 1.5 ms per 50 M events on H100), lets the launch end with an INCOMPLETE grid and adds this mark to the
- * caller's `oob` counter -- the device never hangs.  Counter values >= the mark mean "result invalid", not index errors. */
-#define EVK_ROUTED_ABORT_MARK (1ull << 62)
+#define EVK_VARIANT_ROUTED (5u << EVK_VARIANT_SHIFT)     /* voxel: retired, the same as EVK_VARIANT_AUTO (DESIGN.md section 4); the value stays for binary compatibility */
 
 #define EVK_TS_REVERSE 0x80u  /* timestamp images: timestamp_reverse=True (image.py:318-319) */
 #define EVK_TS_RAW 0x1000u    /* timestamp images: normalize_timestamps=False (image.py:261): weights = t as given */

@@ -391,7 +391,7 @@ WORKSPACE_FACTOR = {"evk_voxel_negpos_f32": 2}     # evk.h: 2 * evk_voxel_worksp
 ACC_FLAG, BILINEAR, CLIP, NEGPOS_TRUTHY = 0x1, 0x2, 0x4, 0x8
 TS_REVERSE, TS_RAW = 0x80, 0x1000
 WINDOW_PAIRS, WINDOW_NEGPOS, AUTO_SPAN = 0x100000, 0x400000, 0x200000
-AUTO, GLOBAL_RED, VECTOR_RED, SMEM_TILE, WARP_AGG = (v << 8 for v in (0, 1, 2, 3, 4))   # never ROUTED, AUTO only below 2^20 events
+AUTO, GLOBAL_RED, VECTOR_RED, SMEM_TILE, WARP_AGG = (v << 8 for v in (0, 1, 2, 3, 4))   # AUTO only below 2^20 events
 CMAX_WANT_GRAD = 0x10
 
 

@@ -128,8 +128,8 @@ def exact_streams(seed, kind, n, fine=20000, pos_frac=None):
     """One exactly summable stream of `n` events for the scatter path `kind`:
       voxel     B = 5, t0 = 0.5, dt = 2: tau = (t - t0) / dt * 4 is a multiple of 2^-6 in [-1, 5].  Hot pixel A (96 %
                 of the hot events): p = +-1 at tau = 0, one integer tap in bin 0 (g = 0), so that one table slot takes
-                all of it; hot pixel B (4 %): tau = 7/2, taps of 1/2 in bins 3 and 4 (g = 1), so that the routed tile
-                carries from both of an event's bins.  + run 60 %, - run 40 %: every CTA of the table launches wraps
+                all of it; hot pixel B (4 %): tau = 7/2, taps of 1/2 in bins 3 and 4 (g = 1), so that hot events with
+                two taps are summed too.  + run 60 %, - run 40 %: every CTA of the table launches wraps
                 up and back down (mostly with a zero net carry, so a carry of one direction that is lost or
                 mis-signed shows)
       nearest   hot p = +-2^19: in the 2^10 image table q = 2^29, so a slot wraps every four same-sign adds

@@ -105,7 +105,7 @@ def assert_scalar_within(out, ref, bound, what=""):
 # ---- exactly summable streams (tests/edge_cases.py exact_streams) ----------------------------------------------------
 EXACT_C = 2048            # CTAs that may share a cell in the image and cmax table paths (at most one wave: 4 per SM)
 # The voxel hot-table kernel holds 40 KB of static shared memory, so at most 5 of its CTAs fit on an SM; its launches
-# cover 4 waves: 20 CTAs per SM, 4096 up to 204 SMs.  The routed tile has one owner CTA per cell.
+# cover 4 waves: 20 CTAs per SM, 4096 up to 204 SMs.
 VOXEL_C = 4096
 
 
@@ -237,18 +237,15 @@ def table_launches(c, sms):
     """The table launches of the exact-sum tests on a GPU with `sms` SMs, as the launch code sizes them, and the value
     each event adds to the hottest slot: [(name, v, F, C, threads, vec)].
       voxel     grid_for: 4096 events per CTA (16-byte aligned SoA) / 1024 (misaligned SoA, AoS, packed), capped at 4
-                waves of 4 or 5 resident CTAs per SM (both checked); slot = hot pixel A, bin 0.  Routed: the tile's
-                one owner CTA takes every event of a cell; slot = hot pixel B, bin 4 (the second bin of tau = 7/2)
+                waves of 4 or 5 resident CTAs per SM (both checked); slot = hot pixel A, bin 0
       images    one wave of 512-thread CTAs, 8192 events per CTA, 16-byte loads; slot = the hot point
       cmax      on-chip image: ceil(n / 8192) CTAs, at most one per SM, 1024 threads, two f64 events per 16-byte load"""
     n, k = c["x"].shape[0], c["kind"]
     g, p = c["group"], c["p"].astype(np.float64)
     if k == "voxel":
         v = np.where((g == 1) & (c["t"] == c["t0"]), p, 0.0)
-        out = [("voxel soa4", v, 22, min(-(-n // 4096), sms * 20), 256, 4)]
-        out += [("voxel 1024/CTA r=%d" % r, v, 22, min(-(-n // 1024), sms * r * 4), 256, 1) for r in (4, 5)]
-        out.append(("routed tile", np.where(g == 2, 0.5 * p, 0.0), 22, 1, 1, 1))
-        return out
+        return [("voxel soa4", v, 22, min(-(-n // 4096), sms * 20), 256, 4)] + \
+               [("voxel 1024/CTA r=%d" % r, v, 22, min(-(-n // 1024), sms * r * 4), 256, 1) for r in (4, 5)]
     if k == "nearest":
         return [("nearest", np.where(g == 1, p, 0.0), 10, -(-n // 8192), 512, 4)]
     if k == "bilinear":
@@ -257,9 +254,8 @@ def table_launches(c, sms):
 
 
 def assert_tables_wrap(c, sms, what=""):
-    """Every CTA's hot slot wraps upward and back downward in every table launch of the stream; the image, cmax and
-    routed cells also receive a non-zero net carry over all CTAs, which a carry sent to the wrong cell cannot hide
-    behind."""
+    """Every CTA's hot slot wraps upward and back downward in every table launch of the stream; the image and cmax
+    cells also receive a non-zero net carry over all CTAs, which a carry sent to the wrong cell cannot hide behind."""
     for name, v, F, C, threads, vec in table_launches(c, sms):
         up, down, net = table_wraps(v, F, C, threads, vec)
         assert up.min() >= 1 and down.min() >= 1, "%s %s: a CTA's slot wraps %d up / %d down" % (

@@ -4,7 +4,6 @@ oracle's exact per-cell sums (exact_bounds.assert_within_exact: |gpu - exact| <=
 out-of-range counts exactly.  A tap that is lost, doubled or sent to the wrong cell shows up in the cell it belongs to,
 however hot the rest of the image is."""
 import ctypes
-import os
 
 import numpy as np
 import pytest
@@ -48,11 +47,8 @@ def _lib():
 
 def _voxel_variants():
     _l, _ = _lib()
-    v = [("auto", _l.VARIANT_AUTO), ("global_red", _l.VARIANT_GLOBAL_RED), ("vector_red", _l.VARIANT_VECTOR_RED),
-         ("smem_tile", _l.VARIANT_SMEM_TILE)]
-    if os.environ.get("EVK_TEST_ROUTED", "1") != "0":
-        v.append(("routed", _l.VARIANT_ROUTED))
-    return v
+    return [("auto", _l.VARIANT_AUTO), ("global_red", _l.VARIANT_GLOBAL_RED), ("vector_red", _l.VARIANT_VECTOR_RED),
+            ("smem_tile", _l.VARIANT_SMEM_TILE)]
 
 
 # ---- voxel grids -----------------------------------------------------------------------------------------------------

@@ -2,9 +2,9 @@
 (tests/edge_cases.py exact_streams): every tap is a multiple of 2^-g and no partial sum any summation order, quantisation,
 flush or carry can form exceeds 2^(24-g), so each output cell must equal the f64 sum of its taps exactly
 (exact_bounds.assert_exact).  The hot cells carry most of the events with their signs in one + run and one - run, so
-the shared-memory tables of the voxel hot path (F = 22), the image hot kernel (nearest F = 10, bilinear F = 22), the
-cmax on-chip image (F = 22) and the routed voxel tile (F = 22) wrap and carry upward and downward; a lost, doubled,
-misplaced, mis-signed or biased carry, tap or flush shows in the cell it belongs to, whatever its size."""
+the shared-memory tables of the voxel hot path (F = 22), the image hot kernel (nearest F = 10, bilinear F = 22) and the
+cmax on-chip image (F = 22) wrap and carry upward and downward; a lost, doubled, misplaced, mis-signed or biased carry,
+tap or flush shows in the cell it belongs to, whatever its size."""
 import ctypes
 import functools
 

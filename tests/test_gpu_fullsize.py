@@ -48,9 +48,7 @@ def test_config2_voxel_50m_every_variant_cell_by_cell(oracle, voxel_stream):
     assert ref.shape == (5, 480, 640) and abs(float(ref.astype(np.float64).sum()) - float(p.astype(np.float64).sum())) <= 2.0
     X, Y, T, P = (torch.from_numpy(a).cuda() for a in (x, y, t, p))
     worst = {}
-    for variant in (None, "global_red", "vector_red", "smem_cache", "routed"):
-        if variant == "routed" and __import__("os").environ.get("EVK_TEST_ROUTED", "1") == "0":
-            continue
+    for variant in (None, "global_red", "vector_red", "smem_cache"):
         eu.config.variant = variant
         out = events_to_voxel_torch(X, Y, T, P, 5, sensor_size=(480, 640)).cpu().numpy()
         assert_close_to_max(out, ref, 1e-5, "voxel 50M variant=%s" % variant)

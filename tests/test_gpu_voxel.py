@@ -10,12 +10,7 @@ from conftest import assert_close_to_max, golden, make_events
 
 pytestmark = pytest.mark.gpu
 
-import os as _os
-
-# the routed kernel spins on inter-SM queues; its in-kernel watchdog turns a protocol stall into a RuntimeError instead of a
-# hang.  tools/try_routed.py is the stand-alone gate; EVK_TEST_ROUTED=0 keeps the variant out of this suite
-ROUTED = ["routed"] if _os.environ.get("EVK_TEST_ROUTED", "1") != "0" else []
-VARIANTS = ["global_red", "vector_red", "smem_cache"] + ROUTED + [None]
+VARIANTS = ["global_red", "vector_red", "smem_cache", None]
 
 
 @pytest.fixture(autouse=True)
@@ -165,45 +160,38 @@ def test_hot_pixels(oracle):
         assert np.abs(vp.cpu().numpy() - refp).max() <= bound, variant
 
 
-@pytest.mark.skipif(not ROUTED, reason="EVK_TEST_ROUTED=0")
-def test_auto_probe_picks_between_routed_and_vector_red():
-    """AUTO with the routed kernel enabled (EVK_VOXEL_ROUTED_MIN, read once at library load -> a subprocess): a device-side
-    probe looks at a sample of the stream; unit-polarity uniform streams take the routed kernel, general polarities and
-    hot-pixel streams the vector-reduction kernel; the kernel not chosen returns at once.  All three equal the oracle."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    script = r'''
-import sys
-import numpy as np, torch
-sys.path.insert(0, %r)
-from event_utils_b200.representations.voxel_grid import events_to_voxel_torch
-from oracle import evk_oracle as O
-O.build()
-rng = np.random.default_rng(3)
-n, H, W = 3_000_000, 260, 346
-x = (rng.random(n) * (W - 1)).astype(np.float32); y = (rng.random(n) * (H - 1)).astype(np.float32)
-t = np.sort(rng.random(n)).astype(np.float32)
-cases = {"unit": (x, y, (rng.integers(0, 2, n) * 2 - 1).astype(np.float32)),
-         "general": (x, y, rng.standard_normal(n).astype(np.float32))}
-xh, yh = x.copy(), y.copy()
-hot = rng.random(n) < 0.2
-xh[hot], yh[hot] = 17.0, 33.0
-cases["hot"] = (xh, yh, cases["unit"][2])
-for name, (cx, cy, cp) in cases.items():
-    ref = O.voxel_f32(cx, cy, t, cp, 5, (H, W))
-    out = events_to_voxel_torch(*(torch.from_numpy(a).cuda() for a in (cx, cy, t, cp)), 5, sensor_size=(H, W)).cpu().numpy()
-    err = np.abs(out - ref).max() / np.abs(ref).max()
-    # the hot pixel sums 6e5 signed f32 taps: the sequential f32 oracle itself is ~sqrt(n) eps away from the exact sum
-    # (order-dependent, see test_hot_pixels_*), so that case gets the random-walk allowance instead of 1e-5
-    assert err <= (2e-4 if name == "hot" else 1e-5), (name, err)
-    print(name, "ok %%.2e" %% err)
-''' % root
-    out = subprocess.run([sys.executable, "-c", script], capture_output=True, text=True, timeout=600, cwd=root,
-                         env=dict(os.environ, EVK_VOXEL_ROUTED_MIN="1000000"))
-    assert out.returncode == 0, out.stdout[-2000:] + out.stderr[-3000:]
-    assert "hot ok" in out.stdout
+def test_routed_variant_is_auto():
+    """EVK_VARIANT_ROUTED is a retired value that means AUTO: the same workspace query and, on exactly summable streams
+    (p = +-1, t on a 2^-10 grid, t0 = 0, dt = 1) below and above AUTO's 2^20-event switch, the same grid bit for bit."""
+    import event_utils_b200 as eu
+    from event_utils_b200 import _lib
+    from event_utils_b200.representations.voxel_grid import events_to_voxel_torch
+    L = _lib.lib()
+    for shape in ((5, 480, 640), (5, 260, 346), (1, 10, 10), (8, 10, 10)):
+        for extra in (0, _lib.BILINEAR):
+            assert L.evk_voxel_workspace_bytes(*shape, _lib.VARIANT_ROUTED | extra) == L.evk_voxel_workspace_bytes(*shape, extra)
+    B, H, W = 5, 260, 346
+    rng = np.random.default_rng(5)
+    oob = torch.zeros(1, dtype=torch.int64, device="cuda")
+    for n in (300_000, 3_000_000):
+        x = (rng.random(n) * (W - 1)).astype(np.float32)
+        y = (rng.random(n) * (H - 1)).astype(np.float32)
+        t = (np.sort(rng.integers(0, 1025, n)) / 1024).astype(np.float32)
+        t[0], t[-1] = 0.0, 1.0
+        p = (rng.integers(0, 2, n) * 2 - 1).astype(np.float32)
+        X, Y, T, P = dev(x, y, t, p)
+        grids = []
+        for variant in (_lib.VARIANT_AUTO, _lib.VARIANT_ROUTED):
+            out = torch.empty((B, H, W), device="cuda")
+            ws = torch.empty(L.evk_voxel_workspace_bytes(B, H, W, variant), dtype=torch.uint8, device="cuda")
+            _lib.check(L.evk_voxel_f32(X.data_ptr(), Y.data_ptr(), T.data_ptr(), P.data_ptr(), n, 0.0, 1.0, B, H, W, variant,
+                                       out.data_ptr(), ws.data_ptr(), ws.numel(), oob.data_ptr(), None))
+            grids.append(out.cpu().numpy())
+        assert int(oob.item()) == 0
+        assert np.array_equal(grids[0], grids[1]), n
+        assert float(grids[0].astype(np.float64).sum()) == float(p.astype(np.float64).sum()), n
+        eu.config.variant = "routed"
+        assert np.array_equal(events_to_voxel_torch(X, Y, T, P, B, sensor_size=(H, W)).cpu().numpy(), grids[0]), n
 
 
 def test_host_pipeline_pageable_and_pinned(oracle):

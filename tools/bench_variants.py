@@ -60,8 +60,7 @@ ws = torch.empty(L.evk_voxel_workspace_bytes(B, H, W, 0), dtype=torch.uint8, dev
 oob = torch.zeros(1, dtype=torch.int64, device=dev)
 t0, dt = float(t[0]), float(t[-1] - t[0])
 print("== voxel %d events -> %dx%dx%d" % (N, B, H, W))
-ws = torch.empty(max(ws.numel(), L.evk_voxel_workspace_bytes(B, H, W, _lib.VARIANT_ROUTED)), dtype=torch.uint8, device=dev)
-for name, v in (("global_red", _lib.VARIANT_GLOBAL_RED), ("vector_red", _lib.VARIANT_VECTOR_RED), ("routed", _lib.VARIANT_ROUTED)):
+for name, v in (("global_red", _lib.VARIANT_GLOBAL_RED), ("vector_red", _lib.VARIANT_VECTOR_RED)):
     def run(v=v, fl=0):
         _lib.check(L.evk_voxel_f32(x.data_ptr(), y.data_ptr(), t.data_ptr(), p.data_ptr(), N, t0, dt, B, H, W, v | fl,
                                    out.data_ptr(), ws.data_ptr(), ws.numel(), oob.data_ptr(), None))
@@ -72,7 +71,7 @@ xh, yh = x.clone(), y.clone()
 hm = torch.rand(N, device=dev) < 0.10
 xh[hm] = torch.where(torch.rand(int(hm.sum()), device=dev) < 0.5, 17.0, 400.0)
 yh[hm] = torch.where(xh[hm] == 17.0, 33.0, 301.0)
-for name, v in (("vector_red", _lib.VARIANT_VECTOR_RED), ("smem_cache", _lib.VARIANT_SMEM_TILE), ("routed", _lib.VARIANT_ROUTED), ("auto", 0)):
+for name, v in (("vector_red", _lib.VARIANT_VECTOR_RED), ("smem_cache", _lib.VARIANT_SMEM_TILE), ("auto", 0)):
     for tag, (xx, yy) in (("uniform", (x, y)), ("10% hot pixels", (xh, yh))):
         def run(v=v, xx=xx, yy=yy):
             _lib.check(L.evk_voxel_f32(xx.data_ptr(), yy.data_ptr(), t.data_ptr(), p.data_ptr(), N, t0, dt, B, H, W, v,
